@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- UNet steps/sec of the Paint-with-Words denoising loop on B200 (BASELINE.json metric).
+"""bench.py -- UNet steps/sec of the Paint-with-Words denoising loop on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
 
 Workload (config.workload): BASELINE.json configs[1] -- aurora_1 colour map, SD1.5-shaped UNet (seeded random
@@ -21,7 +21,11 @@ One JSON line on stdout (rank 0):
              with 16 images per launch; `dense_pair` times the round-1 two-launch path on the same inputs
   reference_gpu_eager   comparison only: the reference's loop and inj_forward op sequence as eager fp16 PyTorch on this GPU
   cpu_baseline  the oracle port of the reference loop on this box's host cores (rank 0, N=1 only), bounded sample
+  device     name and power limit of the GPU the numbers were measured on
 --impl reference: only that CPU loop (the reference is pure Python/torch; its CPU path is what is timed).
+--dump-outputs DIR: after the timed steps, the latents the last timed step produced (what a caller of the sampler
+receives) as DIR/latents.npy (float32).  Inputs are seeded, so two builds run with the same arguments can be compared
+output for output.
 """
 from __future__ import annotations
 
@@ -64,12 +68,12 @@ def workload_config(n_gpus: int, cfg_id: int = 2, images_per_gpu: int = 1) -> di
             "images_per_gpu": images_per_gpu, "unet_batch": 2 * images_per_gpu, "global_images": total,
             "latent": [4, size // 8, size // 8], "tokens": 77,
             "parallelism": f"image-sharded x{n_gpus}, weights replicated (1 broadcast), no per-step collective",
-            "l2_policy": "inputs larger than L2: each step streams the fp16 UNet weights (1.7 GB; L2 is 126 MB)"}
+            "l2_policy": "inputs larger than L2: each step streams the fp16 UNet weights (1.7 GB; L2 is 50 MB)"}
 
 
 # BASELINE.json configs (1-based, BASELINE.md section 4 numbering).  The driver runs the default (2 = configs[1], the
-# configuration the metric is quoted on); `--config N` measures the others with the same machinery
-# (scripts/bench_configs.sh fills BASELINE.md's table from them).  "weak": one image per GPU; "strong": a fixed set of
+# configuration the metric is quoted on); `--config N` measures the others with the same machinery.
+# "weak": one image per GPU; "strong": a fixed set of
 # images sharded over the GPUs (image i -> rank i mod G).
 CONFIGS = {
     1: dict(tag="configs[0]", what="runner.py cat/dog colour map, SD1.5-shape UNet 256x256, 10-step LMS, CFG 7.5 "
@@ -135,23 +139,13 @@ def build_images(cfg: dict, device, image_ids, tok, enc, sch):
     return conds, unconds, torch.cat(lats, 0).to(device), extra
 
 
-def ncu_traffic(key: str):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` capture of the
-    one-launch kernel (profiles/r02_xattn_traffic.json, written by scripts/ncu_summary.py); None if absent."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02_xattn_traffic.json")) as f:
-            return float(json.load(f)[key]["traffic_bytes"])
-    except Exception:
-        return None
-
-
 def measured_peaks():
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             p = json.load(f)
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -406,7 +400,7 @@ def xattn_roofline(device, B: int, biased: int, N=4096, H=8, D=40, T=77, target_
 
 
 def eager_torch_xattn_us(device, N=4096, H=8, D=40, T=77, iters=20, dtype=torch.float16):
-    """Comparison only (SURVEY 8d: "time the reference path on the B200"): the op sequence of the reference's
+    """Comparison only (SURVEY 8d: "time the reference path on the GPU"): the op sequence of the reference's
     inj_forward between to_q/to_k/to_v and to_out (paint_with_words.py:83-118) as eager PyTorch on this device, for
     one conditional call (bias = 0.4*w*log(1+sigma)*qk.max()) plus one unconditional call -- the work one B=2 launch
     pair (pww_xattn_stats_f16 + pww_xattn_fwd_f16) of this repo does.  Returns microseconds per cond+uncond pair."""
@@ -526,6 +520,26 @@ def _claim_stdout():
         os.dup2(2, 1)
 
 
+def dump_outputs(out_dir: str, latents: torch.Tensor, rank: int) -> None:
+    """The latents the timed path returned after its last step, float32, one file per rank."""
+    os.makedirs(out_dir, exist_ok=True)
+    name = "latents.npy" if rank == 0 else f"latents_rank{rank}.npy"
+    np.save(os.path.join(out_dir, name), latents.detach().float().cpu().numpy())
+
+
+def device_info(index: int) -> dict:
+    """Name and power limit of the GPU: part of every number this script reports."""
+    info = {"name": torch.cuda.get_device_name(index), "power_limit_w": None, "sm_max_mhz": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
+                            "-i", str(index)], capture_output=True, text=True, timeout=20)
+        pl, mx = [c.strip() for c in r.stdout.strip().split(",")[:2]]
+        info["power_limit_w"], info["sm_max_mhz"] = float(pl), float(mx)
+    except Exception:
+        pass
+    return info
+
+
 def emit(line: dict):
     data = (json.dumps(line) + "\n").encode()
     if _REAL_STDOUT is None:
@@ -543,7 +557,9 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true")
-    ap.add_argument("--quick", action="store_true", help="timed region only (for ncu launch lists): no e2e/roofline/cpu legs")
+    ap.add_argument("--quick", action="store_true", help="timed region only: no e2e/roofline/cpu legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the latents of the last timed step to DIR/latents.npy (float32)")
     ap.add_argument("--config", type=int, default=2, choices=sorted(CONFIGS),
                     help="BASELINE.json config (1-based); 2 = configs[1], the one the metric is quoted on (default)")
     args = ap.parse_args()
@@ -553,7 +569,7 @@ def main():
         run_reference_arm(args, rank)
         return
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a CUDA device (B200); use --impl reference for the CPU arm")
+        raise SystemExit("bench.py needs a CUDA device (H100); use --impl reference for the CPU arm")
     args.warmup = max(args.warmup, 3)
     device = torch.device("cuda", local_rank)
     torch.cuda.set_device(device)
@@ -629,6 +645,8 @@ def main():
         with ClockSampler(local_rank) as clk:
             ms = timed_region(args.steps)
         clocks = clk.summary()
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, sampler.latents, rank)
         per_step_launches = sampler.native_launches_per_step
         if per_step_launches is None:
             per_step_launches = (_native.launch_count - launches_before) // max(1, args.steps)
@@ -662,7 +680,7 @@ def main():
             "ms_per_step": ms / args.steps, "higher_is_better": True,
             "scaling": "strong" if cfg["total_images"] else "weak", "vs_baseline": None,
             "dtype": "f16", "data": "synthetic", "config": workload_config(world, args.config, m_img),
-            "clocks": clocks,
+            "clocks": clocks, "device": device_info(local_rank),
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                     "ms_per_step": ms_e2e / args.steps},
             "gpu_launches": int(per_step_launches) * args.steps,
@@ -682,7 +700,6 @@ def main():
                 "kernel": "pww_xattn_fused_f16 (one launch: statistic + packed-map bias + softmax + PV) N=4096 C=320 H=8 "
                           "T=77, B=2 (cond+uncond) as launched by this workload",
                 "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                "traffic": ncu_traffic("B2_fused"),
                 "peak_source": peak_src, "us_per_launch": r2["us_op"], "alg_bytes_per_launch": r2["alg_bytes"],
                 "alg_bytes_note": "SURVEY 8d formula with the PACKED map (64 B per pixel + 80 B index) instead of the "
                                   "dense fp32 map (308 B per pixel); alg_bytes_dense_map is the round-1 figure",
@@ -692,7 +709,7 @@ def main():
                 "dense_pair": {"us_stats": r2.get("us_dense_stats"), "us_fwd": r2.get("us_dense_fwd"),
                                "note": "round-1 path (pww_xattn_stats_f16 + pww_xattn_fwd_f16, dense fp32 map), same inputs"},
                 "batched": {"B": 16, "biased": 8, "us_per_launch": r16["us_op"], "achieved": ach16, "frac": ach16 / peak,
-                            "alg_bytes_per_launch": r16["alg_bytes"], "traffic": ncu_traffic("B16_fused"),
+                            "alg_bytes_per_launch": r16["alg_bytes"],
                             "alg_bytes_dense_map": r16["alg_bytes_dense_map"],
                             "frac_with_dense_map_bytes": r16["alg_bytes_dense_map"] / (r16["us_op"] * 1e-6) / 1e9 / peak,
                             "op_frac": ach16 / peak,
@@ -700,7 +717,7 @@ def main():
                 "method": "CUDA events around a CUDA graph of back-to-back launches cycling through buffer sets > L2"}
         except Exception as e:  # keep the headline even if the micro-bench fails
             line["roofline"] = {"bound": "hbm", "achieved": None, "peak": peak, "unit": "GB/s", "frac": None,
-                                "traffic": None, "error": repr(e)}
+                                "error": repr(e)}
         try:    # comparison only: the reference's eager op sequence on this GPU, same shapes, cond + uncond call
             us = eager_torch_xattn_us(device)
             line["roofline"]["eager_torch_fp16"] = {
@@ -717,7 +734,7 @@ def main():
             line["reference_gpu_eager"] = {
                 "value": rg["steps_per_s"], "unit": UNIT, "steps": rg["steps"], "warmup": rg["warmup"],
                 "ms_per_step": rg["ms_per_step"], "dtype": "f16 (torch.autocast)",
-                "what": "reference control flow on this B200: 2 batch-1 eager UNet forwards/step, inj_forward op sequence "
+                "what": "reference control flow on this GPU: 2 batch-1 eager UNet forwards/step, inj_forward op sequence "
                         "(paint_with_words.py:60-125) under autocast, stock PyTorch ops, no graph / caching / fused kernels",
                 "speedup_value": value / total_images / rg["steps_per_s"],
                 "speedup_e2e": e2e_value / total_images / rg["steps_per_s"]}

@@ -1,5 +1,5 @@
 /*
- * pww_b200.h -- C ABI of the B200-native Paint-with-Words attention path (libpww_b200.so).
+ * pww_b200.h -- C ABI of the H100-native Paint-with-Words attention path (libpww_b200.so).
  *
  * The reference (cloneofsimo/paint-with-words-sd) has no FFI: its boundary is the Python callable
  * `inj_forward(self, hidden_states, context=None, mask=None)` that it monkey-patches over
@@ -55,7 +55,7 @@ const char* pww_status_str(int status);
 /* cudaGetErrorString of the last CUDA failure seen by this library on the calling thread ("" if none). */
 const char* pww_last_cuda_error(void);
 
-/* 1 if the running device is compute capability 10.x (the only target), 0 otherwise, <0 on error. */
+/* 1 if the running device is compute capability 9.x (H100, the only target), 0 otherwise, <0 on error. */
 int pww_device_supported(void);
 
 /* Bytes of scratch `pww_xattn_stats_f16` needs for this problem size.  The scratch must be zero-filled
@@ -98,7 +98,7 @@ int pww_xattn_fwd_f16(const void* q, const void* k, const void* v, void* out,
  * ONE-LAUNCH Paint-with-Words cross-attention: statistic + bias + softmax + P.V (paint_with_words.py:87-118 with the
  * weight function of paint_with_words.py:402-405 inlined).  Replaces the pww_xattn_stats_f16 + pww_xattn_fwd_f16 pair:
  * the per-image statistic is reduced inside the kernel (cooperative launch, deterministic fixed-order reduction of
- * per-CTA partials) and the bias enters as two extra k-steps of the Q K^T tensor-core chain.
+ * per-CTA partials) and the bias is rebuilt from the packed map in shared memory.
  *
  * The weight map is passed in PACKED form (SURVEY 8f-4).  The reference's dense [N, T] fp32 map
  * (paint_with_words.py:255-272) has one distinct non-zero column per painted region, so it is a column dictionary

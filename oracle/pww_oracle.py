@@ -4,7 +4,7 @@ TEST INFRASTRUCTURE.  Only tests/, __graft_entry__.smoke() and bench.py's cpu_ba
 legs may import this file, and only as the checker (or as the timed CPU baseline).  The product package
 `paint_with_words_sd_b200` never imports it and has no CPU fallback.
 
-Every function restates one reference function (file:line relative to /root/reference) in plain
+Every function restates one reference function (file:line relative to the reference checkout's root) in plain
 torch-CPU / numpy.  Pinning: the reference ships NO tests or golden vectors for this path (SURVEY.md
 section 4), so the restatement is pinned against outputs of the reference's own functions executed in
 the build container through `oracle/ref_loader.py`; `tests/golden/make_golden.py` generated the

@@ -1,15 +1,15 @@
 """Load the UNMODIFIED reference module by path (test infrastructure only).
 
 TEST INFRASTRUCTURE -- only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline leg may
-import anything under oracle/.  This file is usable only where /root/reference exists (the build
-container); it never travels to the GPU box.  It is how the restatement in `pww_oracle.py` is pinned:
+import anything under oracle/.  This file is usable only where a checkout of the reference exists and
+PWW_REFERENCE_ROOT names it; nothing else in the project needs it.  It is how the restatement in `pww_oracle.py` is pinned:
 `tests/golden/make_golden.py` runs the real reference functions through this loader and commits their
 outputs as fixtures.
 
 The reference cannot be imported as a package here (SURVEY.md section 8c): `diffusers` is absent and
 transformers>=5 has no `CLIPFeatureExtractor`.  Recipe: register placeholder `diffusers` modules, alias
 `CLIPFeatureExtractor`, then exec `paint_with_words/paint_with_words.py` by path.  No reference source
-is copied; nothing is written under /root/reference.
+is copied; nothing is written under the reference checkout.
 """
 from __future__ import annotations
 
@@ -18,13 +18,13 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get("PWW_REFERENCE_ROOT", "/root/reference")
-_REF_FILE = os.path.join(REFERENCE_ROOT, "paint_with_words", "paint_with_words.py")
+REFERENCE_ROOT = os.environ.get("PWW_REFERENCE_ROOT", "")
+_REF_FILE = os.path.join(REFERENCE_ROOT, "paint_with_words", "paint_with_words.py") if REFERENCE_ROOT else ""
 _CACHE = {}
 
 
 def reference_available() -> bool:
-    return os.path.isfile(_REF_FILE)
+    return bool(_REF_FILE) and os.path.isfile(_REF_FILE)
 
 
 def _install_stubs() -> None:

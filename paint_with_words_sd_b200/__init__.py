@@ -1,4 +1,4 @@
-"""paint_with_words_sd_b200 -- B200-native Paint-with-Words attention path.
+"""paint_with_words_sd_b200 -- H100-native Paint-with-Words attention path.
 
 Same public names as the reference package (paint_with_words/__init__.py:1-3) plus the native pieces.
 The repo root also carries the hyphenated alias `paint-with-words-sd_b200` (a symlink to this

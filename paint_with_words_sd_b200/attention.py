@@ -131,10 +131,10 @@ def _rows(t: torch.Tensor) -> torch.Tensor:
 
 
 # "fused" / "auto" (default): ONE launch (statistic + bias + softmax + PV, packed maps; csrc/xattn_fused2.cuh) at every head
-# dim -- it matches or beats the two-launch pair on this hardware at every SD1.5 and SD2.1 shape (N = 4096 d = 40: 15.8 vs
-# 22.5 us at the cond+uncond launch, 45 vs 65 us at 16 images; N = 9216 d = 64: 21.6 vs 23.8 / 82 vs 81;
-# profiles/r02_microbench_sd15_final.jsonl, ..._sd21_final.jsonl); "dense": round 1's pair of launches on the dense fp32 map,
-# kept for maps that cannot be packed (> 10 distinct columns -- those always take it) and as a test / bench comparison.
+# dim -- it beats the two-launch pair at every SD1.5 and SD2.1 shape (cond + uncond launch, CUDA events, H100 80GB HBM3 at
+# 700 W: N = 4096 d = 40: 26.9 vs 34.2 us; N = 1024 d = 80: 40.2 vs 48.4; N = 9216 d = 64: 40.2 vs 47.3); "dense": the
+# pair of launches on the dense fp32 map, kept for maps that cannot be packed (> 10 distinct columns -- those always take
+# it) and as a test / bench comparison.
 XATTN_IMPL = "auto"
 
 
@@ -224,13 +224,13 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
     return out
 
 
-# Self-attention (context=None): "native" = pww_attn_fwd_f16, the tcgen05 flash-attention kernel of libpww_b200;
-# "torch-sdpa" = torch's library attention (cuDNN) -- like cuBLAS for the projections, a library call; "auto" (default) =
-# whichever is faster on this hardware: native up to 512 keys (23 vs 37 us at N = 256, 22 vs 31 us at N = 64), the library
-# above (N = 4096 d = 40: 144 vs 92 us, N = 1024 d = 80: 28 vs 24 us; profiles/r02_selfattn_microbench.jsonl -- the native
-# kernel is bound by its 8 softmax warps, see profiles/r02_notes.md).  bench.py records the setting in `config.self_attn`.
+# Self-attention (context=None): "native" = pww_attn_fwd_f16, the flash-attention kernel of libpww_b200 (csrc/attn_tc.cuh);
+# "torch-sdpa" = torch's library attention -- like cuBLAS for the projections, a library call; "auto" (default) = whichever
+# is faster on the H100: native up to 1024 keys, the library above.  Batch 2, CUDA events, H100 80GB HBM3 at 700 W, native
+# vs library: N = 64 d = 160: 21 vs 29 us; N = 576 d = 64: 27 vs 42; N = 1024 d = 80: 33 vs 43; N = 256 d = 160: 31 vs 29;
+# N = 2304 d = 64: 150 vs 71; N = 4096 d = 40: 284 vs 154.  bench.py records the setting in `config.self_attn`.
 SELF_ATTN_IMPL = "auto"
-SELF_ATTN_NATIVE_MAX_KEYS = 512
+SELF_ATTN_NATIVE_MAX_KEYS = 1024
 
 
 def self_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, scale: float) -> torch.Tensor:
@@ -283,7 +283,7 @@ def refresh_kv_cache(context: dict) -> None:
 def inj_forward(self, hidden_states, context=None, mask=None):
     """Replacement for `CrossAttention.__call__` (reference: paint_with_words.py:60-125)."""
     if not hidden_states.is_cuda:
-        raise _native.NativeError("paint_with_words_sd_b200 attention runs on a B200 GPU only (no CPU path)")
+        raise _native.NativeError("paint_with_words_sd_b200 attention runs on an H100 GPU only (no CPU path)")
     is_dict = isinstance(context, dict)
     if context is None:
         ctx = hidden_states

@@ -95,7 +95,7 @@ def _tokens_img_attention_factors(img_context_seperated, tokenized_texts, ratio:
     paint_with_words.py:259-268; 0/1 unless labels repeat or overlap).  Regions whose label is not in the prompt are
     dropped exactly like the reference drops them.  R is the number of painted regions (5 in the reference's examples),
     so (M, C) is N*R + 77*R numbers instead of N*77 -- the packed mask format of SURVEY 8f-4: the bias
-    g*M_b*W = (g*M_b*M) C^T is one extra k-step of the Q K^T UMMA instead of 77 loads and FMAs per query row.
+    g*M_b*W = (g*M_b*M) C^T is a dictionary lookup per token instead of a dense [N, 77] fp32 map read per query row.
     Not consumed by a kernel yet (DESIGN.md 8)."""
     token_lis = tokenized_texts["input_ids"][0].tolist()
     dim0, dim1 = img_context_seperated[0][1].shape

@@ -1,412 +1,192 @@
-// Self-attention (context=None in the reference's inj_forward, paint_with_words.py:71-72, 87-118) as a flash
-// attention forward on tcgen05 tensor cores: softmax(scale * Q_h K_h^T) V_h with keys = the image's own N pixels.
+// Self-attention (context=None in the reference's inj_forward, paint_with_words.py:71-72, 87-118) as a flash attention
+// forward on Hopper tensor cores: softmax(scale * Q_h K_h^T) V_h with keys = the image's own N pixels.
 //
-// One CTA = (image, head, NQ query tiles of 128 rows).  K and V tiles of BN keys stream through two TMA rings and are
-// shared by the NQ query tiles; softmax group g (4 warps, one thread per query row) owns tile g's S, P and O buffers
-// in tensor memory:
-//     S_g = Q_g K_j^T   (UMMA M=128 N=BN)      -> TMEM, double-buffered: S_g(j+1) is issued while softmax(j) runs
-//     online softmax with LAZY rescaling: the running max only moves (and O_g is rescaled in TMEM) when the tile max
-//       exceeds it by more than 2^8, so the correction pass is rare; P = 2^(s - m) <= 256 fits fp16
-//     P_g (packed fp16)                         -> TMEM (double-buffered where it fits), the A operand of
-//     O_g += P_g V_j    (TS-form UMMA M=128 N=D K=BN, V MN-major) accumulating in TMEM over all key tiles;
-//       for D = 40 / 80 a ones column in V makes accumulator column D the row sum of the fp16 P that was multiplied
-// Warp roles (384 threads): warp 0 Q by TMA, then the K loader | warp 1 S-UMMA issuer + TMEM owner | warp 2 V loader |
-// warp 3 PV-UMMA issuer | warps 4-7 and 8-11 the two softmax groups.  K / V tiles do not use the TMA: a head slice of a
-// key row is 80 bytes (D = 40) at an 80-byte offset, and the engine moves such rows at ~12 cycles each whatever the ring
-// depth (scripts/tma_probe.cu) -- two [64 x 80 B] boxes per key tile cost more than the tile's 1024 MUFU cycles.  The
-// loader warps copy the rows with 16-byte cp.async straight into the swizzled atoms (rows beyond N are zero-filled, the
-// ones column and the zero padding are written once per ring stage) and arrive on the stage's mbarrier.  The control
-// warps run warp-uniform loops and elect one lane only for the tcgen05 / TMA instructions (see xattn_fused2.cuh).  Every barrier that takes several arrivals per
-// phase is per buffer, so a warp's next arrival on it is causally behind the completion of the current phase.
-// Padding (d >= D, key >= N, row >= N) comes from TMA out-of-bounds zero fill; padded keys of the last tile are masked
-// to -inf.
+// One CTA = (image, head, 128 query rows); warp w owns rows [16 w, 16 w + 16) and keeps its Q fragments in registers.
+// Key tiles of BN = 64 rows of K and V stream through a two-stage cp.async ring in shared memory (the copies of tile j + 1
+// are in flight while tile j is computed):
+//     S = Q K_j^T     mma.m16n8k16, 8 n-tiles per warp, fp32 accumulators in registers
+//     online softmax: running row max m and row sum l; O and l are rescaled by 2^(m_old - m_new) when the max moves
+//     O += P V_j      P packed to fp16 straight from the S accumulators (the C layout of two n-tiles is the A layout of one
+//                     k-step), V fragments by ldmatrix.trans
+// Padding (d >= D, key >= N, row >= N) is zero-filled by the copies; padded keys of the last tile are masked to -inf.
 #pragma once
-#include "ptx_sm100.cuh"
+#include "mma_sm90.cuh"
 #include "pww_common.cuh"
-#include "xattn_tc.cuh"   // make_tmap, num_sms, tc_error_buf
+#include "xattn_core.cuh"
+#include "xattn_tc.cuh"   // num_sms, cur_device
 
 namespace pww {
 namespace fa {
 
-constexpr int kThreads = 384;
+constexpr int kThreads = core::kThreads;
+constexpr int kBM = core::kBM;
+constexpr int kBN = 64;                                    // keys per tile
 
 template <int D>
 struct Cfg {
-  static constexpr int NA = (D + 63) / 64;
-  static constexpr int DP = (D + 15) / 16 * 16;
-  static constexpr int BN = 64;                            // keys per tile
-  static constexpr int NQ = (D <= 80) ? 2 : 1;             // query tiles per CTA
-  static constexpr int NK = (D <= 80) ? 4 : 3;             // K ring depth
-  static constexpr int NV = (D <= 80) ? 3 : 2;             // V ring depth
-  // Row sums ride on the P.V UMMA where the last V atom has a spare column (see xattn_tc.cuh): accumulator column D.
-  static constexpr bool ONES = (D == 40 || D == 80);
-  static constexpr int DPV = ONES ? (D + 16) / 16 * 16 : DP;   // UMMA N of P.V: 48, 64, 96, 160
-  static constexpr uint32_t QATOM = 128 * 128, KATOM = BN * 128, PATOM = 128 * 128;
-  static constexpr uint32_t QBYTES = NA * QATOM;           // one query tile
-  static constexpr uint32_t KSTAGE = NA * KATOM, VSTAGE = NA * KATOM;
-  static constexpr uint32_t OFF_K = NQ * QBYTES;
-  static constexpr uint32_t OFF_V = OFF_K + NK * KSTAGE;
-  static constexpr uint32_t OFF_BAR = OFF_V + NV * VSTAGE;
-  static constexpr uint32_t SMEM = OFF_BAR + 256 + 1024;
-  static constexpr int TMEM_COLS = 512;
-  static constexpr int OSTRIDE = (DPV + 31) / 32 * 32;
-  static constexpr int NP = (D == 80) ? 1 : 2;             // P buffers per query tile (TMEM is full at D = 80)
-  static_assert(NQ * 2 * BN + NQ * NP * 32 + NQ * OSTRIDE <= 512, "TMEM budget");
+  using T_ = core::Tile<D>;
+  static constexpr uint32_t KVBYTES = kBN * T_::LD * 2;
+  static constexpr uint32_t OFF_KV = T_::QBYTES;
+  static constexpr uint32_t SMEM = T_::QBYTES + 2 * 2 * KVBYTES;   // Q | 2 x (K | V)
   static_assert(SMEM <= 232448, "shared memory budget");
-  // S is double-buffered per query tile so the next S = Q K^T is issued while the softmax of the current one runs
-  __host__ __device__ static constexpr uint32_t col_s(int g, int buf) { return (g * 2 + buf) * BN; }
-  // P (64 fp16 per row = 32 columns) is the A operand of the P.V UMMA, read straight from tensor memory
-  // double-buffered where TMEM allows, so the softmax of tile j+1 never waits for the P.V of tile j
-  __host__ __device__ static constexpr uint32_t col_p(int g, int buf) { return NQ * 2 * BN + (g * NP + buf) * 32; }
-  __host__ __device__ static constexpr uint32_t col_o(int g) { return NQ * 2 * BN + NQ * NP * 32 + g * OSTRIDE; }
 };
 
 struct Params {
-  __half* out;
+  const __half* q;
   const __half* k;
   const __half* v;
+  __half* out;
   int B, H, N;
   int64_t bs, rs;          // q/k/v element strides (batch, row)
   int64_t o_bs, o_rs;
   float scale;
 };
 
-__device__ __forceinline__ bool elect_one() {     // true on exactly one lane of a converged warp
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {   // src_bytes = 0: zero fill
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async_arrive(uint32_t bar) {   // arrives once this thread's cp.async so far have landed
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-template <int N>
-__device__ __forceinline__ void tmem_ld_row(uint32_t ta, float* v) {
-  if constexpr (N == 128) { ptx::tmem_ld64_sync(ta, v); ptx::tmem_ld64_sync(ta + 64, v + 64); }
-  else if constexpr (N == 64) { ptx::tmem_ld64_sync(ta, v); }
-  else if constexpr (N == 48) { ptx::tmem_ld32_sync(ta, v); ptx::tmem_ld16_sync(ta + 32, v + 32); }
-  else if constexpr (N == 80) { ptx::tmem_ld64_sync(ta, v); ptx::tmem_ld16_sync(ta + 64, v + 64); }
-  else if constexpr (N == 96) { ptx::tmem_ld64_sync(ta, v); ptx::tmem_ld32_sync(ta + 64, v + 64); }
-  else if constexpr (N == 160) { ptx::tmem_ld64_sync(ta, v); ptx::tmem_ld64_sync(ta + 64, v + 64); ptx::tmem_ld32_sync(ta + 128, v + 128); }
-}
-template <int N>
-__device__ __forceinline__ void tmem_st_row(uint32_t ta, const float* v) {
-  if constexpr (N == 64) { ptx::tmem_st64(ta, v); }
-  else if constexpr (N == 48) { ptx::tmem_st32(ta, v); ptx::tmem_st16(ta + 32, v + 32); }
-  else if constexpr (N == 80) { ptx::tmem_st64(ta, v); ptx::tmem_st16(ta + 64, v + 64); }
-  else if constexpr (N == 96) { ptx::tmem_st64(ta, v); ptx::tmem_st32(ta + 64, v + 64); }
-  else if constexpr (N == 160) { ptx::tmem_st64(ta, v); ptx::tmem_st64(ta + 64, v + 64); ptx::tmem_st32(ta + 128, v + 128); }
-  ptx::tmem_st_wait();
-}
-
 template <int D>
-__global__ void __launch_bounds__(kThreads, 1)
-attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmq, const Params p) {
-  using C = Cfg<D>;
-  extern __shared__ unsigned char smem_raw[];
-  const uint32_t smem0 = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
-  unsigned char* smem_gen = smem_raw + (smem0 - ptx::smem_u32(smem_raw));
-  const uint32_t bar0 = smem0 + C::OFF_BAR;
-  auto BAR = [&](int i) { return bar0 + 8u * i; };
-  constexpr int B_QFULL = 0, B_KFULL = 1, B_KEMPTY = 5, B_VFULL = 9, B_VEMPTY = 12, B_SREADY = 15, B_SFREE = 19,
-                B_PREADY = 23, B_PFREE = 27, B_TMEMPTR = 31;   // SREADY/SFREE/PREADY/PFREE: [g*2 + buf]
-  // PREADY is per P buffer like PFREE: a 4-arrival barrier shared by both buffers could be completed by one fast
-  // warp arriving for tiles j and j+1 before a slow warp has written its rows of P(j).  With one barrier per buffer a
-  // warp's next arrival on it (tile j+NP) is ordered behind PFREE, i.e. behind the P.V that consumed phase j.
+__global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const Params p) {
+  using C = core::Tile<D>;
+  using CF = Cfg<D>;
+  extern __shared__ __align__(128) unsigned char smem[];
+  const uint32_t smem0 = ptx::smem_u32(smem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // Progress words (one per role) so a barrier time-out can say where every role stands: [0] Q/K producer tile,
-  // [1] S issuer tile, [2] V producer tile, [3] P.V issuer tile (x2 + group), [4..5] softmax group 0/1 tile.
-  __shared__ int s_prog[8];
-  auto wait = [&](uint32_t bar, uint32_t parity, int tag) {
-    if (ptx::mbar_try_wait(bar, parity)) return;
-    const long long t0 = clock64();
-    while (!ptx::mbar_try_wait(bar, parity)) {
-      if (clock64() - t0 > 4000000000LL) {
-        if ((threadIdx.x & 31) == 0)
-          printf("pww-attn: timeout block %d warp %d tag %d bar %d parity %u | prog qk %d s %d v %d pv %d sm0 %d sm1 %d (n_kv %d)\n",
-                 blockIdx.x, threadIdx.x >> 5, tag, (int)((bar - bar0) >> 3), parity, s_prog[0], s_prog[1], s_prog[2], s_prog[3],
-                 s_prog[4], s_prog[5], (p.N + C::BN - 1) / C::BN);
-        __trap();
-      }
-    }
+  const int qtiles = (p.N + kBM - 1) / kBM;
+  const int bh = blockIdx.x / qtiles, qt = blockIdx.x - bh * qtiles;
+  const int b = bh / p.H, h = bh - b * p.H;
+  const int row_base = qt * kBM;
+  const __half* qb = p.q + (int64_t)b * p.bs + h * D;
+  const __half* kb = p.k + (int64_t)b * p.bs + h * D;
+  const __half* vb = p.v + (int64_t)b * p.bs + h * D;
+  const int ntiles = (p.N + kBN - 1) / kBN;
+  auto issue_kv = [&](int j) {
+    const uint32_t st = smem0 + CF::OFF_KV + (j & 1) * 2 * CF::KVBYTES;
+    const int rows = p.N - j * kBN < kBN ? p.N - j * kBN : kBN;
+    core::load_rows<D>(st, kb + (int64_t)j * kBN * p.rs, p.rs, kBN, rows);
+    core::load_rows<D>(st + CF::KVBYTES, vb + (int64_t)j * kBN * p.rs, p.rs, kBN, rows);
+    ptx::cp_async_commit();
   };
-  if (threadIdx.x < 8) s_prog[threadIdx.x] = -1;
-  // block -> (image, head, query super-tile)
-  const int qtiles = (p.N + 128 * C::NQ - 1) / (128 * C::NQ);
-  const int qt = blockIdx.x % qtiles;
-  const int h = (blockIdx.x / qtiles) % p.H;
-  const int b = blockIdx.x / (qtiles * p.H);
-  const int row0 = qt * 128 * C::NQ;
-  const int n_kv = (p.N + C::BN - 1) / C::BN;
-  // a query tile that starts beyond N has no rows: its softmax group idles and no UMMA is issued for it
-  const int nq_live = (row0 + 128 < p.N && C::NQ == 2) ? 2 : 1;
-
-  if (warp == 0 && lane == 0) {
-    ptx::prefetch_tmap(&tmq);
-    ptx::mbar_init(BAR(B_QFULL), 1);
-    for (int s = 0; s < C::NK; ++s) { ptx::mbar_init(BAR(B_KFULL + s), 32); ptx::mbar_init(BAR(B_KEMPTY + s), 1); }   // 32: one cp.async arrival per loader lane
-    for (int s = 0; s < C::NV; ++s) { ptx::mbar_init(BAR(B_VFULL + s), 32); ptx::mbar_init(BAR(B_VEMPTY + s), 1); }
-    for (int i = 0; i < 4; ++i) {
-      ptx::mbar_init(BAR(B_SREADY + i), 1);
-      ptx::mbar_init(BAR(B_SFREE + i), 4);
-      ptx::mbar_init(BAR(B_PFREE + i), 1);
-      ptx::mbar_init(BAR(B_PREADY + i), 4);
-    }
-    ptx::fence_barrier_init();
-  }
-  // Ring-stage padding, written once (the per-tile copies only touch the D / 8 data chunks of a row): K columns D .. DP-1
-  // are zero; V columns D .. DPV-1 hold the ones column ([1, 0 x 7] at column D: accumulator column D of the P.V UMMA becomes
-  // the row sum; padded keys have P = 0, so every row may carry the 1) followed by zeros.
   {
-    constexpr int kpad = (C::DP - D) / 8, vpad = (C::DPV - D) / 8;      // 16-byte chunks
-    if constexpr (kpad > 0) {
-      for (int idx = threadIdx.x; idx < C::NK * C::BN * kpad; idx += kThreads) {
-        const int st = idx / (C::BN * kpad), rem = idx % (C::BN * kpad), r = rem / kpad, c = D / 8 + rem % kpad;
-        *reinterpret_cast<uint4*>(smem_gen + C::OFF_K + st * C::KSTAGE + (c / 8) * C::KATOM + r * 128 + (((c % 8) ^ (r & 7)) << 4)) =
-            make_uint4(0, 0, 0, 0);
-      }
-    }
-    if constexpr (vpad > 0) {
-      for (int idx = threadIdx.x; idx < C::NV * C::BN * vpad; idx += kThreads) {
-        const int st = idx / (C::BN * vpad), rem = idx % (C::BN * vpad), r = rem / vpad, c = D / 8 + rem % vpad;
-        *reinterpret_cast<uint4*>(smem_gen + C::OFF_V + st * C::VSTAGE + (c / 8) * C::KATOM + r * 128 + (((c % 8) ^ (r & 7)) << 4)) =
-            make_uint4((C::ONES && c == D / 8) ? 0x00003C00u : 0u, 0, 0, 0);
-      }
-    }
-    ptx::fence_proxy_async_smem();
+    const int rows = p.N - row_base < kBM ? p.N - row_base : kBM;
+    core::load_rows<D>(smem0, qb + (int64_t)row_base * p.rs, p.rs, kBM, rows);
   }
-  if (warp == 1) ptx::tmem_alloc<C::TMEM_COLS>(BAR(B_TMEMPTR));
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem_gen + C::OFF_BAR + 8 * B_TMEMPTR);
-  // (no setmaxnreg re-distribution: the two-pass softmax keeps every role under the 168-register budget)
-
-  // One key tile of K or V for this head: rows j*BN .. j*BN+63 (zero beyond N), D / 8 chunks of 16 bytes per row, into the
-  // swizzled atoms of a ring stage; a lane owns whole rows.
-  auto copy_tile = [&](uint32_t stage, const __half* base, int j, uint32_t bar) {
-    const __half* src = base + (int64_t)b * p.bs + h * D;
+  issue_kv(0);                                     // one group: Q and the first key tile
+  uint32_t qa[C::KS][4];
+  float o[C::NT][4];
 #pragma unroll
-    for (int rr = 0; rr < C::BN / 32; ++rr) {
-      const int r = lane + 32 * rr, n = j * C::BN + r;
-      const bool ok = n < p.N;
-      const uint4* srow = reinterpret_cast<const uint4*>(src + (int64_t)(ok ? n : 0) * p.rs);
-      const uint32_t drow = stage + r * 128;
-      const int x7 = r & 7;
+  for (int j = 0; j < C::NT; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+  const float sl2 = p.scale * 1.4426950408889634f;
+  const uint32_t qs = smem0 + (uint32_t)(warp * 16 * C::LD) * 2u;
+#pragma unroll 1
+  for (int jt = 0; jt < ntiles; ++jt) {
+    if (jt + 1 < ntiles) {
+      issue_kv(jt + 1);
+      ptx::cp_async_wait<1>();
+    } else {
+      ptx::cp_async_wait<0>();
+    }
+    __syncthreads();
+    if (jt == 0) {
 #pragma unroll
-      for (int c = 0; c < D / 8; ++c)
-        cp_async16(drow + (c / 8) * C::KATOM + (((c % 8) ^ x7) << 4), srow + c, ok ? 16u : 0u);
+      for (int kk = 0; kk < C::KS; ++kk)
+        ptx::ldsm_x4(qs + (uint32_t)((lane & 15) * C::LD + kk * 16 + (lane >> 4) * 8) * 2u, qa[kk][0], qa[kk][1], qa[kk][2], qa[kk][3]);
     }
-    cp_async_arrive(bar);
-  };
-
-  if (warp == 0) {
-    // ------------------------------------------------ Q tiles once (TMA), then the K loader
-    if (elect_one()) {
-      ptx::mbar_arrive_expect_tx(BAR(B_QFULL), nq_live * C::QBYTES);
-      for (int g = 0; g < nq_live; ++g)
+    const uint32_t ks = smem0 + CF::OFF_KV + (jt & 1) * 2 * CF::KVBYTES, vs = ks + CF::KVBYTES;
+    float s[8][4];
 #pragma unroll
-        for (int a = 0; a < C::NA; ++a)
-          ptx::tma_load_4d(smem0 + g * C::QBYTES + a * C::QATOM, &tmq, BAR(B_QFULL), a * 64, h, row0 + g * 128, b);
-    }
-    __syncwarp();
-    for (int j = 0; j < n_kv; ++j) {
-      if (lane == 0) s_prog[0] = j;
-      const int st = j % C::NK;
-      wait(BAR(B_KEMPTY + st), (uint32_t)(((j / C::NK) & 1) ^ 1), 1);
-      copy_tile(smem0 + C::OFF_K + st * C::KSTAGE, p.k, j, BAR(B_KFULL + st));
-    }
-  } else if (warp == 2) {
-    // ------------------------------------------------ V loader
-    for (int j = 0; j < n_kv; ++j) {
-      if (lane == 0) s_prog[2] = j;
-      const int st = j % C::NV;
-      wait(BAR(B_VEMPTY + st), (uint32_t)(((j / C::NV) & 1) ^ 1), 2);
-      copy_tile(smem0 + C::OFF_V + st * C::VSTAGE, p.v, j, BAR(B_VFULL + st));
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------ UMMA issuer: S_g = Q_g K_j^T  (warp-uniform loop, elected issue)
-    constexpr uint32_t idesc = ptx::make_idesc_f16(128, C::BN, false, false);
-    wait(BAR(B_QFULL), 0, 3);
-    for (int j = 0; j < n_kv; ++j) {
-      if (lane == 0) s_prog[1] = j;
-      const int st = j % C::NK;
-      wait(BAR(B_KFULL + st), (uint32_t)((j / C::NK) & 1), 4);
-      ptx::fence_proxy_async_smem();               // K tile: cp.async (generic proxy) writes -> the UMMA's async-proxy reads
-      const int buf = j & 1;
-      for (int g = 0; g < nq_live; ++g) {
-        wait(BAR(B_SFREE + g * 2 + buf), (uint32_t)(((j >> 1) & 1) ^ 1), 5);   // softmax done with this S buffer
-        ptx::tc_fence_after();
-        const uint32_t qb = smem0 + g * C::QBYTES, kb = smem0 + C::OFF_K + st * C::KSTAGE;
-        if (elect_one()) {
+    for (int j = 0; j < 8; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
 #pragma unroll
-          for (int ks = 0; ks < C::DP / 16; ++ks)
-            ptx::umma_ss(tmem_base + C::col_s(g, buf),
-                         ptx::make_sw128_desc(qb + (ks / 4) * C::QATOM + (ks % 4) * 32, 16, 1024),
-                         ptx::make_sw128_desc(kb + (ks / 4) * C::KATOM + (ks % 4) * 32, 16, 1024), idesc, ks > 0);
-          ptx::umma_commit(BAR(B_SREADY + g * 2 + buf));
-          if (g == nq_live - 1) ptx::umma_commit(BAR(B_KEMPTY + st));
-        }
-        __syncwarp();
+    for (int kk = 0; kk < C::KS; ++kk) {
+#pragma unroll
+      for (int jp = 0; jp < 4; ++jp) {
+        const int t = 16 * jp + (lane & 7) + ((lane >> 4) << 3), d = kk * 16 + ((lane >> 3) & 1) * 8;
+        uint32_t b0, b1, b2, b3;
+        ptx::ldsm_x4(ks + (uint32_t)(t * C::LD + d) * 2u, b0, b1, b2, b3);
+        ptx::mma16816(s[2 * jp], qa[kk], b0, b1);
+        ptx::mma16816(s[2 * jp + 1], qa[kk], b2, b3);
       }
     }
-  } else if (warp == 3) {
-    // ------------------------------------------------ UMMA issuer: O_g += P_g V_j  (warp-uniform loop, elected issue)
-    constexpr uint32_t idesc = ptx::make_idesc_f16(128, C::DPV, false, true);
-    for (int j = 0; j < n_kv; ++j) {
-      const int st = j % C::NV;
-      wait(BAR(B_VFULL + st), (uint32_t)((j / C::NV) & 1), 6);
-      ptx::fence_proxy_async_smem();               // V tile: cp.async (generic proxy) writes -> the UMMA's async-proxy reads
-      for (int g = 0; g < nq_live; ++g) {
-        if (lane == 0) s_prog[3] = 2 * j + g;
-        const int pb = j % C::NP;
-        wait(BAR(B_PREADY + g * 2 + pb), (uint32_t)((j / C::NP) & 1), 7);
-        ptx::tc_fence_after();
-        const uint32_t vb = smem0 + C::OFF_V + st * C::VSTAGE;
-        if (elect_one()) {
+    const int valid = p.N - jt * kBN;              // keys of this tile that exist
+    float t0 = -INFINITY, t1 = -INFINITY;
 #pragma unroll
-          for (int ks = 0; ks < C::BN / 16; ++ks)
-            ptx::umma_ts(tmem_base + C::col_o(g), tmem_base + C::col_p(g, pb) + ks * 8,
-                         ptx::make_sw128_desc(vb + ks * 16 * 128, C::KATOM, 1024), idesc, (j > 0) || (ks > 0));
-          ptx::umma_commit(BAR(B_PFREE + g * 2 + pb));    // P buffer consumed == O_g holds tiles 0..j
-          if (g == nq_live - 1) ptx::umma_commit(BAR(B_VEMPTY + st));
-        }
-        __syncwarp();
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        if (core::tok(j, e, lane) >= valid) s[j][e] = -INFINITY;
+        if (e < 2) t0 = fmaxf(t0, s[j][e]); else t1 = fmaxf(t1, s[j][e]);
+      }
+    t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, 1));
+    t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, 2));
+    t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, 1));
+    t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, 2));
+    const float mn0 = fmaxf(m0, t0), mn1 = fmaxf(m1, t1);
+    const float a0 = ptx::ex2((m0 - mn0) * sl2), a1 = ptx::ex2((m1 - mn1) * sl2);   // 0 on the first tile (m = -inf)
+    m0 = mn0; m1 = mn1;
+    const float n0 = -mn0 * sl2, n1 = -mn1 * sl2;
+    uint32_t pa[4][4];
+    float r0 = 0.f, r1 = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const uint32_t p01 = ptx::pack_h2(ptx::ex2(fmaf(s[j][0], sl2, n0)), ptx::ex2(fmaf(s[j][1], sl2, n0)));
+      const uint32_t p23 = ptx::pack_h2(ptx::ex2(fmaf(s[j][2], sl2, n1)), ptx::ex2(fmaf(s[j][3], sl2, n1)));
+      const float2 f01 = ptx::unpack_h2(p01), f23 = ptx::unpack_h2(p23);
+      r0 += f01.x + f01.y;
+      r1 += f23.x + f23.y;
+      pa[j >> 1][(j & 1) * 2] = p01;
+      pa[j >> 1][(j & 1) * 2 + 1] = p23;
+    }
+    l0 = l0 * a0 + r0;                             // per-thread partial row sums; reduced over the quad at the end
+    l1 = l1 * a1 + r1;
+#pragma unroll
+    for (int j = 0; j < C::NT; ++j) {
+      o[j][0] *= a0; o[j][1] *= a0; o[j][2] *= a1; o[j][3] *= a1;
+    }
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      const int t = 16 * kk + (lane & 7) + ((lane >> 3) & 1) * 8;
+#pragma unroll
+      for (int jp = 0; jp < C::NT / 2; ++jp) {
+        uint32_t b0, b1, b2, b3;
+        ptx::ldsm_x4_t(vs + (uint32_t)(t * C::LD + 16 * jp + (lane >> 4) * 8) * 2u, b0, b1, b2, b3);
+        ptx::mma16816(o[2 * jp], pa[kk], b0, b1);
+        ptx::mma16816(o[2 * jp + 1], pa[kk], b2, b3);
+      }
+      if constexpr (C::NT & 1) {
+        uint32_t b0, b1;
+        ptx::ldsm_x2_t(vs + (uint32_t)(t * C::LD + 8 * (C::NT - 1)) * 2u, b0, b1);
+        ptx::mma16816(o[C::NT - 1], pa[kk], b0, b1);
       }
     }
-  } else {
-    // ------------------------------------------------ softmax groups
-    const int g = (warp >> 2) - 1;
-    if (g < nq_live) {
-      const int row = ((warp & 3) << 5) | lane;
-      const uint32_t lane_addr = (uint32_t)((warp & 3) << 5) << 16;
-      const float sl2 = p.scale * 1.4426950408889634f;
-      float m_run = -INFINITY, l_run = 0.f;
-      for (int j = 0; j < n_kv; ++j) {
-        if ((warp & 3) == 0 && lane == 0) s_prog[4 + g] = j;
-        const int buf = j & 1;
-        wait(BAR(B_SREADY + g * 2 + buf), (uint32_t)((j >> 1) & 1), 8);
-        ptx::tc_fence_after();
-        const uint32_t ts = tmem_base + lane_addr + C::col_s(g, buf);
-        const int valid = p.N - j * C::BN;          // keys of this tile that exist (>= BN except in the last tile)
-        // pass 1 over S (TMEM reads are cheap): row max of the tile
-        float m_tile;
-        {
-          float s[64];
-          ptx::tmem_ld64_sync(ts, s);
-          if (valid < C::BN) {
-#pragma unroll
-            for (int c = 0; c < 64; ++c)
-              if (c >= valid) s[c] = -INFINITY;
-          }
-          float m0 = s[0], m1 = s[1], m2 = s[2], m3 = s[3];
-#pragma unroll
-          for (int c = 4; c < 64; c += 4) {
-            m0 = fmaxf(m0, s[c]); m1 = fmaxf(m1, s[c + 1]); m2 = fmaxf(m2, s[c + 2]); m3 = fmaxf(m3, s[c + 3]);
-          }
-          m_tile = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-        }
-        // lazy rescale: move the reference max only when the tile exceeds it by more than 2^8
-        const bool need = (j == 0) || ((m_tile - m_run) * sl2 > 8.0f);
-        float factor = 1.f;
-        if (need) {
-          factor = (j == 0) ? 0.f : ptx::ex2((m_run - m_tile) * sl2);
-          m_run = m_tile;
-        }
-        const float nm = -m_run * sl2;
-        // this tile's P buffer must have been consumed by its previous P.V ...
-        const int pbuf = j % C::NP;
-        wait(BAR(B_PFREE + g * 2 + pbuf), (uint32_t)(((j / C::NP) & 1) ^ 1), 9);
-        // ... and O may only be rescaled once the P.V of the previous tile has landed (rare path): that is the PFREE
-        // phase of the previous tile's buffer, which this warp last waited on one phase earlier (no parity aliasing)
-        if (j >= 1 && __any_sync(0xffffffffu, need)) {
-          wait(BAR(B_PFREE + g * 2 + (j - 1) % C::NP), (uint32_t)((((j - 1) / C::NP)) & 1), 10);
-          ptx::tc_fence_after();
-          float o[C::DPV];
-          tmem_ld_row<C::DPV>(tmem_base + lane_addr + C::col_o(g), o);
-#pragma unroll
-          for (int c = 0; c < C::DPV; ++c) o[c] *= factor;
-          tmem_st_row<C::DPV>(tmem_base + lane_addr + C::col_o(g), o);
-        }
-        // pass 2: p = 2^((s - m) * scale * log2 e) -> fp16 -> swizzled P tile, 32 columns at a time
-        float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-#pragma unroll
-        for (int c0 = 0; c0 < C::BN; c0 += 32) {
-          float s[32];
-          ptx::tmem_ld32_sync(ts + c0, s);
-          if (c0 + 32 == C::BN) {                   // last read of this S buffer: hand it back to the S-UMMA issuer
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(BAR(B_SFREE + g * 2 + buf));
-          }
-          if (valid < C::BN) {
-#pragma unroll
-            for (int c = 0; c < 32; ++c)
-              if (c0 + c >= valid) s[c] = -INFINITY;
-          }
-          uint32_t pk[16];
-#pragma unroll
-          for (int c = 0; c < 32; c += 4) {
-            const float e0 = ptx::ex2(fmaf(s[c], sl2, nm)), e1 = ptx::ex2(fmaf(s[c + 1], sl2, nm));
-            const float e2 = ptx::ex2(fmaf(s[c + 2], sl2, nm)), e3 = ptx::ex2(fmaf(s[c + 3], sl2, nm));
-            if constexpr (!C::ONES) { a0 += e0; a1 += e1; a2 += e2; a3 += e3; }
-            const __half2 h01 = __floats2half2_rn(e0, e1), h23 = __floats2half2_rn(e2, e3);
-            pk[c / 2] = *reinterpret_cast<const uint32_t*>(&h01);
-            pk[c / 2 + 1] = *reinterpret_cast<const uint32_t*>(&h23);
-          }
-          ptx::tmem_st16_u32(tmem_base + lane_addr + C::col_p(g, pbuf) + c0 / 2, pk);   // 32 fp16 = 16 columns of P
-        }
-        ptx::tmem_st_wait();
-        if constexpr (!C::ONES) l_run = l_run * factor + ((a0 + a1) + (a2 + a3));
-        ptx::fence_proxy_async_smem();
-        ptx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(BAR(B_PREADY + g * 2 + pbuf));
-      }
-      // epilogue: O / l -> fp16 -> global
-      wait(BAR(B_PFREE + g * 2 + (n_kv - 1) % C::NP), (uint32_t)(((n_kv - 1) / C::NP) & 1), 11);
-      ptx::tc_fence_after();
-      float o[C::DPV];
-      tmem_ld_row<C::DPV>(tmem_base + lane_addr + C::col_o(g), o);
-      const float inv = 1.f / (C::ONES ? o[D] : l_run);
-      const int n = row0 + g * 128 + row;
-      if (n < p.N) {
-        __half* orow = p.out + (int64_t)b * p.o_bs + (int64_t)n * p.o_rs + h * D;
-#pragma unroll
-        for (int c = 0; c < D / 8; ++c) {
-          __align__(16) __half2 hk[4];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) hk[q] = __floats2half2_rn(o[c * 8 + 2 * q] * inv, o[c * 8 + 2 * q + 1] * inv);
-          reinterpret_cast<uint4*>(orow)[c] = *reinterpret_cast<const uint4*>(hk);
-        }
-      }
-    }
+    __syncthreads();                               // stage jt & 1 is refilled by the copies issued next iteration
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc<C::TMEM_COLS>(tmem_base);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float i0 = 1.f / l0, i1 = 1.f / l1;
+#pragma unroll
+  for (int j = 0; j < C::NT; ++j) {
+    o[j][0] *= i0; o[j][1] *= i0; o[j][2] *= i1; o[j][3] *= i1;
+  }
+  core::warp_store<D>(o, smem + warp * 16 * C::LD * 2, lane, p.out + (int64_t)b * p.o_bs + h * D, p.o_rs,
+                      row_base + warp * 16, p.N);
 }
 
 template <int D>
 cudaError_t launch(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int64_t bs, int64_t rs,
                    int64_t o_bs, int64_t o_rs, float scale, cudaStream_t s) {
-  using C = Cfg<D>;
-  CUtensorMap tq;
-  if (!tc::make_tmap(&tq, q, D, H, N, B, rs, bs, 128)) return cudaErrorInvalidValue;
+  using CF = Cfg<D>;
   Params p;
-  p.out = (__half*)out; p.k = (const __half*)k; p.v = (const __half*)v; p.B = B; p.H = H; p.N = N; p.bs = bs; p.rs = rs;
-  p.o_bs = o_bs; p.o_rs = o_rs; p.scale = scale;
+  p.q = (const __half*)q; p.k = (const __half*)k; p.v = (const __half*)v; p.out = (__half*)out;
+  p.B = B; p.H = H; p.N = N; p.bs = bs; p.rs = rs; p.o_bs = o_bs; p.o_rs = o_rs; p.scale = scale;
   static bool attr_set[tc::kMaxDevices] = {false};
   if (!attr_set[tc::cur_device()]) {
-    cudaError_t e = cudaFuncSetAttribute(attn_fwd_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, CF::SMEM);
     if (e != cudaSuccess) return e;
     attr_set[tc::cur_device()] = true;
   }
-  const int qtiles = (N + 128 * C::NQ - 1) / (128 * C::NQ);
-  attn_fwd_tc_kernel<D><<<B * H * qtiles, kThreads, C::SMEM, s>>>(tq, p);
+  const long long grid = (long long)B * H * ((N + kBM - 1) / kBM);
+  if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+  attn_fwd_kernel<D><<<(unsigned)grid, kThreads, CF::SMEM, s>>>(p);
   return cudaGetLastError();
 }
 

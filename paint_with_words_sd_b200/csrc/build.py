@@ -1,8 +1,9 @@
-"""Build libpww_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libpww_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m paint_with_words_sd_b200.csrc.build [--force] [--verbose]
 
-The .so is git-ignored but NOT gpurun-ignored, so the prebuilt file travels to the GPU box.
+The .so is a build product (git-ignored); the stamp file holds a fingerprint of the sources and flags, so a stale
+library is rebuilt.
 """
 from __future__ import annotations
 
@@ -18,7 +19,7 @@ LIB = os.path.join(PKG, "libpww_b200.so")
 STAMP = os.path.join(PKG, ".libpww_b200.stamp")
 SOURCES = ["pww_abi.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "-shared", "-cudart", "static",
     "-Xptxas", "-v",

@@ -68,7 +68,7 @@ int pww_device_supported(void) {
   if (e != cudaSuccess) return cuda_fail(e);
   e = cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   if (e != cudaSuccess) return cuda_fail(e);
-  return major == 10 ? 1 : 0;
+  return major == 9 ? 1 : 0;
 }
 
 size_t pww_xattn_workspace_bytes(int B, int H, int N, int T, int D) {
@@ -218,10 +218,10 @@ int pww_xattn_fused_f16(const void* q, const void* k, const void* v, void* out, 
     c.wmap = mpack ? (const float*)mp : nullptr;                   // non-null marks "maps present" for the kernel
     cudaError_t e = cudaErrorInvalidValue;
     switch (D) {
-      case 40: e = pww::fx2::launch_fused2<40>(c, mp, mpack_batch_stride, Bw, ci, s); break;
-      case 64: e = pww::fx2::launch_fused2<64>(c, mp, mpack_batch_stride, Bw, ci, s); break;
-      case 80: e = pww::fx2::launch_fused2<80>(c, mp, mpack_batch_stride, Bw, ci, s); break;
-      case 160: e = pww::fx2::launch_fused2<160>(c, mp, mpack_batch_stride, Bw, ci, s); break;
+      case 40: e = pww::fx2::launch_fused2<40>(c, mp, mpack_batch_stride, ci, s); break;
+      case 64: e = pww::fx2::launch_fused2<64>(c, mp, mpack_batch_stride, ci, s); break;
+      case 80: e = pww::fx2::launch_fused2<80>(c, mp, mpack_batch_stride, ci, s); break;
+      case 160: e = pww::fx2::launch_fused2<160>(c, mp, mpack_batch_stride, ci, s); break;
     }
     if (e == cudaErrorInvalidConfiguration) return PWW_ERR_UNSUPPORTED;
     if (e != cudaSuccess) return cuda_fail(e);
@@ -311,22 +311,6 @@ int pww_add_layernorm_f16(const void* x, const void* res, const void* gamma, con
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 
-// Test infrastructure (not declared in the public header): point the kernels' debug timeline at a device buffer of
-// kTlTags*kTlIts int64 clock64 stamps [tag][iteration] written by CTA 0; pass NULL to disable.
-int pww_debug_set_timeline(void* device_buffer) {
-  pww::tc::debug_timeline() = (long long*)device_buffer;
-  return PWW_OK;
-}
-
-// Test infrastructure (not declared in the public header): structure of the tcgen05 forward kernel, for A/B timing.
-// 0 = per-thread global stores, 1 = TMA-store epilogue at D = 40 (default), 3 = TMA-store epilogue at every head dim
-// (see xattn_tc.cuh).
-int pww_debug_set_variant(int variant) {
-  if (variant != 0 && variant != 1 && variant != 3) return PWW_ERR_BAD_ARG;
-  pww::tc::fwd_variant() = variant;
-  return PWW_OK;
-}
-
 // Test infrastructure (not declared in the public header): replay the forward kernel's unit schedule on the host.
 // wmap_index and out are HOST pointers; out receives 8 int32 per unit (see fwd_schedule_host); returns the number of
 // units written or a negative value for bad arguments.  No GPU needed.
@@ -341,20 +325,14 @@ int pww_debug_set_fused_grid(int grid) {
   pww::fx::debug_grid() = grid < 0 ? 0 : grid;
   return PWW_OK;
 }
-// Test infrastructure: clock64 timeline of one CTA of the fused kernel ([16][64] int64 device buffer, NULL = off).
-int pww_debug_set_fused_timeline(void* device_buffer, int cta) {
-  pww::fx::debug_timeline() = (long long*)device_buffer;
-  pww::fx::debug_timeline_cta() = cta;
-  return PWW_OK;
-}
 // Host replay of the grouped-head kernel's job lists (14 int32 per job, see fused2_schedule_host).
 int pww_debug_fused2_schedule(int B, int H, int G, int tiles, int grid, const int* wmap_index, int* out, int max_jobs) {
   if (!wmap_index || !out) return PWW_ERR_BAD_ARG;
   return pww::fx2::fused2_schedule_host(B, H, G, tiles, grid, wmap_index, out, max_jobs);
 }
-// Test infrastructure: device buffer of grid * (2 + 1024) uint32 the grouped-head kernel copies every CTA's job table to.
-// Heads per unit of the grouped-head kernel (a build-time constant).
+// Heads per unit of the grouped-head kernel at head dim 40 (a build-time constant).
 int pww_debug_fused2_heads_per_unit(void) { return pww::fx2::Cfg2<40>::G; }
+// Test infrastructure: device buffer of grid * (2 + 1024) uint32 the grouped-head kernel copies every CTA's job table to.
 int pww_debug_set_fused_jobs_dump(void* device_buffer) {
   pww::fx::debug_jobs_dump() = (unsigned*)device_buffer;
   return PWW_OK;

@@ -1,4 +1,4 @@
-// Shared host/device helpers for libpww_b200.so (sm_100a only).
+// Shared host/device helpers for libpww_b200.so (sm_90a).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>

@@ -1,55 +1,43 @@
 // Shared pieces of the one-launch Paint-with-Words cross-attention kernel (csrc/xattn_fused2.cuh): constants, launch
 // parameters, the unit order (FxWalk: which (image, row tile, head group) a CTA's contiguous range covers and in which order),
-// the grid-barrier membership test, small PTX helpers, the packed-map tensor map and the host-side knobs.
+// the grid-barrier membership test and the host-side knobs.
 //
 // Packed weight map (SURVEY 8f-4).  The reference's dense [N, 77] fp32 map has at most a handful of distinct non-zero
 // columns (one per painted region, paint_with_words.py:255-272), so it is stored as a column dictionary:
 //     W[n, t] = Mu[n, cidx[t]]      Mu [N, R] fp32 (R <= 10 distinct columns), cidx [77] (-1 = zero column)
 // and Mu is split into fp16 hi/lo halves:  mpack[n] = [ hi(Mu[n,0..9]) | lo(Mu[n,0..9]) | hi(Mu[n,0..9]) | 0 0 ]  (32 fp16,
-// 64 bytes per row instead of 308).  With x = g * M_b split the same way (xh, xl) the B operand row of token t is
-// [ xh at cidx[t] | xh at 10 + cidx[t] | xl at 20 + cidx[t] ], so two extra k-steps of the Q K^T UMMA chain add
-// hi*xh + lo*xh + hi*xl = W * x to 2^-22 relative -- the 77 loads + 77 FMAs per biased row of the dense kernel are gone.
+// 64 bytes per row instead of 308).  The kernel rebuilds W[n, t] = hi + lo in fp32 (exact to 2^-22 relative) from the row
+// tile's 8 KB of packed map in shared memory and adds x * W to the fp32 scores, x = g(sigma) * statistic.
 //
 // Unit order.  `img` lists the biased images first, then the unbiased ones; pair groups (a biased image with an unbiased
 // one: classifier-free guidance supplies both) come first, tile-major, biased unit before unbiased, then the solo groups of
 // the images without a partner.  A CTA takes a contiguous range of this order, so it gets the same number of biased and
 // unbiased units (+-1) whatever the image order of the batch, and its unbiased units' softmax overlaps the grid barrier.
 #pragma once
-#include "ptx_sm100.cuh"
+#include "mma_sm90.cuh"
 #include "pww_common.cuh"
-#include "xattn_tc.cuh"   // make_tmap_out, encode_fn, num_sms, tc_error_buf
+#include "xattn_tc.cuh"   // num_sms, tc_error_buf
 
 namespace pww {
 namespace fx {
 
 constexpr int kBM = 128;          // query rows per tile
 constexpr int kTP = 80;           // padded key count
-constexpr int kThreads = 640;     // 20 warps
 constexpr int kMaxBatch = 32;     // images per launch (the C ABI splits larger batches)
 constexpr int kMaxLocal = 4;      // biased images one CTA's unit range may touch (checked on the host)
-constexpr int kMW = 32;           // packed-map columns per row = two 16-wide k-steps
+constexpr int kMW = 32;           // packed-map columns per row (64 bytes)
 constexpr int kRC = 10;           // dictionary capacity (distinct non-zero columns)
-constexpr uint32_t kQAtom = 128 * 128, kKAtom = kTP * 128, kMAtom = 128 * 64, kCoefTile = kTP * 64;
 
 struct FxParams {
   XattnParams x;            // q/k/v/out, strides, wmap_index, g_sigma, scale, stat, stats_out, counters, partials
   const int8_t* cidx;       // [Bw, 80] dictionary column per token, -1 = none
-  int tiles, units, k_batched;
+  const void* mpack;        // [Bw, N, 32] fp16 packed maps (see above)
+  int64_t mpack_bs;         // elements
+  int tiles, units;
   int grid;                 // CTAs (== gridDim.x): partial slots per image
-  long long* timeline;      // debug only: clock64 stamps [tag][job] of CTA `tl_cta` (see FX_TL)
-  int tl_cta;
   int hg;                   // head groups per row tile (grouped-head kernel, xattn_fused2.cuh)
   unsigned* jobs_dump;      // debug only: [grid][2 + 2 * 512] = njobs, nstat, job table of every CTA (grouped-head kernel)
 };
-constexpr int kFxTlTags = 24, kFxTlIts = 64;
-#define FX_TL(tag, it)                                                                                     \
-  do {                                                                                                     \
-    if constexpr (kTimeline) {                                                                             \
-      if (fp.timeline != nullptr && (int)blockIdx.x == fp.tl_cta && (it) >= 0 && (it) < kFxTlIts)         \
-        fp.timeline[(tag) * kFxTlIts + (it)] = clock64();                                                  \
-    }                                                                                                      \
-  } while (0)
-
 // ------------------------------------------------------------------------------------------------------------------
 // unit order (shared by the kernel and the host replay)
 // ------------------------------------------------------------------------------------------------------------------
@@ -131,85 +119,8 @@ __host__ __device__ __forceinline__ bool fx_cta_has_image(int cta, int grid, int
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// small PTX helpers local to this kernel
-// ------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-// Shared-memory matrix descriptor, K-major SWIZZLE_64B: rows of 64 bytes, 8-row groups of 512 bytes (layout type 4).
-__device__ __forceinline__ uint64_t make_sw64_desc(uint32_t saddr) {
-  uint64_t d = (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)(16u >> 4) << 16;
-  d |= (uint64_t)(512u >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)4 << 61;
-  return d;
-}
-__device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
-  unsigned v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-// 40 consecutive TMEM columns of this thread's lane (x32 + x8), one wait.
-__device__ __forceinline__ void tmem_ld40_sync(uint32_t taddr, float* v) {
-  uint32_t r[40];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%40];\n\t"
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%32, %33, %34, %35, %36, %37, %38, %39}, [%41];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-        "=r"(r[30]), "=r"(r[31]), "=r"(r[32]), "=r"(r[33]), "=r"(r[34]), "=r"(r[35]), "=r"(r[36]), "=r"(r[37]), "=r"(r[38]), "=r"(r[39])
-      : "r"(taddr), "r"(taddr + 32)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 40; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld1_sync(uint32_t taddr, float* v) {
-  uint32_t r;
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r) : "r"(taddr) : "memory");
-  v[0] = __uint_as_float(r);
-}
-__device__ __forceinline__ void tmem_st4_u32(uint32_t taddr, const uint32_t* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};"
-               :: "r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]) : "memory");
-}
-__device__ __forceinline__ void bulk_wait_group_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-
-// ------------------------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------------------------
-// Packed map [Bw, N, 32] fp16 viewed as (col, row, image); box = 32 x 128 x 1, 64-byte swizzle.
-inline bool make_tmap_mpack(CUtensorMap* m, const void* base, int N, int Bw, int64_t batch_stride) {
-  tc::EncodeTiledFn fn = tc::encode_fn();
-  if (!fn) return false;
-  cuuint64_t dims[3] = {(cuuint64_t)kMW, (cuuint64_t)N, (cuuint64_t)Bw};
-  cuuint64_t strides[2] = {(cuuint64_t)kMW * 2, (cuuint64_t)batch_stride * 2};
-  cuuint32_t box[3] = {(cuuint32_t)kMW, (cuuint32_t)kBM, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS)
-    snprintf(tc::tc_error_buf(), 256, "cuTensorMapEncodeTiled(mpack) failed (CUresult %d): base %p N %d Bw %d stride %lld",
-             (int)r, base, N, Bw, (long long)batch_stride);
-  return r == CUDA_SUCCESS;
-}
-
-inline long long*& debug_timeline() {   // test infrastructure: device buffer [kFxTlTags][kFxTlIts] or null
-  static long long* t = nullptr;
-  return t;
-}
-inline int& debug_timeline_cta() {
-  static int c = 0;
-  return c;
-}
 inline unsigned*& debug_jobs_dump() {   // test infrastructure: device buffer the grouped-head kernel copies its job tables to
   static unsigned* p = nullptr;
   return p;

@@ -1,84 +1,43 @@
-// Paint-with-Words cross-attention, ONE launch, head-dim 40 (the 64x64-latent level of SD1.5: N = 4096, 8 heads of 40).
+// Paint-with-Words cross-attention in ONE launch (statistic + bias + softmax + P.V) on Hopper tensor cores, keys T <= 80.
 //
-// Same math, barrier rules, softmax / P.V / epilogue code and packed-map bias as xattn_fused.cuh (read its header first);
-// what changes is HOW Q REACHES SHARED MEMORY.  A head slice of a query row is 80 bytes at an 80-byte offset, and the TMA
-// engine streams such rows at ~1100-1300 cycles per [128 x 80 B] box per SM whatever the ring depth (1.9 TB/s over the
-// chip, scripts/tma_probe.cu / profiles/r02_tma_probe.txt) -- the one-launch kernel was bound by exactly that.  Full
-// 128-byte lines stream 1.6-2x faster, so here
-//     work unit = (image, 128-row tile, group of G = 4 heads);  Q tile = [128 rows x 192 columns] = 3 swizzle atoms of
-//                 whole 128-byte lines covering the unit's 160 columns, loaded ONCE per unit pass and shared by its heads;
-//     S_h       = Q[:, 16-column blocks covering head h] . K'_h^T with 3 k-steps whose A descriptors point INTO the shared
-//                 Q tile.  Head h starts at column 40 h, i.e. 0 or 8 columns into its first block, so the K operand of an
-//                 odd head is loaded 8 columns to the right (TMA box at d = -8: out-of-bounds columns are zero-filled on
-//                 both sides), and the neighbouring heads' Q columns inside the blocks meet zeros.
-// A CTA whose whole unit range fits the Q ring (<= 2 units: the cond + uncond launch of the denoising loop puts at most
-// one unit on a CTA) keeps its Q tiles resident: the statistic pass and the softmax pass read Q from HBM once.
-// K and V tiles of a head ([80 x 64] fp16 atoms) do NOT use the TMA: a [77 x 80 B] box costs the engine ~930 cycles even from
-// L2 (it is row-rate bound, ~12 cycles per short misaligned row; timeline in profiles/r02_fused2_uniform_timeline_*), more
-// than the 616 MUFU cycles of the job's softmax.  Two loader warps copy them straight into
-// the swizzled atoms (K shifted by one 16-byte chunk for odd heads, V with its ones column and zero padding written once
-// per ring stage) as 16-byte cp.async copies that arrive on the stage's mbarrier -- no staging registers, a whole ring of
-// tiles in flight.
+// The per-image statistic (max or std of Q K^T over all heads, rows and tokens) is a grid-wide dependency of every
+// biased score, so the kernel is a persistent cooperative launch (one CTA per SM, all co-resident) that runs three passes
+// over its contiguous range of work units:
+//     1. statistic jobs of the units of biased images: S = Q K^T, folded into per-warp partials, then published to the
+//        image's word in the workspace (max: one atomic max of an order-preserving key; std: a partial slot per CTA,
+//        summed by the waiters in CTA order -- deterministic for a given grid);
+//     2. softmax jobs of the unbiased units: they need no statistic and overlap the other CTAs' statistic pass;
+//     3. grid barrier (per biased image, only the CTAs that publish for it), then the softmax jobs of the biased units
+//        with the bias x * W, x = g(sigma) * fp16(statistic), W rebuilt from the packed map (xattn_fused.cuh).
+// Work unit = (image, 128-row tile, group of G heads); a unit expands into one job per head.  Each job is computed by the
+// 8 warps of the CTA with the warp-level MMA tiles of xattn_core.cuh; the cp.async copies of job i + 1 (Q rows, K, V
+// and, for biased softmax jobs, the row tile's packed map) are in flight while job i is computed.
 #pragma once
-#include <type_traits>
-#include "ptx_sm100.cuh"
+#include "mma_sm90.cuh"
 #include "pww_common.cuh"
-#include "xattn_tc.cuh"   // make_tmap, make_tmap_out, encode_fn, num_sms, tc_error_buf
-#include "xattn_fused.cuh"   // FxWalk, fx_range, fx_cta_has_image, PTX helpers, debug knobs
+#include "xattn_core.cuh"
+#include "xattn_tc.cuh"      // num_sms, cur_device, tc_error_buf
+#include "xattn_fused.cuh"   // FxWalk, fx_range, fx_cta_has_image, debug knobs
 
 namespace pww {
 namespace fx2 {
-using namespace fx;   // unit walk, helpers and constants shared with the per-head kernel
+using namespace fx;   // unit walk, helpers and constants shared with the host replay
 
 template <int D>
 struct Cfg2 {
-  static_assert(D == 40 || D == 64 || D == 80 || D == 160, "head dims of SD1.5 (40 / 80 / 160) and SD2.x (64)");
-#ifndef PWW_FX2_G
-#define PWW_FX2_G 2
-#endif
-#ifndef PWW_FX2_KVCOAL
-#define PWW_FX2_KVCOAL 2
-#endif
-  // heads per unit: 2 x 40 columns at head dim 40 (the unit's 80 columns sit inside 2 atoms wherever they start); one
-  // head at 80 (2 atoms) and at 160 (3 atoms)
-  static constexpr int G = (D == 40) ? PWW_FX2_G : (D == 64 ? 2 : 1);     // 64: two heads = two whole atoms
-  static_assert(G == 1 || G == 2 || G == 4, "heads per unit");
-  // 64-column atoms that cover the unit's G * D columns wherever they start (head dim 64: units are atom aligned)
-  static constexpr int NAQ = (D == 64) ? G : ((G * D > 80) ? 3 : 2);
-  static constexpr int NA = (D + 63) / 64;          // 64-column atoms of a head's K / V tile
-  static constexpr int DP = (D + 15) / 16 * 16;
-  static constexpr int KSTEPS = DP / 16;            // 16-column blocks per head (at 40: 3, the head starts 0 or 8 columns into its first block)
-  static constexpr bool ONES = (D == 40 || D == 80);            // row sums ride on the P.V UMMA (spare V column = 1.0)
-  static constexpr int DPV = ONES ? (D + 16) / 16 * 16 : DP;    // UMMA N of P.V: 48, 96, 160
-  static constexpr int NS = (D <= 80) ? 4 : 2;      // score slots (80 fp32 columns each; P overwrites the S it came from)
-  static constexpr int NO = (D == 40) ? 4 : 2;      // output accumulators
-  static constexpr uint32_t O_STRIDE = DPV;
-  __host__ __device__ static constexpr uint32_t col_s(int slot) { return (uint32_t)slot * 80u; }
-  __host__ __device__ static constexpr uint32_t col_o(int os) { return (uint32_t)NS * 80u + (uint32_t)os * O_STRIDE; }
-  static_assert(NS * 80 + NO * DPV <= 512, "TMEM budget");
-  static constexpr int NQ = (D == 160) ? 1 : 2;     // Q ring: unit passes in flight (or resident units)
-  static constexpr int NK = (D <= 64) ? 3 : 2;      // K ring: jobs in flight
-  static constexpr int NV = (D <= 64) ? 3 : (D == 80 ? 2 : 1);  // V ring: main jobs in flight
-  static constexpr uint32_t QBYTES = NAQ * kQAtom;
-  static constexpr uint32_t QSTAGE = QBYTES + kMAtom;           // Q atoms | packed-map atom of the row tile
-  static constexpr uint32_t KSTAGE = NA * kKAtom, VSTAGE = NA * kKAtom;
-  // output columns of the two threads of a row; every piece is a multiple of 8 columns (16-byte TMA boxes)
-  static constexpr int C0 = (D == 40) ? 24 : D / 2;
-  static constexpr int C1 = D - C0;
-  static constexpr int EPI_W = (D == 160) ? 40 : C0;            // columns per epilogue pass (staging row width)
-  static constexpr int EPI_NPASS = (D == 160) ? 2 : 1;
-  static constexpr uint32_t STG_WARP = 32 * EPI_W * 2;
-  static constexpr uint32_t OFF_K = NQ * QSTAGE;
-  static constexpr uint32_t OFF_V = OFF_K + NK * KSTAGE;
-  static constexpr uint32_t OFF_COEF = OFF_V + NV * VSTAGE;     // 2 B-operand tiles [80 x 32 fp16], 64-byte-swizzled rows
-  static constexpr uint32_t OFF_STG = OFF_COEF + 2 * kCoefTile;
-  static constexpr uint32_t OFF_XCHG = OFF_STG + 16 * STG_WARP; // [group][buf][half][128] fp32 row maxima, then row sums
-  static constexpr uint32_t OFF_BAR = OFF_XCHG + 2 * 2 * 2 * 128 * 4 * 2;
-  static constexpr uint32_t SMEM = OFF_BAR + 512 + 1024;        // + alignment slack
-  static_assert(SMEM + 7680 <= 232448, "shared memory budget (dynamic + ~7.3 KB of static tables incl. the 4 KB job table)");
-  static_assert(16 * STG_WARP >= 64 * 16, "the job-table scratch (kMaxUnits x 16 bytes) lives in the staging area");
+  // heads per unit (the granularity of a CTA's range): 2 at head dims 40 and 64, one head at 80 and 160
+  static constexpr int G = (D == 40 || D == 64) ? 2 : 1;
+  using T_ = core::Tile<D>;
+  static constexpr uint32_t MBYTES = kBM * kMW * 2;                    // packed-map rows of the row tile
+  static constexpr uint32_t OFF_M = T_::QBYTES + 2 * T_::KBYTES;
+  static constexpr uint32_t STAGE = OFF_M + MBYTES;                    // Q | K | V | map of one job
+  static constexpr uint32_t SMEM = 2 * STAGE;
+  static_assert(SMEM + 8192 <= 232448, "shared memory budget (dynamic + ~7 KB of static tables incl. the 4 KB job table)");
 };
 
+// ------------------------------------------------------------------------------------------------------------------
+// job lists (shared by the kernel and the host replay)
+// ------------------------------------------------------------------------------------------------------------------
 // ------------------------------------------------------------------------------------------------------------------
 // job lists (shared by the kernel and the host replay)
 // ------------------------------------------------------------------------------------------------------------------
@@ -153,20 +112,10 @@ struct Fx2Jobs {
 // the kernel
 // ------------------------------------------------------------------------------------------------------------------
 // Job table.  One warp builds the CTA's job list in shared memory during the prologue (parallel over the units of the
-// range: ballots and warp scans, no sequential walk) and every role then runs a WARP-UNIFORM loop over it.  That matters
-// more than it looks: tcgen05.mma, the TMA instructions and tcgen05.commit take their operands from uniform registers, and
-// a loop driven by one lane (`if (lane == 0)`) makes the compiler wrap every such instruction in an R2UR "waterfall" loop
-// (~30 instructions, 100-250 cycles per issue; measured on the first version of this kernel: ~2000 cycles of issuing
-// thread per job).  With the whole warp running the loop and `elect.sync` guarding only the issue, the descriptors are
-// computed on the uniform datapath and the UMMAs of a job go out back to back.
+// range: ballots and warp scans, no sequential walk); the whole CTA then walks it.
 //   s_jobs[i].x = b | h << 8 | tile << 16          s_jobs[i].y = flags, see the JF_* masks
 constexpr int kMaxUnits = 64;        // units per CTA (host-checked: the C ABI splits larger batches)
 constexpr int kMaxJobs = 512;        // kMaxUnits * G heads * 2 passes
-// K / V tile copies with consecutive lanes along a row's chunks: 0 = never, 1 = always, 2 = every head dim but 40.  Measured
-// (profiles/r02_kvcoal_*): 4-12 % faster launches at head dims 64 / 80 / 160; at 40 the 5- and 6-chunk rows make the index
-// arithmetic dearer than the wavefronts it saves (B = 16: +2.8 %), so that head dim keeps one lane per row.
-template <int D>
-constexpr bool kKvCoalesced = PWW_FX2_KVCOAL == 1 || (PWW_FX2_KVCOAL == 2 && D != 40);
 constexpr uint32_t JF_MAIN = 1u, JF_BIASED = 2u, JF_FIRST = 4u, JF_LAST = 8u;   // | li << 4 (2 bits) | ul << 8 (8 bits)
 
 // Order-preserving map float -> unsigned (0 is below every real number: a zero-filled workspace reads as -infinity).
@@ -177,54 +126,19 @@ __device__ __forceinline__ unsigned f32_key(float f) {
 __device__ __forceinline__ float key_f32(unsigned k) {
   return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
 }
-// 16-byte asynchronous copy global -> shared (LDGSTS): no staging registers, many tiles in flight.  src_bytes = 0 writes zeros.
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
-}
-// one arrival on `bar` once every cp.async this thread has issued so far has landed (the count is part of the barrier's
-// expected arrivals: 32 lanes -> init 32)
-__device__ __forceinline__ void cp_async_arrive(uint32_t bar) {
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
-}
-// Per-image synchronisation word of the grid barrier (workspace + 256 + 8 b): low half = order-preserving key of the running
-// maximum (atomic max), high half = number of CTAs that have published.  One acquire load returns both.
-__device__ __forceinline__ unsigned long long ld_acquire_gpu_u64(const unsigned long long* p) {
-  unsigned long long v;
-  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ bool elect_one() {     // true on exactly one lane of a converged warp
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
 
-// kTimeline = true compiles the clock64 stamps in (scripts/fused_timeline.py); the production instantiation has none of
-// them -- at the denoising loop's launch sizes every role runs its code once or twice, so kernel time tracks CODE SIZE
-// (instruction-cache misses were 20 % of the stall samples of a 197 KB build; this one is under 100 KB).
-template <int D, int TT, bool kTimeline>
-__global__ void __launch_bounds__(kThreads, 1)
-xattn_fused2_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ CUtensorMap tmm,
-                    const __grid_constant__ CUtensorMap tmo0, const __grid_constant__ CUtensorMap tmo1,
-                    const FxParams fp) {
-  using C = Cfg2<D>;
+template <int D>
+__global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const FxParams fp) {
+  using C = core::Tile<D>;
+  using CF = Cfg2<D>;
   const XattnParams& p = fp.x;
-  if (threadIdx.x == 0) FX_TL(21, 0);
-  extern __shared__ unsigned char smem_raw[];
-  const uint32_t smem0 = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
-  unsigned char* smem_gen = smem_raw + (smem0 - ptx::smem_u32(smem_raw));
-  const uint32_t bar0 = smem0 + C::OFF_BAR;
-  auto BAR = [&](int i) { return bar0 + 8u * i; };
-  constexpr int B_QFULL = 0, B_QEMPTY = 2, B_KFULL = 4, B_KEMPTY = 7, B_VFULL = 10, B_VEMPTY = 13, B_SREADY = 16,
-                B_SFREE = 20, B_PREADY = 24, B_PVDONE = 28, B_OFREE = 32, B_COEF = 36, B_TMEMPTR = 38, B_STATS = 39;
+  extern __shared__ __align__(128) unsigned char smem[];
+  const uint32_t smem0 = ptx::smem_u32(smem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int T = TT ? TT : p.T;
+  const int T = p.T;
   int u0, u1;
   fx_range(blockIdx.x, gridDim.x, fp.units, u0, u1);
   const int n_it = u1 - u0;
-  // Resident mode: the CTA's whole unit range fits the Q ring, so unit ul owns stage ul for the whole kernel (loaded once,
-  // read by the statistic pass AND the softmax pass); otherwise a stage is loaded per unit pass and released after it.
-  const bool resident = n_it <= C::NQ;
   const int HG = fp.hg;
 
   __shared__ int s_widx[kMaxBatch];
@@ -232,71 +146,13 @@ xattn_fused2_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_consta
   __shared__ int s_nb, s_njobs, s_nstat, s_nl;
   __shared__ int s_lb[kMaxLocal], s_lp[kMaxLocal];   // image / group position of the CTA's local biased images
   __shared__ float s_coef[kMaxLocal];             // g(sigma) * statistic of the CTA's local biased images
-  __shared__ StatPartial s_part[16][kMaxLocal];   // [softmax warp][local biased image]
+  __shared__ StatPartial s_part[core::kWarps][kMaxLocal];   // [warp][local biased image]
   __shared__ uint2 s_jobs[kMaxJobs];
+  __shared__ uint4 s_unit[kMaxUnits];              // job-table build scratch: one entry per unit of the range
   __shared__ int s_expect[kMaxLocal];              // CTAs that publish a partial for each local biased image
-  __shared__ unsigned s_key[16][kMaxLocal];        // max statistic: order-preserving keys of the softmax warps' partial maxima
   __shared__ signed char s_cidx[kMaxLocal][kTP];   // token -> dictionary column of the CTA's local biased images
-  __shared__ int s_img0[kMaxBatch], s_widx0[kMaxBatch], s_pre;   // producer warp's own copy of the partition; early Q loads
 
   if (warp == 0) {
-    // ---- early Q: the first unit passes' tiles are requested BEFORE the prologue's block-wide sync, so the ~2 us of cold
-    //      HBM latency overlap TMEM allocation and the job-table build.  The warp partitions the images itself (same
-    //      ballots as warp 2), initialises the Q barriers and issues the loads of unit passes 0 .. s_pre - 1. ----
-    const int b = lane;
-    const int wi = (b < p.B && p.wmap != nullptr) ? (p.wmap_index ? p.wmap_index[b] : b) : -1;
-    const bool valid = b < p.B, bi = valid && wi >= 0;
-    const unsigned mbk = __ballot_sync(0xffffffffu, bi), muk = __ballot_sync(0xffffffffu, valid && !bi);
-    const unsigned ltk = (1u << lane) - 1u;
-    const int nb0 = __popc(mbk);
-    if (bi) s_img0[__popc(mbk & ltk)] = b;
-    else if (valid) s_img0[nb0 + __popc(muk & ltk)] = b;
-    if (valid) s_widx0[b] = wi;
-    __syncwarp();
-    if (lane == 0) {
-      ptx::prefetch_tmap(&tmq);
-      ptx::prefetch_tmap(&tmm);
-      for (int s = 0; s < C::NQ; ++s) {
-        ptx::mbar_init(BAR(B_QFULL + s), 1);
-        ptx::mbar_init(BAR(B_QEMPTY + s), 1);
-      }
-      ptx::fence_barrier_init();
-      // unit passes in job order: biased units (statistic pass; in resident mode the one load serves both passes), then
-      // unbiased units.  Resident: unit ul -> stage ul.  Ring: pass up -> stage up % NQ, only the first NQ go out here.
-      int pre = 0;
-      FxWalk w(u0, p.B, HG, fp.tiles, nb0, s_img0);
-      if (resident) {
-        for (int ul = 0; ul < n_it; ++ul, w.next()) {
-          const FxUnit u = w.get();
-          const uint32_t qb = smem0 + ul * C::QSTAGE;
-          ptx::mbar_arrive_expect_tx(BAR(B_QFULL + ul), C::QBYTES + (u.biased ? kMAtom : 0u));
-          const int atom0 = (u.h * C::G * D) / 64;
-          for (int a = 0; a < C::NAQ; ++a)
-            tma_load_3d(qb + a * kQAtom, &tmq, BAR(B_QFULL + ul), (atom0 + a) * 64, u.tile * kBM, u.b);
-          if (u.biased) tma_load_3d(qb + C::QBYTES, &tmm, BAR(B_QFULL + ul), 0, u.tile * kBM, s_widx0[u.b]);
-        }
-        pre = n_it;
-      } else {
-        for (int pass = 0; pass < 2 && pre < C::NQ; ++pass) {        // pass 0: biased units, pass 1: unbiased units
-          if (pass == 0 && nb0 == 0) continue;
-          FxWalk w2 = w;
-          for (int it = 0; it < n_it && pre < C::NQ; ++it, w2.next()) {
-            const FxUnit u = w2.get();
-            if ((u.biased != 0) != (pass == 0)) continue;
-            const uint32_t qb = smem0 + pre * C::QSTAGE;
-            ptx::mbar_arrive_expect_tx(BAR(B_QFULL + pre), C::QBYTES);    // statistic / unbiased passes read no map
-            const int atom0 = (u.h * C::G * D) / 64;
-            for (int a = 0; a < C::NAQ; ++a)
-              tma_load_3d(qb + a * kQAtom, &tmq, BAR(B_QFULL + pre), (atom0 + a) * 64, u.tile * kBM, u.b);
-            ++pre;
-          }
-        }
-      }
-      s_pre = pre;
-    }
-    __syncwarp();
-  }
-  if (warp == 2) {
     // ---- stable partition of the images by "has a weight map" ----
     {
       const int b = lane;
@@ -314,7 +170,6 @@ xattn_fused2_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_consta
     // ---- job table: pass 1 gives every unit its place in the three lists, pass 2 expands units into head jobs ----
     const int nbi = s_nb;
     const unsigned lt = (1u << lane) - 1u;
-    uint4* s_unit = reinterpret_cast<uint4*>(smem_gen + C::OFF_STG);     // scratch: the staging tiles are idle until the first epilogue
     int c_sj = 0, c_uj = 0, c_li = -1, c_lastb = -1;
     for (int base = 0; base < n_it; base += 32) {
       const int ul = base + lane;
@@ -331,7 +186,7 @@ xattn_fused2_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_consta
       const bool newimg = isb && u.b != bprev;
       const unsigned mn = __ballot_sync(0xffffffffu, newimg);
       const int li = c_li + __popc(mn & (lt | (1u << lane)));
-      const int nh = valid ? ((p.H - u.h * C::G) < C::G ? (p.H - u.h * C::G) : C::G) : 0;
+      const int nh = valid ? ((p.H - u.h * CF::G) < CF::G ? (p.H - u.h * CF::G) : CF::G) : 0;
       int sb = isb ? nh : 0, su = isu ? nh : 0;            // inclusive warp scans of the head counts
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1) {
@@ -355,7 +210,7 @@ xattn_fused2_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_consta
       const unsigned bi = r.y & 1u, li = (r.y >> 4) & 3u, nh = (r.y >> 8) & 0xffu, hg = (r.x >> 8) & 0xffu;
       const unsigned base_x = (r.x & 0xffu) | (r.x & 0xffff0000u);
       for (unsigned hl = 0; hl < nh; ++hl) {
-        const unsigned x = base_x | ((hg * C::G + hl) << 8);
+        const unsigned x = base_x | ((hg * CF::G + hl) << 8);
         const unsigned fl = (hl == 0 ? JF_FIRST : 0u) | (hl == nh - 1 ? JF_LAST : 0u) | (li << 4) | ((unsigned)(ul & 0xff) << 8);
         if (bi) {
           s_jobs[r.z + hl] = make_uint2(x, fl | JF_BIASED);
@@ -366,667 +221,225 @@ xattn_fused2_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_consta
       }
     }
     if (lane == 0) { s_njobs = 2 * ns + nuj; s_nstat = ns; s_nl = c_li + 1; }
-    if (lane == 0) FX_TL(22, 0);
   }
-  for (int i = threadIdx.x; i < 16 * kMaxLocal; i += kThreads) {
+  for (int i = threadIdx.x; i < core::kWarps * kMaxLocal; i += blockDim.x) {
     StatPartial sp;
     sp.vmax = -INFINITY; sp.sum = 0.0; sp.sumsq = 0.0; sp.pad = 0.0;
     s_part[i / kMaxLocal][i % kMaxLocal] = sp;
-    s_key[i / kMaxLocal][i % kMaxLocal] = 0u;      // key 0 is below every real number
   }
-  // K / V ring stages, once: zero rows T..79 (the per-job copies never touch them); V columns D .. DPV-1 = [1.0, 0 ...] for
-  // real tokens -- the spare column that makes accumulator column D of the P.V UMMA the row sum -- and zero for padded ones.
-  {
-    constexpr int kch = C::DP / 8, vch = C::DPV / 8;           // 16-byte chunks the UMMAs read per row
-    for (int idx = threadIdx.x; idx < C::NK * (kTP - T) * kch; idx += kThreads) {
-      const int stz = idx / ((kTP - T) * kch), rem = idx - stz * ((kTP - T) * kch);
-      const int t = T + rem / kch, ch = rem % kch;
-      *reinterpret_cast<uint4*>(smem_gen + C::OFF_K + stz * C::KSTAGE + (ch >> 3) * kKAtom + t * 128 + (((ch & 7) ^ (t & 7)) << 4)) =
-          make_uint4(0, 0, 0, 0);
-    }
-    for (int idx = threadIdx.x; idx < C::NV * kTP; idx += kThreads) {
-      const int stz = idx / kTP, t = idx - stz * kTP;
-      unsigned char* vrow = smem_gen + C::OFF_V + stz * C::VSTAGE + t * 128;
-      if (t >= T) {
-#pragma unroll 1
-        for (int ch = 0; ch < D / 8; ++ch)
-          *reinterpret_cast<uint4*>(vrow + (ch >> 3) * kKAtom + (((ch & 7) ^ (t & 7)) << 4)) = make_uint4(0, 0, 0, 0);
-      }
-#pragma unroll 1
-      for (int ch = D / 8; ch < vch; ++ch)
-        *reinterpret_cast<uint4*>(vrow + (ch >> 3) * kKAtom + (((ch & 7) ^ (t & 7)) << 4)) =
-            make_uint4((C::ONES && ch == D / 8 && t < T) ? 0x00003C00u : 0u, 0, 0, 0);
-    }
-  }
-  ptx::fence_proxy_async_smem();                   // generic-proxy writes above -> visible to the UMMAs (async proxy)
-  if (warp == 3 && lane == 0) {
-    ptx::prefetch_tmap(&tmo0);
-    ptx::prefetch_tmap(&tmo1);
-    for (int s = 0; s < 3; ++s) {
-      ptx::mbar_init(BAR(B_KFULL + s), 32);      // one cp.async arrival per lane of the loader warp
-      ptx::mbar_init(BAR(B_KEMPTY + s), 1);
-      ptx::mbar_init(BAR(B_VFULL + s), 32);
-      ptx::mbar_init(BAR(B_VEMPTY + s), 1);
-    }
-    for (int s = 0; s < 4; ++s) {
-      ptx::mbar_init(BAR(B_SREADY + s), 1);
-      ptx::mbar_init(BAR(B_SFREE + s), 8);       // one elected arrive per warp of the slot's softmax group
-      ptx::mbar_init(BAR(B_PREADY + s), 8);
-      ptx::mbar_init(BAR(B_PVDONE + s), 1);
-      ptx::mbar_init(BAR(B_OFREE + s), 8);
-    }
-    ptx::mbar_init(BAR(B_COEF + 0), 1);
-    ptx::mbar_init(BAR(B_COEF + 1), 1);
-    ptx::mbar_init(BAR(B_STATS), 16);             // every softmax warp has written its statistic partials
-    ptx::fence_barrier_init();
-  }
-  if (warp == 1) {
-    ptx::tmem_alloc<512>(BAR(B_TMEMPTR));
-    if (lane == 0) FX_TL(23, 0);
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem_gen + C::OFF_BAR + 8 * B_TMEMPTR);
   const int nb = s_nb;
-  const int njobs = s_njobs, ns = s_nstat;
-  if (threadIdx.x == 0) FX_TL(13, 0);
+  const int njobs = s_njobs, ns = s_nstat, nl = s_nl;
   if (fp.jobs_dump != nullptr) {                              // debug: the job table as built on the device
     unsigned* d = fp.jobs_dump + (size_t)blockIdx.x * (2 + 2 * kMaxJobs);
     if (threadIdx.x == 0) { d[0] = (unsigned)njobs; d[1] = (unsigned)ns; }
 #pragma unroll 1
-    for (int i = threadIdx.x; i < njobs; i += kThreads) { d[2 + 2 * i] = s_jobs[i].x; d[3 + 2 * i] = s_jobs[i].y; }
+    for (int i = threadIdx.x; i < njobs; i += blockDim.x) { d[2 + 2 * i] = s_jobs[i].x; d[3 + 2 * i] = s_jobs[i].y; }
   }
   const int nu_img = p.B - nb;
   const int np = nb < nu_img ? nb : nu_img;
+  const int nuj = njobs - 2 * ns;                             // softmax jobs of unbiased units
 
   if (blockIdx.x == 0 && p.stats_out != nullptr)            // images without a weight map report statistic 0
 #pragma unroll 1
-    for (int b = threadIdx.x; b < p.B; b += kThreads)
+    for (int b = threadIdx.x; b < p.B; b += blockDim.x)
       if (s_widx[b] < 0) p.stats_out[b] = 0.f;
-
-  // One head's K or V rows ([T x D] fp16 = 5 chunks of 16 bytes per row) into a swizzled [80 x 128 B] atom with 16-byte
-  // asynchronous copies, data chunk `ch` landing in chunk column ch + shift; chunk column `zc` (< 0: none) is zero-filled.
-  auto copy_kv = [&](uint32_t tile, const __half* base, unsigned x, int shift, int zc, uint32_t bar) {
-    const int b = x & 0xff, h = (x >> 8) & 0xff;
-    const __half* src = base + (fp.k_batched ? (int64_t)b * p.k_bs : 0) + h * D;
-    if constexpr (kKvCoalesced<D>) {
-      // Consecutive lanes take consecutive 16-byte chunks of a row (then the next row): one warp instruction reads a few
-      // whole rows, i.e. a handful of LSU wavefronts, instead of one chunk of 32 different rows = 32 wavefronts.
-      auto rows = [&](auto cpr_tag) {
-        constexpr int CPR = decltype(cpr_tag)::value;      // chunk columns written per row
-        const int total = T * CPR;
-#pragma unroll 4
-        for (int idx = lane; idx < total; idx += 32) {
-          const int t = idx / CPR, c = idx - t * CPR;      // destination chunk column c of row t
-          const bool zero = c == zc;
-          const int ch = zero ? 0 : c - shift;             // source chunk of the head's row
-          const uint4* srow = reinterpret_cast<const uint4*>(src + (int64_t)t * p.k_rs);
-          cp_async16(tile + t * 128 + (c >> 3) * kKAtom + (((c & 7) ^ (t & 7)) << 4), srow + ch, zero ? 0u : 16u);
-        }
-      };
-      if (zc >= 0) rows(std::integral_constant<int, D / 8 + 1>{});   // K at head dim 40: the data chunks and the zeroed one
-      else rows(std::integral_constant<int, D / 8>{});
-      cp_async_arrive(bar);
-      return;
-    }
-#pragma unroll
-    for (int jj = 0; jj < (kTP + 31) / 32; ++jj) {       // a lane owns whole rows: one address computation per row
-      const int t = lane + 32 * jj;
-      if (t < T) {
-        const uint4* srow = reinterpret_cast<const uint4*>(src + (int64_t)t * p.k_rs);
-        const uint32_t drow = tile + t * 128;
-        const int x7 = t & 7;
-#pragma unroll
-        for (int ch = 0; ch < D / 8; ++ch) {             // chunk ch -> atom (ch + shift) / 8, chunk column (ch + shift) % 8
-          const int cc = ch + shift;
-          cp_async16(drow + (cc >> 3) * kKAtom + (((cc & 7) ^ x7) << 4), srow + ch, 16u);
-        }
-        if (zc >= 0) cp_async16(drow + ((zc ^ x7) << 4), srow, 0u);
-      }
-    }
-    cp_async_arrive(bar);
-  };
-
-  if (warp == 0) {
-    // ============================== producer: Q (+ packed map) by TMA per unit pass, K tiles by loads per job ==============================
-    auto load_q = [&](int qst, int b, int tile, int hgi, bool with_map) {     // elected lane only
-      const uint32_t qb = smem0 + qst * C::QSTAGE;
-      ptx::mbar_arrive_expect_tx(BAR(B_QFULL + qst), C::QBYTES + (with_map ? kMAtom : 0u));
-      const int atom0 = (hgi * C::G * D) / 64;             // first 64-column atom of the unit's heads
-#pragma unroll
-      for (int a = 0; a < C::NAQ; ++a)
-        tma_load_3d(qb + a * kQAtom, &tmq, BAR(B_QFULL + qst), (atom0 + a) * 64, tile * kBM, b);
-      if (with_map) tma_load_3d(qb + C::QBYTES, &tmm, BAR(B_QFULL + qst), 0, tile * kBM, s_widx[b]);
-    };
-    const int pre = s_pre;                         // unit passes whose Q tile was requested in the prologue
-    int up = -1;
-    for (int i = 0; i < njobs; ++i) {
-      const uint2 r = s_jobs[i];
-      const int b = r.x & 0xff, h = (r.x >> 8) & 0xff, tile = r.x >> 16;
-      if (r.y & JF_FIRST) {
-        ++up;
-        if (!resident && up >= pre) {                // ring mode: one load per unit pass
-          const int qst = up % C::NQ;
-          ptx::mbar_wait(BAR(B_QEMPTY + qst), (uint32_t)(((up / C::NQ) & 1) ^ 1));
-          if (elect_one()) {
-            // the packed map of the row tile rides with Q in the pass that reads it
-            load_q(qst, b, tile, h / C::G, (r.y & (JF_BIASED | JF_MAIN)) == (JF_BIASED | JF_MAIN));
-            FX_TL(0, i);
-          }
-          __syncwarp();
-        }
-      }
-      // ---- K'_h tile: the head's rows into the swizzled atom, shifted by one 16-byte chunk for odd heads (the head starts
-      //      8 columns into its first 16-column block); the chunk column the shift leaves free is zeroed ----
-      const int st = i % C::NK;
-      ptx::mbar_wait(BAR(B_KEMPTY + st), (uint32_t)(((i / C::NK) & 1) ^ 1));
-      if (lane == 0) FX_TL(16, i);
-      const int sh = ((h * D) % 16) ? 1 : 0;         // only head dim 40 has heads that start mid-block
-      copy_kv(smem0 + C::OFF_K + st * C::KSTAGE, p.k, r.x, sh, (D == 40) ? (sh ? 0 : 5) : -1, BAR(B_KFULL + st));
-      if (lane == 0) FX_TL(17, i);
+  if (warp == 1) {
+    // how many CTAs publish a partial for each of my local biased images
+#pragma unroll 1
+    for (int l = 0; l < nl && l < kMaxLocal; ++l) {
+      int e = 0;
+      const int pos = s_lp[l];
+#pragma unroll 1
+      for (int c = lane; c < (int)gridDim.x; c += 32) e += fx_cta_has_image(c, gridDim.x, fp.units, pos, HG, fp.tiles, np) ? 1 : 0;
+      e = __reduce_add_sync(0xffffffffu, e);
+      if (lane == 0) s_expect[l] = e;
     }
   } else if (warp == 2) {
-    // ============================== loader: V tiles of the main jobs (+ statistic publish) ==============================
-    auto publish = [&]() {
-      const int nl = s_nl;
-      if (p.stat == PWW_STAT_MAX) {
-        // the maximum is order independent: 16 keys -> one warp reduction -> one atomic max on the image's word
+    for (int idx = lane; idx < nl * kTP && idx < kMaxLocal * kTP; idx += 32) {
+      const int l = idx / kTP, t = idx - l * kTP;
+      s_cidx[l][t] = (t < T) ? fp.cidx[(int64_t)s_widx[s_lb[l]] * kTP + t] : (signed char)-1;
+    }
+  }
+
+  // the copies of job i into stage i % 2
+  auto issue = [&](int i) {
+    const uint2 r = s_jobs[i];
+    const int b = r.x & 0xff, h = (r.x >> 8) & 0xff, tile = r.x >> 16;
+    const bool is_main = (r.y & JF_MAIN) != 0, biased = (r.y & JF_BIASED) != 0;
+    const uint32_t st = smem0 + (i & 1) * CF::STAGE;
+    const int rows = p.N - tile * kBM < kBM ? p.N - tile * kBM : kBM;
+    core::load_rows<D>(st, p.q + (int64_t)b * p.q_bs + (int64_t)tile * kBM * p.q_rs + h * D, p.q_rs, kBM, rows);
+    core::load_rows<D>(st + C::QBYTES, p.k + (int64_t)b * p.k_bs + h * D, p.k_rs, kTP, T);
+    if (is_main) core::load_rows<D>(st + C::QBYTES + C::KBYTES, p.v + (int64_t)b * p.k_bs + h * D, p.k_rs, kTP, T);
+    if (is_main && biased) {
+      const __half* mp = reinterpret_cast<const __half*>(fp.mpack) + (int64_t)s_widx[b] * fp.mpack_bs + (int64_t)tile * kBM * kMW;
+      for (int idx = threadIdx.x; idx < kBM * (kMW / 8); idx += blockDim.x) {
+        const int rr = idx >> 2, c = idx & 3;
+        const bool ok = rr < rows;
+        ptx::cp_async16(st + CF::OFF_M + (uint32_t)(rr * kMW + c * 8) * 2u, ok ? (const void*)(mp + rr * kMW + c * 8) : fp.mpack,
+                        ok ? 16u : 0u);
+      }
+    }
+    ptx::cp_async_commit();
+  };
+
+  const float sl2 = p.scale * 1.4426950408889634f;
+  const bool is_max = p.stat == PWW_STAT_MAX;
+  const float gsig = (nb > 0 && p.g_sigma != nullptr) ? __ldg(p.g_sigma) : 0.f;
+  const unsigned long long* sync_words = reinterpret_cast<const unsigned long long*>(p.counters + 64);
+  float vmax = -INFINITY;                          // this thread's statistic partial of local image cur_li
+  double dsum = 0.0, dsq = 0.0;
+  int cur_li = -1;
+  auto flush = [&]() {
+    if (cur_li < 0) return;
+    double m = vmax, a = dsum, q = dsq;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+      a += __shfl_xor_sync(0xffffffffu, a, o);
+      q += __shfl_xor_sync(0xffffffffu, q, o);
+    }
+    if (lane == 0 && cur_li < kMaxLocal) {
+      StatPartial sp;
+      sp.vmax = m; sp.sum = a; sp.sumsq = q; sp.pad = 1.0;
+      s_part[warp][cur_li] = sp;
+    }
+    vmax = -INFINITY; dsum = 0.0; dsq = 0.0;
+  };
+
+  if (njobs > 0) issue(0);
+#pragma unroll 1
+  for (int i = 0; i < njobs; ++i) {
+    if (i + 1 < njobs) {
+      issue(i + 1);
+      ptx::cp_async_wait<1>();
+    } else {
+      ptx::cp_async_wait<0>();
+    }
+    __syncthreads();
+    if (i == ns && ns > 0 && warp == 0) {
+      // ---- publish the CTA's statistic partials: the 8 warps' partials in a fixed order, folded into the image's word ----
+      if (is_max) {
         for (int l = 0; l < nl && l < kMaxLocal; ++l) {
-          const unsigned k = __reduce_max_sync(0xffffffffu, lane < 16 ? s_key[lane][l] : 0u);
+          const unsigned k = __reduce_max_sync(0xffffffffu, lane < core::kWarps ? f32_key((float)s_part[lane][l].vmax) : 0u);
           if (lane == 0) {
             unsigned* word = p.counters + 64 + 2 * s_lb[l];        // {max key, count}, see ld_acquire_gpu_u64
             asm volatile("red.relaxed.gpu.global.max.u32 [%0], %1;" ::"l"(word), "r"(k) : "memory");
-            // release: the maximum above is visible to whoever acquires the new count; nothing is waited for here
+            // release: the maximum above is visible to whoever acquires the new count
             asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(word + 1) : "memory");
           }
         }
       } else if (lane < nl && lane < kMaxLocal) {
-        // std: fixed-order sums of the 16 warps' partials into this CTA's slot (the waiters add the slots in CTA order)
         const int lbv = s_lb[lane];
         StatPartial sp = s_part[0][lane];
 #pragma unroll 1
-        for (int w2 = 1; w2 < 16; ++w2) {
+        for (int w2 = 1; w2 < core::kWarps; ++w2) {
           sp.sum += s_part[w2][lane].sum;
           sp.sumsq += s_part[w2][lane].sumsq;
         }
         p.partials[(int64_t)lbv * gridDim.x + blockIdx.x] = sp;
         asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(p.counters + 64 + 2 * lbv + 1) : "memory");
       }
-      if (lane == 0) FX_TL(12, 0);
-      __syncwarp();
-    };
-    for (int i = ns; i < njobs; ++i) {
-      const int m = i - ns, st = m % C::NV;
-      if (m == C::NV && ns > 0) {
-        // ---- publish the CTA's statistic partials (the first NV tiles of V are already on their way): one lane per local
-        //      image reduces the 16 softmax warps' partials in a fixed order, folds them into the image's word, arrives ----
-        ptx::mbar_wait(BAR(B_STATS), 0);
-        publish();
-      }
-      ptx::mbar_wait(BAR(B_VEMPTY + st), (uint32_t)(((m / C::NV) & 1) ^ 1));
-      if (lane == 0) FX_TL(18, i);
-      copy_kv(smem0 + C::OFF_V + st * C::VSTAGE, p.v, s_jobs[i].x, 0, -1, BAR(B_VFULL + st));
-      if (lane == 0) FX_TL(19, i);
-    }
-    if (ns > 0 && njobs - ns <= C::NV) {           // fewer main jobs than ring stages: not published inside the loop
-      ptx::mbar_wait(BAR(B_STATS), 0);
-      publish();
-    }
-  } else if (warp == 1) {
-    // ============================== UMMA issuer: S of every job (+ grid barrier and the bias operand) ==============================
-    constexpr uint32_t idesc_qk = ptx::make_idesc_f16(128, kTP, false, false);
-    bool stats_ready = false;
-    int cur_li = -1, up = -1;
-    // how many CTAs publish a partial for each of my local biased images: counted now, off the critical path
-    {
-      const int nl = s_nl, G = (int)gridDim.x;
-#pragma unroll 1
-      for (int l = 0; l < nl && l < kMaxLocal; ++l) {
-        int e = 0;
-        const int pos = s_lp[l];
-#pragma unroll 1
-        for (int c = lane; c < G; c += 32) e += fx_cta_has_image(c, G, fp.units, pos, HG, fp.tiles, np) ? 1 : 0;
-        e = __reduce_add_sync(0xffffffffu, e);
-        if (lane == 0) s_expect[l] = e;
-      }
       __syncwarp();
     }
-    const unsigned long long* sync_words = reinterpret_cast<const unsigned long long*>(p.counters + 64);
-    // everything the bias operand needs besides the statistic is fetched now, not after the barrier
-    const float gsig = (nb > 0 && p.g_sigma != nullptr) ? __ldg(p.g_sigma) : 0.f;
-    {
-      const int nl = s_nl;
-      for (int idx = lane; idx < nl * kTP && idx < kMaxLocal * kTP; idx += 32) {
-        const int l = idx / kTP, t = idx - l * kTP;
-        s_cidx[l][t] = (t < T) ? fp.cidx[(int64_t)s_widx[s_lb[l]] * kTP + t] : (signed char)-1;
-      }
-      __syncwarp();
-    }
-    // Jobs are issued in PAIRS where two consecutive jobs are of the same kind (one per softmax group): the loop's fixed
-    // cost -- table read, barrier probes, fences, elect, warp sync, ~1000 cycles of a single warp's dependent chain -- is
-    // paid once per two heads, and both groups get their S at the same time.
-    for (int i = 0; i < njobs;) {
-      const uint2 r = s_jobs[i];
-      const int b = r.x & 0xff;
-      const bool is_main = (r.y & JF_MAIN) != 0, biased = (r.y & JF_BIASED) != 0;
-      const int li = (r.y >> 4) & 3;
-      int npair = 1;
-      if (i + 1 < njobs) {
-        const unsigned y1 = s_jobs[i + 1].y, km = JF_MAIN | JF_BIASED;
-        bool same = (r.y & km) == (y1 & km);
-        if (same && (r.y & km) == km) same = li == (int)((y1 >> 4) & 3);        // biased softmax jobs: same image's bias operand
-        // both jobs' Q tiles must be able to sit in shared memory at once: same unit pass, resident stages, or a ring of >= 2
-        if (same && (y1 & JF_FIRST) && !resident && C::NQ < 2) same = false;
-        if (same) npair = 2;
-      }
-      if (is_main && biased) {
-        if (!stats_ready) {
-          // ---- grid barrier: every CTA owning units of my biased images has published its partial ----
-          const int nl = s_nl;
-          const int G = (int)gridDim.x;
-          if (lane == 0) FX_TL(10, 0);
+    if (i == ns + nuj && ns > 0) {
+      if (warp == 0) {
+        // ---- grid barrier: every CTA owning units of my biased images has published its partial ----
+        const int G = (int)gridDim.x;
 #pragma unroll 1
-          for (int l = 0; l < nl && l < kMaxLocal; ++l) {
-            const int bl = s_lb[l], pos = s_lp[l];
-            const unsigned expect = (unsigned)s_expect[l];
-            unsigned long long word = 0;
-            if (lane == 0) {
-              const long long t0 = clock64();
-              while ((unsigned)((word = ld_acquire_gpu_u64(sync_words + bl)) >> 32) < expect) {
-                if (clock64() - t0 > 20000000000LL) {
-                  printf("pww: grid barrier timeout block %d image %d have %u want %u\n", blockIdx.x, bl,
-                         (unsigned)(word >> 32), expect);
-                  __trap();
-                }
+        for (int l = 0; l < nl && l < kMaxLocal; ++l) {
+          const int bl = s_lb[l], pos = s_lp[l];
+          const unsigned expect = (unsigned)s_expect[l];
+          unsigned long long word = 0;
+          if (lane == 0) {
+            const long long t0 = clock64();
+            while ((unsigned)((word = ptx::ld_acquire_gpu_u64(sync_words + bl)) >> 32) < expect) {
+              if (clock64() - t0 > 20000000000LL) {
+                printf("pww: grid barrier timeout block %d image %d have %u want %u\n", blockIdx.x, bl,
+                       (unsigned)(word >> 32), expect);
+                __trap();
               }
             }
-            __syncwarp();
-            double m = -INFINITY, a = 0.0, q = 0.0;
-            if (p.stat == PWW_STAT_MAX) {
-              // the maximum is order independent: every publisher folded its partial into the word with an atomic max
-              m = (double)key_f32((unsigned)word);
+          }
+          __syncwarp();
+          double m = -INFINITY, a = 0.0, q = 0.0;
+          if (is_max) {
+            // the maximum is order independent: every publisher folded its partial into the word with an atomic max
+            m = (double)key_f32((unsigned)__shfl_sync(0xffffffffu, (unsigned)word, 0));
+          } else {
+            (void)ptx::ld_acquire_gpu_u64(sync_words + bl);      // every lane orders its partial loads behind the count
+            for (int c = lane; c < G; c += 32)
+              if (fx_cta_has_image(c, G, fp.units, pos, HG, fp.tiles, np)) {
+                const StatPartial* pp = p.partials + (int64_t)bl * G + c;
+                a += __ldcg(&pp->sum);
+                q += __ldcg(&pp->sumsq);
+              }
+#pragma unroll 1
+            for (int o = 16; o > 0; o >>= 1) {
+              a += __shfl_xor_sync(0xffffffffu, a, o);
+              q += __shfl_xor_sync(0xffffffffu, q, o);
+            }
+          }
+          if (lane == 0) {
+            const double cnt = (double)p.H * (double)p.N * (double)p.T;
+            double rr;
+            if (is_max) {
+              rr = m;
             } else {
-              (void)ld_acquire_gpu_u64(sync_words + bl);           // every lane orders its partial loads behind the count
-              for (int c = lane; c < G; c += 32)
-                if (fx_cta_has_image(c, G, fp.units, pos, HG, fp.tiles, np)) {
-                  const StatPartial* pp = p.partials + (int64_t)bl * G + c;
-                  a += __ldcg(&pp->sum);
-                  q += __ldcg(&pp->sumsq);
-                }
-#pragma unroll 1
-              for (int o = 16; o > 0; o >>= 1) {
-                a += __shfl_xor_sync(0xffffffffu, a, o);
-                q += __shfl_xor_sync(0xffffffffu, q, o);
-              }
+              const double var = (q - a * a / cnt) / (cnt - 1.0);
+              rr = sqrt(var > 0.0 ? var : 0.0);
             }
-            if (lane == 0) {
-              const double cnt = (double)p.H * (double)p.N * (double)p.T;
-              double rr;
-              if (p.stat == PWW_STAT_MAX) {
-                rr = m;
-              } else {
-                const double var = (q - a * a / cnt) / (cnt - 1.0);
-                rr = sqrt(var > 0.0 ? var : 0.0);
-              }
-              const float st16 = round_to_f16((float)rr);         // qk.max() / qk.std() return fp16 in the reference
-              s_coef[l] = gsig * st16;
-              if (p.stats_out != nullptr) p.stats_out[bl] = st16;   // every CTA of the image writes the same value
-            }
+            const float st16 = round_to_f16((float)rr);         // qk.max() / qk.std() return fp16 in the reference
+            s_coef[l] = gsig * st16;
+            if (p.stats_out != nullptr) p.stats_out[bl] = st16;   // every CTA of the image writes the same value
           }
-          __syncwarp();
-          if (lane == 0) FX_TL(11, 0);
-          stats_ready = true;
         }
-        if (li != cur_li) {
-          // ---- B operand of the bias k-steps for this image: [80 tokens x 32] fp16, 64-byte-swizzled rows ----
-          const int buf = li & 1;
-          if (cur_li >= 0) {                                       // UMMAs reading the old tile
-            if (elect_one()) ptx::umma_commit(BAR(B_COEF + (cur_li & 1)));
-            __syncwarp();
-          }
-          if (li >= 2) ptx::mbar_wait(BAR(B_COEF + buf), (uint32_t)(((li >> 1) - 1) & 1));
-          const float x = s_coef[li < kMaxLocal ? li : 0];
-          const __half xh = __float2half_rn(x);
-          const __half xl = __float2half_rn(x - __half2float(xh));
-          unsigned char* tile = smem_gen + C::OFF_COEF + buf * kCoefTile;
-          const signed char* ci = s_cidx[li < kMaxLocal ? li : 0];
-          for (int t = lane; t < kTP; t += 32) {
-            uint4* rowp = reinterpret_cast<uint4*>(tile + t * 64);
-#pragma unroll
-            for (int ch = 0; ch < 4; ++ch) rowp[ch] = make_uint4(0, 0, 0, 0);
-            const int rc = (int)ci[t];
-            if (rc >= 0 && rc < kRC) {
-              auto put = [&](int k, __half v) {
-                *reinterpret_cast<__half*>(tile + t * 64 + ((((k >> 3) ^ ((t >> 1) & 3))) << 4) + (k & 7) * 2) = v;
-              };
-              put(rc, xh);
-              put(kRC + rc, xh);
-              put(2 * kRC + rc, xl);
-            }
-          }
-          ptx::fence_proxy_async_smem();
-          __syncwarp();
-          cur_li = li;
-        }
+        __syncwarp();
       }
-      int qst_t[2] = {0, 0};
-#pragma unroll
-      for (int t = 0; t < 2; ++t) {
-        if (t >= npair) break;
-        const int it = i + t;
-        const uint2 rt = s_jobs[it];
-        const int kst = it % C::NK, slot = it % C::NS;
-        if (rt.y & JF_FIRST) ++up;
-        const int qst = resident ? (int)((rt.y >> 8) & 0xff) : up % C::NQ;
-        qst_t[t] = qst;
-        // the unit's Q tile (resident stages complete exactly one phase; ring stages one phase per unit pass): first job only
-        if (rt.y & JF_FIRST) ptx::mbar_wait(BAR(B_QFULL + qst), resident ? 0u : (uint32_t)((up / C::NQ) & 1));
-        if (lane == 0) FX_TL(1, it);
-        if constexpr (kTimeline) {                   // timeline builds only: the K wait on its own, so that it gets a stamp
-          ptx::mbar_wait(BAR(B_KFULL + kst), (uint32_t)((it / C::NK) & 1));
-          if (lane == 0) FX_TL(7, it);
-        }
-        // this job's K tile, and the score slot: the previous job on it (it - NS) must be done with it
-        if (it >= C::NS) {
-          const int prev = it - C::NS;
-          const bool by_sfree = !is_main || prev < ns;
-          ptx::mbar_wait2(BAR(B_KFULL + kst), (uint32_t)((it / C::NK) & 1),
-                          BAR((by_sfree ? B_SFREE : B_PVDONE) + slot),
-                          by_sfree ? (uint32_t)((prev / C::NS) & 1) : (uint32_t)(((prev - ns) / C::NS) & 1));
-        } else {
-          ptx::mbar_wait(BAR(B_KFULL + kst), (uint32_t)((it / C::NK) & 1));
-        }
-      }
-      ptx::fence_proxy_async_smem();                 // K tiles: cp.async (generic proxy) writes -> the UMMA's async-proxy reads
-      ptx::tc_fence_after();
-      if (lane == 0) FX_TL(2, i);
-      if (elect_one()) {
-#pragma unroll
-        for (int t = 0; t < 2; ++t) {
-          if (t >= npair) break;
-          const int it = i + t;
-          const uint2 rt = s_jobs[it];
-          const int h = (rt.x >> 8) & 0xff, kst = it % C::NK, slot = it % C::NS, qst = qst_t[t];
-          const uint32_t qb = smem0 + qst * C::QSTAGE, kb = smem0 + C::OFF_K + kst * C::KSTAGE;
-          const int atom0 = ((h / C::G) * C::G * D) / 64;
-          const int blk0 = (h * D) / 16;             // first 16-column block of the head inside the query row
-#pragma unroll
-          for (int ks = 0; ks < C::KSTEPS; ++ks) {
-            const int blk = blk0 + ks;
-            const uint32_t qa = qb + (uint32_t)(blk / 4 - atom0) * kQAtom + (uint32_t)(blk % 4) * 32u;
-            ptx::umma_ss(tmem_base + C::col_s(slot), ptx::make_sw128_desc(qa, 16, 1024),
-                         ptx::make_sw128_desc(kb + (ks / 4) * kKAtom + (ks % 4) * 32, 16, 1024), idesc_qk, ks > 0);
-          }
-          if (is_main && biased) {
-            const uint32_t ma = qb + C::QBYTES, ca = smem0 + C::OFF_COEF + (li & 1) * kCoefTile;
-#pragma unroll
-            for (int ks = 0; ks < kMW / 16; ++ks)
-              ptx::umma_ss(tmem_base + C::col_s(slot), make_sw64_desc(ma + ks * 32), make_sw64_desc(ca + ks * 32), idesc_qk, true);
-          }
-          ptx::umma_commit(BAR(B_SREADY + slot));
-          ptx::umma_commit(BAR(B_KEMPTY + kst));     // the K tile is dead once S exists
-          if ((rt.y & JF_LAST) && !resident) ptx::umma_commit(BAR(B_QEMPTY + qst));   // ... and so is the unit's Q tile after its last head
-          FX_TL(3, it);
-        }
-      }
-      __syncwarp();
-      i += npair;
+      __syncthreads();
     }
-  } else if (warp == 3) {
-    // ============================== UMMA issuer: O = P V of every main job ==============================
-    constexpr uint32_t idesc_pv = ptx::make_idesc_f16(128, C::DPV, false, true);
-    for (int i = ns; i < njobs; ++i) {
-      const int m = i - ns;
-      const int st = m % C::NV, slot = i % C::NS, os = i % C::NO;
-      // the V tile, the group's P (written over S in tensor memory) and the output accumulator of 4 jobs ago
-      if constexpr (kTimeline) {                     // timeline builds only: the V wait on its own, so that it gets a stamp
-        ptx::mbar_wait(BAR(B_VFULL + st), (uint32_t)((m / C::NV) & 1));
-        if (lane == 0) FX_TL(20, i);
-      }
-      if (m >= C::NO)
-        ptx::mbar_wait3(BAR(B_VFULL + st), (uint32_t)((m / C::NV) & 1), BAR(B_PREADY + slot), (uint32_t)((m / C::NS) & 1),
-                        BAR(B_OFREE + os), (uint32_t)(((m / C::NO) - 1) & 1));
-      else
-        ptx::mbar_wait2(BAR(B_VFULL + st), (uint32_t)((m / C::NV) & 1), BAR(B_PREADY + slot), (uint32_t)((m / C::NS) & 1));
-      ptx::fence_proxy_async_smem();                 // V tile: cp.async (generic proxy) writes -> the UMMA's async-proxy reads
-      ptx::tc_fence_after();
-      if (lane == 0) FX_TL(8, i);
-      const uint32_t vb = smem0 + C::OFF_V + st * C::VSTAGE;
-      if (elect_one()) {
-#pragma unroll
-        for (int ks = 0; ks < kTP / 16; ++ks)          // A = P from tensor memory: 8 columns (16 fp16) per k-step
-          ptx::umma_ts(tmem_base + C::col_o(os), tmem_base + C::col_s(slot) + ks * 8,
-                       ptx::make_sw128_desc(vb + ks * 16 * 128, kKAtom, 1024), idesc_pv, ks > 0);
-        ptx::umma_commit(BAR(B_PVDONE + slot));
-        ptx::umma_commit(BAR(B_VEMPTY + st));
-        FX_TL(9, i);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ============================== softmax groups: 8 warps = 128 rows x 2 column halves ==============================
-    const int sw = warp - 4;                       // 0..15
-    const int g = sw >> 3;                         // softmax group
-    const int c = (sw >> 2) & 1;                   // column half: S columns [40c, 40c + 40)
-    const int qd = sw & 3;                         // TMEM lane quarter (== warp % 4)
-    const int row = (qd << 5) | lane;
-    const uint32_t lane_addr = (uint32_t)(qd << 5) << 16;
-    const float sl2 = p.scale * 1.4426950408889634f;
-    const int pair_bar = 1 + g * 4 + qd;           // named barrier shared by the two warps of a row quarter
-    float* xchg = reinterpret_cast<float*>(smem_gen + C::OFF_XCHG);          // [g][buf][half][128] maxima
-    float* xsum = xchg + 2 * 2 * 2 * 128;                                     // [g][buf][half][128] row sums (!ONES)
-    const uint32_t stg_off = C::OFF_STG + (uint32_t)sw * C::STG_WARP;
-    const int oc0 = c ? C::C0 : 0;                 // first output column of this thread
-    const int ocn = c ? C::C1 : C::C0;             // number of output columns of this thread
-
-    auto warp_arrive = [&](uint32_t bar) {         // one arrive per warp (barrier counts are per warp)
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(bar);
-    };
-
-    // ---- stat jobs: per-thread partial of the statistic over this thread's 40 columns ----
-    float vmax = -INFINITY;
-    double dsum = 0.0, dsq = 0.0;
-    int cur_li = -1;
-    auto flush = [&]() {
-      if (cur_li < 0) return;
-      if (p.stat == PWW_STAT_MAX) {
-        const unsigned kmax = __reduce_max_sync(0xffffffffu, f32_key(vmax));
-        if (lane == 0 && cur_li < kMaxLocal) s_key[sw][cur_li] = kmax;
-      } else {
-        double a = dsum, q = dsq;
-#pragma unroll 1
-        for (int o = 16; o > 0; o >>= 1) {
-          a += __shfl_xor_sync(0xffffffffu, a, o);
-          q += __shfl_xor_sync(0xffffffffu, q, o);
-        }
-        if (lane == 0 && cur_li < kMaxLocal) {
-          StatPartial sp;
-          sp.vmax = 0.0; sp.sum = a; sp.sumsq = q; sp.pad = 1.0;
-          s_part[sw][cur_li] = sp;
-        }
-      }
-      vmax = -INFINITY; dsum = 0.0; dsq = 0.0;
-    };
-
-    for (int i = g; i < ns; i += 2) {              // group g takes the jobs with i % 2 == g
-      const uint2 r = s_jobs[i];
-      const int li = (r.y >> 4) & 3, tile = r.x >> 16;
-      const int slot = i % C::NS;
+    // ---- the job ----
+    const uint2 r = s_jobs[i];
+    const int b = r.x & 0xff, h = (r.x >> 8) & 0xff, tile = r.x >> 16;
+    const bool is_main = (r.y & JF_MAIN) != 0, biased = (r.y & JF_BIASED) != 0;
+    const int li = (r.y >> 4) & 3;
+    const uint32_t st = smem0 + (i & 1) * CF::STAGE;
+    const int row0 = tile * kBM + warp * 16;
+    float s[10][4];
+    core::warp_qk<D>(st + (uint32_t)(warp * 16 * C::LD) * 2u, st + C::QBYTES, lane, s);
+    if (!is_main) {
       if (li != cur_li) { flush(); cur_li = li; }
-      ptx::mbar_wait(BAR(B_SREADY + slot), (uint32_t)((i / C::NS) & 1));
-      ptx::tc_fence_after();
-      if ((sw & 7) == 0 && lane == 0) FX_TL(4, i);
-      float s[40];
-      tmem_ld40_sync(tmem_base + lane_addr + C::col_s(slot) + c * 40, s);
-      ptx::tc_fence_before();
-      warp_arrive(BAR(B_SFREE + slot));
-      if ((sw & 7) == 0 && lane == 0) FX_TL(5, i);
-      if (tile * kBM + row < p.N) {
-        if (p.stat == PWW_STAT_MAX) {
-          // max(fp16(s)) == fp16(max(s)): rounding is monotonic, so round once at the very end
-          float m0 = -INFINITY, m1 = -INFINITY;
+      float sum = 0.f, sumsq = 0.f;
+      core::warp_stat(s, T, p.N - row0, lane, is_max, vmax, sum, sumsq);
+      dsum += (double)sum;
+      dsq += (double)sumsq;
+      if (i == ns - 1) flush();
+    } else {
+      if (biased) {
+        const float x = s_coef[li];
+        const signed char* ci = s_cidx[li];
+        const __half* mrow = reinterpret_cast<const __half*>(smem + (i & 1) * CF::STAGE + CF::OFF_M) + (warp * 16 + (lane >> 2)) * kMW;
 #pragma unroll
-          for (int j = 0; j < 40; j += 2) {
-            if (c * 40 + j < T) m0 = fmaxf(m0, s[j]);
-            if (c * 40 + j + 1 < T) m1 = fmaxf(m1, s[j + 1]);
-          }
-          vmax = fmaxf(vmax, fmaxf(m0, m1));
-        } else {
-          float a0 = 0.f, a1 = 0.f, q0 = 0.f, q1 = 0.f;
+        for (int j = 0; j < 10; ++j)
 #pragma unroll
-          for (int j = 0; j < 40; j += 2) {
-            // padded columns hold exact zeros (K rows >= T are zero-filled), so they add nothing
-            const __half2 hh = __floats2half2_rn(s[j], s[j + 1]);
-            const float2 f = __half22float2(hh);
-            a0 += f.x; a1 += f.y;
-            q0 = fmaf(f.x, f.x, q0); q1 = fmaf(f.y, f.y, q1);
+          for (int e = 0; e < 4; ++e) {
+            const int c = ci[core::tok(j, e, lane)];
+            if (c >= 0) {
+              const __half* mr = mrow + (e >> 1) * 8 * kMW;
+              s[j][e] = fmaf(x, __half2float(mr[c]) + __half2float(mr[kRC + c]), s[j][e]);
+            }
           }
-          dsum += (double)(a0 + a1);
-          dsq += (double)(q0 + q1);
-        }
       }
+      float o[C::NT][4];
+      core::warp_softmax_pv<D>(s, T, sl2, st + C::QBYTES + C::KBYTES, lane, o);
+      core::warp_store<D>(o, smem + (i & 1) * CF::STAGE + warp * 16 * C::LD * 2, lane, p.out + (int64_t)b * p.o_bs + h * D,
+                          p.o_rs, row0, p.N);
     }
-    if (ns > 0) {
-      flush();
-      warp_arrive(BAR(B_STATS));                   // the V loader warp publishes the CTA's partials (off this warp's path)
-    }
-
-    // ---- main jobs ----
-    int pend = 0;                                  // 1 = a job of this group has its P.V in flight / finished
-    int pend_slot = 0, pend_os = 0, pend_ph = 0, pend_n0 = 0, pend_b = 0, pend_h = 0, pend_xb = 0;
-    float pend_sum = 0.f;
-    int xb = 0;                                    // exchange buffer parity of this group's next job
-
-    auto epilogue = [&]() {                        // O (fp32, TMEM) -> * 1/rowsum -> fp16 -> staging -> TMA store
-      ptx::mbar_wait(BAR(B_PVDONE + pend_slot), (uint32_t)pend_ph);
-      ptx::tc_fence_after();
-      const uint32_t ta = tmem_base + lane_addr + C::col_o(pend_os);
-#pragma unroll
-      for (int ps = 0; ps < C::EPI_NPASS; ++ps) {
-        float o[41];
-        if constexpr (D == 40) {
-          // columns [oc0, oc0 + 24) (the second half only uses 16 of them) and the row-sum column 40
-          ptx::tmem_ld16_sync(ta + oc0, o);
-          ptx::tmem_ld8_sync(ta + oc0 + 16, o + 16);
-          tmem_ld1_sync(ta + 40, o + 40);
-        } else if constexpr (D == 64) {
-          ptx::tmem_ld32_sync(ta + oc0, o);
-        } else if constexpr (D == 80) {
-          tmem_ld40_sync(ta + oc0, o);
-          tmem_ld1_sync(ta + 80, o + 40);
-        } else {
-          tmem_ld40_sync(ta + oc0 + ps * 40, o);
-        }
-        if (ps == C::EPI_NPASS - 1) {
-          ptx::tc_fence_before();
-          warp_arrive(BAR(B_OFREE + pend_os));     // O is in registers: the next P.V on this accumulator may start
-        }
-        float inv;
-        if constexpr (C::ONES) inv = 1.f / o[40];
-        else inv = 1.f / (pend_sum + xsum[((g * 2 + pend_xb) * 2 + (c ^ 1)) * 128 + row]);
-        // the staging tile is free once the previous store of this warp has been read out (lane 0 owns the groups)
-        if (lane == 0) bulk_wait_group_read0();
-        __syncwarp();
-        const int w8 = (D == 160) ? 5 : (ocn >> 3);      // 16-byte chunks this thread writes
-#pragma unroll
-        for (int ch = 0; ch < C::EPI_W / 8; ++ch) {
-          if (ch < w8) {
-            __align__(16) __half2 pk[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) pk[k] = __floats2half2_rn(o[ch * 8 + 2 * k] * inv, o[ch * 8 + 2 * k + 1] * inv);
-            // staging rows are exactly ocn (or 40) columns wide for the store's box: pitch = box width
-            *reinterpret_cast<uint4*>(smem_gen + stg_off + lane * (((D == 160) ? 40 : ocn) * 2) + ch * 16) =
-                *reinterpret_cast<const uint4*>(pk);
-          }
-        }
-        ptx::fence_proxy_async_smem();             // generic-proxy writes -> visible to the TMA (async proxy)
-        __syncwarp();
-        if (lane == 0 && pend_n0 < p.N) {          // rows >= N are clipped by the TMA
-          ptx::tma_store_4d(c ? &tmo1 : &tmo0, smem0 + stg_off, oc0 + ps * 40, pend_h, pend_n0, pend_b);
-          ptx::bulk_commit_group();
-        }
-      }
-    };
-
-    for (int i = ns + ((ns & 1) ^ g); i < njobs; i += 2) {          // main jobs with i % 2 == g
-      {
-        const uint2 r = s_jobs[i];
-        const int m = i - ns;
-        const int slot = i % C::NS;
-        const uint32_t ts = tmem_base + lane_addr + C::col_s(slot);
-        ptx::mbar_wait(BAR(B_SREADY + slot), (uint32_t)((i / C::NS) & 1));
-        ptx::tc_fence_after();
-        if ((sw & 7) == 0 && lane == 0) FX_TL(4, i);
-        float s[40];
-        tmem_ld40_sync(ts + c * 40, s);
-        // row max over this thread's columns (padded keys excluded), then over the row via the partner thread
-        if constexpr (TT == 77) {
-          if (c) { s[37] = -INFINITY; s[38] = -INFINITY; s[39] = -INFINITY; }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 40; ++j)
-            if (c * 40 + j >= T) s[j] = -INFINITY;
-        }
-        float m0 = s[0], m1 = s[1], m2 = s[2], m3 = s[3];
-#pragma unroll
-        for (int j = 4; j < 40; j += 4) {
-          m0 = fmaxf(m0, s[j]); m1 = fmaxf(m1, s[j + 1]); m2 = fmaxf(m2, s[j + 2]); m3 = fmaxf(m3, s[j + 3]);
-        }
-        float mx = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-        float* xm = xchg + ((g * 2 + xb) * 2) * 128;
-        xm[c * 128 + row] = mx;
-        ptx::named_bar_sync(pair_bar, 64);
-        mx = fmaxf(mx, xm[(c ^ 1) * 128 + row]);
-        const float nm = -mx * sl2;
-        // p_j = 2^(s_j*sl2 - mx*sl2), UNNORMALISED, packed to fp16; O is scaled by 1/rowsum in the epilogue (fp32)
-        float a0 = 0.f, a1 = 0.f;
-        uint32_t pk[20];
-#pragma unroll
-        for (int j = 0; j < 40; j += 2) {
-          const float e0 = ptx::ex2(fmaf(s[j], sl2, nm)), e1 = ptx::ex2(fmaf(s[j + 1], sl2, nm));
-          const __half2 h = __floats2half2_rn(e0, e1);
-          pk[j / 2] = *reinterpret_cast<const uint32_t*>(&h);
-          if constexpr (!C::ONES) {
-            const float2 f = __half22float2(h);       // sum exactly what the UMMA will multiply
-            a0 += f.x; a1 += f.y;
-          }
-        }
-        if constexpr (!C::ONES) xsum[((g * 2 + xb) * 2 + c) * 128 + row] = a0 + a1;
-        // P (packed fp16) over the S columns it came from: this half owns P columns [20c, 20c + 20)
-        ptx::tmem_st16_u32(ts + c * 20, pk);
-        tmem_st4_u32(ts + c * 20 + 16, pk + 16);
-        ptx::tmem_st_wait();
-        ptx::tc_fence_before();
-        warp_arrive(BAR(B_PREADY + slot));
-        if ((sw & 7) == 0 && lane == 0) FX_TL(5, i);
-        if (pend) epilogue();                      // overlaps with this job's P.V
-        if ((sw & 7) == 0 && lane == 0) FX_TL(6, i);
-        pend = 1;
-        pend_slot = slot;
-        pend_os = i % C::NO;
-        pend_ph = (m / C::NS) & 1;
-        pend_n0 = (int)(r.x >> 16) * kBM + (qd << 5);
-        pend_b = r.x & 0xff;
-        pend_h = (r.x >> 8) & 0xff;
-        pend_xb = xb;
-        pend_sum = a0 + a1;
-        xb ^= 1;
-      }
-    }
-    if (pend) {
-      if constexpr (!C::ONES) ptx::named_bar_sync(pair_bar, 64);   // the partner's row sum of the last job is written
-      epilogue();
-    }
-    if (lane == 0) ptx::bulk_wait_group0();        // the staging tile must outlive the last store
-    if ((sw & 7) == 0 && lane == 0) FX_TL(14, g);
+    __syncthreads();
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x == 0) FX_TL(15, 0);
-  if (warp == 1) ptx::tmem_dealloc<512>(tmem_base);
   // the last CTA to leave resets the arrival counters for the next launch (every waiter has passed its barrier)
+  __syncthreads();
   if (threadIdx.x == 0 && nb > 0) {
     __threadfence();
     const unsigned prev = atomicAdd(p.counters + kMaxBatch, 1u);
@@ -1043,24 +456,6 @@ xattn_fused2_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_consta
 // ------------------------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------------------------
-// Q [B, N, H*D] fp16 viewed as (column, row, image): boxes of [64 columns x 128 rows x 1] = whole 128-byte lines,
-// 128-byte swizzle.  Columns beyond H*D and rows beyond N are zero-filled.
-inline bool make_tmap_qfull(CUtensorMap* m, const void* base, int C, int N, int B, int64_t row_stride, int64_t batch_stride) {
-  tc::EncodeTiledFn fn = tc::encode_fn();
-  if (!fn) return false;
-  cuuint64_t dims[3] = {(cuuint64_t)C, (cuuint64_t)N, (cuuint64_t)B};
-  cuuint64_t strides[2] = {(cuuint64_t)row_stride * 2, (cuuint64_t)(batch_stride > 0 ? batch_stride : (int64_t)N * row_stride) * 2};
-  cuuint32_t box[3] = {64, (cuuint32_t)kBM, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS)
-    snprintf(tc::tc_error_buf(), 256, "cuTensorMapEncodeTiled(q rows) failed (CUresult %d): base %p C %d N %d B %d strides %lld %lld",
-             (int)r, base, C, N, B, (long long)row_stride, (long long)batch_stride);
-  return r == CUDA_SUCCESS;
-}
-
 // A launch fits when every CTA's unit range touches at most kMaxLocal biased images and holds at most kMaxUnits units
 // (job table in shared memory); the C ABI halves the images per launch until it does.
 inline bool fused2_fits(int B, int hg, int tiles, int grid) {
@@ -1069,56 +464,38 @@ inline bool fused2_fits(int B, int hg, int tiles, int grid) {
 }
 
 template <int D>
-cudaError_t launch_fused2(const XattnParams& x, const void* mpack, int64_t mpack_bs, int Bw, const int8_t* cidx,
-                          cudaStream_t s) {
-  using C = Cfg2<D>;
-  CUtensorMap tq, tm, to0, to1;
-  if (!make_tmap_qfull(&tq, x.q, x.H * D, x.N, x.B, x.q_rs, x.q_bs)) return cudaErrorInvalidValue;
-  if (mpack != nullptr) {
-    if (!make_tmap_mpack(&tm, mpack, x.N, Bw, mpack_bs)) return cudaErrorInvalidValue;
-  } else {
-    tm = tq;                                       // never dereferenced: no image is biased
-  }
-  const int w0 = (D == 160) ? 40 : C::C0, w1 = (D == 160) ? 40 : C::C1;      // store boxes: one epilogue pass wide
-  if (!tc::make_tmap_out(&to0, x.out, D, x.H, x.N, x.B, x.o_rs, x.o_bs, 32, w0, false) ||
-      !tc::make_tmap_out(&to1, x.out, D, x.H, x.N, x.B, x.o_rs, x.o_bs, 32, w1, false))
-    return cudaErrorInvalidValue;
+cudaError_t launch_fused2(const XattnParams& x, const void* mpack, int64_t mpack_bs, const int8_t* cidx, cudaStream_t s) {
+  using CF = Cfg2<D>;
   FxParams fp;
+  memset(&fp, 0, sizeof(fp));
   fp.x = x;
   fp.cidx = cidx;
+  fp.mpack = mpack;
+  fp.mpack_bs = mpack_bs;
   fp.tiles = ceil_div(x.N, kBM);
-  fp.hg = ceil_div(x.H, C::G);
+  fp.hg = ceil_div(x.H, CF::G);
   fp.units = x.B * fp.tiles * fp.hg;
-  fp.k_batched = x.k_bs > 0 ? 1 : 0;
   fp.grid = fused_grid(fp.units);
-  fp.timeline = debug_timeline();
-  fp.tl_cta = debug_timeline_cta();
   fp.jobs_dump = debug_jobs_dump();
   if (!fused2_fits(x.B, fp.hg, fp.tiles, fp.grid)) return cudaErrorInvalidConfiguration;
   static bool attr_set[tc::kMaxDevices] = {false};
   if (!attr_set[tc::cur_device()]) {
-    cudaError_t e = cudaFuncSetAttribute(xattn_fused2_kernel<D, 77, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(xattn_fused2_kernel<D, 0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(xattn_fused2_kernel<D, 77, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(xattn_fused2_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, CF::SMEM);
     if (e != cudaSuccess) return e;
     attr_set[tc::cur_device()] = true;
   }
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(fp.grid);
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = C::SMEM;
+  cfg.blockDim = dim3(core::kThreads);
+  cfg.dynamicSmemBytes = CF::SMEM;
   cfg.stream = s;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeCooperative;     // all CTAs co-resident: the in-kernel grid barrier cannot deadlock
   attr[0].val.cooperative = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  if (x.T == 77 && fp.timeline != nullptr) return cudaLaunchKernelEx(&cfg, xattn_fused2_kernel<D, 77, true>, tq, tm, to0, to1, fp);
-  if (x.T == 77) return cudaLaunchKernelEx(&cfg, xattn_fused2_kernel<D, 77, false>, tq, tm, to0, to1, fp);
-  return cudaLaunchKernelEx(&cfg, xattn_fused2_kernel<D, 0, false>, tq, tm, to0, to1, fp);
+  return cudaLaunchKernelEx(&cfg, xattn_fused2_kernel<D>, fp);
 }
 
 // Host replay of the job lists (test infrastructure): out[job] = {cta, i, kind, m, b, h, tile, biased, li, gi, up, ul,

@@ -1,119 +1,45 @@
-// Paint-with-Words cross-attention on tcgen05 tensor cores (sm_100a), keys T <= 80.
+// Paint-with-Words cross-attention on Hopper tensor cores (sm_90a), keys T <= 80: the two-launch pair that takes the
+// reference's dense [N, T] fp32 weight map (maps with more than 10 distinct columns cannot be packed for the one-launch
+// kernel of xattn_fused2.cuh).
 //
 // Fused region of the reference's inj_forward (paint_with_words.py:87-118), per image b / head h / 128-row tile:
-//     S = Q_h K_h^T            UMMA M=128 N=80 K=D(+pad)   operands staged by TMA, accumulator in TMEM
-//     P = softmax(scale*(S + g*M_b*w[b]))                   one thread per query row, mask tile in shared memory
-//     O = P V_h                UMMA M=128 N=D K=80           P (fp16) written over S in TMEM and read from there (TS form)
-// Work unit = (image, row tile, head).  Every CTA owns a contiguous range of units in an order (FwdWalk) that pairs one
-// image with a weight map and one without, alternates their heads, and fetches the [128 x T] fp32 mask tile of the
-// pair once for all heads.
-//
-// Forward-kernel warp roles (384 threads): warp 0 TMA producer for Q/K | warp 1 UMMA issuer S = Q K^T + TMEM owner |
-// warps 2-5 softmax group 0 | warps 6-9 softmax group 1 | warp 10 TMA producer for V and the mask | warp 11 UMMA issuer
-// O = P V.  Group g handles units it % 2 == g with its own score buffers (two per group for D <= 80) and O accumulator
-// in TMEM; the epilogue of a unit is deferred until the group has handed the next unit's P to the tensor pipe.
-//
-// Shared-memory tiles are 128-byte-swizzled "atoms" of 64 fp16 columns: Q [128 x 64], K/V [80 x 64] rows of 128 B.
-// TMA's out-of-bounds zero fill supplies every padding the UMMAs need (d >= D, token >= T, row >= N).
+//     statistics kernel:  per-image max / (sum, sumsq) of fp16(Q_h K_h^T) over all heads, rows and tokens
+//     forward kernel:     S = Q_h K_h^T;  P = softmax(scale * (S + g * M_b * w[b]));  O = P V_h
+// with the warp-level MMA tiles of xattn_core.cuh.  Work unit = (image, row tile, head); every CTA of the persistent grid
+// owns a contiguous range of units and double-buffers them: the cp.async copies of unit i + 1 are in flight while unit i
+// is computed.  The forward kernel walks its range in the FwdWalk order, which pairs one image with a weight map and one
+// without and alternates their heads, so that every CTA gets the same mix of biased and unbiased units.
 #pragma once
 #include <cuda.h>
 #include <stdio.h>
 #include <stdlib.h>
 
-#include "ptx_sm100.cuh"
+#include "mma_sm90.cuh"
 #include "pww_common.cuh"
+#include "xattn_core.cuh"
 
 namespace pww {
 namespace tc {
 
-constexpr int kBM = 128;         // query rows per tile
-constexpr int kTP = 80;          // padded key count
-constexpr int kThreads = 320;        // stats kernel
-constexpr int kFwdThreads = 384;     // forward kernel: 12 warps
-constexpr uint32_t kQAtom = 128 * 128;   // bytes
-constexpr uint32_t kKAtom = kTP * 128;
-constexpr uint32_t kPAtom = 128 * 128;
-constexpr uint32_t kPBuf = 2 * kPAtom;   // token columns 0-63 | 64-79
-constexpr uint32_t kMaskBytes = kBM * kTP * 4;
-constexpr int kTmemCols = 512;
+constexpr int kBM = core::kBM;   // query rows per tile
+constexpr int kTP = core::kTP;   // padded key count
+constexpr int kThreads = core::kThreads;
 constexpr int kMaxBatch = 256;   // images per launch (the C ABI splits larger batches)
-constexpr int kMaxLocal = 4;     // images one CTA's unit range can touch: B/148 + 2 <= 4 for B <= 256
-// TMEM column map (512 columns).  Each softmax group g owns NSB score buffers of 80 fp32 columns and one O accumulator
-// of up to 160 columns.  P (80 packed fp16 = 40 columns, the A operand of the P.V UMMA, read straight from tensor
-// memory) overwrites the first 40 columns of the S buffer it was computed from, so a buffer cycles S -> P -> free and
-// the only thing that gates its reuse is the P.V that consumed it.  With NSB = 2 (D <= 80) the next S = Q K^T of a
-// group is issued while the group is still working on the current one: the softmax never waits for the tensor pipe.
-template <int D> __host__ __device__ constexpr int nsb() { return D <= 80 ? 2 : 1; }
-template <int D> __host__ __device__ constexpr uint32_t s_stride() { return D == 80 ? 80u : 96u; }
-template <int D> __host__ __device__ constexpr uint32_t o_stride() { return D <= 64 ? 64u : (D == 80 ? 96u : 160u); }
-template <int D> __host__ __device__ constexpr uint32_t col_s(int g, int buf) { return (uint32_t)(g * nsb<D>() + buf) * s_stride<D>(); }
-template <int D> __host__ __device__ constexpr uint32_t col_o(int g) { return 2u * nsb<D>() * s_stride<D>() + (uint32_t)g * o_stride<D>(); }
-static_assert(col_o<40>(1) + 48 <= 512 && col_o<64>(1) + 64 <= 512 && col_o<80>(1) + 96 <= 512 && col_o<160>(1) + 160 <= 512,
-              "TMEM budget");
+constexpr int kMaxLocal = 4;     // images one CTA's unit range can touch: B/132 + 2 <= 4 for B <= 256
 
 template <int D>
 struct Cfg {
-  static constexpr int NA = (D + 63) / 64;          // 64-column atoms along the head dim
-  static constexpr int DP = (D + 15) / 16 * 16;     // UMMA extent of the head dim
-  static constexpr int KSTEPS = DP / 16;
-  // Q/K tiles and V tiles live in separate rings: Q/K of a unit are released as soon as S = Q K^T is done (long
-  // before P.V), so the next units' Q/K loads -- ~2 us of TMA latency for 200+ short rows -- are issued early.
-  static constexpr int NQK = (D <= 64) ? 4 : (D <= 80 ? 2 : 1);
-  static constexpr int NV = (D <= 64) ? 3 : 2;
-  static constexpr uint32_t QKSTAGE = NA * (kQAtom + kKAtom);
-  static constexpr uint32_t VSTAGE = NA * kKAtom;
-  // Row sums ride on the P.V UMMA: when the last 64-column V atom has a spare column (D = 40, 80) that column is
-  // set to 1.0 for every real token, so accumulator column D holds sum_j fp16(P_j) -- exactly the normaliser of
-  // the P that was multiplied -- and the softmax threads never add the 80 exponentials themselves.
-  static constexpr bool ONES = (D == 40 || D == 80);
-  static constexpr int DPV = ONES ? (D + 16) / 16 * 16 : DP;   // UMMA N of P.V: 48, 64, 96, 160
-  static constexpr uint32_t OFF_V = NQK * QKSTAGE;
-  static constexpr uint32_t OFF_MASK = OFF_V + NV * VSTAGE;
-  static constexpr int NSB = nsb<D>();             // score buffers per softmax group (see the TMEM map above)
-  static constexpr uint32_t OFF_BAR = OFF_MASK + kMaskBytes;
-  static constexpr uint32_t SMEM = OFF_BAR + 256 + 1024;   // + alignment slack
-  // TMA-store epilogue: one [32 rows x EPI_CW columns] fp16 staging tile per softmax warp, stored in D / EPI_CW passes.
-  // D = 40: the whole row in one pass, plain layout (80-byte rows are bank-conflict free).  D = 64: one pass, rows of
-  // 128 bytes in the 128-byte swizzle (plain rows would make every 16-byte store an 8-way bank conflict).  D = 80, 160:
-  // 40-column passes so the staging fits beside the operand rings.
-  static constexpr int EPI_CW = (D == 64) ? 64 : 40;
-  static constexpr int EPI_NPASS = D / EPI_CW;
-  static constexpr bool EPI_SW = (D == 64);
-  static constexpr uint32_t OFF_STG = OFF_BAR + (EPI_SW ? 1024 : 256);
-  static constexpr uint32_t STG_WARP = 32 * EPI_CW * 2;
-  static constexpr uint32_t SMEM_EPI = OFF_STG + 8 * STG_WARP + 1024;
-  // stats kernel: Q and K only
-  static constexpr uint32_t SSTAGE = NA * (kQAtom + kKAtom);
-  static constexpr int S_NSTAGE = (D <= 80) ? 3 : 2;
-  static constexpr uint32_t S_OFF_BAR = S_NSTAGE * SSTAGE;
-  static constexpr uint32_t S_SMEM = S_OFF_BAR + 256 + 1024;
+  using T_ = core::Tile<D>;
+  static constexpr uint32_t STAGE = T_::QBYTES + 2 * T_::KBYTES;   // Q | K | V of one unit
+  static constexpr uint32_t SMEM = 2 * STAGE;
+  static_assert(SMEM <= 232448 - 8192, "shared memory budget (dynamic + static tables)");
 };
-
-// Debug timeline (test infrastructure): when TcParams::timeline is non-null, CTA 0 records clock64 per
-// (tag, iteration) in shared memory and dumps the table to global memory when the kernel ends.
-constexpr int kTlTags = 14, kTlIts = 40;
-__shared__ long long tl_buf[kTlTags * kTlIts];
-#define PWW_TL(tag, it)                                                                      \
-  do {                                                                                       \
-    if (tp.timeline != nullptr && blockIdx.x == 0 && (it) < kTlIts) tl_buf[(tag) * kTlIts + (it)] = clock64(); \
-  } while (0)
 
 struct TcParams {
   XattnParams x;
   int tiles;        // row tiles per image
   int units;        // B * tiles * H
-  int k_batched;    // 0 when k/v have batch stride 0 (shared context)
-  long long* timeline;   // debug only (see PWW_TL)
 };
-
-__device__ __forceinline__ void tl_init(const TcParams& tp) {
-  if (tp.timeline != nullptr && blockIdx.x == 0)
-    for (int i = threadIdx.x; i < kTlTags * kTlIts; i += blockDim.x) tl_buf[i] = 0;
-}
-__device__ __forceinline__ void tl_dump(const TcParams& tp) {   // call after a __syncthreads at kernel end
-  if (tp.timeline != nullptr && blockIdx.x == 0)
-    for (int i = threadIdx.x; i < kTlTags * kTlIts; i += blockDim.x) tp.timeline[i] = tl_buf[i];
-}
 
 // Walks consecutive units without a div/mod per step.
 struct UnitIter {
@@ -132,12 +58,12 @@ struct UnitIter {
   }
 };
 // Forward-kernel unit order.  Units are tile-major; inside a row tile the images are visited in GROUPS that share one
-// [128 x T] mask tile in shared memory:
+// [128 x T] mask tile:
 //   * pair group: one biased image A (has a weight map) and one unbiased image U (classifier-free guidance puts as many
 //     of each in the batch).  2H units, head h = j/2, in the order  U A | A U | U A | ...  so that (1) biased and
-//     unbiased units alternate at the finest grain -- every CTA's contiguous range and both softmax groups get the same
-//     mix, whatever the image order in the batch -- (2) A's mask tile is reused by all H heads, and (3) the group ends
-//     with its mask no longer needed, so the next group's mask load overlaps the last units.
+//     unbiased units alternate at the finest grain -- every CTA's contiguous range gets the same mix, whatever the image
+//     order in the batch -- (2) A's mask tile is reused by all H heads (it stays in L2), and (3) the group ends with its
+//     mask no longer needed.
 //   * solo group: an image without a partner (all-biased or all-unbiased batches), H units head-minor.
 // s_img lists the biased images first (nb of them), then the unbiased ones.
 struct FwdUnit {
@@ -198,7 +124,7 @@ struct FwdWalk {
     return r;
   }
 };
-// Position (inside its group) of the unit at which every softmax warp releases the group's mask tile: the last
+// Position (inside its group) of the last unit of the CTA's range that reads the group's mask tile: the last
 // mask-reading unit if the CTA's range [it - j_lo .., it + rest] contains it, else the last unit of the group in range.
 __host__ __device__ __forceinline__ int mask_release_pos(const FwdUnit& f, int it, int n_it) {
   const int j_lo = f.j > it ? f.j - it : 0;
@@ -206,9 +132,7 @@ __host__ __device__ __forceinline__ int mask_release_pos(const FwdUnit& f, int i
   if (j_hi > f.gsize - 1) j_hi = f.gsize - 1;
   return (f.jl >= j_lo && f.jl <= j_hi) ? f.jl : j_hi;
 }
-// Mask-barrier rule (shared by the kernel and the host replay): EVERY softmax warp waits for B_MFULL at the first unit
-// of each mask group of its CTA, whether or not it reads the tile.  A warp therefore observes the phases of B_MFULL
-// in order 0, 1, 2, ... and a parity wait can never be satisfied by a phase it skipped.
+// First unit of a mask group inside a CTA's range.
 __host__ __device__ __forceinline__ bool mask_group_starts_here(const FwdUnit& f, int it) { return f.j == 0 || it == 0; }
 __device__ __forceinline__ void cta_range(int units, int& u0, int& u1) {
   u0 = (int)((long long)blockIdx.x * units / gridDim.x);
@@ -219,42 +143,33 @@ __device__ __forceinline__ int image_widx(const XattnParams& p, int b) {
   return p.wmap_index ? p.wmap_index[b] : b;
 }
 
+// Copies of one unit's operands into a stage: Q rows of the tile, K (and V) rows of the head.
+template <int D>
+__device__ __forceinline__ void load_unit(uint32_t st, const XattnParams& p, int b, int h, int tile, bool with_v) {
+  using C = core::Tile<D>;
+  const int rows = p.N - tile * kBM;
+  core::load_rows<D>(st, p.q + (int64_t)b * p.q_bs + (int64_t)tile * kBM * p.q_rs + h * D, p.q_rs, kBM, rows < kBM ? rows : kBM);
+  core::load_rows<D>(st + C::QBYTES, p.k + (int64_t)b * p.k_bs + h * D, p.k_rs, kTP, p.T);
+  if (with_v) core::load_rows<D>(st + C::QBYTES + C::KBYTES, p.v + (int64_t)b * p.k_bs + h * D, p.k_rs, kTP, p.T);
+  ptx::cp_async_commit();
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // forward kernel
 // ---------------------------------------------------------------------------------------------------------
-// TT = 77 compiles the key-length checks away (the Stable Diffusion case); TT = 0 keeps them for any T <= 80.
-// EPI_TMA: the epilogue goes through shared memory and TMA stores (one [32 x D] fp16 tile per softmax warp) instead of
-// 16-byte global stores from every thread (32 distinct lines per store instruction, 640 LSU wavefronts per unit);
-// both forms are built so one process can A/B them on the same device (pww_debug_set_variant).
-template <int D, int TT, bool EPI_TMA>
-__global__ void __launch_bounds__(kFwdThreads, 1)
-xattn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ CUtensorMap tmk,
-                    const __grid_constant__ CUtensorMap tmv, const __grid_constant__ CUtensorMap tmo,
-                    const TcParams tp) {
-  using C = Cfg<D>;
+template <int D>
+__global__ void __launch_bounds__(kThreads, 1) xattn_fwd_kernel(const TcParams tp) {
+  using C = core::Tile<D>;
   const XattnParams& p = tp.x;
-  extern __shared__ unsigned char smem_raw[];
-  const uint32_t smem0 = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
-  unsigned char* smem_gen = smem_raw + (smem0 - ptx::smem_u32(smem_raw));
-  const uint32_t bar0 = smem0 + C::OFF_BAR;
-  // barrier slots (8 bytes each)
-  auto BAR = [&](int i) { return bar0 + 8u * i; };
-  // SREADY / PREADY / PVDONE are per score buffer, indexed [g*2 + buf]; a group's unit `local` uses buffer
-  // local % NSB in phase (local / NSB) & 1.  Every multi-arrival barrier keeps the rule that a warp's next arrival is
-  // causally behind the completion of the current phase (PREADY: via PVDONE -> next S; OFREE: via the next P.V).
-  constexpr int B_QFULL = 0, B_QEMPTY = 4, B_VFULL = 8, B_VEMPTY = 11, B_MFULL = 14, B_MEMPTY = 15, B_SREADY = 16,
-                B_PREADY = 20, B_PVDONE = 24, B_OFREE = 28, B_TMEMPTR = 30;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  int u0, u1;
-  cta_range(tp.units, u0, u1);
-  const int n_it = u1 - u0;
-  // per-image weight-map index and bias coefficient g(sigma)*M_b, staged once (no global loads in the loops)
+  extern __shared__ __align__(128) unsigned char smem[];
+  const uint32_t smem0 = ptx::smem_u32(smem);
+  __shared__ int s_img[kMaxBatch];
   __shared__ int s_widx[kMaxBatch];
   __shared__ float s_coef[kMaxBatch];
-  __shared__ int s_img[kMaxBatch];             // biased images first, then unbiased (see fwd_unit)
   __shared__ int s_nb;
-  tl_init(tp);
-  if (warp == 2) {                             // stable partition of the images by "has a weight map"
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (warp == 0) {
+    // stable partition of the images by "has a weight map"
     int nb_total = 0;
     for (int base = 0; base < p.B; base += 32) {
       const int b = base + lane;
@@ -273,350 +188,66 @@ xattn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_consta
     }
     if (lane == 0) s_nb = nb_total;
   }
-  for (int b = threadIdx.x; b < p.B; b += kFwdThreads) {
+  for (int b = threadIdx.x; b < p.B; b += kThreads) {
     const int wi = image_widx(p, b);
     s_widx[b] = wi;
     s_coef[b] = wi >= 0 ? __ldg(p.g_sigma) * __ldg(p.stats + b) : 0.f;
   }
-
-  if (warp == 0 && lane == 0) {
-    ptx::prefetch_tmap(&tmq);
-    ptx::prefetch_tmap(&tmk);
-    ptx::prefetch_tmap(&tmv);
-    if constexpr (EPI_TMA) ptx::prefetch_tmap(&tmo);
-    for (int s = 0; s < C::NQK; ++s) {
-      ptx::mbar_init(BAR(B_QFULL + s), 1);
-      ptx::mbar_init(BAR(B_QEMPTY + s), 1);
-    }
-    for (int s = 0; s < C::NV; ++s) {
-      ptx::mbar_init(BAR(B_VFULL + s), 1);
-      ptx::mbar_init(BAR(B_VEMPTY + s), 1);
-    }
-    ptx::mbar_init(BAR(B_MFULL), 1);
-    ptx::mbar_init(BAR(B_MEMPTY), 8);          // one elected arrive per softmax warp
-    for (int i = 0; i < 4; ++i) {
-      ptx::mbar_init(BAR(B_SREADY + i), 1);
-      ptx::mbar_init(BAR(B_PREADY + i), 4);
-      ptx::mbar_init(BAR(B_PVDONE + i), 1);
-    }
-    for (int g = 0; g < 2; ++g) ptx::mbar_init(BAR(B_OFREE + g), 4);
-    ptx::fence_barrier_init();
-  }
-  if (warp == 1) ptx::tmem_alloc<kTmemCols>(BAR(B_TMEMPTR));
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem_gen + C::OFF_BAR + 8 * B_TMEMPTR);
-
-  if (warp == 0) {
-    // ===================================== TMA producer: Q and K tiles =====================================
-    if (lane == 0) {
-      FwdWalk wq(u0, p.B, p.H, s_nb, s_img);
-      for (int it = 0; it < n_it; ++it, wq.next()) {
-        const FwdUnit uq = wq.get();
-        const int st = it % C::NQK;
-        ptx::mbar_wait(BAR(B_QEMPTY + st), (uint32_t)(((it / C::NQK) & 1) ^ 1));
-        PWW_TL(1, it);
-        const uint32_t sb = smem0 + st * C::QKSTAGE;
-        ptx::mbar_arrive_expect_tx(BAR(B_QFULL + st), C::QKSTAGE);
-        const int kb = tp.k_batched ? uq.b : 0;
-#pragma unroll
-        for (int a = 0; a < C::NA; ++a) {
-          ptx::tma_load_4d(sb + a * kQAtom, &tmq, BAR(B_QFULL + st), a * 64, uq.h, uq.tile * kBM, uq.b);
-          ptx::tma_load_4d(sb + C::NA * kQAtom + a * kKAtom, &tmk, BAR(B_QFULL + st), a * 64, uq.h, 0, kb);
-        }
-      }
+  int u0, u1;
+  cta_range(tp.units, u0, u1);
+  const int n_it = u1 - u0;
+  if (n_it <= 0) return;
+  const float sl2 = p.scale * 1.4426950408889634f;
+  FwdWalk w(u0, p.B, p.H, s_nb, s_img);
+  FwdUnit nxt = w.get();
+  load_unit<D>(smem0, p, nxt.b, nxt.h, nxt.tile, true);
+  for (int it = 0; it < n_it; ++it) {
+    const FwdUnit f = nxt;
+    if (it + 1 < n_it) {
+      w.next();
+      nxt = w.get();
+      load_unit<D>(smem0 + ((it + 1) & 1) * Cfg<D>::STAGE, p, nxt.b, nxt.h, nxt.tile, true);
+      ptx::cp_async_wait<1>();
+    } else {
+      ptx::cp_async_wait<0>();
     }
-    __syncwarp();
-  } else if (warp == 10) {
-    // ===================================== TMA producer: mask tiles and V tiles =====================================
-    FwdWalk wv(u0, p.B, p.H, s_nb, s_img);
-    int grp = -1;
-    for (int it = 0; it < n_it; ++it, wv.next()) {
-      const FwdUnit uv = wv.get();
-      if (it == 0 || uv.j == 0) {                 // first unit of a group in this CTA's range: stage its mask tile
-        ++grp;
-        ptx::mbar_wait(BAR(B_MEMPTY), (uint32_t)((grp & 1) ^ 1));
-        // (a range that starts behind the group's last mask-reading unit does not need the tile)
-        const int widx = (uv.mask_b >= 0 && uv.j <= uv.jl) ? s_widx[uv.mask_b] : -1;
-        if (widx >= 0) {
-          const int rows = min(kBM, p.N - uv.tile * kBM);
-          const uint32_t bytes = (uint32_t)rows * p.T * 4u;
-          const float* src = p.wmap + (int64_t)widx * p.wmap_bs + (int64_t)uv.tile * kBM * p.T;
-          if ((bytes & 15u) == 0 && (reinterpret_cast<uintptr_t>(src) & 15u) == 0) {
-            if (lane == 0) {
-              ptx::mbar_arrive_expect_tx(BAR(B_MFULL), bytes);
-              ptx::bulk_load_1d(smem0 + C::OFF_MASK, src, bytes, BAR(B_MFULL));
-            }
-          } else {                                // ragged tail tile: plain loads by the whole warp
-            float* dst = reinterpret_cast<float*>(smem_gen + C::OFF_MASK);
-            for (int i = lane; i < rows * p.T; i += 32) dst[i] = __ldg(src + i);
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(BAR(B_MFULL));
-          }
-        } else if (lane == 0) {
-          ptx::mbar_arrive(BAR(B_MFULL));         // keep the phases in lock-step for unbiased images
-        }
-      }
-      const int st = it % C::NV;
-      ptx::mbar_wait(BAR(B_VEMPTY + st), (uint32_t)(((it / C::NV) & 1) ^ 1));
-      if (lane == 0) {
-        const uint32_t sb = smem0 + C::OFF_V + st * C::VSTAGE;
-        ptx::mbar_arrive_expect_tx(BAR(B_VFULL + st), C::VSTAGE);
-        const int kb = tp.k_batched ? uv.b : 0;
+    __syncthreads();
+    const uint32_t st = smem0 + (it & 1) * Cfg<D>::STAGE;
+    const uint32_t qs = st + (uint32_t)(warp * 16 * C::LD) * 2u;
+    float s[10][4];
+    core::warp_qk<D>(qs, st + C::QBYTES, lane, s);
+    const int row0 = f.tile * kBM + warp * 16;
+    const int widx = s_widx[f.b];
+    if (widx >= 0) {
+      const float x = s_coef[f.b];
+      const float* wm = p.wmap + (int64_t)widx * p.wmap_bs;
 #pragma unroll
-        for (int a = 0; a < C::NA; ++a) ptx::tma_load_4d(sb + a * kKAtom, &tmv, BAR(B_VFULL + st), a * 64, uv.h, 0, kb);
-      }
-      __syncwarp();
+      for (int j = 0; j < 10; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int t = core::tok(j, e, lane), r = row0 + (lane >> 2) + (e >> 1) * 8;
+          if (t < p.T && r < p.N) s[j][e] = fmaf(x, __ldg(wm + (int64_t)r * p.T + t), s[j][e]);
+        }
     }
-  } else if (warp == 1) {
-    // ===================================== UMMA issuer: S = Q K^T of every unit, in unit order =====================================
-    // (One issuer warp per softmax group -- each issuing its group's S and P.V -- was tried and gave wrong results at
-    //  D = 64: see profiles/.  Warp 1 issues every SS-form chain, warp 11 every TS-form chain.)
-    if (lane == 0) {
-      constexpr uint32_t idesc_qk = ptx::make_idesc_f16(128, kTP, false, false);
-      for (int it = 0; it < n_it; ++it) {
-        // S[g][buf] = Q K^T of unit `it` (the group's unit `local`)
-        const int st = it % C::NQK, g = it & 1, local = it >> 1, buf = local % C::NSB, k = local / C::NSB;
-        ptx::mbar_wait(BAR(B_QFULL + st), (uint32_t)((it / C::NQK) & 1));
-        if (k >= 1)                                      // the P.V that read P out of this buffer has finished
-          ptx::mbar_wait(BAR(B_PVDONE + g * 2 + buf), (uint32_t)((k - 1) & 1));
-        PWW_TL(2, it);
-        ptx::tc_fence_after();
-        const uint32_t sb = smem0 + st * C::QKSTAGE;
-#pragma unroll
-        for (int ks = 0; ks < C::KSTEPS; ++ks) {
-          const uint32_t qa = sb + (ks / 4) * kQAtom + (ks % 4) * 32;
-          const uint32_t ka = sb + C::NA * kQAtom + (ks / 4) * kKAtom + (ks % 4) * 32;
-          ptx::umma_ss(tmem_base + col_s<D>(g, buf), ptx::make_sw128_desc(qa, 16, 1024),
-                       ptx::make_sw128_desc(ka, 16, 1024), idesc_qk, ks > 0);
-        }
-        ptx::umma_commit(BAR(B_SREADY + g * 2 + buf));
-        ptx::umma_commit(BAR(B_QEMPTY + st));      // Q/K tiles are dead once S exists
-        PWW_TL(4, it);
-      }
-    }
-    __syncwarp();
-  } else if (warp == 11) {
-    // ===================================== UMMA issuer: O = P V of every unit, in unit order =====================================
-    // The whole warp waits for the V tile (so every VFULL phase of every stage is observed by the same threads, in
-    // order) and, for D = 40 / 80, sets the spare column of the last V atom to 1.0 for every real token: accumulator
-    // column D of the P.V UMMA is then the row sum of the fp16 P that was multiplied.
-    constexpr uint32_t idesc_pv = ptx::make_idesc_f16(128, C::DPV, false, true);
-    for (int j = 0; j < n_it; ++j) {
-      const int st = j % C::NV, g = j & 1, local = j >> 1, buf = local % C::NSB, k = local / C::NSB;
-      ptx::mbar_wait(BAR(B_VFULL + st), (uint32_t)((j / C::NV) & 1));
-      if constexpr (C::ONES) {
-        unsigned char* vlast = smem_gen + C::OFF_V + st * C::VSTAGE + (C::NA - 1) * kKAtom;
-        constexpr int cc = D % 64;                 // spare column inside the last atom
-        for (int r = lane; r < (TT ? TT : p.T); r += 32)
-          *reinterpret_cast<__half*>(vlast + r * 128 + ((((cc >> 3) ^ (r & 7))) << 4) + (cc & 7) * 2) = __float2half(1.0f);
-        ptx::fence_proxy_async_smem();             // generic-proxy writes -> visible to the UMMA (async proxy)
-        __syncwarp();
-      }
-      if (lane == 0) {
-        // O[g] = P V of unit `j`; P is read from the score buffer it overwrote
-        ptx::mbar_wait(BAR(B_PREADY + g * 2 + buf), (uint32_t)(k & 1));
-        if (local >= 1) ptx::mbar_wait(BAR(B_OFREE + g), (uint32_t)((local - 1) & 1));
-        PWW_TL(3, j);
-        ptx::tc_fence_after();
-        const uint32_t vb = smem0 + C::OFF_V + st * C::VSTAGE;
-#pragma unroll
-        for (int ks = 0; ks < kTP / 16; ++ks)          // A = P from tensor memory: 8 columns (16 fp16) per k-step
-          ptx::umma_ts(tmem_base + col_o<D>(g), tmem_base + col_s<D>(g, buf) + ks * 8,
-                       ptx::make_sw128_desc(vb + ks * 16 * 128, kKAtom, 1024), idesc_pv, ks > 0);
-        ptx::umma_commit(BAR(B_PVDONE + g * 2 + buf));
-        ptx::umma_commit(BAR(B_VEMPTY + st));
-        PWW_TL(8, j);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ===================================== softmax / epilogue groups =====================================
-    const int g = (warp - 2) >> 2;
-    const int row = ((warp & 3) << 5) | lane;                  // TMEM lane == tile row
-    const uint32_t lane_addr = (uint32_t)((warp & 3) << 5) << 16;
-    const float sl2 = p.scale * 1.4426950408889634f;
-    const float* mask_row = reinterpret_cast<const float*>(smem_gen + C::OFF_MASK) + row * (TT ? TT : p.T);
-    FwdWalk ws(u0, p.B, p.H, s_nb, s_img);
-    int grp = -1;
-    // deferred epilogue state: iteration `pend` of this group has its P.V in flight / finished
-    int pend_local = -1, pend_n = 0, pend_b = 0, pend_h = 0;
-    __half* pend_out = nullptr;
-    float pend_inv = 0.f;
-    // TMA-store epilogue: this warp's [32 x D] fp16 staging tile (row = lane)
-    const uint32_t stg_off = C::OFF_STG + (uint32_t)(warp - 2) * C::STG_WARP;
-
-    auto warp_arrive = [&](uint32_t bar) {       // one arrive per warp (barrier counts are per warp)
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(bar);
-    };
-    auto epilogue = [&]() {                      // O[g] (fp32, TMEM) -> * 1/rowsum -> fp16 -> global
-      ptx::mbar_wait(BAR(B_PVDONE + g * 2 + pend_local % C::NSB), (uint32_t)((pend_local / C::NSB) & 1));
-      ptx::tc_fence_after();
-      const uint32_t ta = tmem_base + lane_addr + col_o<D>(g);
-      float o[C::DPV];
-      // whole accumulator row in as few TMEM loads as possible
-      if constexpr (C::DPV == 48) { ptx::tmem_ld32_sync(ta, o); ptx::tmem_ld16_sync(ta + 32, o + 32); }
-      else if constexpr (C::DPV == 64) { ptx::tmem_ld64_sync(ta, o); }
-      else if constexpr (C::DPV == 96) { ptx::tmem_ld64_sync(ta, o); ptx::tmem_ld32_sync(ta + 64, o + 64); }
-      else { ptx::tmem_ld64_sync(ta, o); ptx::tmem_ld64_sync(ta + 64, o + 64); ptx::tmem_ld32_sync(ta + 128, o + 128); }
-      ptx::tc_fence_before();
-      warp_arrive(BAR(B_OFREE + g));             // O[g] is in registers: the next P.V may overwrite it
-      const float inv = C::ONES ? 1.f / o[D] : pend_inv;
-      if constexpr (EPI_TMA) {
-#pragma unroll
-        for (int ps = 0; ps < C::EPI_NPASS; ++ps) {
-          // the staging tile is free once the previous store of this warp has been read out (lane 0 owns the groups)
-          if (lane == 0) ptx::bulk_wait_group_read0();
-          __syncwarp();
-          unsigned char* dst = smem_gen + stg_off + lane * (C::EPI_CW * 2);
-#pragma unroll
-          for (int c = 0; c < C::EPI_CW / 8; ++c) {
-            __align__(16) __half2 pk[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q)
-              pk[q] = __floats2half2_rn(o[ps * C::EPI_CW + c * 8 + 2 * q] * inv, o[ps * C::EPI_CW + c * 8 + 2 * q + 1] * inv);
-            const int cs = C::EPI_SW ? (c ^ (lane & 7)) : c;       // 16-byte chunk position inside the (swizzled) row
-            reinterpret_cast<uint4*>(dst)[cs] = *reinterpret_cast<const uint4*>(pk);
-          }
-          ptx::fence_proxy_async_smem();           // generic-proxy writes -> visible to the TMA (async proxy)
-          __syncwarp();
-          const int n0 = pend_n - lane;            // first row of this warp's 32-row slice; rows >= N are clipped by TMA
-          if (lane == 0 && n0 < p.N) {
-            ptx::tma_store_4d(&tmo, smem0 + stg_off, ps * C::EPI_CW, pend_h, n0, pend_b);
-            ptx::bulk_commit_group();
-          }
-        }
-      } else {
-        if (pend_n < p.N) {
-#pragma unroll
-          for (int c = 0; c < D / 8; ++c) {
-            __align__(16) __half2 pk[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) pk[q] = __floats2half2_rn(o[c * 8 + 2 * q] * inv, o[c * 8 + 2 * q + 1] * inv);
-            reinterpret_cast<uint4*>(pend_out)[c] = *reinterpret_cast<const uint4*>(pk);
-          }
-        }
-      }
-    };
-
-    for (int it = 0; it < n_it; ++it, ws.next()) {
-      const FwdUnit ui = ws.get();
-      if (mask_group_starts_here(ui, it)) {
-        // all 8 softmax warps, both groups: observe this group's MFULL phase before any read or release of the tile
-        ++grp;
-        ptx::mbar_wait(BAR(B_MFULL), (uint32_t)(grp & 1));
-      }
-      // every softmax warp releases the group's mask tile exactly once, at this position of the group
-      const bool release_here = (ui.j == mask_release_pos(ui, it, n_it));
-      if ((it & 1) == g) {
-        const int local = it >> 1, buf = local % C::NSB;
-        const int widx = s_widx[ui.b];
-        const float coef = s_coef[ui.b];
-        const uint32_t ts = tmem_base + lane_addr + col_s<D>(g, buf);
-        ptx::mbar_wait(BAR(B_SREADY + g * 2 + buf), (uint32_t)((local / C::NSB) & 1));
-        if ((threadIdx.x & 127) == 64) PWW_TL(5, it);
-        ptx::tc_fence_after();
-        float s[kTP];
-        ptx::tmem_ld64_sync(ts, s);
-        ptx::tmem_ld16_sync(ts + 64, s + 64);
-        if ((threadIdx.x & 127) == 64) PWW_TL(0, it);
-        // logits t_j = S_j + coef*w_j (unscaled), row max with 4 independent chains
-        if (widx >= 0) {                            // (this group's MFULL phase was observed at the group's first unit)
-          if constexpr (TT == 77) {
-#pragma unroll
-            for (int j = 0; j < 77; ++j) s[j] = fmaf(coef, mask_row[j], s[j]);
-          } else {
-#pragma unroll
-            for (int j = 0; j < kTP; ++j)
-              if (j < p.T) s[j] = fmaf(coef, mask_row[j], s[j]);
-          }
-        }
-        if (release_here) warp_arrive(BAR(B_MEMPTY));   // the mask values are in registers: the next tile may land
-        if constexpr (TT == 77) {
-          s[77] = s[78] = s[79] = -INFINITY;
-        } else {
-#pragma unroll
-          for (int j = 0; j < kTP; ++j)
-            if (j >= p.T) s[j] = -INFINITY;
-        }
-        float m0 = s[0], m1 = s[1], m2 = s[2], m3 = s[3];
-#pragma unroll
-        for (int j = 4; j < kTP; j += 4) {
-          m0 = fmaxf(m0, s[j]); m1 = fmaxf(m1, s[j + 1]); m2 = fmaxf(m2, s[j + 2]); m3 = fmaxf(m3, s[j + 3]);
-        }
-        const float mx = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-        const float nm = -mx * sl2;
-        // p_j = 2^(t_j*sl2 - mx*sl2), UNNORMALISED, packed to fp16; O is scaled by 1/rowsum in the epilogue (fp32).
-        // (ex2.approx.f16x2 was tried: on sm_100a it lowers to two MUFU.EX2.F16 plus a PRMT -- no MUFU saving and
-        //  40 extra instructions per row -- so the exponentials stay fp32.)
-        float a0 = 0.f, a1 = 0.f;
-        uint32_t pk[kTP / 2];
-#pragma unroll
-        for (int j = 0; j < kTP; j += 2) {
-          const float e0 = ptx::ex2(fmaf(s[j], sl2, nm)), e1 = ptx::ex2(fmaf(s[j + 1], sl2, nm));
-          const __half2 h = __floats2half2_rn(e0, e1);
-          pk[j / 2] = *reinterpret_cast<const uint32_t*>(&h);
-          if constexpr (!C::ONES) {
-            const float2 f = __half22float2(h);       // sum exactly what the UMMA will multiply
-            a0 += f.x; a1 += f.y;
-          }
-        }
-        const float sum = a0 + a1;
-        if (lane == 0) { const int qd = warp & 3; PWW_TL((qd == 2 ? 7 : (qd == 3 ? 9 : (qd == 0 ? 10 : 11))), it); }
-        // P row (packed fp16) over the S row it came from: this thread has the whole row in registers
-        ptx::tmem_st32_u32(ts, pk);
-        ptx::tmem_st8_u32(ts + 32, pk + 32);
-        ptx::tmem_st_wait();
-        ptx::fence_proxy_async_smem();
-        ptx::tc_fence_before();
-        warp_arrive(BAR(B_PREADY + g * 2 + buf));
-        if ((threadIdx.x & 127) == 64) PWW_TL(6, it);
-        if (pend_local >= 0) {                     // overlaps with this iteration's P.V
-          epilogue();
-          if ((threadIdx.x & 127) == 64) PWW_TL(12, it);
-        }
-
-        pend_local = local;
-        pend_n = ui.tile * kBM + row;
-        pend_b = ui.b;
-        pend_h = ui.h;
-        pend_out = p.out + (int64_t)ui.b * p.o_bs + (int64_t)pend_n * p.o_rs + ui.h * D;
-        pend_inv = 1.f / sum;
-      } else if (release_here) {
-        warp_arrive(BAR(B_MEMPTY));                     // the other group's unit: this warp's mask reads are all behind it
-      }
-    }
-    if (pend_local >= 0) epilogue();
-    if constexpr (EPI_TMA) {
-      if (lane == 0) ptx::bulk_wait_group0();    // the staging tile must outlive the last store
-    }
+    float o[C::NT][4];
+    core::warp_softmax_pv<D>(s, p.T, sl2, st + C::QBYTES + C::KBYTES, lane, o);
+    core::warp_store<D>(o, smem + (it & 1) * Cfg<D>::STAGE + warp * 16 * C::LD * 2, lane,
+                        p.out + (int64_t)f.b * p.o_bs + f.h * D, p.o_rs, row0, p.N);
+    __syncthreads();
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  tl_dump(tp);
-  if (warp == 1) ptx::tmem_dealloc<kTmemCols>(tmem_base);
 }
 
 // ---------------------------------------------------------------------------------------------------------
 // statistics kernel: per-image max / (sum, sumsq) of fp16(S) over all heads, rows and tokens
 // ---------------------------------------------------------------------------------------------------------
-constexpr int kStatTmemCols = 256;
-
-template <int D, int TT>
-__global__ void __launch_bounds__(kThreads, 1)
-xattn_stats_tc_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ CUtensorMap tmk,
-                      const TcParams tp) {
-  using C = Cfg<D>;
+template <int D>
+__global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams tp) {
+  using C = core::Tile<D>;
   const XattnParams& p = tp.x;
-  extern __shared__ unsigned char smem_raw[];
-  const uint32_t smem0 = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
-  unsigned char* smem_gen = smem_raw + (smem0 - ptx::smem_u32(smem_raw));
-  const uint32_t bar0 = smem0 + C::S_OFF_BAR;
-  auto BAR = [&](int i) { return bar0 + 8u * i; };
-  constexpr int B_FULL = 0, B_EMPTY = 3, B_SREADY = 6, B_SFREE = 8, B_TMEMPTR = 10;
-  __shared__ StatPartial s_part[8][kMaxLocal];                  // [reducer warp][local image]
+  extern __shared__ __align__(128) unsigned char smem[];
+  const uint32_t smem0 = ptx::smem_u32(smem);
+  __shared__ StatPartial s_part[core::kWarps][kMaxLocal];     // [warp][local image]
   __shared__ unsigned char s_skip[kMaxBatch];
   __shared__ int is_last;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -625,94 +256,22 @@ xattn_stats_tc_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_cons
   const int n_it = u1 - u0;
   const int upi = tp.tiles * p.H;                               // units per image
   const int b_first = n_it > 0 ? u0 / upi : 0;
-  tl_init(tp);
   for (int b = threadIdx.x; b < p.B; b += kThreads) s_skip[b] = (p.wmap_index != nullptr && p.wmap_index[b] < 0) ? 1 : 0;
-  if (threadIdx.x < 8 * kMaxLocal) {
+  if (threadIdx.x < core::kWarps * kMaxLocal) {
     StatPartial sp;
     sp.vmax = -INFINITY; sp.sum = 0.0; sp.sumsq = 0.0; sp.pad = 0.0;
     s_part[threadIdx.x / kMaxLocal][threadIdx.x % kMaxLocal] = sp;
   }
-
-  if (warp == 0 && lane == 0) {
-    ptx::prefetch_tmap(&tmq);
-    ptx::prefetch_tmap(&tmk);
-    for (int s = 0; s < C::S_NSTAGE; ++s) {
-      ptx::mbar_init(BAR(B_FULL + s), 1);
-      ptx::mbar_init(BAR(B_EMPTY + s), 1);
-    }
-    for (int g = 0; g < 2; ++g) {
-      ptx::mbar_init(BAR(B_SREADY + g), 1);
-      ptx::mbar_init(BAR(B_SFREE + g), 4);
-    }
-    ptx::fence_barrier_init();
-  }
-  if (warp == 1) ptx::tmem_alloc<kStatTmemCols>(BAR(B_TMEMPTR));
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem_gen + C::S_OFF_BAR + 8 * B_TMEMPTR);
-
   auto skip = [&](int b) { return s_skip[b] != 0; };
-
-  if (warp == 0) {
-    int k = 0;                                                  // index among non-skipped iterations
-    UnitIter un(u0, tp.tiles, p.H);
-    for (int it = 0; it < n_it; ++it, un.next()) {
-      if (skip(un.b)) continue;
-      const int st = k % C::S_NSTAGE;
-      ptx::mbar_wait(BAR(B_EMPTY + st), (uint32_t)(((k / C::S_NSTAGE) & 1) ^ 1));
-      if (lane == 0) {
-        PWW_TL(1, k);
-        const uint32_t sb = smem0 + st * C::SSTAGE;
-        ptx::mbar_arrive_expect_tx(BAR(B_FULL + st), C::SSTAGE);
-        const int kb = tp.k_batched ? un.b : 0;
-#pragma unroll
-        for (int a = 0; a < C::NA; ++a) {
-          ptx::tma_load_4d(sb + a * kQAtom, &tmq, BAR(B_FULL + st), a * 64, un.h, un.tile * kBM, un.b);
-          ptx::tma_load_4d(sb + C::NA * kQAtom + a * kKAtom, &tmk, BAR(B_FULL + st), a * 64, un.h, 0, kb);
-        }
-      }
-      __syncwarp();
-      ++k;
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_qk = ptx::make_idesc_f16(128, kTP, false, false);
-      int k = 0;
-      UnitIter un(u0, tp.tiles, p.H);
-      for (int it = 0; it < n_it; ++it, un.next()) {
-        if (skip(un.b)) continue;
-        const int st = k % C::S_NSTAGE, g = k & 1, local = k >> 1;
-        ptx::mbar_wait(BAR(B_FULL + st), (uint32_t)((k / C::S_NSTAGE) & 1));
-        PWW_TL(2, k);
-        if (local >= 1) ptx::mbar_wait(BAR(B_SFREE + g), (uint32_t)((local - 1) & 1));
-        PWW_TL(3, k);
-        ptx::tc_fence_after();
-        const uint32_t sb = smem0 + st * C::SSTAGE;
-#pragma unroll
-        for (int ks = 0; ks < C::KSTEPS; ++ks) {
-          const uint32_t qa = sb + (ks / 4) * kQAtom + (ks % 4) * 32;
-          const uint32_t ka = sb + C::NA * kQAtom + (ks / 4) * kKAtom + (ks % 4) * 32;
-          ptx::umma_ss(tmem_base + g * 128, ptx::make_sw128_desc(qa, 16, 1024), ptx::make_sw128_desc(ka, 16, 1024),
-                       idesc_qk, ks > 0);
-        }
-        ptx::umma_commit(BAR(B_SREADY + g));
-        ptx::umma_commit(BAR(B_EMPTY + st));
-        PWW_TL(4, k);
-        ++k;
-      }
-    }
-    __syncwarp();
-  } else {
-    const int g = (warp - 2) >> 2;
-    const int row = ((warp & 3) << 5) | lane;
-    const uint32_t lane_addr = (uint32_t)((warp & 3) << 5) << 16;
-    float vmax = -INFINITY, sum = 0.f, sumsq = 0.f;
-    double dsum = 0.0, dsq = 0.0;                               // per-image accumulators across units
-    int cur_b = -1, k = 0;
+  const bool is_max = p.stat == PWW_STAT_MAX;
+  {
+    float vmax = -INFINITY;
+    double dsum = 0.0, dsq = 0.0;
+    int cur_b = -1;
     auto flush = [&]() {
       if (cur_b < 0) return;
-      double m = vmax, a = dsum + (double)sum, q = dsq + (double)sumsq;
+      double m = vmax, a = dsum, q = dsq;
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) {
         m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
@@ -722,73 +281,48 @@ xattn_stats_tc_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_cons
       if (lane == 0) {
         StatPartial sp;
         sp.vmax = m; sp.sum = a; sp.sumsq = q; sp.pad = 1.0;
-        s_part[warp - 2][cur_b - b_first] = sp;
+        s_part[warp][cur_b - b_first] = sp;
       }
-      vmax = -INFINITY; sum = 0.f; sumsq = 0.f; dsum = 0.0; dsq = 0.0;
+      vmax = -INFINITY; dsum = 0.0; dsq = 0.0;
     };
-    UnitIter un(u0, tp.tiles, p.H);
-    for (int it = 0; it < n_it; ++it, un.next()) {
-      if (skip(un.b)) continue;
-      if ((k & 1) == g) {
-        if (un.b != cur_b) { flush(); cur_b = un.b; }
-        const int local = k >> 1;
-        ptx::mbar_wait(BAR(B_SREADY + g), (uint32_t)(local & 1));
-        if (threadIdx.x == 64 || threadIdx.x == 192) PWW_TL(5, k);
-        ptx::tc_fence_after();
-        float s[kTP];
-        ptx::tmem_ld64_sync(tmem_base + lane_addr + g * 128, s);
-        ptx::tmem_ld16_sync(tmem_base + lane_addr + g * 128 + 64, s + 64);
-        ptx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(BAR(B_SFREE + g));
-        if (threadIdx.x == 64 || threadIdx.x == 192) PWW_TL(6, k);
-        if (un.tile * kBM + row < p.N) {
-          if (p.stat == PWW_STAT_MAX) {
-            // max(fp16(s)) == fp16(max(s)): rounding is monotonic, so round once at the very end
-            if constexpr (TT == 77) {
-              s[77] = s[78] = s[79] = -INFINITY;
-            } else {
-#pragma unroll
-              for (int j = 0; j < kTP; ++j)
-                if (j >= p.T) s[j] = -INFINITY;
-            }
-            float m0 = s[0], m1 = s[1], m2 = s[2], m3 = s[3];
-#pragma unroll
-            for (int j = 4; j < kTP; j += 4) {
-              m0 = fmaxf(m0, s[j]); m1 = fmaxf(m1, s[j + 1]); m2 = fmaxf(m2, s[j + 2]); m3 = fmaxf(m3, s[j + 3]);
-            }
-            vmax = fmaxf(vmax, fmaxf(fmaxf(m0, m1), fmaxf(m2, m3)));
-          } else {
-            float a0 = 0.f, a1 = 0.f, q0 = 0.f, q1 = 0.f;
-#pragma unroll
-            for (int j = 0; j < kTP; j += 2) {
-              // padded columns hold exact zeros (K rows >= T are zero-filled), so they add nothing
-              const __half2 h = __floats2half2_rn(s[j], s[j + 1]);
-              const float2 f = __half22float2(h);
-              a0 += f.x; a1 += f.y;
-              q0 = fmaf(f.x, f.x, q0); q1 = fmaf(f.y, f.y, q1);
-            }
-            sum = a0 + a1; sumsq = q0 + q1;
-          }
-        }
-        dsum += (double)sum; dsq += (double)sumsq; sum = 0.f; sumsq = 0.f;
+    // the units of images with a map, in order; `nxt` runs one unit ahead (its copies overlap this unit's MMAs)
+    UnitIter nxt(u0, tp.tiles, p.H);
+    int it_n = 0;
+    auto advance = [&]() { while (it_n < n_it && skip(nxt.b)) { nxt.next(); ++it_n; } };
+    advance();
+    if (it_n < n_it) load_unit<D>(smem0, p, nxt.b, nxt.h, nxt.tile, false);
+    for (int k = 0; it_n < n_it; ++k) {
+      const int b = nxt.b, tile = nxt.tile;
+      nxt.next();
+      ++it_n;
+      advance();
+      if (it_n < n_it) {
+        load_unit<D>(smem0 + ((k + 1) & 1) * Cfg<D>::STAGE, p, nxt.b, nxt.h, nxt.tile, false);
+        ptx::cp_async_wait<1>();
+      } else {
+        ptx::cp_async_wait<0>();
       }
-      if ((threadIdx.x == 64 || threadIdx.x == 192) && ((k & 1) == g)) PWW_TL(7, k);
-      ++k;
+      __syncthreads();
+      if (b != cur_b) { flush(); cur_b = b; }
+      const uint32_t st = smem0 + (k & 1) * Cfg<D>::STAGE;
+      float s[10][4];
+      core::warp_qk<D>(st + (uint32_t)(warp * 16 * C::LD) * 2u, st + C::QBYTES, lane, s);
+      float sum = 0.f, sumsq = 0.f;
+      core::warp_stat(s, p.T, p.N - tile * kBM - warp * 16, lane, is_max, vmax, sum, sumsq);
+      dsum += (double)sum;
+      dsq += (double)sumsq;
+      __syncthreads();
     }
     flush();
   }
   // ---- per-CTA partials (fixed warp order), then the last CTA to arrive finalises every image ----
-  ptx::tc_fence_before();
   __syncthreads();
-  tl_dump(tp);
-  if (warp == 1) ptx::tmem_dealloc<kStatTmemCols>(tmem_base);
   const int G = gridDim.x;
   if (threadIdx.x < kMaxLocal && n_it > 0) {
     const int b = b_first + threadIdx.x;
     if (b < p.B && (int64_t)b * upi < u1 && !skip(b)) {
       StatPartial sp = s_part[0][threadIdx.x];
-      for (int w = 1; w < 8; ++w) {
+      for (int w = 1; w < core::kWarps; ++w) {
         sp.vmax = fmax(sp.vmax, s_part[w][threadIdx.x].vmax);
         sp.sum += s_part[w][threadIdx.x].sum;
         sp.sumsq += s_part[w][threadIdx.x].sumsq;
@@ -805,8 +339,8 @@ xattn_stats_tc_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_cons
   __syncthreads();
   if (!is_last) return;
   __threadfence();
-  // warp w finalises images w, w+10, ...: lanes stride over the CTAs whose unit range intersects the image
-  for (int b = warp; b < p.B; b += kThreads / 32) {
+  // warp w finalises images w, w+8, ...: lanes stride over the CTAs whose unit range intersects the image
+  for (int b = warp; b < p.B; b += core::kWarps) {
     if (skip(b)) {
       if (lane == 0) p.stats_out[b] = 0.f;
       continue;
@@ -831,7 +365,7 @@ xattn_stats_tc_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_cons
     if (lane == 0) {
       const double cnt = (double)p.H * (double)p.N * (double)p.T;
       double r;
-      if (p.stat == PWW_STAT_MAX) {
+      if (is_max) {
         r = m;
       } else {
         const double var = (q - a * a / cnt) / (cnt - 1.0);
@@ -846,49 +380,10 @@ xattn_stats_tc_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_cons
 // ---------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-inline EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* sym = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(sym);
-  }
-  return fn;
-}
-
-// [B, L, H*D] fp16 viewed as (d, head, row, batch); box = 64 d x 1 head x box_rows rows x 1, 128-byte swizzle.
-// Diagnostics of the last host-side failure in this file (read by pww_abi.cu into pww_last_cuda_error()).
+// Diagnostics of the last host-side failure in the launchers (read by pww_abi.cu into pww_last_cuda_error()).
 inline char* tc_error_buf() {
   static thread_local char buf[256] = "";
   return buf;
-}
-
-inline bool make_tmap(CUtensorMap* m, const void* base, int D, int H, int L, int B, int64_t row_stride,
-                      int64_t batch_stride, int box_rows) {
-  EncodeTiledFn fn = encode_fn();
-  if (!fn) {
-    snprintf(tc_error_buf(), 256, "cuTensorMapEncodeTiled entry point not found");
-    return false;
-  }
-  cuuint64_t dims[4] = {(cuuint64_t)D, (cuuint64_t)H, (cuuint64_t)L, (cuuint64_t)B};
-  cuuint64_t strides[3] = {(cuuint64_t)D * 2, (cuuint64_t)row_stride * 2,
-                           (cuuint64_t)(batch_stride > 0 ? batch_stride : (int64_t)L * row_stride) * 2};
-  cuuint32_t box[4] = {64, 1, (cuuint32_t)box_rows, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS)
-    snprintf(tc_error_buf(), 256,
-             "cuTensorMapEncodeTiled failed (CUresult %d): base %p dims {%d,%d,%d,%d} strides {%lld,%lld,%lld} box rows %d",
-             (int)r, base, D, H, L, B, (long long)strides[0], (long long)strides[1], (long long)strides[2], box_rows);
-  return r == CUDA_SUCCESS;
 }
 
 // Per-device host state: the current device decides (the Python shim makes the tensors' device current).
@@ -907,14 +402,10 @@ inline int num_sms() {
 
 inline int stats_grid(int units) { return units < num_sms() ? units : num_sms(); }
 
-inline long long*& debug_timeline() {
-  static long long* ptr = nullptr;
-  return ptr;
-}
 // Host replay of the forward kernel's unit schedule (test infrastructure): the same FwdWalk / cta_range /
-// mask_release_pos / mask_group_starts_here code the kernel runs, executed on the CPU.  out[u] = {cta, it, b, h, tile,
-// group_id, mask_b, flags} for every unit in launch order of each CTA; flags bit 0 = every softmax warp releases the
-// mask tile at this unit, bit 1 = every softmax warp (both groups) waits for B_MFULL at this unit.
+// mask_release_pos / mask_group_starts_here code, executed on the CPU.  out[u] = {cta, it, b, h, tile, group_id, mask_b,
+// flags} for every unit in launch order of each CTA; flags bit 0 = last unit of the group in the CTA's range that reads
+// the mask tile, bit 1 = first unit of a mask group in the CTA's range.
 inline int fwd_schedule_host(int B, int H, int tiles, int grid, const int* wmap_index, int* out) {
   if (B <= 0 || B > kMaxBatch || H <= 0 || tiles <= 0 || grid <= 0) return -1;
   int img[kMaxBatch];
@@ -941,105 +432,38 @@ inline int fwd_schedule_host(int B, int H, int tiles, int grid, const int* wmap_
   return row;
 }
 
-// Forward-kernel epilogue: 0 = per-thread global stores everywhere, 1 = TMA-store epilogue at D = 40 only,
-// 3 = TMA-store epilogue at every head dim (default); pww_debug_set_variant overrides it for A/B timing.
-constexpr int kDefaultFwdVariant = 3;   // parity-green and faster at D = 64 / 80 / 160 on hardware (profiles/r02_call1_*)
-inline int& fwd_variant() {
-  static int v = kDefaultFwdVariant;
-  return v;
-}
-// Row-major [B, L, H, D] fp16 output as a TMA tensor: boxes of [box_cols x 1 x rows x 1], plain or 128-byte swizzled.
-inline bool make_tmap_out(CUtensorMap* m, const void* base, int D, int H, int L, int B, int64_t row_stride,
-                          int64_t batch_stride, int box_rows, int box_cols, bool swizzle128) {
-  EncodeTiledFn fn = encode_fn();
-  if (!fn) return false;
-  cuuint64_t dims[4] = {(cuuint64_t)D, (cuuint64_t)H, (cuuint64_t)L, (cuuint64_t)B};
-  cuuint64_t strides[3] = {(cuuint64_t)D * 2, (cuuint64_t)row_stride * 2, (cuuint64_t)batch_stride * 2};
-  cuuint32_t box[4] = {(cuuint32_t)box_cols, 1, (cuuint32_t)box_rows, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
-                  CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS;
-}
-
-template <int D, bool EPI_TMA>
-cudaError_t launch_fwd_var(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& to,
-                           const TcParams& tp, cudaStream_t s) {
-  using C = Cfg<D>;
-  constexpr uint32_t smem = EPI_TMA ? C::SMEM_EPI : C::SMEM;
-  static_assert(smem <= 232448 - 8192, "shared memory budget (dynamic + static tables)");
-  static bool attr_set[kMaxDevices] = {false};       // cudaFuncSetAttribute is per device
-  if (!attr_set[cur_device()]) {
-    cudaError_t e = cudaFuncSetAttribute(xattn_fwd_tc_kernel<D, 77, EPI_TMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(xattn_fwd_tc_kernel<D, 0, EPI_TMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    attr_set[cur_device()] = true;
-  }
-  const int grid = tp.units < num_sms() ? tp.units : num_sms();
-  if (tp.x.T == 77)
-    xattn_fwd_tc_kernel<D, 77, EPI_TMA><<<grid, kFwdThreads, smem, s>>>(tq, tk, tv, to, tp);
-  else
-    xattn_fwd_tc_kernel<D, 0, EPI_TMA><<<grid, kFwdThreads, smem, s>>>(tq, tk, tv, to, tp);
-  return cudaGetLastError();
+template <int D>
+cudaError_t set_smem(const void* fn, uint32_t bytes, bool (&done)[kMaxDevices]) {
+  if (done[cur_device()]) return cudaSuccess;
+  cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  if (e == cudaSuccess) done[cur_device()] = true;
+  return e;
 }
 
 template <int D>
 cudaError_t launch_fwd(const XattnParams& x, cudaStream_t s) {
-  using C = Cfg<D>;
-  CUtensorMap tq, tk, tv;
-  const int kB = x.k_bs > 0 ? x.B : 1;
-  if (!make_tmap(&tq, x.q, D, x.H, x.N, x.B, x.q_rs, x.q_bs, kBM) ||
-      !make_tmap(&tk, x.k, D, x.H, x.T, kB, x.k_rs, x.k_bs, kTP) ||
-      !make_tmap(&tv, x.v, D, x.H, x.T, kB, x.k_rs, x.k_bs, kTP))
-    return cudaErrorInvalidValue;
   TcParams tp;
   tp.x = x;
   tp.tiles = ceil_div(x.N, kBM);
   tp.units = x.B * tp.tiles * x.H;
-  tp.k_batched = x.k_bs > 0 ? 1 : 0;
-  tp.timeline = debug_timeline();
-  // The TMA-store epilogue needs a 16-byte aligned, 16-byte strided output.  It is the default at D = 40 (the 64x64-latent
-  // layers, where this kernel spends its time; verified and A/B-timed on hardware); for the other head dims it is built
-  // but only selected by variant 3 until it has been through the parity tests on a GPU.
-  CUtensorMap to = tq;
-  const int var = fwd_variant();
-  const bool want = (D == 40) ? (var >= 1) : (var == 3);
-  const bool tma_ok = (reinterpret_cast<uintptr_t>(x.out) & 15u) == 0 && (x.o_rs * 2) % 16 == 0 &&
-                      (x.o_bs * 2) % 16 == 0 && x.o_bs > 0;
-  if (want && tma_ok && make_tmap_out(&to, x.out, D, x.H, x.N, x.B, x.o_rs, x.o_bs, 32, C::EPI_CW, C::EPI_SW)) {
-    return launch_fwd_var<D, true>(tq, tk, tv, to, tp, s);
-  }
-  return launch_fwd_var<D, false>(tq, tk, tv, to, tp, s);
+  static bool attr_set[kMaxDevices] = {false};
+  cudaError_t e = set_smem<D>((const void*)xattn_fwd_kernel<D>, Cfg<D>::SMEM, attr_set);
+  if (e != cudaSuccess) return e;
+  const int grid = tp.units < num_sms() ? tp.units : num_sms();
+  xattn_fwd_kernel<D><<<grid, kThreads, Cfg<D>::SMEM, s>>>(tp);
+  return cudaGetLastError();
 }
 
 template <int D>
 cudaError_t launch_stats(const XattnParams& x, cudaStream_t s) {
-  using C = Cfg<D>;
-  CUtensorMap tq, tk;
-  const int kB = x.k_bs > 0 ? x.B : 1;
-  if (!make_tmap(&tq, x.q, D, x.H, x.N, x.B, x.q_rs, x.q_bs, kBM) ||
-      !make_tmap(&tk, x.k, D, x.H, x.T, kB, x.k_rs, x.k_bs, kTP))
-    return cudaErrorInvalidValue;
   TcParams tp;
   tp.x = x;
   tp.tiles = ceil_div(x.N, kBM);
   tp.units = x.B * tp.tiles * x.H;
-  tp.k_batched = x.k_bs > 0 ? 1 : 0;
-  tp.timeline = debug_timeline();
   static bool attr_set[kMaxDevices] = {false};
-  if (!attr_set[cur_device()]) {
-    cudaError_t e = cudaFuncSetAttribute(xattn_stats_tc_kernel<D, 77>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::S_SMEM);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(xattn_stats_tc_kernel<D, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::S_SMEM);
-    if (e != cudaSuccess) return e;
-    attr_set[cur_device()] = true;
-  }
-  if (x.T == 77)
-    xattn_stats_tc_kernel<D, 77><<<stats_grid(tp.units), kThreads, C::S_SMEM, s>>>(tq, tk, tp);
-  else
-    xattn_stats_tc_kernel<D, 0><<<stats_grid(tp.units), kThreads, C::S_SMEM, s>>>(tq, tk, tp);
+  cudaError_t e = set_smem<D>((const void*)xattn_stats_kernel<D>, Cfg<D>::SMEM, attr_set);
+  if (e != cudaSuccess) return e;
+  xattn_stats_kernel<D><<<stats_grid(tp.units), kThreads, Cfg<D>::SMEM, s>>>(tp);
   return cudaGetLastError();
 }
 

@@ -1,6 +1,6 @@
 """Public API: `paint_with_words()`, `paint_with_words_inpaint()`, `pww_load_tools()` -- same keyword
 arguments, defaults and return type as the reference (paint_with_words/paint_with_words.py:128-204,
-391-510; paint_with_words_inpaint.py:137-270) -- plus `PwWSampler`, the B200-first engine behind them.
+391-510; paint_with_words_inpaint.py:137-270) -- plus `PwWSampler`, the GPU-first engine behind them.
 
 What is different underneath (results equal within the stated fp16 tolerance):
   * the attention of every UNet block runs in libpww_b200.so (see attention.py);

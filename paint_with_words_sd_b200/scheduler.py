@@ -1,13 +1,13 @@
 """Minimal LMS discrete scheduler with the diffusers-0.10.0 `LMSDiscreteScheduler` call surface used at
 paint_with_words.py:197-202, 431-476, 506 and paint_with_words_inpaint.py:180-197, 266.
 
-diffusers is a third-party dependency that is not vendored under /root/reference (requirements.txt:1
+diffusers is a third-party dependency that is not vendored in the reference (requirements.txt:1
 pins 0.10.0) and is not installed here, so the published algorithm is restated: scaled-linear betas
 0.00085..0.012 over 1000 train steps, Karras-style sigmas = sqrt((1-abar)/abar) interpolated at
 linspace(0,999,n)[::-1] with a trailing 0, epsilon prediction, order-4 linear multistep with
 coefficients from scipy.integrate.quad(epsrel=1e-4).
 
-B200-first change: the multistep coefficients of every step are integrated once in `set_timesteps`
+GPU-first change: the multistep coefficients of every step are integrated once in `set_timesteps`
 (the stock implementation calls scipy.quad on the host inside every `step`, stalling the stream), and
 `step_index_of` avoids the `.nonzero().item()` device sync of paint_with_words.py:473.
 """

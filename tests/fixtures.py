@@ -1,4 +1,5 @@
-"""Shared test/bench inputs rebuilt from the committed golden fixtures (no /root/reference needed)."""
+"""Shared test/bench inputs rebuilt from the committed golden fixtures (no reference checkout needed)."""
+import math
 import os
 
 import numpy as np
@@ -35,3 +36,17 @@ def moon_mask_image(size: int = 512) -> Image.Image:
     cm = np.load(os.path.join(GOLDEN, "color_maps.npz"))
     img = Image.fromarray((cm["moon_mask"] * 255).astype(np.uint8), mode="L")
     return img if size == 512 else img.resize((size, size), Image.NEAREST)
+
+
+def exact_digest(t) -> np.ndarray:
+    """[sum, sum of squares, weighted checksum] of a float32 array too big to commit.  Every term is exact in float64
+    (a float32 value, its square, its product with an integer below 2^14) and each sum is math.fsum's correctly rounded
+    one, so the digest does not depend on the order in which a machine adds."""
+    x = np.asarray(t.detach().cpu().numpy() if hasattr(t, "detach") else t)
+    if x.dtype != np.float32:
+        raise TypeError(f"exact_digest needs float32 values, got {x.dtype}")
+    x = x.astype(np.float64).ravel()
+    w = np.arange(1, x.size + 1, dtype=np.float64) % 9973
+    nz = x != 0                                  # zeros add nothing to any of the three sums
+    x, w = x[nz], w[nz]
+    return np.array([math.fsum(x.tolist()), math.fsum((x * x).tolist()), math.fsum((x * w).tolist())])

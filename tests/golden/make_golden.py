@@ -1,6 +1,6 @@
 """Generate the committed golden fixtures by running the UNMODIFIED reference functions.
 
-    python tests/golden/make_golden.py          (build container only: needs /root/reference)
+    python tests/golden/make_golden.py          (needs a reference checkout named by PWW_REFERENCE_ROOT)
 
 The reference has no tests or golden vectors for the Paint-with-Words path (SURVEY.md section 4), so the
 oracle (oracle/pww_oracle.py) is pinned against the reference's own code executed here through
@@ -9,7 +9,7 @@ oracle/ref_loader.py.  Outputs (all under tests/golden/, all small):
   color_maps.npz     region-index maps derived from contents/example_input.png, contents/aurora_1.png
                      (0 = pixel matches no context colour, i+1 = i-th colour of the runner.py setting) and
                      the binarised contents/moon_mask.png -- the only inputs the mask builder looks at, so
-                     the GPU box (which has no /root/reference) can rebuild equivalent PIL images.
+                     a machine without the reference can rebuild equivalent PIL images.
   mask_builder.npz   reference outputs of always_round, _extract_seed_and_sigma_from_context,
                      _image_context_seperator, _tokens_img_attention_weight (ratios 8/16/32/64 and ORIG
                      digests), _get_binary_mask, _blur_image_mask for the runner.py settings.
@@ -31,6 +31,7 @@ sys.path.insert(0, ROOT)
 from oracle.ref_loader import REFERENCE_ROOT, load_reference  # noqa: E402
 from paint_with_words_sd_b200.synthetic import SimpleWordTokenizer  # noqa: E402
 from paint_with_words_sd_b200.unet import CrossAttention  # noqa: E402
+from tests.fixtures import exact_digest  # noqa: E402
 
 OUT = os.path.dirname(os.path.abspath(__file__))
 
@@ -112,7 +113,7 @@ def main():
                 mb[f"{tag}_w{r}"] = wt.numpy()
             orig = ref._tokens_img_attention_weight(sep, text_input, ratio=1, original_shape=True)
             mb[f"{tag}_orig_shape"] = np.array(orig.shape)
-            mb[f"{tag}_orig_digest"] = digest(orig)
+            mb[f"{tag}_orig_digest"] = exact_digest(orig)
             if size == 512 and name == "aurora":
                 # regional seeding + blur (runner.py:61-72 style context)
                 ctx2 = dict(AURORA_SEED_CTX)

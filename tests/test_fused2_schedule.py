@@ -3,7 +3,7 @@ on the host by the library itself (the same code the kernel's host-replay test c
 What must hold: every (image, head, row tile) is a softmax job exactly once; every unit of an image with a weight map is
 a statistic job exactly once, before any softmax job of its CTA; the unbiased softmax jobs of a CTA precede its biased
 ones (they overlap the grid barrier); the jobs of a unit pass are consecutive, flagged first ... last, share one `up`;
-`up` counts the unit passes of a CTA in order (the Q ring index); `ul` is the unit's position in the CTA's range (the
+`up` counts the unit passes of a CTA in order; `ul` is the unit's position in the CTA's range (the
 resident stage); the set of CTAs the barrier of image b waits for is exactly the set that publishes a partial for b."""
 import ctypes
 import itertools
@@ -51,6 +51,10 @@ CASES = [
     (4, 8, 8, 8, [0, -1, 1, -1]),
     (2, 8, 8, 3, [0, -1]),
     (5, 3, 3, 4, [0, -1, 1, -1, 2]),
+    # the same launches on the H100's 132 SMs
+    (16, 8, 32, 132, list(range(8)) + [-1] * 8),
+    (16, 8, 32, 132, [v for i in range(8) for v in (i, -1)]),
+    (3, 5, 72, 132, [0, 1, -1]),
 ]
 
 
@@ -103,11 +107,10 @@ def test_job_lists(B, H, tiles, grid, widx):
 
 
 def test_the_workload_launch_is_resident():
-    """cond + uncond at N = 4096, 8 heads on 148 CTAs: at most two units per CTA (the Q ring depth), so every CTA keeps
-    its Q tiles in shared memory between the statistic pass and the softmax pass; with 2 heads per unit most CTAs hold one
-    biased and one unbiased unit, whose softmax jobs overlap the grid barrier."""
+    """cond + uncond at N = 4096, 8 heads on 132 CTAs (one per H100 SM): at most two units per CTA; with 2 heads per unit
+    most CTAs hold one biased and one unbiased unit, whose softmax jobs overlap the grid barrier."""
     hg = (8 + G - 1) // G
-    grid = min(148, 2 * 32 * hg)
+    grid = min(132, 2 * 32 * hg)
     j = _jobs(2, 8, 32, grid, [0, -1])
     both = 0
     for cta in range(grid):

@@ -35,6 +35,10 @@ CASES = [
     (1, 8, 1, 148, [-1]),                          # fewer units than CTAs
     (5, 10, 3, 7, [0, 1, 2, 3, 4]),                # all biased
     (33, 8, 2, 148, [(-1 if i % 3 else i // 3) for i in range(33)]),
+    # the same launches on the H100's 132 SMs
+    (2, 8, 32, 132, [0, -1]),
+    (16, 8, 32, 132, [v for i in range(8) for v in (i, -1)]),
+    (3, 5, 72, 132, [0, 1, -1]),
 ]
 
 
@@ -66,7 +70,7 @@ def test_every_unit_once_and_mask_protocol(B, H, tiles, grid, widx):
 
 @pytest.mark.parametrize("order", ["cond_first", "uncond_first", "interleaved"])
 def test_cfg_batches_are_balanced_whatever_the_image_order(order):
-    B, H, tiles, grid = 16, 8, 32, 148
+    B, H, tiles, grid = 16, 8, 32, 132
     widx = {"cond_first": list(range(8)) + [-1] * 8, "uncond_first": [-1] * 8 + list(range(8)),
             "interleaved": [v for i in range(8) for v in (i, -1)]}[order]
     s = _schedule(B, H, tiles, grid, widx)
@@ -91,7 +95,7 @@ def test_old_wait_rule_skipped_phases_and_new_rule_does_not():
     mask-reading unit lay in the CTA's SECOND mask group waited for parity 1 of B_MFULL without having observed
     phase 0, so the parity test could pass before the first tile had landed.  The replay shows the old rule skipped
     phases on some CTAs of exactly that launch, and that under the new rule every warp waits on every phase."""
-    B, H, tiles, grid, widx = 1, 8, 32, 148, [0]
+    B, H, tiles, grid, widx = 1, 8, 32, 132, [0]
     s = _schedule(B, H, tiles, grid, widx)
     exposed = []
     for cta in range(grid):

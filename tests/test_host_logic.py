@@ -92,7 +92,7 @@ def test_factored_weight_map_reproduces_the_dense_one(name, size):
         assert torch.equal(m @ c.T, w)
         if w.shape[0] >= 1024:
             assert m.numel() + c.numel() < w.numel() / 5
-        # fp16 storage of the factors (what a UMMA operand would hold) stays far inside the attention tolerance
+        # fp16 storage of the factors (what a tensor-core operand would hold) stays far inside the attention tolerance
         w16 = m.half().float() @ c.T
         assert (w16 - w).abs().max().item() <= 2 ** -11 * w.abs().max().item()
 

@@ -75,8 +75,10 @@ def test_strided_qkv_views():
 
 
 def test_default_dispatch_matches_oracle_on_both_sides_of_the_switch():
-    """The shim's default: native kernel up to 512 keys, torch's library attention above -- same numbers either way."""
-    for N, native in ((256, True), (1024, False)):
+    """The shim's default: native kernel up to SELF_ATTN_NATIVE_MAX_KEYS keys, torch's library attention above -- same
+    numbers either way."""
+    switch = A.SELF_ATTN_NATIVE_MAX_KEYS
+    for N, native in ((switch // 4, True), (2 * switch, False)):
         q, k, v = _qkv(1, N, 8, 40, seed=N)
         before = _native.launch_count
         got = A.self_attention(q.cuda(), k.cuda(), v.cuda(), 8, 40 ** -0.5).float().cpu()

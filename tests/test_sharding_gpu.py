@@ -1,6 +1,6 @@
 """SURVEY 4 item 4 / 8e on hardware: with images sharded over 2 GPUs (NCCL, weights broadcast once from rank 0, nothing
 exchanged per step) every image's final latents are BIT-IDENTICAL to the same image run alone on one GPU.  Needs two
-GPUs (`gpurun --gpus 2`); skipped on a one-GPU box."""
+GPUs; skipped on a one-GPU machine."""
 import math
 import os
 import socket

@@ -266,11 +266,10 @@ def test_fused_long_job_lists(N, H, D, B, grid, stat):
 
 
 def test_fused_std_long_job_lists_repeat_bit_identically():
-    """compute-sanitizer racecheck reports write-after-write hazards on the V ring for the std statistic at head dim 40
-    (profiles/r02_sanitizer_all.txt; max and the other head dims are clean).  The ring's release is a tcgen05.commit
-    arrival on an mbarrier, which the tool does not model; a real overwrite of a V tile that is still being read would make
-    the output depend on timing.  40 launches of that configuration must agree bit for bit (fixed grid: the std partials
-    are summed in CTA order) and with the oracle."""
+    """Long job lists with the std statistic at head dim 40: every CTA reuses its two operand stages many times and spans
+    several images.  A stage overwritten while it is still being read would make the output depend on timing, so 40
+    launches of that configuration must agree bit for bit (fixed grid: the std partials are summed in CTA order) and with
+    the oracle."""
     N, H, D, T, B = 1024, 8, 40, 77, 4
     q, k, v, w = _inputs(B, N, H, D, T, seed=4242)
     idx = torch.tensor([0, -1, 1, -1], dtype=torch.int32)

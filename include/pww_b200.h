@@ -24,6 +24,10 @@
  *            (paint_with_words.py:255-268, 370-377) stacked along dim 0
  *   wmap_index : [B] int32, image b uses wmap[wmap_index[b]]; -1 = no bias for that image (the
  *            reference's uncond dict / tensor context, paint_with_words.py:107-110, 379-386, 493)
+ *
+ * Key lengths: T <= 80 (Stable Diffusion's 77-token context), or a long prompt of k = 2 or 3 CLIP chunks
+ * concatenated along tokens (T = 154 or 231; each chunk is [BOS] + up to 75 tokens + [EOS] + padding, encoded
+ * on its own).  Any other T returns PWW_ERR_UNSUPPORTED.  Workspace sizes do not depend on T.
  */
 #ifndef PWW_B200_H_
 #define PWW_B200_H_
@@ -84,7 +88,7 @@ int pww_xattn_stats_f16(const void* q, const void* k,
  * `g_sigma` is a 1-element device array holding G(sigma) = coef*ln(1+sigma^p) for this step (a device
  * scalar so a captured CUDA graph can be replayed with a new sigma).  wmap/wmap_index/stats/g_sigma may
  * all be NULL: plain cross-attention (tensor context, paint_with_words.py:67-69,107-108).
- * Requires T <= 80 (Stable Diffusion's 77-token context).
+ * Requires T <= 80 or T = 154 / 231 (see "Key lengths" above; wmap stays [Bw, N, T], no padding columns).
  */
 int pww_xattn_fwd_f16(const void* q, const void* k, const void* v, void* out,
                       int B, int H, int N, int T, int D,
@@ -106,14 +110,17 @@ int pww_xattn_fwd_f16(const void* q, const void* k, const void* v, void* out,
  *   mpack : [Bw, N, 32] fp16, row n = [ hi(Mu[n,0..9]) | lo(Mu[n,0..9]) | hi(Mu[n,0..9]) | 0 0 ] with
  *           hi(x) = fp16(x), lo(x) = fp16(x - hi(x));  64 bytes per pixel instead of 308
  *           (element (w,n,c) at w*mpack_batch_stride + n*32 + c; 16-byte aligned)
- *   cidx  : [Bw, 80] int8, dictionary column of token t (0..9) or -1 (also for t >= T)
+ *   cidx  : [Bw, 80 k] int8, k = 1 for T <= 80, else T / 77: dictionary column (0..9) or -1 of token 77 c + j at
+ *           column 80 c + j (for k = 1: token t at column t, -1 for t >= T; for k > 1 the columns 80 c + 77 .. 80 c + 79
+ *           of every chunk are -1)
  * `paint_with_words_sd_b200.conditioning.pack_weight_map` builds both, bit-exactly reversible to the dense map.
  * Maps with more than 10 distinct columns use the two-launch dense path above.
  *
  *   stats [B] out : the per-image statistic (fp16-rounded, as float; 0 for images without a map); may be NULL
  *   workspace     : pww_xattn_fused_workspace_bytes() bytes, zero-filled ONCE after allocation (self-cleaning)
  * mpack == NULL (or every wmap_index[b] < 0): plain cross-attention, workspace may be NULL.
- * Requires T <= 80, B <= 32 per launch (larger batches are split internally), 16-byte aligned `out` strides.
+ * Requires T <= 80 or T = 154 / 231, B <= 32 per launch (larger batches are split internally), 16-byte aligned `out`
+ * strides.
  */
 size_t pww_xattn_fused_workspace_bytes(void);
 int pww_xattn_fused_f16(const void* q, const void* k, const void* v, void* out,

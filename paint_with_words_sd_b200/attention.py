@@ -4,9 +4,11 @@ Same calling convention, context-dict schema and patch mechanism as the referenc
 (paint_with_words/paint_with_words.py:60-125 `inj_forward`, 193-195 / 556-559 patch sites):
 
     inj_forward(self, hidden_states, context=None, mask=None) -> Tensor[B, N, C]
-    context: None (self-attention) | Tensor[B,77,Dc] | dict with
-        "CONTEXT_TENSOR", "CROSS_ATTENTION_WEIGHT_{N}" ([N,77] fp32 or int 0),
-        "CROSS_ATTENTION_WEIGHT_ORIG" ([H,W,77] fp32 or int 0), "SIGMA", "WEIGHT_FUNCTION"
+    context: None (self-attention) | Tensor[B,T,Dc] | dict with
+        "CONTEXT_TENSOR", "CROSS_ATTENTION_WEIGHT_{N}" ([N,T] fp32 or int 0),
+        "CROSS_ATTENTION_WEIGHT_ORIG" ([H,W,T] fp32 or int 0), "SIGMA", "WEIGHT_FUNCTION"
+    T = 77 (one CLIP window, any T <= 80 works) or a long prompt of 2 or 3 concatenated 77-token chunks (T = 154, 231;
+    `conditioning.chunk_prompt`, the A1111 / compel layout).
         (optional, ours) "WMAP_INDEX", "G_SIGMA", "CROSS_ATTENTION_PACKED_{N}", "PWW_SCRATCH"
 
 Everything between the q/k/v projections and the output projection runs in libpww_b200.so through
@@ -32,7 +34,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _native
-from .conditioning import expand_orig_weight_map, pack_weight_map, packed_key, weight_key
+from .conditioning import PACK_TOKENS, expand_orig_weight_map, key_chunks, pack_weight_map, packed_key, weight_key
 from .weight_function import g_of_sigma, probe_weight_function
 
 _ORIG_KEY = "CROSS_ATTENTION_WEIGHT_ORIG"
@@ -143,9 +145,9 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                     stat: int = _native.PWW_STAT_MAX, g_sigma: Optional[torch.Tensor] = None,
                     return_stats: bool = False, packed=None, stats_out: Optional[torch.Tensor] = None,
                     workspace: Optional[torch.Tensor] = None):
-    """Fused region for a key sequence of <= 80 tokens.  q [B,N,C]; k,v [B,T,C]; wmap [Bw,N,T] fp32 or None;
-    `packed` = (mpack [Bw,N,32] fp16, cidx [Bw,80] int8) from `conditioning.pack_weight_map` (built from `wmap` and
-    cached when not given).  `g_sigma` is a 1-element fp32 device tensor holding G(sigma).  `stats_out` / `workspace`
+    """Fused region for a key sequence of T <= 80 tokens or of 2 / 3 CLIP chunks (T = 154, 231; any other T raises).
+    q [B,N,C]; k,v [B,T,C]; wmap [Bw,N,T] fp32 or None; `packed` = (mpack [Bw,N,32] fp16, cidx [Bw,80 k] int8, k key
+    chunks) from `conditioning.pack_weight_map` (built from `wmap` and cached when not given).  `g_sigma` is a 1-element fp32 device tensor holding G(sigma).  `stats_out` / `workspace`
     let a caller that captures CUDA graphs own the scratch (defaults: per-device scratch of this module)."""
     L = _native.lib()
     q, k, v = _rows(q), _rows(k), _rows(v)
@@ -182,7 +184,8 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
             mp_bs = bw = ws_bytes = 0
             if biased:
                 mpack, cidx = packed
-                if mpack.shape[1] != N or mpack.dtype != torch.float16 or cidx.dtype != torch.int8:
+                if (mpack.shape[1] != N or mpack.dtype != torch.float16 or cidx.dtype != torch.int8
+                        or cidx.shape[-1] != PACK_TOKENS * max(1, key_chunks(T))):
                     raise ValueError("packed weight map does not match this attention level")
                 st.ensure(B, 0)
                 stats = st.stats if stats_out is None else stats_out

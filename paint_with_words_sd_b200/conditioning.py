@@ -15,7 +15,7 @@ index/downsample step bit-exact.  Differences that do not change results:
 from __future__ import annotations
 
 import math
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -117,7 +117,25 @@ def _tokens_img_attention_factors(img_context_seperated, tokenized_texts, ratio:
 
 PACK_COLS = 32          # fp16 columns per pixel of the packed map (csrc/xattn_fused.cuh: kMW)
 PACK_CAPACITY = 10      # distinct non-zero columns a packed map can hold (kRC)
-PACK_TOKENS = 80        # padded token count of the column index (kTP)
+PACK_TOKENS = 80        # padded token count of the column index (kTP), per key chunk
+CHUNK_TOKENS = 77       # one CLIP window: [BOS] + up to 75 prompt tokens + [EOS] (+ padding)
+MAX_PROMPT_CHUNKS = 3   # longest context the attention kernels take: T = 231
+
+
+def key_chunks(t: int) -> int:
+    """Key chunks of a context of t tokens as the attention kernels stage it: 1 for t <= 80, k for t = 77 k (k = 2, 3),
+    0 for any other length (no kernel)."""
+    if t <= PACK_TOKENS:
+        return 1
+    k, r = divmod(t, CHUNK_TOKENS)
+    return k if r == 0 and 2 <= k <= MAX_PROMPT_CHUNKS else 0
+
+
+def _cidx_columns(t: int) -> torch.Tensor:
+    """Column of token j in the packed column index: j itself for t <= 80; for a chunked context token 77 c + i sits at
+    column 80 c + i (columns 80 c + 77 .. 80 c + 79 stay -1)."""
+    j = torch.arange(t)
+    return j if t <= PACK_TOKENS else j // CHUNK_TOKENS * PACK_TOKENS + j % CHUNK_TOKENS
 
 
 def pack_weight_map(w: torch.Tensor):
@@ -130,18 +148,22 @@ def pack_weight_map(w: torch.Tensor):
         w[n, t] == Mu[n, cidx[t]]        Mu [N, R] fp32 (R <= 10), cidx[t] = -1 for an all-zero column
 
     with Mu split into fp16 halves hi = fp16(Mu), lo = fp16(Mu - hi) so that hi + lo reproduces Mu to 2^-22:
-        mpack [Bw, N, 32] fp16 = [ hi(0..9) | lo(0..9) | hi(0..9) | 0 0 ],   cidx [Bw, 80] int8.
+        mpack [Bw, N, 32] fp16 = [ hi(0..9) | lo(0..9) | hi(0..9) | 0 0 ],   cidx [Bw, 80 k] int8.
+    k is the number of key chunks: 1 for T <= 80; for a long context of k CLIP chunks (T = 154, 231) token 77 c + j is
+    at column 80 c + j and the three padding columns of each chunk are -1.
     Works on CPU or CUDA tensors (torch ops only; the map builder is host-side set-up work, as in the reference).
-    Returns None when a map has more than PACK_CAPACITY distinct non-zero columns or values outside fp16 range --
-    such maps take the dense two-launch path."""
+    Returns None when a map has more than PACK_CAPACITY distinct non-zero columns, values outside fp16 range or a
+    token count without a kernel -- such maps take the dense two-launch path."""
     if w.dim() == 2:
         w = w.unsqueeze(0)
     bw, n, t = w.shape
-    if t > PACK_TOKENS:
+    k = key_chunks(t)
+    if k == 0:
         return None
     w = w.to(torch.float32)
     mpack = torch.zeros((bw, n, PACK_COLS), dtype=torch.float16, device=w.device)
-    cidx = torch.full((bw, PACK_TOKENS), -1, dtype=torch.int8, device=w.device)
+    cidx = torch.full((bw, PACK_TOKENS * k), -1, dtype=torch.int8, device=w.device)
+    col = _cidx_columns(t).to(w.device)
     for i in range(bw):
         cols = torch.nonzero((w[i] != 0).any(dim=0)).flatten()
         if cols.numel() == 0:
@@ -155,7 +177,7 @@ def pack_weight_map(w: torch.Tensor):
         mpack[i, :, 0:r] = hi.t()
         mpack[i, :, PACK_CAPACITY:PACK_CAPACITY + r] = lo.t()
         mpack[i, :, 2 * PACK_CAPACITY:2 * PACK_CAPACITY + r] = hi.t()
-        cidx[i, cols] = inv.to(torch.int8)
+        cidx[i, col[cols]] = inv.to(torch.int8)
     return mpack, cidx
 
 
@@ -164,8 +186,9 @@ def unpack_weight_map(mpack: torch.Tensor, cidx: torch.Tensor, tokens: int = 77)
     bw, n, _ = mpack.shape
     mu = mpack[..., :PACK_CAPACITY].to(torch.float32) + mpack[..., PACK_CAPACITY:2 * PACK_CAPACITY].to(torch.float32)
     out = torch.zeros((bw, n, tokens), dtype=torch.float32, device=mpack.device)
+    col = _cidx_columns(tokens).to(cidx.device)
     for i in range(bw):
-        idx = cidx[i, :tokens].to(torch.int64)
+        idx = cidx[i, col].to(torch.int64)
         sel = idx >= 0
         out[i][:, sel] = mu[i][:, idx[sel]]
     return out
@@ -225,14 +248,96 @@ def weight_key(n: int) -> str:
     return f"CROSS_ATTENTION_WEIGHT_{n}"
 
 
+def _special_ids(tokenizer, length: int) -> Tuple[int, int, int]:
+    """(BOS, EOS, padding id) as the tokenizer lays out one padded window."""
+    row = list(tokenizer([""], padding="max_length", max_length=length)["input_ids"][0])
+    return row[0], row[1], row[-1]
+
+
+def _prompt_windows(ids: List[int], labels: List[List[int]], max_chunks: int, width: int) -> List[List[int]]:
+    """Split prompt token ids (without BOS / EOS) into at most `max_chunks` windows of at most `width` tokens.  A window
+    never ends inside a span where a region label matches: it ends before the span instead, so every label that fits is
+    matched inside one chunk.  Tokens past the last window are dropped (truncation, as with one window)."""
+    spans = [(s, s + len(lab)) for lab in labels if lab for s in _match_positions(ids, lab)]
+    windows: List[List[int]] = []
+    pos = 0
+    while pos < len(ids) and len(windows) < max_chunks:
+        end = min(pos + width, len(ids))
+        if end < len(ids):
+            cut = end
+            while True:
+                inside = [a for a, b in spans if a < cut < b]
+                if not inside:
+                    break
+                cut = min(inside)
+            if cut > pos:                  # overlapping spans longer than a window: keep the plain cut
+                end = cut
+        windows.append(ids[pos:end])
+        pos = end
+    return windows
+
+
+def _chunked_ids(tokenizer, windows: List[List[int]], chunks: int) -> torch.Tensor:
+    """[1, 77 * chunks] ids: each window as [BOS] + window + [EOS] padded to one 77-token chunk, then empty chunks."""
+    length = tokenizer.model_max_length
+    bos, eos, pad = _special_ids(tokenizer, length)
+    rows = []
+    for c in range(chunks):
+        win = windows[c] if c < len(windows) else []
+        rows += [bos] + list(win) + [eos] + [pad] * (length - 2 - len(win))
+    return torch.tensor([rows], dtype=torch.long)
+
+
+def _encode_chunked(text_encoder, ids: torch.Tensor, device) -> torch.Tensor:
+    """Each 77-token chunk through the text encoder on its own, concatenated along tokens (the A1111 / compel layout)."""
+    length = CHUNK_TOKENS
+    return torch.cat([text_encoder(ids[:, c:c + length].to(device))[0] for c in range(0, ids.shape[1], length)], 1)
+
+
+def chunk_prompt(tokenizer, prompt: str, labels: Sequence[str] = (), max_prompt_chunks: int = 1) -> torch.Tensor:
+    """Token ids [1, 77 k] of `prompt` in k <= `max_prompt_chunks` CLIP windows of up to 75 tokens (k = 1: the
+    tokenizer's own padded, truncated window).  `labels` are the region labels: no window ends inside one of their
+    matches.  A label longer than one window raises ValueError."""
+    if not 1 <= max_prompt_chunks <= MAX_PROMPT_CHUNKS:
+        raise ValueError(f"max_prompt_chunks must be 1 .. {MAX_PROMPT_CHUNKS}, got {max_prompt_chunks}")
+    length = tokenizer.model_max_length
+    if max_prompt_chunks == 1:
+        return tokenizer([prompt], padding="max_length", max_length=length, truncation=True,
+                         return_tensors="pt")["input_ids"]
+    width = length - 2
+    ids = list(tokenizer(prompt)["input_ids"])[1:-1]
+    lab_ids = []
+    for label in labels:
+        li = list(tokenizer(label)["input_ids"])[1:-1]
+        if len(li) > width:
+            raise ValueError(f"region label {label!r} is {len(li)} tokens long; a label must fit one {width}-token window")
+        lab_ids.append(li)
+    windows = _prompt_windows(ids, lab_ids, max_prompt_chunks, width)
+    return _chunked_ids(tokenizer, windows, max(1, len(windows)))
+
+
 def _encode_text_color_inputs(text_encoder, tokenizer, device, color_map_image, color_context,
-                              input_prompt, unconditional_input_prompt, use_blur: bool = True):
+                              input_prompt, unconditional_input_prompt, use_blur: bool = True,
+                              max_prompt_chunks: int = 1):
     """paint_with_words.py:315-388 (and the pipeline-class copy 561-627, which ignores blur sigmas:
     pass use_blur=False for that behaviour).  Returns
-    (extra_seeds, seperated_word_contexts, encoder_hidden_states, uncond_encoder_hidden_states)."""
+    (extra_seeds, seperated_word_contexts, encoder_hidden_states, uncond_encoder_hidden_states).
+
+    `max_prompt_chunks` > 1 lets a prompt longer than 75 tokens fill up to that many 77-token CLIP chunks (T = 77 k,
+    see `chunk_prompt`); the uncond prompt is encoded to the same number of chunks, each chunk by the text encoder on its
+    own.  A prompt that fits one chunk gives the same dicts as max_prompt_chunks=1 (the reference's behaviour)."""
+    if not 1 <= max_prompt_chunks <= MAX_PROMPT_CHUNKS:
+        raise ValueError(f"max_prompt_chunks must be 1 .. {MAX_PROMPT_CHUNKS}, got {max_prompt_chunks}")
     text_input = tokenizer([input_prompt], padding="max_length", max_length=tokenizer.model_max_length,
                            truncation=True, return_tensors="pt")
     color_context, extra_seeds, extra_sigmas = _extract_seed_and_sigma_from_context(color_context)
+    chunks = 1
+    if max_prompt_chunks > 1:
+        labels = [spec.rpartition(",")[0] for spec in color_context.values()] if color_map_image is not None else []
+        ids = chunk_prompt(tokenizer, input_prompt, labels, max_prompt_chunks)
+        chunks = ids.shape[1] // CHUNK_TOKENS
+        if chunks > 1:
+            text_input = {"input_ids": ids}
     seperated_word_contexts, width, height = _image_context_seperator(color_map_image, color_context, tokenizer)
     if use_blur and len(extra_sigmas) > 0:
         print("Use extra sigma to smooth mask", extra_sigmas)
@@ -249,6 +354,13 @@ def _encode_text_color_inputs(text_encoder, tokenizer, device, color_map_image, 
         cond[key] = _tokens_img_attention_weight(seperated_word_contexts, text_input, ratio=r).to(device)
         uncond[key] = 0
 
+    if chunks > 1:
+        cond["CONTEXT_TENSOR"] = _encode_chunked(text_encoder, text_input["input_ids"], device)
+        width = tokenizer.model_max_length - 2
+        un_ids = list(tokenizer(unconditional_input_prompt)["input_ids"])[1:-1]
+        un_windows = _prompt_windows(un_ids, [], chunks, width)
+        uncond["CONTEXT_TENSOR"] = _encode_chunked(text_encoder, _chunked_ids(tokenizer, un_windows, chunks), device)
+        return extra_seeds, seperated_word_contexts, cond, uncond
     cond["CONTEXT_TENSOR"] = text_encoder(text_input.input_ids.to(device))[0]
     uncond_input = tokenizer([unconditional_input_prompt], padding="max_length",
                              max_length=text_input.input_ids.shape[-1], return_tensors="pt")

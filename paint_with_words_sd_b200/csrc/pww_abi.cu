@@ -26,8 +26,33 @@ int check_common(const void* q, const void* k, int B, int H, int N, int T, int D
   if (!aligned16(q) || !aligned16(k)) return PWW_ERR_BAD_ARG;
   if ((q_bs | q_rs | k_bs | k_rs) & 7) return PWW_ERR_BAD_ARG;  // 16-byte vector access on rows
   if (q_rs < (int64_t)H * D || k_rs < (int64_t)H * D) return PWW_ERR_BAD_ARG;
-  if (!supported_head_dim(D) || T > pww::tc::kTP) return PWW_ERR_UNSUPPORTED;
+  if (!supported_head_dim(D) || !pww::core::supported_keys(T)) return PWW_ERR_UNSUPPORTED;
   return PWW_OK;
+}
+
+// Kernel instance for a (head dim, key chunk count) pair: f(Shape<D, KC>{}) with KC = 1 for T <= 80, else T / 77.
+template <int D_, int KC_>
+struct Shape {
+  static constexpr int D = D_, KC = KC_;
+};
+template <int D, typename F>
+cudaError_t with_chunks(int T, F&& f) {
+  switch (pww::core::chunks_of(T)) {
+    case 1: return f(Shape<D, 1>{});
+    case 2: return f(Shape<D, 2>{});
+    case 3: return f(Shape<D, 3>{});
+  }
+  return cudaErrorInvalidValue;
+}
+template <typename F>
+cudaError_t with_shape(int D, int T, F&& f) {
+  switch (D) {
+    case 40: return with_chunks<40>(T, f);
+    case 64: return with_chunks<64>(T, f);
+    case 80: return with_chunks<80>(T, f);
+    case 160: return with_chunks<160>(T, f);
+  }
+  return cudaErrorInvalidValue;
 }
 
 size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
@@ -47,13 +72,13 @@ int cuda_fail(cudaError_t e) {
 
 extern "C" {
 
-int pww_version(void) { return 100; }  // 0.1.0
+int pww_version(void) { return 200; }  // 0.2.0: long contexts (T = 154, 231)
 
 const char* pww_status_str(int status) {
   switch (status) {
     case PWW_OK: return "ok";
     case PWW_ERR_BAD_ARG: return "bad argument (null/misaligned pointer, non-positive size or stride not a multiple of 8)";
-    case PWW_ERR_UNSUPPORTED: return "unsupported shape (head dim must be 40/64/80/160, T <= 80)";
+    case PWW_ERR_UNSUPPORTED: return "unsupported shape (head dim must be 40/64/80/160, T <= 80, 154 or 231)";
     case PWW_ERR_CUDA: return "CUDA error (see pww_last_cuda_error)";
     case PWW_ERR_WORKSPACE: return "workspace too small (see pww_xattn_workspace_bytes)";
     default: return "unknown status";
@@ -104,13 +129,7 @@ int pww_xattn_stats_f16(const void* q, const void* k, int B, int H, int N, int T
       c.k = p.k + (int64_t)b0 * p.k_bs;
       c.wmap_index = p.wmap_index ? p.wmap_index + b0 : nullptr;
       c.stats_out = p.stats_out + b0;
-      cudaError_t e = cudaErrorInvalidValue;
-      switch (D) {
-        case 40: e = pww::tc::launch_stats<40>(c, s); break;
-        case 64: e = pww::tc::launch_stats<64>(c, s); break;
-        case 80: e = pww::tc::launch_stats<80>(c, s); break;
-        case 160: e = pww::tc::launch_stats<160>(c, s); break;
-      }
+      const cudaError_t e = with_shape(D, T, [&](auto k) { return pww::tc::launch_stats<k.D, k.KC>(c, s); });
       if (e != cudaSuccess) return cuda_fail(e);
     }
     return PWW_OK;
@@ -147,13 +166,7 @@ int pww_xattn_fwd_f16(const void* q, const void* k, const void* v, void* out, in
       c.wmap_index = (p.wmap && p.wmap_index) ? p.wmap_index + b0 : nullptr;
       c.stats = p.stats ? p.stats + b0 : nullptr;
       if (p.wmap && !p.wmap_index) c.wmap = p.wmap + (int64_t)b0 * p.wmap_bs;   // identity mapping
-      cudaError_t e = cudaErrorInvalidValue;
-      switch (D) {
-        case 40: e = pww::tc::launch_fwd<40>(c, s); break;
-        case 64: e = pww::tc::launch_fwd<64>(c, s); break;
-        case 80: e = pww::tc::launch_fwd<80>(c, s); break;
-        case 160: e = pww::tc::launch_fwd<160>(c, s); break;
-      }
+      const cudaError_t e = with_shape(D, T, [&](auto k) { return pww::tc::launch_fwd<k.D, k.KC>(c, s); });
       if (e != cudaSuccess) return cuda_fail(e);
     }
     return PWW_OK;
@@ -213,16 +226,11 @@ int pww_xattn_fused_f16(const void* q, const void* k, const void* v, void* out, 
     } else if (mpack) {                                            // identity mapping: image b uses map b
       c.wmap_index = nullptr;
       mp = (const __half*)mpack + (int64_t)b0 * mpack_batch_stride;
-      ci = cidx + (int64_t)b0 * pww::fx::kTP;
+      ci = cidx + (int64_t)b0 * pww::fx::kTP * pww::core::chunks_of(T);   // [Bw, 80 k]
     }
     c.wmap = mpack ? (const float*)mp : nullptr;                   // non-null marks "maps present" for the kernel
-    cudaError_t e = cudaErrorInvalidValue;
-    switch (D) {
-      case 40: e = pww::fx2::launch_fused2<40>(c, mp, mpack_batch_stride, ci, s); break;
-      case 64: e = pww::fx2::launch_fused2<64>(c, mp, mpack_batch_stride, ci, s); break;
-      case 80: e = pww::fx2::launch_fused2<80>(c, mp, mpack_batch_stride, ci, s); break;
-      case 160: e = pww::fx2::launch_fused2<160>(c, mp, mpack_batch_stride, ci, s); break;
-    }
+    const cudaError_t e =
+        with_shape(D, T, [&](auto k) { return pww::fx2::launch_fused2<k.D, k.KC>(c, mp, mpack_batch_stride, ci, s); });
     if (e == cudaErrorInvalidConfiguration) return PWW_ERR_UNSUPPORTED;
     if (e != cudaSuccess) return cuda_fail(e);
   }

@@ -3,7 +3,7 @@
 // A CTA of 8 warps works on one [128-row x head] tile at a time; warp w owns query rows [16 w, 16 w + 16).  Operands are
 // staged in shared memory by 16-byte cp.async copies (rows of LD = DP + 8 halfs: the 16-byte pad makes every ldmatrix
 // phase hit 8 distinct bank groups), read into registers with ldmatrix and multiplied with mma.m16n8k16 (fp16 in, fp32
-// accumulate).  Cross-attention (keys T <= 80):
+// accumulate).  Cross-attention (keys T <= 80; longer contexts of 2 or 3 CLIP chunks stream one tile per chunk, below):
 //     S = Q K^T   16 x 80 per warp, DP / 16 k-steps      accumulators: 10 n-tiles x 4 fp32 per thread
 //     P = 2^(log2e * scale * (S + bias - rowmax))        in registers; packed to fp16 it is the A operand of
 //     O = P V     16 x D per warp, 5 k-steps over the 80 padded keys, V fragments by ldmatrix.trans
@@ -150,6 +150,98 @@ __device__ __forceinline__ void warp_store(const float (&o)[Tile<D>::NT][4], uns
           *reinterpret_cast<const uint4*>(stage + (r * C::LD + c * 8) * 2);
   }
   __syncwarp();
+}
+
+// ---- long contexts: k CLIP chunks of 77 keys (T = 154, 231) ----
+// Chunk c (keys 77 c .. 77 c + 76) is staged as its own 80-row K / V tile, rows 77 .. 79 zero-filled and masked to -inf,
+// so warp_qk runs unchanged on every chunk.  The softmax streams over the chunks (running row max and sum, O rescaled
+// when the max moves, as in attn_tc.cuh); P is packed to fp16 and the row sum is the sum of the fp16 P values that were
+// multiplied, rescaled in fp32.
+constexpr int kChunk = 77;      // keys per CLIP chunk
+constexpr int kMaxChunks = 3;
+__host__ __device__ __forceinline__ constexpr int chunks_of(int T) { return T <= kTP ? 1 : T / kChunk; }
+// T <= 80 (one tile) or a whole number of chunks, at most kMaxChunks.
+__host__ __device__ __forceinline__ constexpr bool supported_keys(int T) {
+  return T <= kTP || T == 2 * kChunk || T == kMaxChunks * kChunk;
+}
+
+template <int D>
+__device__ __forceinline__ void warp_online_begin(float (&o)[Tile<D>::NT][4], float& m0, float& m1, float& l0, float& l1) {
+#pragma unroll
+  for (int j = 0; j < Tile<D>::NT; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
+  m0 = m1 = -INFINITY;
+  l0 = l1 = 0.f;
+}
+
+// One chunk: s holds S + bias of the chunk's 80 padded keys, vs is its V tile.  l0 / l1 are per-thread partial row sums.
+template <int D>
+__device__ __forceinline__ void warp_online_chunk(float (&s)[10][4], float sl2, uint32_t vs, int lane,
+                                                  float (&o)[Tile<D>::NT][4], float& m0, float& m1, float& l0, float& l1) {
+  using C = Tile<D>;
+  float t0 = -INFINITY, t1 = -INFINITY;
+#pragma unroll
+  for (int j = 0; j < 10; ++j)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      if (tok(j, e, lane) >= kChunk) s[j][e] = -INFINITY;
+      if (e < 2) t0 = fmaxf(t0, s[j][e]); else t1 = fmaxf(t1, s[j][e]);
+    }
+  t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, 1));
+  t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, 2));
+  t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, 1));
+  t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, 2));
+  const float mn0 = fmaxf(m0, t0), mn1 = fmaxf(m1, t1);
+  const float a0 = ptx::ex2((m0 - mn0) * sl2), a1 = ptx::ex2((m1 - mn1) * sl2);   // 0 on the first chunk (m = -inf)
+  m0 = mn0; m1 = mn1;
+  const float n0 = -mn0 * sl2, n1 = -mn1 * sl2;
+  uint32_t pa[5][4];
+  float r0 = 0.f, r1 = 0.f;
+#pragma unroll
+  for (int j = 0; j < 10; ++j) {
+    const uint32_t p01 = ptx::pack_h2(ptx::ex2(fmaf(s[j][0], sl2, n0)), ptx::ex2(fmaf(s[j][1], sl2, n0)));
+    const uint32_t p23 = ptx::pack_h2(ptx::ex2(fmaf(s[j][2], sl2, n1)), ptx::ex2(fmaf(s[j][3], sl2, n1)));
+    const float2 f01 = ptx::unpack_h2(p01), f23 = ptx::unpack_h2(p23);    // sum exactly what the MMA multiplies
+    r0 += f01.x + f01.y;
+    r1 += f23.x + f23.y;
+    pa[j >> 1][(j & 1) * 2] = p01;
+    pa[j >> 1][(j & 1) * 2 + 1] = p23;
+  }
+  l0 = l0 * a0 + r0;
+  l1 = l1 * a1 + r1;
+#pragma unroll
+  for (int j = 0; j < C::NT; ++j) {
+    o[j][0] *= a0; o[j][1] *= a0; o[j][2] *= a1; o[j][3] *= a1;
+  }
+#pragma unroll
+  for (int kk = 0; kk < 5; ++kk) {
+    const int t = 16 * kk + (lane & 7) + ((lane >> 3) & 1) * 8;
+#pragma unroll
+    for (int jp = 0; jp < C::NT / 2; ++jp) {
+      uint32_t b0, b1, b2, b3;
+      ptx::ldsm_x4_t(vs + (uint32_t)(t * C::LD + 16 * jp + (lane >> 4) * 8) * 2u, b0, b1, b2, b3);
+      ptx::mma16816(o[2 * jp], pa[kk], b0, b1);
+      ptx::mma16816(o[2 * jp + 1], pa[kk], b2, b3);
+    }
+    if constexpr (C::NT & 1) {
+      uint32_t b0, b1;
+      ptx::ldsm_x2_t(vs + (uint32_t)(t * C::LD + 8 * (C::NT - 1)) * 2u, b0, b1);
+      ptx::mma16816(o[C::NT - 1], pa[kk], b0, b1);
+    }
+  }
+}
+
+// Divides O by the row sums (reduced over the quad) once every chunk has been accumulated.
+template <int D>
+__device__ __forceinline__ void warp_online_end(float (&o)[Tile<D>::NT][4], float l0, float l1) {
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float i0 = 1.f / l0, i1 = 1.f / l1;
+#pragma unroll
+  for (int j = 0; j < Tile<D>::NT; ++j) {
+    o[j][0] *= i0; o[j][1] *= i0; o[j][2] *= i1; o[j][3] *= i1;
+  }
 }
 
 // Statistic partials of S over the warp's valid elements (row < N, token < T): running max of S (rounding to fp16 is

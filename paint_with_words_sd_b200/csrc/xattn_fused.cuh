@@ -30,7 +30,7 @@ constexpr int kRC = 10;           // dictionary capacity (distinct non-zero colu
 
 struct FxParams {
   XattnParams x;            // q/k/v/out, strides, wmap_index, g_sigma, scale, stat, stats_out, counters, partials
-  const int8_t* cidx;       // [Bw, 80] dictionary column per token, -1 = none
+  const int8_t* cidx;       // [Bw, 80 k] dictionary column per token (k key chunks; token 77 c + j at 80 c + j), -1 = none
   const void* mpack;        // [Bw, N, 32] fp16 packed maps (see above)
   int64_t mpack_bs;         // elements
   int tiles, units;

@@ -1,4 +1,5 @@
-// Paint-with-Words cross-attention in ONE launch (statistic + bias + softmax + P.V) on Hopper tensor cores, keys T <= 80.
+// Paint-with-Words cross-attention in ONE launch (statistic + bias + softmax + P.V) on Hopper tensor cores, keys T <= 80
+// or 2 / 3 CLIP chunks of 77 (T = 154, 231).
 //
 // The per-image statistic (max or std of Q K^T over all heads, rows and tokens) is a grid-wide dependency of every
 // biased score, so the kernel is a persistent cooperative launch (one CTA per SM, all co-resident) that runs three passes
@@ -12,6 +13,11 @@
 // Work unit = (image, 128-row tile, group of G heads); a unit expands into one job per head.  Each job is computed by the
 // 8 warps of the CTA with the warp-level MMA tiles of xattn_core.cuh; the cp.async copies of job i + 1 (Q rows, K, V
 // and, for biased softmax jobs, the row tile's packed map) are in flight while job i is computed.
+//
+// Long contexts (KC = 2 or 3 chunks): a stage holds one 80-row K and V tile per chunk; a job loops over the chunks
+// (statistic: S of every chunk; softmax: per-chunk bias and the streaming softmax of xattn_core.cuh).  Where two such
+// stages do not fit in shared memory (head dim 80 at 3 chunks, head dim 160 at 2 and 3) the kernel runs on one stage and
+// the copies of job i + 1 start once job i is done.  The unit and job order do not depend on KC.
 #pragma once
 #include "mma_sm90.cuh"
 #include "pww_common.cuh"
@@ -23,15 +29,16 @@ namespace pww {
 namespace fx2 {
 using namespace fx;   // unit walk, helpers and constants shared with the host replay
 
-template <int D>
+template <int D, int KC = 1>
 struct Cfg2 {
   // heads per unit (the granularity of a CTA's range): 2 at head dims 40 and 64, one head at 80 and 160
   static constexpr int G = (D == 40 || D == 64) ? 2 : 1;
   using T_ = core::Tile<D>;
   static constexpr uint32_t MBYTES = kBM * kMW * 2;                    // packed-map rows of the row tile
-  static constexpr uint32_t OFF_M = T_::QBYTES + 2 * T_::KBYTES;
-  static constexpr uint32_t STAGE = OFF_M + MBYTES;                    // Q | K | V | map of one job
-  static constexpr uint32_t SMEM = 2 * STAGE;
+  static constexpr uint32_t OFF_M = T_::QBYTES + 2 * KC * T_::KBYTES;
+  static constexpr uint32_t STAGE = OFF_M + MBYTES;                    // Q | K chunks | V chunks | map of one job
+  static constexpr int NST = (2 * STAGE + 8192 <= 232448) ? 2 : 1;     // stages (see the header)
+  static constexpr uint32_t SMEM = NST * STAGE;
   static_assert(SMEM + 8192 <= 232448, "shared memory budget (dynamic + ~7 KB of static tables incl. the 4 KB job table)");
 };
 
@@ -127,10 +134,11 @@ __device__ __forceinline__ float key_f32(unsigned k) {
   return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
 }
 
-template <int D>
+template <int D, int KC>
 __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const FxParams fp) {
   using C = core::Tile<D>;
-  using CF = Cfg2<D>;
+  using CF = Cfg2<D, KC>;
+  constexpr int CW = kTP * KC;                     // cidx columns: token 77 c + j of chunk c at column 80 c + j
   const XattnParams& p = fp.x;
   extern __shared__ __align__(128) unsigned char smem[];
   const uint32_t smem0 = ptx::smem_u32(smem);
@@ -150,7 +158,7 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
   __shared__ uint2 s_jobs[kMaxJobs];
   __shared__ uint4 s_unit[kMaxUnits];              // job-table build scratch: one entry per unit of the range
   __shared__ int s_expect[kMaxLocal];              // CTAs that publish a partial for each local biased image
-  __shared__ signed char s_cidx[kMaxLocal][kTP];   // token -> dictionary column of the CTA's local biased images
+  __shared__ signed char s_cidx[kMaxLocal][CW];    // token -> dictionary column of the CTA's local biased images
 
   if (warp == 0) {
     // ---- stable partition of the images by "has a weight map" ----
@@ -256,22 +264,29 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
       if (lane == 0) s_expect[l] = e;
     }
   } else if (warp == 2) {
-    for (int idx = lane; idx < nl * kTP && idx < kMaxLocal * kTP; idx += 32) {
-      const int l = idx / kTP, t = idx - l * kTP;
-      s_cidx[l][t] = (t < T) ? fp.cidx[(int64_t)s_widx[s_lb[l]] * kTP + t] : (signed char)-1;
+    for (int idx = lane; idx < nl * CW && idx < kMaxLocal * CW; idx += 32) {
+      const int l = idx / CW, t = idx - l * CW;
+      const bool real = KC == 1 ? t < T : t % kTP < core::kChunk;
+      s_cidx[l][t] = real ? fp.cidx[(int64_t)s_widx[s_lb[l]] * CW + t] : (signed char)-1;
     }
   }
 
-  // the copies of job i into stage i % 2
+  // the copies of job i into stage i % 2 (stage 0 when there is one)
+  auto stage = [&](int i) { return (uint32_t)(CF::NST == 2 ? (i & 1) : 0) * CF::STAGE; };
   auto issue = [&](int i) {
     const uint2 r = s_jobs[i];
     const int b = r.x & 0xff, h = (r.x >> 8) & 0xff, tile = r.x >> 16;
     const bool is_main = (r.y & JF_MAIN) != 0, biased = (r.y & JF_BIASED) != 0;
-    const uint32_t st = smem0 + (i & 1) * CF::STAGE;
+    const uint32_t st = smem0 + stage(i);
     const int rows = p.N - tile * kBM < kBM ? p.N - tile * kBM : kBM;
     core::load_rows<D>(st, p.q + (int64_t)b * p.q_bs + (int64_t)tile * kBM * p.q_rs + h * D, p.q_rs, kBM, rows);
-    core::load_rows<D>(st + C::QBYTES, p.k + (int64_t)b * p.k_bs + h * D, p.k_rs, kTP, T);
-    if (is_main) core::load_rows<D>(st + C::QBYTES + C::KBYTES, p.v + (int64_t)b * p.k_bs + h * D, p.k_rs, kTP, T);
+    const int kv = KC == 1 ? T : core::kChunk;
+#pragma unroll 1
+    for (int c = 0; c < KC; ++c) {
+      const int64_t off = (int64_t)b * p.k_bs + (int64_t)c * core::kChunk * p.k_rs + h * D;
+      core::load_rows<D>(st + C::QBYTES + c * C::KBYTES, p.k + off, p.k_rs, kTP, kv);
+      if (is_main) core::load_rows<D>(st + C::QBYTES + (KC + c) * C::KBYTES, p.v + off, p.k_rs, kTP, kv);
+    }
     if (is_main && biased) {
       const __half* mp = reinterpret_cast<const __half*>(fp.mpack) + (int64_t)s_widx[b] * fp.mpack_bs + (int64_t)tile * kBM * kMW;
       for (int idx = threadIdx.x; idx < kBM * (kMW / 8); idx += blockDim.x) {
@@ -311,10 +326,15 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
   if (njobs > 0) issue(0);
 #pragma unroll 1
   for (int i = 0; i < njobs; ++i) {
-    if (i + 1 < njobs) {
-      issue(i + 1);
-      ptx::cp_async_wait<1>();
-    } else {
+    if constexpr (CF::NST == 2) {
+      if (i + 1 < njobs) {
+        issue(i + 1);
+        ptx::cp_async_wait<1>();
+      } else {
+        ptx::cp_async_wait<0>();
+      }
+    } else {                                        // one stage: job i - 1 is done with it (barrier at the loop's end)
+      if (i > 0) issue(i);
       ptx::cp_async_wait<0>();
     }
     __syncthreads();
@@ -404,8 +424,53 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
     const int b = r.x & 0xff, h = (r.x >> 8) & 0xff, tile = r.x >> 16;
     const bool is_main = (r.y & JF_MAIN) != 0, biased = (r.y & JF_BIASED) != 0;
     const int li = (r.y >> 4) & 3;
-    const uint32_t st = smem0 + (i & 1) * CF::STAGE;
+    const uint32_t st = smem0 + stage(i);
     const int row0 = tile * kBM + warp * 16;
+    if constexpr (KC > 1) {
+      const uint32_t qs = st + (uint32_t)(warp * 16 * C::LD) * 2u;
+      if (!is_main) {
+        if (li != cur_li) { flush(); cur_li = li; }
+        float sum = 0.f, sumsq = 0.f;
+#pragma unroll 1
+        for (int c = 0; c < KC; ++c) {              // the real tokens of every chunk
+          float s[10][4];
+          core::warp_qk<D>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
+          core::warp_stat(s, core::kChunk, p.N - row0, lane, is_max, vmax, sum, sumsq);
+        }
+        dsum += (double)sum;
+        dsq += (double)sumsq;
+        if (i == ns - 1) flush();
+      } else {
+        const float x = biased ? s_coef[li] : 0.f;
+        const __half* mrow = reinterpret_cast<const __half*>(smem + stage(i) + CF::OFF_M) + (warp * 16 + (lane >> 2)) * kMW;
+        float o[C::NT][4], m0, m1, l0, l1;
+        core::warp_online_begin<D>(o, m0, m1, l0, l1);
+#pragma unroll 1
+        for (int c = 0; c < KC; ++c) {
+          float s[10][4];
+          core::warp_qk<D>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
+          if (biased) {
+            const signed char* ci = s_cidx[li] + c * kTP;
+#pragma unroll
+            for (int j = 0; j < 10; ++j)
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const int cc = ci[core::tok(j, e, lane)];
+                if (cc >= 0) {
+                  const __half* mr = mrow + (e >> 1) * 8 * kMW;
+                  s[j][e] = fmaf(x, __half2float(mr[cc]) + __half2float(mr[kRC + cc]), s[j][e]);
+                }
+              }
+          }
+          core::warp_online_chunk<D>(s, sl2, st + C::QBYTES + (KC + c) * C::KBYTES, lane, o, m0, m1, l0, l1);
+        }
+        core::warp_online_end<D>(o, l0, l1);
+        core::warp_store<D>(o, smem + stage(i) + warp * 16 * C::LD * 2, lane, p.out + (int64_t)b * p.o_bs + h * D, p.o_rs,
+                            row0, p.N);
+      }
+      __syncthreads();
+      continue;
+    }
     float s[10][4];
     core::warp_qk<D>(st + (uint32_t)(warp * 16 * C::LD) * 2u, st + C::QBYTES, lane, s);
     if (!is_main) {
@@ -463,9 +528,9 @@ inline bool fused2_fits(int B, int hg, int tiles, int grid) {
   return fused_range_ok(B, hg, tiles, grid) && fused_units_ok(units, grid) && (units + grid - 1) / grid + 1 <= kMaxUnits;
 }
 
-template <int D>
+template <int D, int KC>
 cudaError_t launch_fused2(const XattnParams& x, const void* mpack, int64_t mpack_bs, const int8_t* cidx, cudaStream_t s) {
-  using CF = Cfg2<D>;
+  using CF = Cfg2<D, KC>;
   FxParams fp;
   memset(&fp, 0, sizeof(fp));
   fp.x = x;
@@ -480,7 +545,7 @@ cudaError_t launch_fused2(const XattnParams& x, const void* mpack, int64_t mpack
   if (!fused2_fits(x.B, fp.hg, fp.tiles, fp.grid)) return cudaErrorInvalidConfiguration;
   static bool attr_set[tc::kMaxDevices] = {false};
   if (!attr_set[tc::cur_device()]) {
-    cudaError_t e = cudaFuncSetAttribute(xattn_fused2_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, CF::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(xattn_fused2_kernel<D, KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, CF::SMEM);
     if (e != cudaSuccess) return e;
     attr_set[tc::cur_device()] = true;
   }
@@ -495,7 +560,7 @@ cudaError_t launch_fused2(const XattnParams& x, const void* mpack, int64_t mpack
   attr[0].val.cooperative = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, xattn_fused2_kernel<D>, fp);
+  return cudaLaunchKernelEx(&cfg, xattn_fused2_kernel<D, KC>, fp);
 }
 
 // Host replay of the job lists (test infrastructure): out[job] = {cta, i, kind, m, b, h, tile, biased, li, gi, up, ul,

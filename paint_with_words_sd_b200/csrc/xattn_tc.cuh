@@ -1,6 +1,7 @@
-// Paint-with-Words cross-attention on Hopper tensor cores (sm_90a), keys T <= 80: the two-launch pair that takes the
-// reference's dense [N, T] fp32 weight map (maps with more than 10 distinct columns cannot be packed for the one-launch
-// kernel of xattn_fused2.cuh).
+// Paint-with-Words cross-attention on Hopper tensor cores (sm_90a), keys T <= 80 or 2 / 3 CLIP chunks (T = 154, 231):
+// the two-launch pair that takes the reference's dense [N, T] fp32 weight map (maps with more than 10 distinct columns
+// cannot be packed for the one-launch kernel of xattn_fused2.cuh).  KC = chunks of the key sequence: each chunk is one
+// 80-row K / V tile of the stage, and the softmax streams over them (xattn_core.cuh).
 //
 // Fused region of the reference's inj_forward (paint_with_words.py:87-118), per image b / head h / 128-row tile:
 //     statistics kernel:  per-image max / (sum, sumsq) of fp16(Q_h K_h^T) over all heads, rows and tokens
@@ -27,11 +28,13 @@ constexpr int kThreads = core::kThreads;
 constexpr int kMaxBatch = 256;   // images per launch (the C ABI splits larger batches)
 constexpr int kMaxLocal = 4;     // images one CTA's unit range can touch: B/132 + 2 <= 4 for B <= 256
 
-template <int D>
+template <int D, int KC = 1>
 struct Cfg {
   using T_ = core::Tile<D>;
-  static constexpr uint32_t STAGE = T_::QBYTES + 2 * T_::KBYTES;   // Q | K | V of one unit
-  static constexpr uint32_t SMEM = 2 * STAGE;
+  static constexpr uint32_t STAGE = T_::QBYTES + 2 * KC * T_::KBYTES;   // Q | K chunks | V chunks of one unit
+  // two stages (the copies of unit i + 1 overlap unit i) where they fit; one at the long contexts of head dim 160
+  static constexpr int NST = (2 * STAGE <= 232448 - 8192) ? 2 : 1;
+  static constexpr uint32_t SMEM = NST * STAGE;
   static_assert(SMEM <= 232448 - 8192, "shared memory budget (dynamic + static tables)");
 };
 
@@ -143,23 +146,29 @@ __device__ __forceinline__ int image_widx(const XattnParams& p, int b) {
   return p.wmap_index ? p.wmap_index[b] : b;
 }
 
-// Copies of one unit's operands into a stage: Q rows of the tile, K (and V) rows of the head.
-template <int D>
+// Copies of one unit's operands into a stage: Q rows of the tile, K (and V) rows of the head, one 80-row tile per chunk.
+template <int D, int KC>
 __device__ __forceinline__ void load_unit(uint32_t st, const XattnParams& p, int b, int h, int tile, bool with_v) {
   using C = core::Tile<D>;
   const int rows = p.N - tile * kBM;
   core::load_rows<D>(st, p.q + (int64_t)b * p.q_bs + (int64_t)tile * kBM * p.q_rs + h * D, p.q_rs, kBM, rows < kBM ? rows : kBM);
-  core::load_rows<D>(st + C::QBYTES, p.k + (int64_t)b * p.k_bs + h * D, p.k_rs, kTP, p.T);
-  if (with_v) core::load_rows<D>(st + C::QBYTES + C::KBYTES, p.v + (int64_t)b * p.k_bs + h * D, p.k_rs, kTP, p.T);
+  const int kv = KC == 1 ? p.T : core::kChunk;
+#pragma unroll 1
+  for (int c = 0; c < KC; ++c) {
+    const int64_t off = (int64_t)b * p.k_bs + (int64_t)c * core::kChunk * p.k_rs + h * D;
+    core::load_rows<D>(st + C::QBYTES + c * C::KBYTES, p.k + off, p.k_rs, kTP, kv);
+    if (with_v) core::load_rows<D>(st + C::QBYTES + (KC + c) * C::KBYTES, p.v + off, p.k_rs, kTP, kv);
+  }
   ptx::cp_async_commit();
 }
 
 // ---------------------------------------------------------------------------------------------------------
 // forward kernel
 // ---------------------------------------------------------------------------------------------------------
-template <int D>
+template <int D, int KC>
 __global__ void __launch_bounds__(kThreads, 1) xattn_fwd_kernel(const TcParams tp) {
   using C = core::Tile<D>;
+  using CF = Cfg<D, KC>;
   const XattnParams& p = tp.x;
   extern __shared__ __align__(128) unsigned char smem[];
   const uint32_t smem0 = ptx::smem_u32(smem);
@@ -201,24 +210,55 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_fwd_kernel(const TcParams t
   const float sl2 = p.scale * 1.4426950408889634f;
   FwdWalk w(u0, p.B, p.H, s_nb, s_img);
   FwdUnit nxt = w.get();
-  load_unit<D>(smem0, p, nxt.b, nxt.h, nxt.tile, true);
+  load_unit<D, KC>(smem0, p, nxt.b, nxt.h, nxt.tile, true);
   for (int it = 0; it < n_it; ++it) {
     const FwdUnit f = nxt;
-    if (it + 1 < n_it) {
-      w.next();
-      nxt = w.get();
-      load_unit<D>(smem0 + ((it + 1) & 1) * Cfg<D>::STAGE, p, nxt.b, nxt.h, nxt.tile, true);
-      ptx::cp_async_wait<1>();
-    } else {
+    if constexpr (CF::NST == 2) {
+      if (it + 1 < n_it) {
+        w.next();
+        nxt = w.get();
+        load_unit<D, KC>(smem0 + ((it + 1) & 1) * CF::STAGE, p, nxt.b, nxt.h, nxt.tile, true);
+        ptx::cp_async_wait<1>();
+      } else {
+        ptx::cp_async_wait<0>();
+      }
+    } else {                                       // one stage: refilled once the previous unit is done with it
+      if (it > 0) load_unit<D, KC>(smem0, p, f.b, f.h, f.tile, true);
       ptx::cp_async_wait<0>();
+      if (it + 1 < n_it) { w.next(); nxt = w.get(); }
     }
     __syncthreads();
-    const uint32_t st = smem0 + (it & 1) * Cfg<D>::STAGE;
+    const uint32_t st = smem0 + (CF::NST == 2 ? (it & 1) : 0) * CF::STAGE;
     const uint32_t qs = st + (uint32_t)(warp * 16 * C::LD) * 2u;
-    float s[10][4];
-    core::warp_qk<D>(qs, st + C::QBYTES, lane, s);
     const int row0 = f.tile * kBM + warp * 16;
     const int widx = s_widx[f.b];
+    if constexpr (KC > 1) {
+      float o[C::NT][4], m0, m1, l0, l1;
+      core::warp_online_begin<D>(o, m0, m1, l0, l1);
+#pragma unroll 1
+      for (int c = 0; c < KC; ++c) {
+        float s[10][4];
+        core::warp_qk<D>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
+        if (widx >= 0) {
+          const float x = s_coef[f.b];
+          const float* wm = p.wmap + (int64_t)widx * p.wmap_bs + c * core::kChunk;   // chunk c, slot t = column 77 c + t
+#pragma unroll
+          for (int j = 0; j < 10; ++j)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const int t = core::tok(j, e, lane), r = row0 + (lane >> 2) + (e >> 1) * 8;
+              if (t < core::kChunk && r < p.N) s[j][e] = fmaf(x, __ldg(wm + (int64_t)r * p.T + t), s[j][e]);
+            }
+        }
+        core::warp_online_chunk<D>(s, sl2, st + C::QBYTES + (KC + c) * C::KBYTES, lane, o, m0, m1, l0, l1);
+      }
+      core::warp_online_end<D>(o, l0, l1);
+      core::warp_store<D>(o, smem + (st - smem0) + warp * 16 * C::LD * 2, lane, p.out + (int64_t)f.b * p.o_bs + f.h * D, p.o_rs, row0, p.N);
+      __syncthreads();
+      continue;
+    }
+    float s[10][4];
+    core::warp_qk<D>(qs, st + C::QBYTES, lane, s);
     if (widx >= 0) {
       const float x = s_coef[f.b];
       const float* wm = p.wmap + (int64_t)widx * p.wmap_bs;
@@ -232,7 +272,7 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_fwd_kernel(const TcParams t
     }
     float o[C::NT][4];
     core::warp_softmax_pv<D>(s, p.T, sl2, st + C::QBYTES + C::KBYTES, lane, o);
-    core::warp_store<D>(o, smem + (it & 1) * Cfg<D>::STAGE + warp * 16 * C::LD * 2, lane,
+    core::warp_store<D>(o, smem + (it & 1) * CF::STAGE + warp * 16 * C::LD * 2, lane,
                         p.out + (int64_t)f.b * p.o_bs + f.h * D, p.o_rs, row0, p.N);
     __syncthreads();
   }
@@ -241,9 +281,10 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_fwd_kernel(const TcParams t
 // ---------------------------------------------------------------------------------------------------------
 // statistics kernel: per-image max / (sum, sumsq) of fp16(S) over all heads, rows and tokens
 // ---------------------------------------------------------------------------------------------------------
-template <int D>
+template <int D, int KC>
 __global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams tp) {
   using C = core::Tile<D>;
+  using CF = Cfg<D, KC>;
   const XattnParams& p = tp.x;
   extern __shared__ __align__(128) unsigned char smem[];
   const uint32_t smem0 = ptx::smem_u32(smem);
@@ -290,25 +331,29 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams
     int it_n = 0;
     auto advance = [&]() { while (it_n < n_it && skip(nxt.b)) { nxt.next(); ++it_n; } };
     advance();
-    if (it_n < n_it) load_unit<D>(smem0, p, nxt.b, nxt.h, nxt.tile, false);
+    if (it_n < n_it) load_unit<D, KC>(smem0, p, nxt.b, nxt.h, nxt.tile, false);
     for (int k = 0; it_n < n_it; ++k) {
-      const int b = nxt.b, tile = nxt.tile;
+      const int b = nxt.b, h = nxt.h, tile = nxt.tile;
+      if (CF::NST == 1 && k > 0) load_unit<D, KC>(smem0, p, b, h, tile, false);   // one stage: refilled here
       nxt.next();
       ++it_n;
       advance();
-      if (it_n < n_it) {
-        load_unit<D>(smem0 + ((k + 1) & 1) * Cfg<D>::STAGE, p, nxt.b, nxt.h, nxt.tile, false);
+      if (CF::NST == 2 && it_n < n_it) {
+        load_unit<D, KC>(smem0 + ((k + 1) & 1) * CF::STAGE, p, nxt.b, nxt.h, nxt.tile, false);
         ptx::cp_async_wait<1>();
       } else {
         ptx::cp_async_wait<0>();
       }
       __syncthreads();
       if (b != cur_b) { flush(); cur_b = b; }
-      const uint32_t st = smem0 + (k & 1) * Cfg<D>::STAGE;
-      float s[10][4];
-      core::warp_qk<D>(st + (uint32_t)(warp * 16 * C::LD) * 2u, st + C::QBYTES, lane, s);
+      const uint32_t st = smem0 + (CF::NST == 2 ? (k & 1) : 0) * CF::STAGE;
       float sum = 0.f, sumsq = 0.f;
-      core::warp_stat(s, p.T, p.N - tile * kBM - warp * 16, lane, is_max, vmax, sum, sumsq);
+#pragma unroll 1
+      for (int c = 0; c < KC; ++c) {                // the real tokens of every chunk
+        float s[10][4];
+        core::warp_qk<D>(st + (uint32_t)(warp * 16 * C::LD) * 2u, st + C::QBYTES + c * C::KBYTES, lane, s);
+        core::warp_stat(s, KC == 1 ? p.T : core::kChunk, p.N - tile * kBM - warp * 16, lane, is_max, vmax, sum, sumsq);
+      }
       dsum += (double)sum;
       dsq += (double)sumsq;
       __syncthreads();
@@ -440,30 +485,30 @@ cudaError_t set_smem(const void* fn, uint32_t bytes, bool (&done)[kMaxDevices]) 
   return e;
 }
 
-template <int D>
+template <int D, int KC>
 cudaError_t launch_fwd(const XattnParams& x, cudaStream_t s) {
   TcParams tp;
   tp.x = x;
   tp.tiles = ceil_div(x.N, kBM);
   tp.units = x.B * tp.tiles * x.H;
   static bool attr_set[kMaxDevices] = {false};
-  cudaError_t e = set_smem<D>((const void*)xattn_fwd_kernel<D>, Cfg<D>::SMEM, attr_set);
+  cudaError_t e = set_smem<D>((const void*)xattn_fwd_kernel<D, KC>, Cfg<D, KC>::SMEM, attr_set);
   if (e != cudaSuccess) return e;
   const int grid = tp.units < num_sms() ? tp.units : num_sms();
-  xattn_fwd_kernel<D><<<grid, kThreads, Cfg<D>::SMEM, s>>>(tp);
+  xattn_fwd_kernel<D, KC><<<grid, kThreads, Cfg<D, KC>::SMEM, s>>>(tp);
   return cudaGetLastError();
 }
 
-template <int D>
+template <int D, int KC>
 cudaError_t launch_stats(const XattnParams& x, cudaStream_t s) {
   TcParams tp;
   tp.x = x;
   tp.tiles = ceil_div(x.N, kBM);
   tp.units = x.B * tp.tiles * x.H;
   static bool attr_set[kMaxDevices] = {false};
-  cudaError_t e = set_smem<D>((const void*)xattn_stats_kernel<D>, Cfg<D>::SMEM, attr_set);
+  cudaError_t e = set_smem<D>((const void*)xattn_stats_kernel<D, KC>, Cfg<D, KC>::SMEM, attr_set);
   if (e != cudaSuccess) return e;
-  xattn_stats_kernel<D><<<stats_grid(tp.units), kThreads, Cfg<D>::SMEM, s>>>(tp);
+  xattn_stats_kernel<D, KC><<<stats_grid(tp.units), kThreads, Cfg<D, KC>::SMEM, s>>>(tp);
   return cudaGetLastError();
 }
 

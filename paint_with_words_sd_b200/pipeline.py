@@ -170,9 +170,13 @@ class PwWSampler:
         return torch.tensor(rows, dtype=torch.float32)
 
     def _merge_contexts(self, conds, unconds) -> dict:
-        """Batch the per-image dicts: CONTEXT_TENSOR -> [2m,77,Dc]; weight maps -> [m,N,77] stacks;
+        """Batch the per-image dicts: CONTEXT_TENSOR -> [2m,T,Dc]; weight maps -> [m,N,T] stacks;
         WMAP_INDEX = [0..m-1, -1 x m]."""
         m = self.m
+        lengths = {int(c["CONTEXT_TENSOR"].shape[1]) for c in list(conds) + list(unconds)}
+        if len(lengths) != 1:
+            raise ValueError(f"all images of a sampler need the same text length (got T = {sorted(lengths)}); encode them "
+                             "with the same max_prompt_chunks or use one sampler per length")
         ctx = {"CONTEXT_TENSOR": torch.cat([c["CONTEXT_TENSOR"] for c in conds] +
                                            [u["CONTEXT_TENSOR"] for u in unconds], 0).to(self.device)}
         for key in conds[0]:
@@ -329,15 +333,19 @@ def paint_with_words(
     init_image: Optional[Image.Image] = None,
     strength: float = 0.5,
     return_latents: bool = False,
+    max_prompt_chunks: int = 1,
 ):
-    """paint_with_words.py:391-510.  Returns one PIL.Image (or the final latents with return_latents)."""
+    """paint_with_words.py:391-510.  Returns one PIL.Image (or the final latents with return_latents).
+    `max_prompt_chunks` (1 .. 3): a prompt longer than 75 tokens fills up to that many 77-token CLIP chunks instead of
+    being truncated (conditioning.chunk_prompt); 1 is the reference's behaviour."""
     width, height = color_map_image.size
     vae, unet, text_encoder, tokenizer, scheduler = (
         pww_load_tools(device, scheduler_type, local_model_path=local_model_path, hf_model_path=hf_model_path,
                        model_token=model_token)
         if preloaded_utils is None else preloaded_utils)
     extra_seeds, seperated_word_contexts, cond, uncond = _encode_text_color_inputs(
-        text_encoder, tokenizer, device, color_map_image, color_context, input_prompt, unconditional_input_prompt)
+        text_encoder, tokenizer, device, color_map_image, color_context, input_prompt, unconditional_input_prompt,
+        max_prompt_chunks=max_prompt_chunks)
 
     scheduler.set_timesteps(num_inference_steps)
     timesteps = scheduler.timesteps
@@ -410,8 +418,10 @@ def paint_with_words_inpaint(
     model_token: Optional[str] = None,
     strength: float = 1.0,
     return_latents: bool = False,
+    max_prompt_chunks: int = 1,
 ):
-    """paint_with_words_inpaint.py:137-270: 9-channel UNet input cat[latents, mask, masked-image latents]."""
+    """paint_with_words_inpaint.py:137-270: 9-channel UNet input cat[latents, mask, masked-image latents].
+    `max_prompt_chunks` as in `paint_with_words`."""
     vae, unet, text_encoder, tokenizer, scheduler = (
         pww_load_tools(device, scheduler_type, local_model_path=local_model_path, hf_model_path=hf_model_path,
                        model_token=model_token)
@@ -420,7 +430,8 @@ def paint_with_words_inpaint(
     color_map_image = color_map_image.resize((width, height), Image.NEAREST)
     mask_image = mask_image.resize((width, height), Image.NEAREST)
     _, _, cond, uncond = _encode_text_color_inputs(
-        text_encoder, tokenizer, device, color_map_image, color_context, input_prompt, unconditional_input_prompt)
+        text_encoder, tokenizer, device, color_map_image, color_context, input_prompt, unconditional_input_prompt,
+        max_prompt_chunks=max_prompt_chunks)
     mask, masked_image = prepare_mask_and_masked_image(init_image, mask_image)
 
     scheduler.set_timesteps(num_inference_steps)
@@ -515,8 +526,10 @@ class PaintWithWord_StableDiffusionPipeline:
     def __call__(self, prompt, color_map_image=None, color_context={}, weight_function: Callable = default_weight_function,
                  height=None, width=None, num_inference_steps: int = 30, guidance_scale: float = 7.5, negative_prompt="",
                  num_images_per_prompt: int = 1, eta: float = 0.5, seed: int = 0, generator=None, image=None, latents=None,
-                 output_type: str = "pil", return_dict: bool = True, callback=None, callback_steps: int = 1):
+                 output_type: str = "pil", return_dict: bool = True, callback=None, callback_steps: int = 1,
+                 max_prompt_chunks: int = 1):
         extra = {} if image is None else {"init_image": image, "strength": eta}
+        extra["max_prompt_chunks"] = max_prompt_chunks
         return self._run(paint_with_words, prompt, color_map_image, dict(color_context), weight_function,
                          num_inference_steps, guidance_scale, negative_prompt, seed, output_type, return_dict, callback,
                          callback_steps, **extra)
@@ -535,7 +548,9 @@ class PaintWithWord_StableDiffusionInpaintPipeline(PaintWithWord_StableDiffusion
                  weight_function: Callable = default_weight_function, height=None, width=None,
                  num_inference_steps: int = 30, guidance_scale: float = 7.5, negative_prompt="",
                  num_images_per_prompt: int = 1, eta: float = 1.0, seed: int = 0, generator=None, latents=None,
-                 output_type: str = "pil", return_dict: bool = True, callback=None, callback_steps: int = 1):
+                 output_type: str = "pil", return_dict: bool = True, callback=None, callback_steps: int = 1,
+                 max_prompt_chunks: int = 1):
         return self._run(paint_with_words_inpaint, prompt, color_map_image, dict(color_context), weight_function,
                          num_inference_steps, guidance_scale, negative_prompt, seed, output_type, return_dict, callback,
-                         callback_steps, mask_image=mask_image, init_image=image, strength=eta)
+                         callback_steps, mask_image=mask_image, init_image=image, strength=eta,
+                         max_prompt_chunks=max_prompt_chunks)

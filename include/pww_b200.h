@@ -133,6 +133,40 @@ int pww_xattn_fused_f16(const void* q, const void* k, const void* v, void* out,
                         float* stats, void* workspace, size_t workspace_bytes, void* stream);
 
 /*
+ * Per-image settings: the three calls above with a statistic kind and a G(sigma) for EACH image, so one launch serves a
+ * batch of images made with different weight functions (max / std, different strengths or sigma exponents).  Same
+ * arguments and rules as the twin without `_multi` (key lengths, head dims, batch splits, workspace), except:
+ *   stat    : [B] int32 device array instead of one int; entry b is image b's kind.  PWW_STAT_STD means std, any
+ *             other value means max.
+ *   g_sigma : [B] fp32 device array instead of one element; entry b is image b's G(sigma).
+ * Entry b belongs to image b of the call; entries of images with wmap_index[b] < 0 are ignored.  A NULL `stat` or
+ * `g_sigma` array where a map is given returns PWW_ERR_BAD_ARG (pww_xattn_stats_multi_f16 always needs `stat`).
+ * With every kind equal and every G equal, the results are bit-identical to the twin's.
+ */
+int pww_xattn_stats_multi_f16(const void* q, const void* k,
+                              int B, int H, int N, int T, int D,
+                              int64_t q_batch_stride, int64_t q_row_stride,
+                              int64_t k_batch_stride, int64_t k_row_stride,
+                              const int32_t* stat, const int32_t* wmap_index,
+                              float* stats /* [B] out */,
+                              void* workspace, size_t workspace_bytes, void* stream);
+int pww_xattn_fwd_multi_f16(const void* q, const void* k, const void* v, void* out,
+                            int B, int H, int N, int T, int D,
+                            int64_t q_batch_stride, int64_t q_row_stride,
+                            int64_t k_batch_stride, int64_t k_row_stride,
+                            int64_t o_batch_stride, int64_t o_row_stride,
+                            const float* wmap, int64_t wmap_batch_stride, const int32_t* wmap_index,
+                            const float* stats, const float* g_sigma, float scale, void* stream);
+int pww_xattn_fused_multi_f16(const void* q, const void* k, const void* v, void* out,
+                              int B, int H, int N, int T, int D,
+                              int64_t q_batch_stride, int64_t q_row_stride,
+                              int64_t k_batch_stride, int64_t k_row_stride,
+                              int64_t o_batch_stride, int64_t o_row_stride,
+                              const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+                              const int32_t* wmap_index, const int32_t* stat, const float* g_sigma, float scale,
+                              float* stats, void* workspace, size_t workspace_bytes, void* stream);
+
+/*
  * Self-attention through the same patched function (context=None, paint_with_words.py:71-72):
  *   out = softmax(scale * Q_h K_h^T) V_h  with keys/values [B, N, H*D]; no bias; online softmax.
  */

@@ -18,6 +18,7 @@ EXPORTS = (
     "pww_version", "pww_status_str", "pww_last_cuda_error", "pww_device_supported",
     "pww_xattn_workspace_bytes", "pww_xattn_stats_f16", "pww_xattn_fwd_f16", "pww_attn_fwd_f16",
     "pww_xattn_fused_workspace_bytes", "pww_xattn_fused_f16",
+    "pww_xattn_stats_multi_f16", "pww_xattn_fwd_multi_f16", "pww_xattn_fused_multi_f16",
     "pww_groupnorm_workspace_bytes", "pww_groupnorm_nhwc_f16", "pww_geglu_f16", "pww_add_layernorm_f16",
 )
 
@@ -58,6 +59,16 @@ def lib() -> ctypes.CDLL:
     L.pww_xattn_fused_f16.restype = c_i
     L.pww_xattn_fused_f16.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i, c_i, c_i, c_i, c_i, c_i64, c_i64, c_i64, c_i64,
                                       c_i64, c_i64, c_vp, c_i64, c_i, c_vp, c_vp, c_i, c_vp, c_f, c_vp, c_vp, c_sz, c_vp]
+    # per-image twins: `stat` is an int32 [B] device array instead of an int, `g_sigma` holds B values
+    L.pww_xattn_stats_multi_f16.restype = c_i
+    L.pww_xattn_stats_multi_f16.argtypes = [c_vp, c_vp, c_i, c_i, c_i, c_i, c_i, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp,
+                                            c_vp, c_vp, c_sz, c_vp]
+    L.pww_xattn_fwd_multi_f16.restype = c_i
+    L.pww_xattn_fwd_multi_f16.argtypes = list(L.pww_xattn_fwd_f16.argtypes)
+    L.pww_xattn_fused_multi_f16.restype = c_i
+    L.pww_xattn_fused_multi_f16.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i, c_i, c_i, c_i, c_i, c_i64, c_i64, c_i64, c_i64,
+                                            c_i64, c_i64, c_vp, c_i64, c_i, c_vp, c_vp, c_vp, c_vp, c_f, c_vp, c_vp, c_sz,
+                                            c_vp]
     L.pww_attn_fwd_f16.restype = c_i
     L.pww_attn_fwd_f16.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i, c_i, c_i, c_i, c_i64, c_i64, c_i64, c_i64, c_f, c_vp]
     L.pww_groupnorm_workspace_bytes.restype = c_sz

@@ -9,7 +9,7 @@ Same calling convention, context-dict schema and patch mechanism as the referenc
         "CROSS_ATTENTION_WEIGHT_ORIG" ([H,W,T] fp32 or int 0), "SIGMA", "WEIGHT_FUNCTION"
     T = 77 (one CLIP window, any T <= 80 works) or a long prompt of 2 or 3 concatenated 77-token chunks (T = 154, 231;
     `conditioning.chunk_prompt`, the A1111 / compel layout).
-        (optional, ours) "WMAP_INDEX", "G_SIGMA", "CROSS_ATTENTION_PACKED_{N}", "PWW_SCRATCH"
+        (optional, ours) "WMAP_INDEX", "G_SIGMA", "STAT_KIND", "CROSS_ATTENTION_PACKED_{N}", "PWW_SCRATCH"
 
 Everything between the q/k/v projections and the output projection runs in libpww_b200.so through
 the C ABI (include/pww_b200.h): ONE launch of `pww_xattn_fused_f16` (per-image max/std of QK^T over all heads,
@@ -23,12 +23,16 @@ Extensions beyond the reference (which is hard-wired to batch 1, paint_with_word
     how images are batched or sharded across GPUs;
   * dict key "WMAP_INDEX" (int32 [B] device tensor): image b uses weight map `WMAP_INDEX[b]` of a
     stacked [Bw,N,77] map, -1 = no bias.  This is what lets the cond and uncond halves of
-    classifier-free guidance run as ONE batch-2 forward instead of two (paint_with_words.py:483-499).
+    classifier-free guidance run as ONE batch-2 forward instead of two (paint_with_words.py:483-499);
+  * per-image weight functions: dict key "STAT_KIND" (int32 [B] device tensor, PWW_STAT_MAX / PWW_STAT_STD per image)
+    with "G_SIGMA" holding B values, both kept by `PwWSampler`.  Image b's bias is G_SIGMA[b] * stat_b(qk) * w, and
+    the call still is one launch (the `_multi` entry points).  A dict without "STAT_KIND" probes its one
+    WEIGHT_FUNCTION as the reference does.
 """
 from __future__ import annotations
 
 import math
-from typing import Dict, Optional
+from typing import Dict, Optional, Union
 
 import torch
 import torch.nn.functional as F
@@ -142,13 +146,16 @@ XATTN_IMPL = "auto"
 
 def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, scale: float,
                     wmap: Optional[torch.Tensor] = None, wmap_index: Optional[torch.Tensor] = None,
-                    stat: int = _native.PWW_STAT_MAX, g_sigma: Optional[torch.Tensor] = None,
+                    stat: Union[int, torch.Tensor] = _native.PWW_STAT_MAX, g_sigma: Optional[torch.Tensor] = None,
                     return_stats: bool = False, packed=None, stats_out: Optional[torch.Tensor] = None,
                     workspace: Optional[torch.Tensor] = None):
     """Fused region for a key sequence of T <= 80 tokens or of 2 / 3 CLIP chunks (T = 154, 231; any other T raises).
     q [B,N,C]; k,v [B,T,C]; wmap [Bw,N,T] fp32 or None; `packed` = (mpack [Bw,N,32] fp16, cidx [Bw,80 k] int8, k key
-    chunks) from `conditioning.pack_weight_map` (built from `wmap` and cached when not given).  `g_sigma` is a 1-element fp32 device tensor holding G(sigma).  `stats_out` / `workspace`
-    let a caller that captures CUDA graphs own the scratch (defaults: per-device scratch of this module)."""
+    chunks) from `conditioning.pack_weight_map` (built from `wmap` and cached when not given).  `stat` is one kind for
+    every image (an int) with `g_sigma` a 1-element fp32 device tensor holding G(sigma), or per-image settings: an int32
+    [B] device tensor of kinds with `g_sigma` an fp32 [B] device tensor (entry b = image b; the `_multi` entry points).
+    `stats_out` / `workspace` let a caller that captures CUDA graphs own the scratch (defaults: per-device scratch of
+    this module)."""
     L = _native.lib()
     q, k, v = _rows(q), _rows(k), _rows(v)
     B, N, C = q.shape
@@ -178,6 +185,15 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
         if biased and wmap_index is None:
             bw = packed[0].shape[0] if packed is not None else wmap.shape[0]
             wmap_index = st.shared_index(B) if bw == 1 else torch.arange(B, dtype=torch.int32, device=q.device)
+        per_image = isinstance(stat, torch.Tensor)
+        kind_ptr = None
+        if per_image and biased:
+            if (stat.dtype != torch.int32 or stat.numel() != B or not stat.is_contiguous() or stat.device != q.device
+                    or g_sigma is None or g_sigma.dtype != torch.float32 or g_sigma.numel() != B
+                    or not g_sigma.is_contiguous() or g_sigma.device != q.device):
+                raise ValueError(f"per-image settings need an int32 [{B}] kind tensor and an fp32 [{B}] G tensor on "
+                                 f"{q.device}")
+            kind_ptr = stat.data_ptr()
         stats = None
         if use_fused:
             mp_ptr = ci_ptr = idx_ptr = g_ptr = st_ptr = ws_ptr = None
@@ -193,11 +209,12 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                 mp_ptr, ci_ptr, idx_ptr = mpack.data_ptr(), cidx.data_ptr(), wmap_index.data_ptr()
                 g_ptr, st_ptr, ws_ptr = g_sigma.data_ptr(), stats.data_ptr(), ws.data_ptr()
                 mp_bs, bw, ws_bytes = mpack.stride(0), mpack.shape[0], ws.numel()
-            rc = L.pww_xattn_fused_f16(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, heads, N, T, D,
-                                       q.stride(0), q.stride(1), k.stride(0), k.stride(1), out.stride(0), out.stride(1),
-                                       mp_ptr, mp_bs, bw, ci_ptr, idx_ptr, stat, g_ptr, float(scale), st_ptr, ws_ptr,
-                                       ws_bytes, stream)
-            _native.check(rc, "pww_xattn_fused_f16")
+            fn = L.pww_xattn_fused_multi_f16 if per_image else L.pww_xattn_fused_f16
+            rc = fn(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, heads, N, T, D,
+                    q.stride(0), q.stride(1), k.stride(0), k.stride(1), out.stride(0), out.stride(1),
+                    mp_ptr, mp_bs, bw, ci_ptr, idx_ptr, kind_ptr if per_image else stat, g_ptr, float(scale), st_ptr,
+                    ws_ptr, ws_bytes, stream)
+            _native.check(rc, fn.__name__)
             _native.launch_count += 1
         else:
             stats_ptr = g_ptr = w_ptr = idx_ptr = None
@@ -210,17 +227,19 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                 ws_bytes = L.pww_xattn_workspace_bytes(B, heads, N, T, D)
                 st.ensure(B, ws_bytes)
                 stats = st.stats if stats_out is None else stats_out
-                rc = L.pww_xattn_stats_f16(q.data_ptr(), k.data_ptr(), B, heads, N, T, D, q.stride(0), q.stride(1),
-                                           k.stride(0), k.stride(1), stat, wmap_index.data_ptr(), stats.data_ptr(),
-                                           st.workspace.data_ptr(), st.workspace.numel(), stream)
-                _native.check(rc, "pww_xattn_stats_f16")
+                fn = L.pww_xattn_stats_multi_f16 if per_image else L.pww_xattn_stats_f16
+                rc = fn(q.data_ptr(), k.data_ptr(), B, heads, N, T, D, q.stride(0), q.stride(1), k.stride(0),
+                        k.stride(1), kind_ptr if per_image else stat, wmap_index.data_ptr(), stats.data_ptr(),
+                        st.workspace.data_ptr(), st.workspace.numel(), stream)
+                _native.check(rc, fn.__name__)
                 _native.launch_count += 1
                 stats_ptr, g_ptr = stats.data_ptr(), g_sigma.data_ptr()
                 w_ptr, idx_ptr, w_bs = wmap.data_ptr(), wmap_index.data_ptr(), wmap.stride(0)
-            rc = L.pww_xattn_fwd_f16(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, heads, N, T, D,
-                                     q.stride(0), q.stride(1), k.stride(0), k.stride(1), out.stride(0), out.stride(1),
-                                     w_ptr, w_bs, idx_ptr, stats_ptr, g_ptr, float(scale), stream)
-            _native.check(rc, "pww_xattn_fwd_f16")
+            fn = L.pww_xattn_fwd_multi_f16 if per_image else L.pww_xattn_fwd_f16
+            rc = fn(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, heads, N, T, D,
+                    q.stride(0), q.stride(1), k.stride(0), k.stride(1), out.stride(0), out.stride(1),
+                    w_ptr, w_bs, idx_ptr, stats_ptr, g_ptr, float(scale), stream)
+            _native.check(rc, fn.__name__)
             _native.launch_count += 1
     if return_stats:
         return out, (stats[:B].clone() if stats is not None else None)
@@ -317,7 +336,17 @@ def inj_forward(self, hidden_states, context=None, mask=None):
         wmap = wmap_index = g_dev = packed = None
         scratch = (None, None)
         stat = _native.PWW_STAT_MAX
-        if is_dict:
+        kinds = context.get("STAT_KIND") if is_dict else None
+        if kinds is not None:
+            # per-image settings kept by PwWSampler: kinds [B] and G_SIGMA [B] on the device, WMAP_INDEX = -1 for the
+            # images whose weight function is zero
+            w = resolve_weight_map(context, q.shape[1], q.device)
+            if isinstance(w, torch.Tensor):
+                wmap, stat, g_dev = w, kinds, context["G_SIGMA"]
+                wmap_index = context.get("WMAP_INDEX")
+                packed = context.get(packed_key(q.shape[1]))
+                scratch = context.get("PWW_SCRATCH", scratch)
+        elif is_dict:
             f = context["WEIGHT_FUNCTION"]
             sigma = context["SIGMA"]
             w = resolve_weight_map(context, q.shape[1], q.device)

@@ -72,7 +72,7 @@ int cuda_fail(cudaError_t e) {
 
 extern "C" {
 
-int pww_version(void) { return 200; }  // 0.2.0: long contexts (T = 154, 231)
+int pww_version(void) { return 300; }  // 0.3.0: per-image statistic kind and G(sigma) (the _multi entry points)
 
 const char* pww_status_str(int status) {
   switch (status) {
@@ -103,20 +103,27 @@ size_t pww_xattn_workspace_bytes(int B, int H, int N, int T, int D) {
          (size_t)B * stats_slots_per_image(H, N) * sizeof(pww::StatPartial);
 }
 
-int pww_xattn_stats_f16(const void* q, const void* k, int B, int H, int N, int T, int D, int64_t q_batch_stride,
-                        int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int stat,
-                        const int32_t* wmap_index, float* stats, void* workspace, size_t workspace_bytes,
-                        void* stream) {
+}  // extern "C"
+
+namespace {
+
+// The statistics launches of pww_xattn_stats_f16 (kinds == NULL: `stat` for every image) and of
+// pww_xattn_stats_multi_f16 (per_image: kinds[b] for image b).
+int xattn_stats(const void* q, const void* k, int B, int H, int N, int T, int D, int64_t q_batch_stride,
+                int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int stat, const int32_t* kinds,
+                bool per_image, const int32_t* wmap_index, float* stats, void* workspace, size_t workspace_bytes,
+                void* stream) {
   int rc = check_common(q, k, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride);
   if (rc) return rc;
-  if (!stats || !workspace || (stat != PWW_STAT_MAX && stat != PWW_STAT_STD)) return PWW_ERR_BAD_ARG;
+  if (!stats || !workspace) return PWW_ERR_BAD_ARG;
+  if (per_image ? !kinds : (stat != PWW_STAT_MAX && stat != PWW_STAT_STD)) return PWW_ERR_BAD_ARG;
   if (workspace_bytes < pww_xattn_workspace_bytes(B, H, N, T, D)) return PWW_ERR_WORKSPACE;
   pww::XattnParams p;
   memset(&p, 0, sizeof(p));
   p.q = (const __half*)q; p.k = (const __half*)k;
   p.B = B; p.H = H; p.N = N; p.T = T; p.D = D;
   p.q_bs = q_batch_stride; p.q_rs = q_row_stride; p.k_bs = k_batch_stride; p.k_rs = k_row_stride;
-  p.wmap_index = wmap_index; p.stat = stat; p.stats_out = stats;
+  p.wmap_index = wmap_index; p.stat = stat; p.stat_kind = per_image ? kinds : nullptr; p.stats_out = stats;
   p.counters = (unsigned int*)workspace;
   p.partials = (pww::StatPartial*)((char*)workspace + align_up((size_t)B * sizeof(unsigned int), 256));
   cudaStream_t s = (cudaStream_t)stream;
@@ -128,6 +135,7 @@ int pww_xattn_stats_f16(const void* q, const void* k, int B, int H, int N, int T
       c.q = p.q + (int64_t)b0 * p.q_bs;
       c.k = p.k + (int64_t)b0 * p.k_bs;
       c.wmap_index = p.wmap_index ? p.wmap_index + b0 : nullptr;
+      c.stat_kind = p.stat_kind ? p.stat_kind + b0 : nullptr;
       c.stats_out = p.stats_out + b0;
       const cudaError_t e = with_shape(D, T, [&](auto k) { return pww::tc::launch_stats<k.D, k.KC>(c, s); });
       if (e != cudaSuccess) return cuda_fail(e);
@@ -136,11 +144,13 @@ int pww_xattn_stats_f16(const void* q, const void* k, int B, int H, int N, int T
   }
 }
 
-int pww_xattn_fwd_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
-                      int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
-                      int64_t o_batch_stride, int64_t o_row_stride, const float* wmap, int64_t wmap_batch_stride,
-                      const int32_t* wmap_index, const float* stats, const float* g_sigma, float scale,
-                      void* stream) {
+// The forward launches of pww_xattn_fwd_f16 (g_stride 0: g_sigma[0] for every image) and of pww_xattn_fwd_multi_f16
+// (g_stride 1: g_sigma[b] for image b).
+int xattn_fwd(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+              int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
+              int64_t o_batch_stride, int64_t o_row_stride, const float* wmap, int64_t wmap_batch_stride,
+              const int32_t* wmap_index, const float* stats, const float* g_sigma, int64_t g_stride, float scale,
+              void* stream) {
   int rc = check_common(q, k, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride);
   if (rc) return rc;
   if (!v || !out || !aligned16(v) || !aligned16(out)) return PWW_ERR_BAD_ARG;
@@ -153,7 +163,7 @@ int pww_xattn_fwd_f16(const void* q, const void* k, const void* v, void* out, in
   p.q_bs = q_batch_stride; p.q_rs = q_row_stride; p.k_bs = k_batch_stride; p.k_rs = k_row_stride;
   p.o_bs = o_batch_stride; p.o_rs = o_row_stride;
   p.wmap = wmap; p.wmap_bs = wmap_batch_stride; p.wmap_index = wmap_index;
-  p.stats = stats; p.g_sigma = g_sigma; p.scale = scale;
+  p.stats = stats; p.g_sigma = g_sigma; p.g_stride = g_stride; p.scale = scale;
   cudaStream_t s = (cudaStream_t)stream;
   {
     for (int b0 = 0; b0 < B; b0 += pww::tc::kMaxBatch) {          // <= 256 images per launch
@@ -165,6 +175,7 @@ int pww_xattn_fwd_f16(const void* q, const void* k, const void* v, void* out, in
       c.out = p.out + (int64_t)b0 * p.o_bs;
       c.wmap_index = (p.wmap && p.wmap_index) ? p.wmap_index + b0 : nullptr;
       c.stats = p.stats ? p.stats + b0 : nullptr;
+      c.g_sigma = p.g_sigma ? p.g_sigma + (int64_t)b0 * p.g_stride : nullptr;
       if (p.wmap && !p.wmap_index) c.wmap = p.wmap + (int64_t)b0 * p.wmap_bs;   // identity mapping
       const cudaError_t e = with_shape(D, T, [&](auto k) { return pww::tc::launch_fwd<k.D, k.KC>(c, s); });
       if (e != cudaSuccess) return cuda_fail(e);
@@ -173,13 +184,14 @@ int pww_xattn_fwd_f16(const void* q, const void* k, const void* v, void* out, in
   }
 }
 
-size_t pww_xattn_fused_workspace_bytes(void) { return pww::fx::fused_workspace_bytes(); }
-
-int pww_xattn_fused_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
-                        int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
-                        int64_t o_batch_stride, int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride,
-                        int Bw, const int8_t* cidx, const int32_t* wmap_index, int stat, const float* g_sigma,
-                        float scale, float* stats, void* workspace, size_t workspace_bytes, void* stream) {
+// The one launch of pww_xattn_fused_f16 (one `stat` and g_sigma[0] for every image) and of pww_xattn_fused_multi_f16
+// (per_image: kinds[b] and g_sigma[b] for image b).
+int xattn_fused(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+                int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
+                int64_t o_batch_stride, int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw,
+                const int8_t* cidx, const int32_t* wmap_index, int stat, const int32_t* kinds, bool per_image,
+                const float* g_sigma, float scale, float* stats, void* workspace, size_t workspace_bytes,
+                void* stream) {
   int rc = check_common(q, k, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride);
   if (rc) return rc;
   if (!v || !out || !aligned16(v) || !aligned16(out)) return PWW_ERR_BAD_ARG;
@@ -187,7 +199,7 @@ int pww_xattn_fused_f16(const void* q, const void* k, const void* v, void* out, 
   if (mpack) {
     if (!cidx || !g_sigma || !workspace || Bw <= 0 || !aligned16(mpack)) return PWW_ERR_BAD_ARG;
     if ((mpack_batch_stride & 7) || mpack_batch_stride < (int64_t)N * pww::fx::kMW) return PWW_ERR_BAD_ARG;
-    if (stat != PWW_STAT_MAX && stat != PWW_STAT_STD) return PWW_ERR_BAD_ARG;
+    if (per_image ? !kinds : (stat != PWW_STAT_MAX && stat != PWW_STAT_STD)) return PWW_ERR_BAD_ARG;
     if (workspace_bytes < pww_xattn_fused_workspace_bytes()) return PWW_ERR_WORKSPACE;
   }
   pww::XattnParams p;
@@ -196,7 +208,8 @@ int pww_xattn_fused_f16(const void* q, const void* k, const void* v, void* out, 
   p.B = B; p.H = H; p.N = N; p.T = T; p.D = D;
   p.q_bs = q_batch_stride; p.q_rs = q_row_stride; p.k_bs = k_batch_stride; p.k_rs = k_row_stride;
   p.o_bs = o_batch_stride; p.o_rs = o_row_stride;
-  p.g_sigma = g_sigma; p.scale = scale; p.stat = stat;
+  p.g_sigma = g_sigma; p.g_stride = per_image ? 1 : 0; p.scale = scale; p.stat = stat;
+  p.stat_kind = per_image ? kinds : nullptr;
   p.counters = (unsigned int*)workspace;
   p.partials = workspace ? (pww::StatPartial*)((char*)workspace + 512) : nullptr;   // header: counters @0, per-image maxima @256
   cudaStream_t s = (cudaStream_t)stream;
@@ -219,6 +232,8 @@ int pww_xattn_fused_f16(const void* q, const void* k, const void* v, void* out, 
     c.v = p.v + (int64_t)b0 * p.k_bs;
     c.out = p.out + (int64_t)b0 * p.o_bs;
     c.stats_out = stats ? stats + b0 : nullptr;
+    c.stat_kind = p.stat_kind ? p.stat_kind + b0 : nullptr;
+    c.g_sigma = p.g_sigma ? p.g_sigma + (int64_t)b0 * p.g_stride : nullptr;
     const void* mp = mpack;
     const int8_t* ci = cidx;
     if (mpack && wmap_index) {
@@ -235,6 +250,67 @@ int pww_xattn_fused_f16(const void* q, const void* k, const void* v, void* out, 
     if (e != cudaSuccess) return cuda_fail(e);
   }
   return PWW_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int pww_xattn_stats_f16(const void* q, const void* k, int B, int H, int N, int T, int D, int64_t q_batch_stride,
+                        int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int stat,
+                        const int32_t* wmap_index, float* stats, void* workspace, size_t workspace_bytes,
+                        void* stream) {
+  return xattn_stats(q, k, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride, stat, nullptr,
+                     false, wmap_index, stats, workspace, workspace_bytes, stream);
+}
+
+int pww_xattn_stats_multi_f16(const void* q, const void* k, int B, int H, int N, int T, int D, int64_t q_batch_stride,
+                              int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, const int32_t* stat,
+                              const int32_t* wmap_index, float* stats, void* workspace, size_t workspace_bytes,
+                              void* stream) {
+  return xattn_stats(q, k, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride, PWW_STAT_MAX,
+                     stat, true, wmap_index, stats, workspace, workspace_bytes, stream);
+}
+
+int pww_xattn_fwd_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+                      int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
+                      int64_t o_batch_stride, int64_t o_row_stride, const float* wmap, int64_t wmap_batch_stride,
+                      const int32_t* wmap_index, const float* stats, const float* g_sigma, float scale,
+                      void* stream) {
+  return xattn_fwd(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+                   o_batch_stride, o_row_stride, wmap, wmap_batch_stride, wmap_index, stats, g_sigma, 0, scale, stream);
+}
+
+int pww_xattn_fwd_multi_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+                            int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
+                            int64_t o_batch_stride, int64_t o_row_stride, const float* wmap, int64_t wmap_batch_stride,
+                            const int32_t* wmap_index, const float* stats, const float* g_sigma, float scale,
+                            void* stream) {
+  return xattn_fwd(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+                   o_batch_stride, o_row_stride, wmap, wmap_batch_stride, wmap_index, stats, g_sigma, 1, scale, stream);
+}
+
+size_t pww_xattn_fused_workspace_bytes(void) { return pww::fx::fused_workspace_bytes(); }
+
+int pww_xattn_fused_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+                        int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
+                        int64_t o_batch_stride, int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride,
+                        int Bw, const int8_t* cidx, const int32_t* wmap_index, int stat, const float* g_sigma,
+                        float scale, float* stats, void* workspace, size_t workspace_bytes, void* stream) {
+  return xattn_fused(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+                     o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, stat, nullptr,
+                     false, g_sigma, scale, stats, workspace, workspace_bytes, stream);
+}
+
+int pww_xattn_fused_multi_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+                              int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride,
+                              int64_t k_row_stride, int64_t o_batch_stride, int64_t o_row_stride, const void* mpack,
+                              int64_t mpack_batch_stride, int Bw, const int8_t* cidx, const int32_t* wmap_index,
+                              const int32_t* stat, const float* g_sigma, float scale, float* stats, void* workspace,
+                              size_t workspace_bytes, void* stream) {
+  return xattn_fused(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+                     o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, PWW_STAT_MAX, stat,
+                     true, g_sigma, scale, stats, workspace, workspace_bytes, stream);
 }
 
 size_t pww_groupnorm_workspace_bytes(int B, int HW, int G) {

@@ -10,6 +10,9 @@
 //     2. softmax jobs of the unbiased units: they need no statistic and overlap the other CTAs' statistic pass;
 //     3. grid barrier (per biased image, only the CTAs that publish for it), then the softmax jobs of the biased units
 //        with the bias x * W, x = g(sigma) * fp16(statistic), W rebuilt from the packed map (xattn_fused.cuh).
+// The statistic kind and g(sigma) are per image when the launch carries per-image arrays (XattnParams::stat_kind,
+// g_stride = 1), else one kind and one g(sigma) for every image; each CTA keeps the kind of its local biased images in
+// shared memory, so the statistic jobs, the publish step and the finalise step branch per image.
 // Work unit = (image, 128-row tile, group of G heads); a unit expands into one job per head.  Each job is computed by the
 // 8 warps of the CTA with the warp-level MMA tiles of xattn_core.cuh; the cp.async copies of job i + 1 (Q rows, K, V
 // and, for biased softmax jobs, the row tile's packed map) are in flight while job i is computed.
@@ -154,6 +157,7 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
   __shared__ int s_nb, s_njobs, s_nstat, s_nl;
   __shared__ int s_lb[kMaxLocal], s_lp[kMaxLocal];   // image / group position of the CTA's local biased images
   __shared__ float s_coef[kMaxLocal];             // g(sigma) * statistic of the CTA's local biased images
+  __shared__ bool s_ismax[kMaxLocal];             // statistic kind of the CTA's local biased images
   __shared__ StatPartial s_part[core::kWarps][kMaxLocal];   // [warp][local biased image]
   __shared__ uint2 s_jobs[kMaxJobs];
   __shared__ uint4 s_unit[kMaxUnits];              // job-table build scratch: one entry per unit of the range
@@ -253,7 +257,7 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
     for (int b = threadIdx.x; b < p.B; b += blockDim.x)
       if (s_widx[b] < 0) p.stats_out[b] = 0.f;
   if (warp == 1) {
-    // how many CTAs publish a partial for each of my local biased images
+    // how many CTAs publish a partial for each of my local biased images, and which statistic each one takes
 #pragma unroll 1
     for (int l = 0; l < nl && l < kMaxLocal; ++l) {
       int e = 0;
@@ -261,7 +265,7 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
 #pragma unroll 1
       for (int c = lane; c < (int)gridDim.x; c += 32) e += fx_cta_has_image(c, gridDim.x, fp.units, pos, HG, fp.tiles, np) ? 1 : 0;
       e = __reduce_add_sync(0xffffffffu, e);
-      if (lane == 0) s_expect[l] = e;
+      if (lane == 0) { s_expect[l] = e; s_ismax[l] = image_is_max(p, s_lb[l]); }
     }
   } else if (warp == 2) {
     for (int idx = lane; idx < nl * CW && idx < kMaxLocal * CW; idx += 32) {
@@ -300,8 +304,6 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
   };
 
   const float sl2 = p.scale * 1.4426950408889634f;
-  const bool is_max = p.stat == PWW_STAT_MAX;
-  const float gsig = (nb > 0 && p.g_sigma != nullptr) ? __ldg(p.g_sigma) : 0.f;
   const unsigned long long* sync_words = reinterpret_cast<const unsigned long long*>(p.counters + 64);
   float vmax = -INFINITY;                          // this thread's statistic partial of local image cur_li
   double dsum = 0.0, dsq = 0.0;
@@ -340,17 +342,17 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
     __syncthreads();
     if (i == ns && ns > 0 && warp == 0) {
       // ---- publish the CTA's statistic partials: the 8 warps' partials in a fixed order, folded into the image's word ----
-      if (is_max) {
-        for (int l = 0; l < nl && l < kMaxLocal; ++l) {
-          const unsigned k = __reduce_max_sync(0xffffffffu, lane < core::kWarps ? f32_key((float)s_part[lane][l].vmax) : 0u);
-          if (lane == 0) {
-            unsigned* word = p.counters + 64 + 2 * s_lb[l];        // {max key, count}, see ld_acquire_gpu_u64
-            asm volatile("red.relaxed.gpu.global.max.u32 [%0], %1;" ::"l"(word), "r"(k) : "memory");
-            // release: the maximum above is visible to whoever acquires the new count
-            asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(word + 1) : "memory");
-          }
+      for (int l = 0; l < nl && l < kMaxLocal; ++l) {
+        if (!s_ismax[l]) continue;                                 // warp-uniform: one kind per image
+        const unsigned k = __reduce_max_sync(0xffffffffu, lane < core::kWarps ? f32_key((float)s_part[lane][l].vmax) : 0u);
+        if (lane == 0) {
+          unsigned* word = p.counters + 64 + 2 * s_lb[l];          // {max key, count}, see ld_acquire_gpu_u64
+          asm volatile("red.relaxed.gpu.global.max.u32 [%0], %1;" ::"l"(word), "r"(k) : "memory");
+          // release: the maximum above is visible to whoever acquires the new count
+          asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(word + 1) : "memory");
         }
-      } else if (lane < nl && lane < kMaxLocal) {
+      }
+      if (lane < nl && lane < kMaxLocal && !s_ismax[lane]) {       // std images: one lane per local image
         const int lbv = s_lb[lane];
         StatPartial sp = s_part[0][lane];
 #pragma unroll 1
@@ -383,6 +385,7 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
             }
           }
           __syncwarp();
+          const bool is_max = s_ismax[l];
           double m = -INFINITY, a = 0.0, q = 0.0;
           if (is_max) {
             // the maximum is order independent: every publisher folded its partial into the word with an atomic max
@@ -411,7 +414,7 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
               rr = sqrt(var > 0.0 ? var : 0.0);
             }
             const float st16 = round_to_f16((float)rr);         // qk.max() / qk.std() return fp16 in the reference
-            s_coef[l] = gsig * st16;
+            s_coef[l] = (p.g_sigma != nullptr ? image_g(p, bl) : 0.f) * st16;
             if (p.stats_out != nullptr) p.stats_out[bl] = st16;   // every CTA of the image writes the same value
           }
         }
@@ -435,7 +438,7 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
         for (int c = 0; c < KC; ++c) {              // the real tokens of every chunk
           float s[10][4];
           core::warp_qk<D>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
-          core::warp_stat(s, core::kChunk, p.N - row0, lane, is_max, vmax, sum, sumsq);
+          core::warp_stat(s, core::kChunk, p.N - row0, lane, s_ismax[li], vmax, sum, sumsq);
         }
         dsum += (double)sum;
         dsq += (double)sumsq;
@@ -476,7 +479,7 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
     if (!is_main) {
       if (li != cur_li) { flush(); cur_li = li; }
       float sum = 0.f, sumsq = 0.f;
-      core::warp_stat(s, T, p.N - row0, lane, is_max, vmax, sum, sumsq);
+      core::warp_stat(s, T, p.N - row0, lane, s_ismax[li], vmax, sum, sumsq);
       dsum += (double)sum;
       dsq += (double)sumsq;
       if (i == ns - 1) flush();

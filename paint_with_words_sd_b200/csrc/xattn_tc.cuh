@@ -5,7 +5,8 @@
 //
 // Fused region of the reference's inj_forward (paint_with_words.py:87-118), per image b / head h / 128-row tile:
 //     statistics kernel:  per-image max / (sum, sumsq) of fp16(Q_h K_h^T) over all heads, rows and tokens
-//     forward kernel:     S = Q_h K_h^T;  P = softmax(scale * (S + g * M_b * w[b]));  O = P V_h
+//     forward kernel:     S = Q_h K_h^T;  P = softmax(scale * (S + g[b] * M_b * w[b]));  O = P V_h
+// The statistic kind and g are one value for the launch or one per image (XattnParams::stat_kind, g_stride).
 // with the warp-level MMA tiles of xattn_core.cuh.  Work unit = (image, row tile, head); every CTA of the persistent grid
 // owns a contiguous range of units and double-buffers them: the cp.async copies of unit i + 1 are in flight while unit i
 // is computed.  The forward kernel walks its range in the FwdWalk order, which pairs one image with a weight map and one
@@ -200,7 +201,7 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_fwd_kernel(const TcParams t
   for (int b = threadIdx.x; b < p.B; b += kThreads) {
     const int wi = image_widx(p, b);
     s_widx[b] = wi;
-    s_coef[b] = wi >= 0 ? __ldg(p.g_sigma) * __ldg(p.stats + b) : 0.f;
+    s_coef[b] = wi >= 0 ? image_g(p, b) * __ldg(p.stats + b) : 0.f;
   }
   __syncthreads();
   int u0, u1;
@@ -290,6 +291,7 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams
   const uint32_t smem0 = ptx::smem_u32(smem);
   __shared__ StatPartial s_part[core::kWarps][kMaxLocal];     // [warp][local image]
   __shared__ unsigned char s_skip[kMaxBatch];
+  __shared__ bool s_ismax[kMaxBatch];                           // statistic kind per image
   __shared__ int is_last;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int u0, u1;
@@ -297,7 +299,10 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams
   const int n_it = u1 - u0;
   const int upi = tp.tiles * p.H;                               // units per image
   const int b_first = n_it > 0 ? u0 / upi : 0;
-  for (int b = threadIdx.x; b < p.B; b += kThreads) s_skip[b] = (p.wmap_index != nullptr && p.wmap_index[b] < 0) ? 1 : 0;
+  for (int b = threadIdx.x; b < p.B; b += kThreads) {
+    s_skip[b] = (p.wmap_index != nullptr && p.wmap_index[b] < 0) ? 1 : 0;
+    s_ismax[b] = s_skip[b] ? true : image_is_max(p, b);        // skipped images: their kind is never read
+  }
   if (threadIdx.x < core::kWarps * kMaxLocal) {
     StatPartial sp;
     sp.vmax = -INFINITY; sp.sum = 0.0; sp.sumsq = 0.0; sp.pad = 0.0;
@@ -305,7 +310,6 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams
   }
   __syncthreads();
   auto skip = [&](int b) { return s_skip[b] != 0; };
-  const bool is_max = p.stat == PWW_STAT_MAX;
   {
     float vmax = -INFINITY;
     double dsum = 0.0, dsq = 0.0;
@@ -346,6 +350,7 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams
       }
       __syncthreads();
       if (b != cur_b) { flush(); cur_b = b; }
+      const bool is_max = s_ismax[b];
       const uint32_t st = smem0 + (CF::NST == 2 ? (k & 1) : 0) * CF::STAGE;
       float sum = 0.f, sumsq = 0.f;
 #pragma unroll 1
@@ -410,7 +415,7 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams
     if (lane == 0) {
       const double cnt = (double)p.H * (double)p.N * (double)p.T;
       double r;
-      if (is_max) {
+      if (s_ismax[b]) {
         r = m;
       } else {
         const double var = (q - a * a / cnt) / (cnt - 1.0);

@@ -1,6 +1,7 @@
 """Public API: `paint_with_words()`, `paint_with_words_inpaint()`, `pww_load_tools()` -- same keyword
 arguments, defaults and return type as the reference (paint_with_words/paint_with_words.py:128-204,
-391-510; paint_with_words_inpaint.py:137-270) -- plus `PwWSampler`, the GPU-first engine behind them.
+391-510; paint_with_words_inpaint.py:137-270) -- plus `PwWSampler`, the GPU-first engine behind them, and
+`paint_with_words_batch()`, which makes many differently configured images in shared samplers.
 
 What is different underneath (results equal within the stated fp16 tolerance):
   * the attention of every UNet block runs in libpww_b200.so (see attention.py);
@@ -12,8 +13,9 @@ What is different underneath (results equal within the stated fp16 tolerance):
 """
 from __future__ import annotations
 
+import inspect
 import math
-from typing import Callable, Dict, List, Optional, Sequence, Tuple
+from typing import Callable, Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -25,7 +27,7 @@ from .conditioning import _encode_text_color_inputs, _get_binary_mask, pack_weig
 from .scheduler import LMSDiscreteScheduler
 from .synthetic import IdentityVAE, RandomTextEncoder, SimpleWordTokenizer
 from .unet import UNet2DConditionModel, UNetConfig, build_unet
-from .weight_function import g_of_sigma, probe_weight_function
+from .weight_function import STAT_MAX, UnsupportedWeightFunction, g_of_sigma, probe_weight_function
 
 
 def default_weight_function(w, sigma, qk):
@@ -118,22 +120,41 @@ def initial_latents(latent_size, seed: int, extra_seeds: Dict[int, int], seperat
 # ---------------------------------------------------------------------------------------------
 # the engine
 # ---------------------------------------------------------------------------------------------
+def _per_image(value, m: int, name: str, is_one) -> list:
+    """One setting for every image, or a sequence of exactly m settings."""
+    if is_one(value):
+        return [value] * m
+    vals = list(value)
+    if len(vals) != m or not all(is_one(v) for v in vals):
+        raise ValueError(f"{name} must be one value or a sequence of {m} (one per image)")
+    return vals
+
+
 class PwWSampler:
     """Denoising loop for a group of images on ONE GPU (paint_with_words.py:471-506 semantics per image).
 
     Each image i has a cond context dict, an uncond context dict and latents; a step runs one UNet
     forward over the batch [cond_0..cond_{m-1}, uncond_0..uncond_{m-1}], the CFG combine and the LMS
     update.  `use_graph=True` captures the step in a CUDA graph.
+
+    `weight_function` is one callable for every image or a sequence of m callables, one per image, and `guidance_scale`
+    one float or m floats: images made with different settings share the sampler, and every cross-attention call is
+    still one launch (per-image statistic kind and G(sigma) on the device).  An identically-zero function leaves its
+    image unbiased.
     """
 
     def __init__(self, unet, scheduler: LMSDiscreteScheduler, cond_ctxs: Sequence[dict], uncond_ctxs: Sequence[dict],
-                 latents: torch.Tensor, weight_function: Callable, guidance_scale: float = 7.5,
+                 latents: torch.Tensor, weight_function: Union[Callable, Sequence[Callable]],
+                 guidance_scale: Union[float, Sequence[float]] = 7.5,
                  extra_input: Optional[torch.Tensor] = None, use_graph: bool = True, timesteps=None):
         self.unet, self.scheduler = unet, scheduler
         self.m = len(cond_ctxs)
         self.device = latents.device
-        self.guidance_scale = float(guidance_scale)
         self.weight_function = weight_function
+        self.guidance_scale = (float(guidance_scale) if isinstance(guidance_scale, (int, float))
+                               else [float(g) for g in guidance_scale])
+        self._fns = _per_image(weight_function, self.m, "weight_function", callable)
+        scales = _per_image(self.guidance_scale, self.m, "guidance_scale", lambda g: isinstance(g, float))
         self.timesteps = list((scheduler.timesteps if timesteps is None else timesteps).tolist())
         self.latents = latents.clone().float()
         self.extra_input = extra_input            # inpaint: [m,5,h,w] (mask + masked-image latents)
@@ -141,18 +162,27 @@ class PwWSampler:
         self._graph = None
         self._kv_graph = None
         self.native_launches_per_step = None
-        self._probed = probe_weight_function(weight_function, 1.0)
+        self._probed = []
+        for i, f in enumerate(self._fns):
+            try:
+                self._probed.append(probe_weight_function(f, 1.0))
+            except UnsupportedWeightFunction as e:
+                if callable(weight_function):
+                    raise
+                raise UnsupportedWeightFunction(f"weight_function of image {i}: {e}") from e
         up = next(iter(unet.parameters()), None)
         self._unet_dtype = up.dtype if up is not None else torch.float32
         self._ctx = self._merge_contexts(cond_ctxs, uncond_ctxs)
         dev = self.device
-        # Per-step scalars (sigma, 1/sqrt(sigma^2+1), t, 4 LMS coefficients, G(sigma)) are tabulated
-        # once on the host and uploaded; a step copies its row into `_params` (one 32-byte D2D copy), so
-        # a captured graph sees new values and the host never feeds the stream mid-loop.
+        # Per-step scalars (sigma, 1/sqrt(sigma^2+1), t, 4 LMS coefficients, G_0(sigma) .. G_{m-1}(sigma)) are
+        # tabulated once on the host and uploaded; a step copies its row into `_params` (one D2D copy), so a captured
+        # graph sees new values and the host never feeds the stream mid-loop.  `_params` has m more entries that stay 0:
+        # G_SIGMA holds one value per image of the UNet batch, and the uncond images are unbiased.
         self._table = self._build_step_table().to(dev)
-        self._params = torch.zeros(8, dtype=torch.float32, device=dev)
+        self._params = torch.zeros(7 + 2 * self.m, dtype=torch.float32, device=dev)
         self._derivs = torch.zeros((4,) + tuple(self.latents.shape), dtype=torch.float32, device=dev)
-        self._ctx["G_SIGMA"] = self._params[7:8]
+        self._ctx["G_SIGMA"] = self._params[7:]
+        self._gscale = torch.tensor(scales, dtype=torch.float32, device=dev).view(self.m, 1, 1, 1)
         self._step_no = 0
 
     def _build_step_table(self) -> torch.Tensor:
@@ -165,13 +195,14 @@ class PwWSampler:
             # missing history (img2img starts mid-schedule) simply contributes nothing (zip truncation).
             coeffs = list(sch._coeffs[si]) if sch._coeffs is not None else sch._lms_coeffs(si, min(si + 1, 4))
             coeffs = (coeffs + [0.0] * 4)[:4]
-            g = g_of_sigma(self.weight_function, self._probed, sch.sigmas[si])
-            rows.append([sigma, 1.0 / math.sqrt(sigma * sigma + 1.0), float(t), *coeffs, g])
+            gs = [g_of_sigma(f, pr, sch.sigmas[si]) for f, pr in zip(self._fns, self._probed)]
+            rows.append([sigma, 1.0 / math.sqrt(sigma * sigma + 1.0), float(t), *coeffs, *gs])
         return torch.tensor(rows, dtype=torch.float32)
 
     def _merge_contexts(self, conds, unconds) -> dict:
         """Batch the per-image dicts: CONTEXT_TENSOR -> [2m,T,Dc]; weight maps -> [m,N,T] stacks;
-        WMAP_INDEX = [0..m-1, -1 x m]."""
+        WMAP_INDEX = [0..m-1, -1 x m] with -1 also for images whose weight function is zero; STAT_KIND = the probed
+        statistic of every image (uncond images: max, ignored)."""
         m = self.m
         lengths = {int(c["CONTEXT_TENSOR"].shape[1]) for c in list(conds) + list(unconds)}
         if len(lengths) != 1:
@@ -197,7 +228,10 @@ class PwWSampler:
                     ctx[packed_key(n)] = (packed[0].to(self.device), packed[1].to(self.device))
             else:
                 ctx[key] = 0
-        ctx["WMAP_INDEX"] = torch.tensor(list(range(m)) + [-1] * m, dtype=torch.int32, device=self.device)
+        ctx["WMAP_INDEX"] = torch.tensor([-1 if pr.is_zero else i for i, pr in enumerate(self._probed)] + [-1] * m,
+                                         dtype=torch.int32, device=self.device)
+        ctx["STAT_KIND"] = torch.tensor([STAT_MAX if pr.is_zero else pr.stat for pr in self._probed] + [STAT_MAX] * m,
+                                        dtype=torch.int32, device=self.device)
         ctx["WEIGHT_FUNCTION"] = self.weight_function
         ctx["SIGMA"] = None
         ctx["KV_CACHE"] = {}       # to_k/to_v of the text context are step-invariant: computed at the first step
@@ -218,7 +252,7 @@ class PwWSampler:
         x2 = torch.cat([x, x], 0).to(self._unet_dtype)      # the reference runs under autocast: feed the UNet its own dtype
         eps = self.unet(x2, self._params[2:3], encoder_hidden_states=self._ctx).sample.float()
         eps_c, eps_u = eps[:m], eps[m:]
-        noise_pred = eps_u + self.guidance_scale * (eps_c - eps_u)
+        noise_pred = eps_u + self._gscale * (eps_c - eps_u)
         # LMS (epsilon prediction): derivative == noise_pred; history kept in a rolling device buffer
         self._derivs.copy_(torch.roll(self._derivs, 1, 0))
         self._derivs[0].copy_(noise_pred)
@@ -226,7 +260,7 @@ class PwWSampler:
         self.latents.add_(upd)
 
     def _set_step_scalars(self, i: int, step_index: int):
-        self._params.copy_(self._table[i])
+        self._params[:self._table.shape[1]].copy_(self._table[i])
         self._ctx["SIGMA"] = self.scheduler.sigmas[step_index]
 
     # -- host-buffer interface (what bench.py's e2e leg drives) -----------------------------------
@@ -368,6 +402,99 @@ def paint_with_words(
     if return_latents:
         return latents
     return _pil_from_latents(vae, latents)[0]
+
+
+# the per-image keyword arguments of paint_with_words that paint_with_words_batch takes per entry
+BATCH_SETTING_KEYS = ("color_context", "color_map_image", "input_prompt", "unconditional_input_prompt", "seed",
+                      "weight_function", "guidance_scale", "max_prompt_chunks")
+
+
+def _batch_settings(settings) -> List[dict]:
+    """Every entry with paint_with_words's defaults filled in; unknown keys and img2img raise ValueError."""
+    params = inspect.signature(paint_with_words).parameters
+    out = []
+    for i, entry in enumerate(settings):
+        unknown = set(entry) - set(BATCH_SETTING_KEYS)
+        if unknown & {"init_image", "strength"}:
+            raise ValueError(f"settings[{i}]: init_image / strength cannot be batched (img2img draws its noise from the "
+                             "global RNG); call paint_with_words for that image")
+        if unknown:
+            raise ValueError(f"settings[{i}]: unknown keys {sorted(unknown)}; the per-image keys are "
+                             f"{', '.join(BATCH_SETTING_KEYS)}")
+        full = {k: params[k].default for k in BATCH_SETTING_KEYS}
+        full.update(entry)
+        if full["color_map_image"] is None:
+            raise ValueError(f"settings[{i}]: color_map_image is required")
+        out.append(full)
+    return out
+
+
+def batch_groups(keys: Sequence, max_batch_size: int) -> List[List[int]]:
+    """Indices of the entries grouped by key (groups in order of first appearance, input order inside a group), each
+    group cut into runs of at most `max_batch_size`: one sampler per run.  A key of None is never shared."""
+    if max_batch_size < 1:
+        raise ValueError("max_batch_size must be >= 1")
+    groups: Dict[object, List[int]] = {}
+    for i, key in enumerate(keys):
+        groups.setdefault(("solo", i) if key is None else key, []).append(i)
+    return [g[j:j + max_batch_size] for g in groups.values() for j in range(0, len(g), max_batch_size)]
+
+
+@torch.no_grad()
+def paint_with_words_batch(
+    settings: Sequence[dict],
+    num_inference_steps: int = 30,
+    scheduler_type=LMSDiscreteScheduler,
+    device: str = "cuda:0",
+    local_model_path: Optional[str] = None,
+    hf_model_path: Optional[str] = "synthetic:sd15",
+    preloaded_utils: Optional[Tuple] = None,
+    model_token: Optional[str] = None,
+    max_batch_size: int = 8,
+    return_latents: bool = False,
+):
+    """Many images, each with its own settings, in as few samplers as possible.  `settings[i]` is a dict of the
+    per-image keyword arguments of `paint_with_words` (BATCH_SETTING_KEYS: color_context, color_map_image, input_prompt,
+    unconditional_input_prompt, seed, weight_function, guidance_scale, max_prompt_chunks); missing keys take
+    paint_with_words's defaults.  Returns a list of PIL images (or [1,4,h,w] latents) in input order; image i equals
+    `paint_with_words(**settings[i])` up to fp16 noise.
+
+    Entries of the same latent size and text length run in one `PwWSampler` of at most `max_batch_size` images (a
+    2 * max_batch_size UNet batch with CFG), whatever their weight functions and guidance scales.  The default of 8 gave
+    the most images/s of k = 1, 2, 4, 8 at 512x512 (BASELINE.md section 4) and bounds memory.  Sizes that are not multiples of 64 need the single-image weight-map fallback and
+    run one image per sampler.  img2img (init_image / strength) is not batched."""
+    entries = _batch_settings(settings)
+    if max_batch_size < 1:
+        raise ValueError("max_batch_size must be >= 1")
+    vae, unet, text_encoder, tokenizer, scheduler = (
+        pww_load_tools(device, scheduler_type, local_model_path=local_model_path, hf_model_path=hf_model_path,
+                       model_token=model_token)
+        if preloaded_utils is None else preloaded_utils)
+    scheduler.set_timesteps(num_inference_steps)
+    encoded, keys = [], []
+    for e in entries:
+        width, height = e["color_map_image"].size
+        extra_seeds, seperated_word_contexts, cond, uncond = _encode_text_color_inputs(
+            text_encoder, tokenizer, device, e["color_map_image"], dict(e["color_context"]), e["input_prompt"],
+            e["unconditional_input_prompt"], max_prompt_chunks=e["max_prompt_chunks"])
+        latents = initial_latents((1, unet.in_channels, height // 8, width // 8), e["seed"], extra_seeds,
+                                  seperated_word_contexts).to(device)
+        encoded.append((cond, uncond, latents * scheduler.init_noise_sigma))
+        solo = width % 64 != 0 or height % 64 != 0
+        keys.append(None if solo else (height // 8, width // 8, int(cond["CONTEXT_TENSOR"].shape[1])))
+    results: List[Optional[torch.Tensor]] = [None] * len(entries)
+    for idx in batch_groups(keys, max_batch_size):
+        sampler = PwWSampler(unet, scheduler, [encoded[i][0] for i in idx], [encoded[i][1] for i in idx],
+                             torch.cat([encoded[i][2] for i in idx], 0),
+                             [entries[i]["weight_function"] for i in idx], [entries[i]["guidance_scale"] for i in idx],
+                             timesteps=scheduler.timesteps)
+        latents = sampler.run()
+        for j, i in enumerate(idx):
+            results[i] = latents[j:j + 1].clone()
+        del sampler
+    if return_latents:
+        return results
+    return [_pil_from_latents(vae, lat)[0] for lat in results]
 
 
 def prepare_mask_and_masked_image(image, mask):

@@ -200,6 +200,35 @@ int pww_geglu_f16(const void* in, void* out, int64_t M, int I, void* stream);
 int pww_add_layernorm_f16(const void* x, const void* res, const void* gamma, const void* beta, void* sum_out, void* y,
                           int64_t M, int C, float eps, void* stream);
 
+/*
+ * The sampler step around the UNet (LMS, Euler, Euler ancestral, DPM++ 2M), two launches per denoising step.
+ * Latents are [m, 4, h, w] fp32 contiguous; dtype codes name the UNet's input / output type.
+ *
+ * pww_sampler_input: the UNet input [2m, channels, h, w] (contiguous, `out_dtype`): rows i and m + i both get
+ *   round(latents[i] * scale[0]) in channels 0..3 and, for channels == 9, round(extra[i]) in channels 4..8 (extra is
+ *   [m, 5, h, w] fp32: the inpaint mask and masked-image latents; NULL for channels == 4).  `scale` is a device scalar.
+ *
+ * pww_sampler_update: classifier-free guidance and one step of the linear step form, latents updated in place:
+ *   eps    = eps_u + guidance[i] (eps_c - eps_u)         eps_c = eps[i], eps_u = eps[m + i] ([2m, 4, h, w], any strides)
+ *   q      = a x + b eps                                 written to history entry `slot`
+ *   x_next = alpha x + (beta[0] q + beta[1] h1 + ... + beta[L-1] h_{L-1}) + gamma z
+ * h_k is history entry (slot - k) mod L, L = history_len (1..4); history is [L, m, 4, h, w] fp32.  z is noise row
+ * `row` of noise [n, m, 4, h, w] fp32 (noise may be NULL; the term is skipped when gamma == 0).  beta is a [4] and
+ * form a [6] device array: form = {alpha, a, b, gamma, slot, row}.  All arithmetic is fp32, rounded after every
+ * operation in the order written; a == 0 gives q = b eps and alpha == 1 gives x + (...).
+ * Both return PWW_ERR_BAD_ARG for null pointers or bad sizes and PWW_ERR_UNSUPPORTED for other dtypes, before any
+ * CUDA call.
+ */
+#define PWW_DTYPE_F32 0
+#define PWW_DTYPE_F16 1
+int pww_sampler_input(const float* latents, const float* scale, const float* extra, void* out, int out_dtype,
+                      int m, int channels, int height, int width, void* stream);
+int pww_sampler_update(const void* eps, int eps_dtype, int64_t eps_batch_stride, int64_t eps_channel_stride,
+                       int64_t eps_row_stride, int64_t eps_col_stride,
+                       float* latents, float* history, int history_len, const float* noise,
+                       const float* guidance, const float* beta, const float* form,
+                       int m, int height, int width, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

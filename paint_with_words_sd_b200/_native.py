@@ -13,6 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("PWW_B200_LIB", os.path.join(_HERE, "libpww_b200.so"))
 
 PWW_STAT_MAX, PWW_STAT_STD = 0, 1
+PWW_DTYPE_F32, PWW_DTYPE_F16 = 0, 1
 
 EXPORTS = (
     "pww_version", "pww_status_str", "pww_last_cuda_error", "pww_device_supported",
@@ -20,6 +21,7 @@ EXPORTS = (
     "pww_xattn_fused_workspace_bytes", "pww_xattn_fused_f16",
     "pww_xattn_stats_multi_f16", "pww_xattn_fwd_multi_f16", "pww_xattn_fused_multi_f16",
     "pww_groupnorm_workspace_bytes", "pww_groupnorm_nhwc_f16", "pww_geglu_f16", "pww_add_layernorm_f16",
+    "pww_sampler_input", "pww_sampler_update",
 )
 
 
@@ -79,6 +81,11 @@ def lib() -> ctypes.CDLL:
     L.pww_geglu_f16.argtypes = [c_vp, c_vp, c_i64, c_i, c_vp]
     L.pww_add_layernorm_f16.restype = c_i
     L.pww_add_layernorm_f16.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i, c_f, c_vp]
+    L.pww_sampler_input.restype = c_i
+    L.pww_sampler_input.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i, c_i, c_i, c_i, c_i, c_vp]
+    L.pww_sampler_update.restype = c_i
+    L.pww_sampler_update.argtypes = [c_vp, c_i, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_i, c_vp, c_vp, c_vp, c_vp,
+                                     c_i, c_i, c_i, c_vp]
     _lib = L
     return L
 

@@ -8,6 +8,7 @@
 #include "xattn_fused2.cuh"
 #include "attn_tc.cuh"
 #include "unet_ops.cuh"
+#include "sampler_step.cuh"
 #include <stdlib.h>
 
 namespace {
@@ -78,7 +79,7 @@ const char* pww_status_str(int status) {
   switch (status) {
     case PWW_OK: return "ok";
     case PWW_ERR_BAD_ARG: return "bad argument (null/misaligned pointer, non-positive size or stride not a multiple of 8)";
-    case PWW_ERR_UNSUPPORTED: return "unsupported shape (head dim must be 40/64/80/160, T <= 80, 154 or 231)";
+    case PWW_ERR_UNSUPPORTED: return "unsupported shape or dtype (head dim must be 40/64/80/160, T <= 80, 154 or 231)";
     case PWW_ERR_CUDA: return "CUDA error (see pww_last_cuda_error)";
     case PWW_ERR_WORKSPACE: return "workspace too small (see pww_xattn_workspace_bytes)";
     default: return "unknown status";
@@ -392,6 +393,45 @@ int pww_add_layernorm_f16(const void* x, const void* res, const void* gamma, con
     default: return PWW_ERR_UNSUPPORTED;
   }
   cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? PWW_OK : cuda_fail(e);
+}
+
+int pww_sampler_input(const float* latents, const float* scale, const float* extra, void* out, int out_dtype, int m,
+                      int channels, int height, int width, void* stream) {
+  if (!latents || !scale || !out || m <= 0 || height <= 0 || width <= 0) return PWW_ERR_BAD_ARG;
+  if (channels != 4 && channels != 9) return PWW_ERR_BAD_ARG;
+  if ((channels == 9) != (extra != nullptr)) return PWW_ERR_BAD_ARG;
+  if (out_dtype != PWW_DTYPE_F32 && out_dtype != PWW_DTYPE_F16) return PWW_ERR_UNSUPPORTED;
+  pww::smp::InputArgs a;
+  a.lat = latents; a.scale = scale; a.extra = extra; a.out = out; a.m = m; a.C = channels; a.hw = height * width;
+  const bool px4 = (a.hw % 4) == 0 && aligned16(latents) && (!extra || aligned16(extra)) && aligned16(out);
+  cudaStream_t s = (cudaStream_t)stream;
+  const cudaError_t e = out_dtype == PWW_DTYPE_F16 ? pww::smp::launch_input<__half>(a, px4, s)
+                                                   : pww::smp::launch_input<float>(a, px4, s);
+  return e == cudaSuccess ? PWW_OK : cuda_fail(e);
+}
+
+int pww_sampler_update(const void* eps, int eps_dtype, int64_t eps_batch_stride, int64_t eps_channel_stride,
+                       int64_t eps_row_stride, int64_t eps_col_stride, float* latents, float* history, int history_len,
+                       const float* noise, const float* guidance, const float* beta, const float* form, int m,
+                       int height, int width, void* stream) {
+  if (!eps || !latents || !history || !guidance || !beta || !form) return PWW_ERR_BAD_ARG;
+  if (m <= 0 || height <= 0 || width <= 0 || history_len < 1 || history_len > 4) return PWW_ERR_BAD_ARG;
+  if (eps_dtype != PWW_DTYPE_F32 && eps_dtype != PWW_DTYPE_F16) return PWW_ERR_UNSUPPORTED;
+  pww::smp::UpdateArgs a;
+  a.eps = eps; a.e_sn = eps_batch_stride; a.e_sc = eps_channel_stride; a.e_sh = eps_row_stride; a.e_sw = eps_col_stride;
+  a.lat = latents; a.hist = history; a.noise = noise; a.gscale = guidance; a.beta = beta; a.form = form;
+  a.m = m; a.h = height; a.w = width; a.nh = history_len;
+  const int64_t hw = (int64_t)height * width;
+  const size_t es = eps_dtype == PWW_DTYPE_F16 ? 2 : 4;
+  const bool px4 = (hw % 4) == 0 && aligned16(latents) && aligned16(history) && (!noise || aligned16(noise));
+  // channels-last packed rows: pixel p's 4 channels at 4p (8 bytes per pixel in fp16, 16 in fp32)
+  const size_t need = px4 ? 16 : 4 * es;
+  const bool cl = eps_channel_stride == 1 && eps_col_stride == 4 && eps_row_stride == 4 * (int64_t)width &&
+                  (reinterpret_cast<uintptr_t>(eps) % need) == 0 && ((size_t)eps_batch_stride * es) % need == 0;
+  cudaStream_t s = (cudaStream_t)stream;
+  const cudaError_t e = eps_dtype == PWW_DTYPE_F16 ? pww::smp::launch_update<__half>(a, px4, cl, s)
+                                                   : pww::smp::launch_update<float>(a, px4, cl, s);
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 

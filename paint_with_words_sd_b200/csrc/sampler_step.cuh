@@ -1,0 +1,227 @@
+// The sampler step around the UNet (pww_sampler_input / pww_sampler_update): the scaled, CFG-doubled UNet input, and
+// the CFG combine + one linear step form that LMS, Euler, Euler ancestral and DPM++ 2M fill with their own coefficients.
+//
+// Every scalar that changes per step is read from device memory (a captured CUDA graph replays with new values), and
+// all arithmetic is fp32 with explicit round-to-nearest intrinsics in the order of the step form, so nvcc cannot
+// contract a multiply and an add into an FMA:
+//   eps    = eps_u + g_i (eps_c - eps_u)
+//   q      = a x + b eps                          (a == 0: q = b eps)
+//   x_next = alpha x + (beta0 q + beta1 h1 + ...)  (alpha == 1: x + (...))   [+ gamma z when gamma != 0 and z exists]
+#pragma once
+#include "pww_common.cuh"
+
+namespace pww {
+namespace smp {
+
+constexpr int kThreads = 256;
+
+// form[] columns (pipeline.FORM_COLUMNS): alpha, a, b, gamma, history slot, noise row
+struct UpdateArgs {
+  const void* eps;                      // [2m, 4, h, w] UNet output: cond rows 0..m-1, uncond rows m..2m-1
+  int64_t e_sn, e_sc, e_sh, e_sw;       // its element strides
+  float* lat;                           // [m, 4, h, w] fp32, updated in place
+  float* hist;                          // [nh, m, 4, h, w] ring of step-form entries
+  const float* noise;                   // [n, m, 4, h, w] per-step noise rows, or NULL
+  const float* gscale;                  // [m] guidance scale per image
+  const float* beta;                    // [4]
+  const float* form;                    // [6]
+  int m, h, w, nh;
+};
+
+struct InputArgs {
+  const float* lat;                     // [m, 4, h, w] fp32
+  const float* scale;                   // [1] 1/sqrt(sigma^2 + 1)
+  const float* extra;                   // [m, C - 4, h, w] fp32 (inpaint mask + masked-image latents), or NULL
+  void* out;                            // [2m, C, h, w] contiguous, UNet dtype
+  int m, C, hw;
+};
+
+template <typename T> __device__ __forceinline__ float to_f(T v);
+template <> __device__ __forceinline__ float to_f<float>(float v) { return v; }
+template <> __device__ __forceinline__ float to_f<__half>(__half v) { return __half2float(v); }
+
+__device__ __forceinline__ float2 h2_to_f2(unsigned u) {
+  __half2 h;
+  memcpy(&h, &u, sizeof(h));
+  return __half22float2(h);
+}
+
+// PX consecutive fp32 values (PX = 4: one 16-byte access).
+template <int PX>
+__device__ __forceinline__ void load_px(const float* p, float (&v)[PX]) {
+  if constexpr (PX == 4) {
+    const float4 t = *reinterpret_cast<const float4*>(p);
+    v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+  } else {
+    v[0] = *p;
+  }
+}
+template <int PX>
+__device__ __forceinline__ void store_px(float* p, const float (&v)[PX]) {
+  if constexpr (PX == 4) {
+    *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
+  } else {
+    *p = v[0];
+  }
+}
+
+// e[c][j] = channel c of pixel p0 + j of one image's eps.  CL: channels-last packed rows (pixel p's 4 channels at
+// 4p .. 4p+3), read with 8- or 16-byte accesses; otherwise one strided load per element.
+template <typename T, int PX, bool CL>
+__device__ __forceinline__ void load_eps(const T* base, const UpdateArgs& a, int p0, float (&e)[4][PX]) {
+  if constexpr (CL && sizeof(T) == 4) {
+    const float4* s = reinterpret_cast<const float4*>(base + (int64_t)p0 * 4);
+#pragma unroll
+    for (int j = 0; j < PX; ++j) {
+      const float4 t = __ldg(s + j);
+      e[0][j] = t.x; e[1][j] = t.y; e[2][j] = t.z; e[3][j] = t.w;
+    }
+  } else if constexpr (CL && PX == 4) {
+    const uint4* s = reinterpret_cast<const uint4*>(base + (int64_t)p0 * 4);
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {                 // one 16-byte access = two pixels
+      const uint4 t = __ldg(s + k);
+      const float2 a0 = h2_to_f2(t.x), a1 = h2_to_f2(t.y), b0 = h2_to_f2(t.z), b1 = h2_to_f2(t.w);
+      e[0][2 * k] = a0.x; e[1][2 * k] = a0.y; e[2][2 * k] = a1.x; e[3][2 * k] = a1.y;
+      e[0][2 * k + 1] = b0.x; e[1][2 * k + 1] = b0.y; e[2][2 * k + 1] = b1.x; e[3][2 * k + 1] = b1.y;
+    }
+  } else if constexpr (CL) {                      // fp16, one pixel: one 8-byte access
+    const uint2 t = __ldg(reinterpret_cast<const uint2*>(base + (int64_t)p0 * 4));
+    const float2 a0 = h2_to_f2(t.x), a1 = h2_to_f2(t.y);
+    e[0][0] = a0.x; e[1][0] = a0.y; e[2][0] = a1.x; e[3][0] = a1.y;
+  } else {
+#pragma unroll
+    for (int j = 0; j < PX; ++j) {
+      const int p = p0 + j, y = p / a.w, x = p - y * a.w;
+      const T* px = base + y * a.e_sh + x * a.e_sw;
+#pragma unroll
+      for (int c = 0; c < 4; ++c) e[c][j] = to_f(px[c * a.e_sc]);
+    }
+  }
+}
+
+// e[c][j] = eps_u + g (eps_c - eps_u) of image i.
+template <typename T, int PX, bool CL>
+__device__ __forceinline__ void guided_eps(const UpdateArgs& a, int i, int p0, float (&e)[4][PX]) {
+  const T* eps = static_cast<const T*>(a.eps);
+  const float g = __ldg(a.gscale + i);
+  float eu[4][PX];
+  load_eps<T, PX, CL>(eps + (int64_t)i * a.e_sn, a, p0, e);
+  load_eps<T, PX, CL>(eps + (int64_t)(i + a.m) * a.e_sn, a, p0, eu);
+#pragma unroll
+  for (int c = 0; c < 4; ++c)
+#pragma unroll
+    for (int j = 0; j < PX; ++j) e[c][j] = __fadd_rn(eu[c][j], __fmul_rn(g, __fsub_rn(e[c][j], eu[c][j])));
+}
+
+// One thread per (image, PX consecutive pixels), all 4 channels.
+template <typename T, int PX, bool CL>
+__global__ void __launch_bounds__(kThreads) sampler_update_kernel(const UpdateArgs a) {
+  const int hw = a.h * a.w, groups = hw / PX;
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (int64_t)a.m * groups) return;
+  const int i = (int)(idx / groups);
+  const int p0 = (int)(idx - (int64_t)i * groups) * PX;
+  float eg[4][PX];
+  guided_eps<T, PX, CL>(a, i, p0, eg);
+  const float alpha = __ldg(a.form + 0), ca = __ldg(a.form + 1), cb = __ldg(a.form + 2), gamma = __ldg(a.form + 3);
+  const int slot = (int)__ldg(a.form + 4), row = (int)__ldg(a.form + 5);
+  const float b0 = __ldg(a.beta + 0);
+  const bool with_noise = a.noise != nullptr && gamma != 0.f;
+  const int64_t entry = (int64_t)a.m * 4 * hw;   // elements of one history entry / noise row
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    const int64_t off = ((int64_t)i * 4 + c) * hw + p0;
+    float x[PX], q[PX], s[PX];
+    load_px<PX>(a.lat + off, x);
+#pragma unroll
+    for (int j = 0; j < PX; ++j) {
+      const float e = eg[c][j];
+      q[j] = ca == 0.f ? __fmul_rn(cb, e) : __fadd_rn(__fmul_rn(ca, x[j]), __fmul_rn(cb, e));
+      s[j] = __fmul_rn(b0, q[j]);
+    }
+    store_px<PX>(a.hist + slot * entry + off, q);
+    for (int k = 1; k < a.nh; ++k) {
+      const float bk = __ldg(a.beta + k);
+      float hk[PX];
+      load_px<PX>(a.hist + ((slot - k + a.nh) % a.nh) * entry + off, hk);
+#pragma unroll
+      for (int j = 0; j < PX; ++j) s[j] = __fadd_rn(s[j], __fmul_rn(bk, hk[j]));
+    }
+#pragma unroll
+    for (int j = 0; j < PX; ++j) x[j] = alpha == 1.f ? __fadd_rn(x[j], s[j]) : __fadd_rn(__fmul_rn(alpha, x[j]), s[j]);
+    if (with_noise) {
+      float z[PX];
+      load_px<PX>(a.noise + row * entry + off, z);
+#pragma unroll
+      for (int j = 0; j < PX; ++j) x[j] = __fadd_rn(x[j], __fmul_rn(gamma, z[j]));
+    }
+    store_px<PX>(a.lat + off, x);
+  }
+}
+
+template <int PX>
+__device__ __forceinline__ void store_out(float* p, const float (&v)[PX]) { store_px<PX>(p, v); }
+template <int PX>
+__device__ __forceinline__ void store_out(__half* p, const float (&v)[PX]) {
+  if constexpr (PX == 4) {
+    const __half2 lo = __floats2half2_rn(v[0], v[1]), hi = __floats2half2_rn(v[2], v[3]);
+    uint2 u;
+    memcpy(&u.x, &lo, 4);
+    memcpy(&u.y, &hi, 4);
+    *reinterpret_cast<uint2*>(p) = u;
+  } else {
+    *p = __float2half_rn(v[0]);
+  }
+}
+
+// One thread per (image, channel, PX consecutive pixels); writes the value to the cond row i and the uncond row m + i.
+template <typename T, int PX>
+__global__ void __launch_bounds__(kThreads) sampler_input_kernel(const InputArgs a) {
+  const int groups = a.hw / PX;
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (int64_t)a.m * a.C * groups) return;
+  const int ic = (int)(idx / groups);
+  const int i = ic / a.C, c = ic - i * a.C;
+  const int p0 = (int)(idx - (int64_t)ic * groups) * PX;
+  float v[PX];
+  if (c < 4) {
+    load_px<PX>(a.lat + ((int64_t)i * 4 + c) * a.hw + p0, v);
+    const float s = __ldg(a.scale);
+#pragma unroll
+    for (int j = 0; j < PX; ++j) v[j] = __fmul_rn(v[j], s);
+  } else {
+    load_px<PX>(a.extra + ((int64_t)i * (a.C - 4) + (c - 4)) * a.hw + p0, v);
+  }
+  T* out = static_cast<T*>(a.out);
+  store_out<PX>(out + ((int64_t)i * a.C + c) * a.hw + p0, v);
+  store_out<PX>(out + ((int64_t)(i + a.m) * a.C + c) * a.hw + p0, v);
+}
+
+inline unsigned blocks_for(int64_t threads) { return (unsigned)((threads + kThreads - 1) / kThreads); }
+
+template <typename T>
+cudaError_t launch_update(const UpdateArgs& a, bool px4, bool cl, cudaStream_t s) {
+  const int64_t hw = (int64_t)a.h * a.w;
+  if (px4) {
+    const unsigned g = blocks_for(a.m * hw / 4);
+    if (cl) sampler_update_kernel<T, 4, true><<<g, kThreads, 0, s>>>(a);
+    else sampler_update_kernel<T, 4, false><<<g, kThreads, 0, s>>>(a);
+  } else {
+    const unsigned g = blocks_for(a.m * hw);
+    if (cl) sampler_update_kernel<T, 1, true><<<g, kThreads, 0, s>>>(a);
+    else sampler_update_kernel<T, 1, false><<<g, kThreads, 0, s>>>(a);
+  }
+  return cudaGetLastError();
+}
+
+template <typename T>
+cudaError_t launch_input(const InputArgs& a, bool px4, cudaStream_t s) {
+  const int64_t n = (int64_t)a.m * a.C * a.hw;
+  if (px4) sampler_input_kernel<T, 4><<<blocks_for(n / 4), kThreads, 0, s>>>(a);
+  else sampler_input_kernel<T, 1><<<blocks_for(n), kThreads, 0, s>>>(a);
+  return cudaGetLastError();
+}
+
+}  // namespace smp
+}  // namespace pww

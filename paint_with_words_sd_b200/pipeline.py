@@ -7,8 +7,9 @@ What is different underneath (results equal within the stated fp16 tolerance):
   * the attention of every UNet block runs in libpww_b200.so (see attention.py);
   * cond and uncond are ONE batch-2 UNet forward with per-image bias enable and per-image score
     statistic instead of two batch-1 forwards (paint_with_words.py:483-499);
-  * the whole step (UNet, CFG combine, LMS update) is captured in a CUDA graph; sigma, G(sigma) and the
-    LMS coefficients are device scalars refreshed by tiny copies, so a replay does no host math;
+  * the whole step (UNet input, UNet, CFG combine + sampler update as two native launches) is captured in a CUDA
+    graph; sigma, G(sigma) and the sampler's step-form coefficients are device scalars refreshed by one tiny copy, so
+    a replay does no host math;
   * K/V of the text context are step-invariant, so the context tensors are staged once per image.
 """
 from __future__ import annotations
@@ -24,7 +25,9 @@ from PIL import Image
 
 from . import attention as _attention
 from .conditioning import _encode_text_color_inputs, _get_binary_mask, pack_weight_map, packed_key
-from .scheduler import LMSDiscreteScheduler
+from . import _native
+from .scheduler import (SIGMA_SCHEDULERS, EulerAncestralDiscreteScheduler, LMSDiscreteScheduler, history_length,
+                        step_form)
 from .synthetic import IdentityVAE, RandomTextEncoder, SimpleWordTokenizer
 from .unet import UNet2DConditionModel, UNetConfig, build_unet
 from .weight_function import STAT_MAX, UnsupportedWeightFunction, g_of_sigma, probe_weight_function
@@ -84,6 +87,11 @@ def pww_load_tools(device: str = "cuda:0", scheduler_type=LMSDiscreteScheduler,
     return vae, unet, text_encoder, tokenizer, scheduler
 
 
+def _dtype_code(dtype) -> int:
+    """The C ABI's dtype code; -1 (rejected by the kernels as unsupported) for anything but fp16 / fp32."""
+    return {torch.float32: _native.PWW_DTYPE_F32, torch.float16: _native.PWW_DTYPE_F16}.get(dtype, -1)
+
+
 def _module_dtype(module, default=torch.float32):
     p = next(iter(module.parameters()), None) if hasattr(module, "parameters") else None
     return p.dtype if p is not None else default
@@ -120,6 +128,18 @@ def initial_latents(latent_size, seed: int, extra_seeds: Dict[int, int], seperat
 # ---------------------------------------------------------------------------------------------
 # the engine
 # ---------------------------------------------------------------------------------------------
+def ancestral_noise(seeds: Sequence[int], shape: Tuple[int, ...], n: int) -> torch.Tensor:
+    """[n, m, *shape] fp32: image i's rows are draws 1..n of `torch.Generator().manual_seed(seeds[i])` on the CPU, each
+    `shape`-sized (draw 0 is that seed's initial noise), as a diffusers pipeline given `generator=torch.manual_seed(seed)`
+    draws them.  Per image, so batching and sharding do not change which noise an image gets."""
+    per_image = []
+    for s in seeds:
+        g = torch.Generator().manual_seed(int(s))
+        torch.randn(shape, generator=g)
+        per_image.append(torch.stack([torch.randn(shape, generator=g) for _ in range(n)]))
+    return torch.stack(per_image, 1)
+
+
 def _per_image(value, m: int, name: str, is_one) -> list:
     """One setting for every image, or a sequence of exactly m settings."""
     if is_one(value):
@@ -134,8 +154,13 @@ class PwWSampler:
     """Denoising loop for a group of images on ONE GPU (paint_with_words.py:471-506 semantics per image).
 
     Each image i has a cond context dict, an uncond context dict and latents; a step runs one UNet
-    forward over the batch [cond_0..cond_{m-1}, uncond_0..uncond_{m-1}], the CFG combine and the LMS
-    update.  `use_graph=True` captures the step in a CUDA graph.
+    forward over the batch [cond_0..cond_{m-1}, uncond_0..uncond_{m-1}], the CFG combine and the sampler update.
+    `use_graph=True` captures the step in a CUDA graph.
+
+    `scheduler` is an LMS, Euler, Euler ancestral or DPM++ 2M scheduler of `scheduler.py` (any other class raises
+    TypeError).  Every sampler is one linear step form per image (`scheduler.step_form`), tabulated for every step at
+    set-up.  The ancestral sampler needs `noise_seed` (one int, or m ints): image i's step noise is
+    `ancestral_noise([seed_i], ...)`; the other samplers ignore it.
 
     `weight_function` is one callable for every image or a sequence of m callables, one per image, and `guidance_scale`
     one float or m floats: images made with different settings share the sampler, and every cross-attention call is
@@ -146,7 +171,11 @@ class PwWSampler:
     def __init__(self, unet, scheduler: LMSDiscreteScheduler, cond_ctxs: Sequence[dict], uncond_ctxs: Sequence[dict],
                  latents: torch.Tensor, weight_function: Union[Callable, Sequence[Callable]],
                  guidance_scale: Union[float, Sequence[float]] = 7.5,
-                 extra_input: Optional[torch.Tensor] = None, use_graph: bool = True, timesteps=None):
+                 extra_input: Optional[torch.Tensor] = None, use_graph: bool = True, timesteps=None,
+                 noise_seed: Union[None, int, Sequence[int]] = None):
+        if not isinstance(scheduler, SIGMA_SCHEDULERS):
+            raise TypeError(f"PwWSampler does not support {type(scheduler).__name__}; use one of "
+                            + ", ".join(c.__name__ for c in SIGMA_SCHEDULERS))
         self.unet, self.scheduler = unet, scheduler
         self.m = len(cond_ctxs)
         self.device = latents.device
@@ -156,8 +185,16 @@ class PwWSampler:
         self._fns = _per_image(weight_function, self.m, "weight_function", callable)
         scales = _per_image(self.guidance_scale, self.m, "guidance_scale", lambda g: isinstance(g, float))
         self.timesteps = list((scheduler.timesteps if timesteps is None else timesteps).tolist())
-        self.latents = latents.clone().float()
-        self.extra_input = extra_input            # inpaint: [m,5,h,w] (mask + masked-image latents)
+        # the sampler kernels index latents [m,4,h,w] and extra_input [m,5,h,w] as contiguous fp32 buffers: a private
+        # contiguous copy, whatever the caller's layout, and shapes checked against the m images
+        if latents.dim() != 4 or tuple(latents.shape[:2]) != (self.m, 4):
+            raise ValueError(f"latents must be [{self.m}, 4, h, w] (one per image), got {tuple(latents.shape)}")
+        self.latents = latents.to(torch.float32, memory_format=torch.contiguous_format, copy=True)
+        if extra_input is not None and tuple(extra_input.shape) != (self.m, 5) + tuple(latents.shape[2:]):
+            raise ValueError(f"extra_input must be [{self.m}, 5, {latents.shape[2]}, {latents.shape[3]}] (mask + masked-"
+                             f"image latents per image), got {tuple(extra_input.shape)}")
+        self.extra_input = (None if extra_input is None else     # inpaint: [m,5,h,w] (mask + masked-image latents)
+                            extra_input.to(self.device, torch.float32, memory_format=torch.contiguous_format))
         self.use_graph = use_graph and latents.is_cuda
         self._graph = None
         self._kv_graph = None
@@ -174,30 +211,51 @@ class PwWSampler:
         self._unet_dtype = up.dtype if up is not None else torch.float32
         self._ctx = self._merge_contexts(cond_ctxs, uncond_ctxs)
         dev = self.device
-        # Per-step scalars (sigma, 1/sqrt(sigma^2+1), t, 4 LMS coefficients, G_0(sigma) .. G_{m-1}(sigma)) are
-        # tabulated once on the host and uploaded; a step copies its row into `_params` (one D2D copy), so a captured
-        # graph sees new values and the host never feeds the stream mid-loop.  `_params` has m more entries that stay 0:
-        # G_SIGMA holds one value per image of the UNet batch, and the uncond images are unbiased.
-        self._table = self._build_step_table().to(dev)
-        self._params = torch.zeros(7 + 2 * self.m, dtype=torch.float32, device=dev)
-        self._derivs = torch.zeros((4,) + tuple(self.latents.shape), dtype=torch.float32, device=dev)
-        self._ctx["G_SIGMA"] = self._params[7:]
-        self._gscale = torch.tensor(scales, dtype=torch.float32, device=dev).view(self.m, 1, 1, 1)
+        # Per-step scalars are tabulated once on the host and uploaded; a step copies its row into `_params` (one D2D
+        # copy), so a captured graph sees new values and the host never feeds the stream mid-loop.  A row is
+        #   [sigma, 1/sqrt(sigma^2+1), t, beta0..beta3, G_0(sigma) .. G_{m-1}(sigma), 0 x m, alpha, a, b, gamma, slot, row]
+        # (`_table` is its first 7 + m columns; FORM_COLUMNS names the last six).  G_SIGMA holds one value per image of
+        # the UNet batch: the m zeros leave the uncond images unbiased.
+        m = self.m
+        table = self._build_step_table()
+        self._hist_len = history_length(scheduler)
+        self._rows = torch.cat([table, torch.zeros(table.shape[0], m), self._build_form_table()], 1).to(dev)
+        self._table = self._rows[:, :7 + m]
+        self._params = torch.zeros(self._rows.shape[1], dtype=torch.float32, device=dev)
+        self._derivs = torch.zeros((self._hist_len,) + tuple(self.latents.shape), dtype=torch.float32, device=dev)
+        self._ctx["G_SIGMA"] = self._params[7:7 + 2 * m]
+        self._gscale = torch.tensor(scales, dtype=torch.float32, device=dev).view(m, 1, 1, 1)
+        self._noise = None
+        if isinstance(scheduler, EulerAncestralDiscreteScheduler):
+            if noise_seed is None:
+                raise ValueError(f"{type(scheduler).__name__} draws noise every step: pass noise_seed (one int or {m})")
+            seeds = _per_image(noise_seed, m, "noise_seed", lambda v: isinstance(v, (int, np.integer)))
+            self._noise = ancestral_noise(seeds, tuple(self.latents.shape[1:]), len(self.timesteps)).to(dev)
+        channels = 4 + (0 if self.extra_input is None else int(self.extra_input.shape[1]))
+        self._unet_in = torch.empty((2 * m, channels) + tuple(self.latents.shape[2:]), dtype=self._unet_dtype,
+                                    device=dev)
         self._step_no = 0
+
+    def step_forms(self) -> List[tuple]:
+        """float64 (alpha, a, b, [beta0..beta3], gamma) of every step of this run (`scheduler.step_form`); the run's
+        first step has no history."""
+        sch = self.scheduler
+        return [step_form(sch, sch.step_index_of(t), first=(i == 0)) for i, t in enumerate(self.timesteps)]
 
     def _build_step_table(self) -> torch.Tensor:
         sch = self.scheduler
         rows = []
-        for t in self.timesteps:
+        for t, (_, _, _, beta, _) in zip(self.timesteps, self.step_forms()):
             si = sch.step_index_of(t)
             sigma = float(sch.sigmas[si])
-            # paint_with_words.py:506 -> LMS order = min(step_index+1, 4) on the ABSOLUTE schedule index;
-            # missing history (img2img starts mid-schedule) simply contributes nothing (zip truncation).
-            coeffs = list(sch._coeffs[si]) if sch._coeffs is not None else sch._lms_coeffs(si, min(si + 1, 4))
-            coeffs = (coeffs + [0.0] * 4)[:4]
             gs = [g_of_sigma(f, pr, sch.sigmas[si]) for f, pr in zip(self._fns, self._probed)]
-            rows.append([sigma, 1.0 / math.sqrt(sigma * sigma + 1.0), float(t), *coeffs, *gs])
+            rows.append([sigma, 1.0 / math.sqrt(sigma * sigma + 1.0), float(t), *beta, *gs])
         return torch.tensor(rows, dtype=torch.float32)
+
+    def _build_form_table(self) -> torch.Tensor:
+        """[steps, 6] = FORM_COLUMNS: alpha, a, b, gamma, the history slot this step writes, the noise row it reads."""
+        return torch.tensor([[alpha, a, b, gamma, float(i % self._hist_len), float(i)]
+                             for i, (alpha, a, b, _, gamma) in enumerate(self.step_forms())], dtype=torch.float32)
 
     def _merge_contexts(self, conds, unconds) -> dict:
         """Batch the per-image dicts: CONTEXT_TENSOR -> [2m,T,Dc]; weight maps -> [m,N,T] stacks;
@@ -245,22 +303,30 @@ class PwWSampler:
 
     # -- one step, expressed only with device tensors / device scalars --------------------------
     def _step_body(self):
-        m = self.m
-        x = self.latents * self._params[1]
-        if self.extra_input is not None:
-            x = torch.cat([x, self.extra_input], dim=1)
-        x2 = torch.cat([x, x], 0).to(self._unet_dtype)      # the reference runs under autocast: feed the UNet its own dtype
-        eps = self.unet(x2, self._params[2:3], encoder_hidden_states=self._ctx).sample.float()
-        eps_c, eps_u = eps[:m], eps[m:]
-        noise_pred = eps_u + self._gscale * (eps_c - eps_u)
-        # LMS (epsilon prediction): derivative == noise_pred; history kept in a rolling device buffer
-        self._derivs.copy_(torch.roll(self._derivs, 1, 0))
-        self._derivs[0].copy_(noise_pred)
-        upd = (self._params[3:7].view(4, 1, 1, 1, 1) * self._derivs).sum(0)
-        self.latents.add_(upd)
+        m, (h, w) = self.m, self.latents.shape[-2:]
+        L = _native.lib()
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        f32 = self._params.element_size()
+        # the UNet input in the UNet's own dtype (the reference runs under autocast): [2m, C, h, w], rows i and m + i
+        # both fp16(latents_i / sqrt(sigma^2 + 1)) [+ the inpaint channels]
+        _native.check(L.pww_sampler_input(self.latents.data_ptr(), self._params.data_ptr() + f32,
+                                          None if self.extra_input is None else self.extra_input.data_ptr(),
+                                          self._unet_in.data_ptr(), _dtype_code(self._unet_in.dtype), m,
+                                          self._unet_in.shape[1], h, w, stream), "pww_sampler_input")
+        eps = self.unet(self._unet_in, self._params[2:3], encoder_hidden_states=self._ctx).sample
+        if tuple(eps.shape) != (2 * m, 4, h, w) or eps.device != self.device:
+            raise ValueError(f"the UNet returned {tuple(eps.shape)} on {eps.device}; expected {(2 * m, 4, h, w)}")
+        # CFG with the per-image scale, then the step form; eps is read in place through its strides
+        form = self._params.data_ptr() + (7 + 2 * m) * f32
+        _native.check(L.pww_sampler_update(eps.data_ptr(), _dtype_code(eps.dtype), *eps.stride(),
+                                           self.latents.data_ptr(), self._derivs.data_ptr(), self._hist_len,
+                                           None if self._noise is None else self._noise.data_ptr(),
+                                           self._gscale.data_ptr(), self._params.data_ptr() + 3 * f32, form, m, h, w,
+                                           stream), "pww_sampler_update")
+        _native.launch_count += 2
 
     def _set_step_scalars(self, i: int, step_index: int):
-        self._params[:self._table.shape[1]].copy_(self._table[i])
+        self._params.copy_(self._rows[i])
         self._ctx["SIGMA"] = self.scheduler.sigmas[step_index]
 
     # -- host-buffer interface (what bench.py's e2e leg drives) -----------------------------------
@@ -302,13 +368,15 @@ class PwWSampler:
         return n
 
     def restart(self, latents: Optional[torch.Tensor] = None):
-        """Rewind to step 0 (fresh LMS history), optionally with new latents."""
+        """Rewind to step 0 (empty history, the first noise row), optionally with new latents."""
         self._step_no = 0
         self._derivs.zero_()
         if latents is not None:
             self.latents.copy_(latents)
 
     def step(self):
+        if not self.latents.is_cuda:
+            raise RuntimeError("PwWSampler steps run on a CUDA device (the sampler kernels have no CPU version)")
         i = self._step_no
         step_index = self.scheduler.step_index_of(self.timesteps[i])
         self._set_step_scalars(i, step_index)
@@ -397,7 +465,7 @@ def paint_with_words(
         latents = scheduler.add_noise(init_latents, noise, timesteps[:1])
 
     sampler = PwWSampler(unet, scheduler, [cond], [uncond], latents, weight_function, guidance_scale,
-                         timesteps=timesteps)
+                         timesteps=timesteps, noise_seed=seed)
     latents = sampler.run()
     if return_latents:
         return latents
@@ -487,7 +555,7 @@ def paint_with_words_batch(
         sampler = PwWSampler(unet, scheduler, [encoded[i][0] for i in idx], [encoded[i][1] for i in idx],
                              torch.cat([encoded[i][2] for i in idx], 0),
                              [entries[i]["weight_function"] for i in idx], [entries[i]["guidance_scale"] for i in idx],
-                             timesteps=scheduler.timesteps)
+                             timesteps=scheduler.timesteps, noise_seed=[entries[i]["seed"] for i in idx])
         latents = sampler.run()
         for j, i in enumerate(idx):
             results[i] = latents[j:j + 1].clone()
@@ -583,7 +651,8 @@ def paint_with_words_inpaint(
             f"num_channels_latents: {latents.shape[1]} + num_channels_mask: {mask.shape[1]} + "
             f"num_channels_masked_image: {masked_image_latents.shape[1]} = {total}.")
     sampler = PwWSampler(unet, scheduler, [cond], [uncond], latents, weight_function, guidance_scale,
-                         extra_input=torch.cat([mask, masked_image_latents], 1).float(), timesteps=timesteps)
+                         extra_input=torch.cat([mask, masked_image_latents], 1).float(), timesteps=timesteps,
+                         noise_seed=seed)
     latents = sampler.run()
     if return_latents:
         return latents

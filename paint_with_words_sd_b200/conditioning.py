@@ -115,7 +115,7 @@ def _tokens_img_attention_factors(img_context_seperated, tokenized_texts, ratio:
     return torch.stack(cols, dim=1), torch.stack(counts, dim=1)
 
 
-PACK_COLS = 32          # fp16 columns per pixel of the packed map (csrc/xattn_fused.cuh: kMW)
+PACK_COLS = 32          # fp16 columns per pixel of the packed map (csrc/xattn_fused2.cuh: kMW)
 PACK_CAPACITY = 10      # distinct non-zero columns a packed map can hold (kRC)
 PACK_TOKENS = 80        # padded token count of the column index (kTP), per key chunk
 CHUNK_TOKENS = 77       # one CLIP window: [BOS] + up to 75 prompt tokens + [EOS] (+ padding)

@@ -4,7 +4,6 @@
 
 #include "pww_common.cuh"
 #include "xattn_tc.cuh"
-#include "xattn_fused.cuh"
 #include "xattn_fused2.cuh"
 #include "attn_tc.cuh"
 #include "unet_ops.cuh"
@@ -217,11 +216,11 @@ int xattn_fused(const void* q, const void* k, const void* v, void* out, int B, i
   // image b is biased iff it has a packed map: with mpack == NULL every index is -1 (the kernel reads wmap_index)
   int chunk = pww::fx::kMaxBatch;                                  // images per launch
   {                                                                // job table of <= 64 units per CTA
-    const int tiles = pww::ceil_div(N, pww::fx::kBM);
-    const int hg = pww::ceil_div(H, D == 40 ? pww::fx2::Cfg2<40>::G : (D == 64 ? pww::fx2::Cfg2<64>::G : 1));
+    const int tiles = pww::ceil_div(N, pww::core::kBM);
+    const int hg = pww::ceil_div(H, D == 40 ? pww::fx::Cfg2<40>::G : (D == 64 ? pww::fx::Cfg2<64>::G : 1));
     while (chunk > 1) {
       const int cb = B < chunk ? B : chunk;
-      if (pww::fx2::fused2_fits(cb, hg, tiles, pww::fx::fused_grid(cb * hg * tiles))) break;
+      if (pww::fx::fused2_fits(cb, hg, tiles, pww::fx::fused_grid(cb * hg * tiles))) break;
       chunk >>= 1;
     }
   }
@@ -242,11 +241,11 @@ int xattn_fused(const void* q, const void* k, const void* v, void* out, int B, i
     } else if (mpack) {                                            // identity mapping: image b uses map b
       c.wmap_index = nullptr;
       mp = (const __half*)mpack + (int64_t)b0 * mpack_batch_stride;
-      ci = cidx + (int64_t)b0 * pww::fx::kTP * pww::core::chunks_of(T);   // [Bw, 80 k]
+      ci = cidx + (int64_t)b0 * pww::core::kTP * pww::core::chunks_of(T);   // [Bw, 80 k]
     }
     c.wmap = mpack ? (const float*)mp : nullptr;                   // non-null marks "maps present" for the kernel
     const cudaError_t e =
-        with_shape(D, T, [&](auto k) { return pww::fx2::launch_fused2<k.D, k.KC>(c, mp, mpack_batch_stride, ci, s); });
+        with_shape(D, T, [&](auto k) { return pww::fx::launch_fused2<k.D, k.KC>(c, mp, mpack_batch_stride, ci, s); });
     if (e == cudaErrorInvalidConfiguration) return PWW_ERR_UNSUPPORTED;
     if (e != cudaSuccess) return cuda_fail(e);
   }
@@ -436,7 +435,7 @@ int pww_sampler_update(const void* eps, int eps_dtype, int64_t eps_batch_stride,
 }
 
 // Test infrastructure (not declared in the public header): replay the forward kernel's unit schedule on the host.
-// wmap_index and out are HOST pointers; out receives 8 int32 per unit (see fwd_schedule_host); returns the number of
+// wmap_index and out are HOST pointers; out receives 5 int32 per unit (see fwd_schedule_host); returns the number of
 // units written or a negative value for bad arguments.  No GPU needed.
 int pww_debug_fwd_schedule(int B, int H, int tiles, int grid, const int* wmap_index, int* out) {
   if (!wmap_index || !out) return PWW_ERR_BAD_ARG;
@@ -449,13 +448,13 @@ int pww_debug_set_fused_grid(int grid) {
   pww::fx::debug_grid() = grid < 0 ? 0 : grid;
   return PWW_OK;
 }
-// Host replay of the grouped-head kernel's job lists (14 int32 per job, see fused2_schedule_host).
+// Host replay of the grouped-head kernel's job lists (8 int32 per job, see fused2_schedule_host).
 int pww_debug_fused2_schedule(int B, int H, int G, int tiles, int grid, const int* wmap_index, int* out, int max_jobs) {
   if (!wmap_index || !out) return PWW_ERR_BAD_ARG;
-  return pww::fx2::fused2_schedule_host(B, H, G, tiles, grid, wmap_index, out, max_jobs);
+  return pww::fx::fused2_schedule_host(B, H, G, tiles, grid, wmap_index, out, max_jobs);
 }
 // Heads per unit of the grouped-head kernel at head dim 40 (a build-time constant).
-int pww_debug_fused2_heads_per_unit(void) { return pww::fx2::Cfg2<40>::G; }
+int pww_debug_fused2_heads_per_unit(void) { return pww::fx::Cfg2<40>::G; }
 // Test infrastructure: device buffer of grid * (2 + 1024) uint32 the grouped-head kernel copies every CTA's job table to.
 int pww_debug_set_fused_jobs_dump(void* device_buffer) {
   pww::fx::debug_jobs_dump() = (unsigned*)device_buffer;

@@ -35,8 +35,7 @@ struct XattnParams {
   const int32_t* stat_kind;   // [B] per-image statistic kind, or NULL = `stat` for every image
   float* stats_out;
   unsigned int* counters;  // [B] arrival counters (zero on entry, zero on exit)
-  StatPartial* partials;   // [B][ctas_per_image]
-  int ctas_per_image;
+  StatPartial* partials;   // [B][grid] partial slots, one per CTA
 };
 
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }

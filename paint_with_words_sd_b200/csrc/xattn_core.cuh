@@ -3,7 +3,7 @@
 // A CTA of 8 warps works on one [128-row x head] tile at a time; warp w owns query rows [16 w, 16 w + 16).  Operands are
 // staged in shared memory by 16-byte cp.async copies (rows of LD = DP + 8 halfs: the 16-byte pad makes every ldmatrix
 // phase hit 8 distinct bank groups), read into registers with ldmatrix and multiplied with mma.m16n8k16 (fp16 in, fp32
-// accumulate).  Cross-attention (keys T <= 80; longer contexts of 2 or 3 CLIP chunks stream one tile per chunk, below):
+// accumulate).  Cross-attention, per chunk of at most 80 keys (the softmax streams over 1, 2 or 3 chunks, below):
 //     S = Q K^T   16 x 80 per warp, DP / 16 k-steps      accumulators: 10 n-tiles x 4 fp32 per thread
 //     P = 2^(log2e * scale * (S + bias - rowmax))        in registers; packed to fp16 it is the A operand of
 //     O = P V     16 x D per warp, 5 k-steps over the 80 padded keys, V fragments by ldmatrix.trans
@@ -70,65 +70,6 @@ __device__ __forceinline__ void warp_qk(uint32_t qs, uint32_t ks, int lane, floa
 // Token of accumulator element e of n-tile j for this lane; the row is lane / 4 (+ 8 for e >= 2).
 __device__ __forceinline__ int tok(int j, int e, int lane) { return 8 * j + 2 * (lane & 3) + (e & 1); }
 
-// Softmax of the warp's 16 rows over the T real tokens (s already holds S + bias) followed by O = P V, normalised.
-template <int D>
-__device__ __forceinline__ void warp_softmax_pv(float (&s)[10][4], int T, float sl2, uint32_t vs, int lane,
-                                                float (&o)[Tile<D>::NT][4]) {
-  using C = Tile<D>;
-  float m0 = -INFINITY, m1 = -INFINITY;
-#pragma unroll
-  for (int j = 0; j < 10; ++j)
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      if (tok(j, e, lane) >= T) s[j][e] = -INFINITY;
-      if (e < 2) m0 = fmaxf(m0, s[j][e]); else m1 = fmaxf(m1, s[j][e]);
-    }
-  m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1));
-  m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
-  m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
-  m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
-  const float n0 = -m0 * sl2, n1 = -m1 * sl2;
-  uint32_t pa[5][4];
-  float l0 = 0.f, l1 = 0.f;
-#pragma unroll
-  for (int j = 0; j < 10; ++j) {
-    const uint32_t p01 = ptx::pack_h2(ptx::ex2(fmaf(s[j][0], sl2, n0)), ptx::ex2(fmaf(s[j][1], sl2, n0)));
-    const uint32_t p23 = ptx::pack_h2(ptx::ex2(fmaf(s[j][2], sl2, n1)), ptx::ex2(fmaf(s[j][3], sl2, n1)));
-    const float2 f01 = ptx::unpack_h2(p01), f23 = ptx::unpack_h2(p23);    // sum exactly what the MMA multiplies
-    l0 += f01.x + f01.y;
-    l1 += f23.x + f23.y;
-    pa[j >> 1][(j & 1) * 2] = p01;
-    pa[j >> 1][(j & 1) * 2 + 1] = p23;
-  }
-  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
-  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
-  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-#pragma unroll
-  for (int j = 0; j < C::NT; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
-#pragma unroll
-  for (int kk = 0; kk < 5; ++kk) {
-    const int t = 16 * kk + (lane & 7) + ((lane >> 3) & 1) * 8;
-#pragma unroll
-    for (int jp = 0; jp < C::NT / 2; ++jp) {
-      uint32_t b0, b1, b2, b3;
-      ptx::ldsm_x4_t(vs + (uint32_t)(t * C::LD + 16 * jp + (lane >> 4) * 8) * 2u, b0, b1, b2, b3);
-      ptx::mma16816(o[2 * jp], pa[kk], b0, b1);
-      ptx::mma16816(o[2 * jp + 1], pa[kk], b2, b3);
-    }
-    if constexpr (C::NT & 1) {
-      uint32_t b0, b1;
-      ptx::ldsm_x2_t(vs + (uint32_t)(t * C::LD + 8 * (C::NT - 1)) * 2u, b0, b1);
-      ptx::mma16816(o[C::NT - 1], pa[kk], b0, b1);
-    }
-  }
-  const float i0 = 1.f / l0, i1 = 1.f / l1;
-#pragma unroll
-  for (int j = 0; j < C::NT; ++j) {
-    o[j][0] *= i0; o[j][1] *= i0; o[j][2] *= i1; o[j][3] *= i1;
-  }
-}
-
 // Normalised O of the warp's 16 rows -> fp16 in global memory: staged over the warp's own Q rows in shared memory (dead
 // once S exists), then written as whole 16-byte pieces of each row.  Rows >= N are dropped.
 template <int D>
@@ -152,17 +93,37 @@ __device__ __forceinline__ void warp_store(const float (&o)[Tile<D>::NT][4], uns
   __syncwarp();
 }
 
-// ---- long contexts: k CLIP chunks of 77 keys (T = 154, 231) ----
-// Chunk c (keys 77 c .. 77 c + 76) is staged as its own 80-row K / V tile, rows 77 .. 79 zero-filled and masked to -inf,
-// so warp_qk runs unchanged on every chunk.  The softmax streams over the chunks (running row max and sum, O rescaled
-// when the max moves, as in attn_tc.cuh); P is packed to fp16 and the row sum is the sum of the fp16 P values that were
-// multiplied, rescaled in fp32.
+// ---- key chunks: T <= 80 is one chunk of T keys; T = 154, 231 are 2 / 3 CLIP chunks of 77 ----
+// Chunk c (keys 77 c .. 77 c + kv - 1) is staged as its own 80-row K / V tile, rows kv .. 79 zero-filled and masked to
+// -inf, so warp_qk runs unchanged on every chunk.  The softmax streams over the chunks (running row max and sum, O
+// rescaled when the max moves, as in attn_tc.cuh); P is packed to fp16 and the row sum is the sum of the fp16 P values
+// that were multiplied, rescaled in fp32.  The first chunk's rescale factor is ex2(-inf * scale) = 0 (scale > 0), so a
+// single chunk gives exactly the one-pass softmax.
 constexpr int kChunk = 77;      // keys per CLIP chunk
 constexpr int kMaxChunks = 3;
 __host__ __device__ __forceinline__ constexpr int chunks_of(int T) { return T <= kTP ? 1 : T / kChunk; }
 // T <= 80 (one tile) or a whole number of chunks, at most kMaxChunks.
 __host__ __device__ __forceinline__ constexpr bool supported_keys(int T) {
   return T <= kTP || T == 2 * kChunk || T == kMaxChunks * kChunk;
+}
+// Real keys of every chunk of a KC-chunk instance.
+template <int KC>
+__host__ __device__ __forceinline__ constexpr int chunk_keys(int T) { return KC == 1 ? T : kChunk; }
+
+// Copies of one job's operands into a stage: Q rows of the tile, then K (and V) rows of head h, one 80-row tile per
+// chunk with chunk_keys<KC>(T) real rows.  The caller commits the group.
+template <int D, int KC>
+__device__ __forceinline__ void load_operands(uint32_t st, const XattnParams& p, int b, int h, int tile, bool with_v) {
+  using C = Tile<D>;
+  const int rows = p.N - tile * kBM;
+  load_rows<D>(st, p.q + (int64_t)b * p.q_bs + (int64_t)tile * kBM * p.q_rs + h * D, p.q_rs, kBM, rows < kBM ? rows : kBM);
+  const int kv = chunk_keys<KC>(p.T);
+#pragma unroll 1
+  for (int c = 0; c < KC; ++c) {
+    const int64_t off = (int64_t)b * p.k_bs + (int64_t)c * kChunk * p.k_rs + h * D;
+    load_rows<D>(st + C::QBYTES + c * C::KBYTES, p.k + off, p.k_rs, kTP, kv);
+    if (with_v) load_rows<D>(st + C::QBYTES + (KC + c) * C::KBYTES, p.v + off, p.k_rs, kTP, kv);
+  }
 }
 
 template <int D>
@@ -173,9 +134,10 @@ __device__ __forceinline__ void warp_online_begin(float (&o)[Tile<D>::NT][4], fl
   l0 = l1 = 0.f;
 }
 
-// One chunk: s holds S + bias of the chunk's 80 padded keys, vs is its V tile.  l0 / l1 are per-thread partial row sums.
+// One chunk: s holds S + bias of the chunk's 80 padded keys, of which the first kv are real; vs is its V tile.  l0 / l1
+// are per-thread partial row sums.
 template <int D>
-__device__ __forceinline__ void warp_online_chunk(float (&s)[10][4], float sl2, uint32_t vs, int lane,
+__device__ __forceinline__ void warp_online_chunk(float (&s)[10][4], int kv, float sl2, uint32_t vs, int lane,
                                                   float (&o)[Tile<D>::NT][4], float& m0, float& m1, float& l0, float& l1) {
   using C = Tile<D>;
   float t0 = -INFINITY, t1 = -INFINITY;
@@ -183,7 +145,7 @@ __device__ __forceinline__ void warp_online_chunk(float (&s)[10][4], float sl2, 
   for (int j = 0; j < 10; ++j)
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
-      if (tok(j, e, lane) >= kChunk) s[j][e] = -INFINITY;
+      if (tok(j, e, lane) >= kv) s[j][e] = -INFINITY;
       if (e < 2) t0 = fmaxf(t0, s[j][e]); else t1 = fmaxf(t1, s[j][e]);
     }
   t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, 1));
@@ -262,6 +224,30 @@ __device__ __forceinline__ void warp_stat(const float (&s)[10][4], int T, int ro
         sumsq = fmaf(h, h, sumsq);
       }
     }
+}
+
+// Warp reduction of a (max, sum, sumsq) partial: every lane ends with the warp's total.
+__device__ __forceinline__ void warp_reduce_stat(double& m, double& a, double& q) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+    a += __shfl_xor_sync(0xffffffffu, a, o);
+    q += __shfl_xor_sync(0xffffffffu, q, o);
+  }
+}
+
+// The statistic of an image from its totals over all H * N * T scores: the maximum, or the unbiased standard deviation
+// (variance clamped at 0), rounded to fp16 as qk.max() / qk.std() return it in the reference.
+__device__ __forceinline__ float stat_value(const XattnParams& p, bool is_max, double m, double a, double q) {
+  const double cnt = (double)p.H * (double)p.N * (double)p.T;
+  double r;
+  if (is_max) {
+    r = m;
+  } else {
+    const double var = (q - a * a / cnt) / (cnt - 1.0);
+    r = sqrt(var > 0.0 ? var : 0.0);
+  }
+  return round_to_f16((float)r);
 }
 
 }  // namespace core

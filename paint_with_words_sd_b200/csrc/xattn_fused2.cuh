@@ -9,7 +9,7 @@
 //        summed by the waiters in CTA order -- deterministic for a given grid);
 //     2. softmax jobs of the unbiased units: they need no statistic and overlap the other CTAs' statistic pass;
 //     3. grid barrier (per biased image, only the CTAs that publish for it), then the softmax jobs of the biased units
-//        with the bias x * W, x = g(sigma) * fp16(statistic), W rebuilt from the packed map (xattn_fused.cuh).
+//        with the bias x * W, x = g(sigma) * fp16(statistic), W rebuilt from the packed map (below).
 // The statistic kind and g(sigma) are per image when the launch carries per-image arrays (XattnParams::stat_kind,
 // g_stride = 1), else one kind and one g(sigma) for every image; each CTA keeps the kind of its local biased images in
 // shared memory, so the statistic jobs, the publish step and the finalise step branch per image.
@@ -17,27 +17,48 @@
 // 8 warps of the CTA with the warp-level MMA tiles of xattn_core.cuh; the cp.async copies of job i + 1 (Q rows, K, V
 // and, for biased softmax jobs, the row tile's packed map) are in flight while job i is computed.
 //
-// Long contexts (KC = 2 or 3 chunks): a stage holds one 80-row K and V tile per chunk; a job loops over the chunks
-// (statistic: S of every chunk; softmax: per-chunk bias and the streaming softmax of xattn_core.cuh).  Where two such
-// stages do not fit in shared memory (head dim 80 at 3 chunks, head dim 160 at 2 and 3) the kernel runs on one stage and
-// the copies of job i + 1 start once job i is done.  The unit and job order do not depend on KC.
+// Key chunks (KC = 1, 2 or 3): a stage holds one 80-row K and V tile per chunk; a job loops over the chunks (statistic:
+// S of every chunk; softmax: per-chunk bias and the streaming softmax of xattn_core.cuh).  Where two such stages do not
+// fit in shared memory (head dim 80 at 3 chunks, head dim 160 at 2 and 3) the kernel runs on one stage and the copies of
+// job i + 1 start once job i is done.  The unit and job order do not depend on KC.
+//
+// Packed weight map (SURVEY 8f-4).  The reference's dense [N, 77] fp32 map has at most a handful of distinct non-zero
+// columns (one per painted region, paint_with_words.py:255-272), so it is stored as a column dictionary:
+//     W[n, t] = Mu[n, cidx[t]]      Mu [N, R] fp32 (R <= 10 distinct columns), cidx [77] (-1 = zero column)
+// and Mu is split into fp16 hi/lo halves:  mpack[n] = [ hi(Mu[n,0..9]) | lo(Mu[n,0..9]) | hi(Mu[n,0..9]) | 0 0 ]  (32 fp16,
+// 64 bytes per row instead of 308).  The kernel rebuilds W[n, t] = hi + lo in fp32 (exact to 2^-22 relative) from the row
+// tile's 8 KB of packed map in shared memory and adds x * W to the fp32 scores.
 #pragma once
 #include "mma_sm90.cuh"
 #include "pww_common.cuh"
 #include "xattn_core.cuh"
 #include "xattn_tc.cuh"      // num_sms, cur_device, tc_error_buf
-#include "xattn_fused.cuh"   // FxWalk, fx_range, fx_cta_has_image, debug knobs
 
 namespace pww {
-namespace fx2 {
-using namespace fx;   // unit walk, helpers and constants shared with the host replay
+namespace fx {
+
+constexpr int kMaxBatch = 32;     // images per launch (the C ABI splits larger batches)
+constexpr int kMaxLocal = 4;      // biased images one CTA's unit range may touch (checked on the host)
+constexpr int kMW = 32;           // packed-map columns per row (64 bytes)
+constexpr int kRC = 10;           // dictionary capacity (distinct non-zero columns)
+
+struct FxParams {
+  XattnParams x;            // q/k/v/out, strides, wmap_index, g_sigma, scale, stat, stats_out, counters, partials
+  const int8_t* cidx;       // [Bw, 80 k] dictionary column per token (k key chunks; token 77 c + j at 80 c + j), -1 = none
+  const void* mpack;        // [Bw, N, 32] fp16 packed maps (see above)
+  int64_t mpack_bs;         // elements
+  int tiles, units;
+  int grid;                 // CTAs (== gridDim.x): partial slots per image
+  int hg;                   // head groups per row tile
+  unsigned* jobs_dump;      // debug only: [grid][2 + 2 * 512] = njobs, nstat, job table of every CTA
+};
 
 template <int D, int KC = 1>
 struct Cfg2 {
   // heads per unit (the granularity of a CTA's range): 2 at head dims 40 and 64, one head at 80 and 160
   static constexpr int G = (D == 40 || D == 64) ? 2 : 1;
   using T_ = core::Tile<D>;
-  static constexpr uint32_t MBYTES = kBM * kMW * 2;                    // packed-map rows of the row tile
+  static constexpr uint32_t MBYTES = core::kBM * kMW * 2;              // packed-map rows of the row tile
   static constexpr uint32_t OFF_M = T_::QBYTES + 2 * KC * T_::KBYTES;
   static constexpr uint32_t STAGE = OFF_M + MBYTES;                    // Q | K chunks | V chunks | map of one job
   static constexpr int NST = (2 * STAGE + 8192 <= 232448) ? 2 : 1;     // stages (see the header)
@@ -46,38 +67,111 @@ struct Cfg2 {
 };
 
 // ------------------------------------------------------------------------------------------------------------------
-// job lists (shared by the kernel and the host replay)
+// unit order (shared by the kernel and the host replay)
 // ------------------------------------------------------------------------------------------------------------------
-// ------------------------------------------------------------------------------------------------------------------
-// job lists (shared by the kernel and the host replay)
-// ------------------------------------------------------------------------------------------------------------------
-// Units are walked with the per-head kernel's FxWalk, "heads" being head GROUPS (hg = ceil(H / G) of them); a unit
-// expands into one job per head of its group.  A CTA runs three passes over its contiguous unit range, as in the
-// per-head kernel: statistic jobs of the biased units, softmax jobs of the unbiased units, softmax jobs of the biased
-// units.  `up` numbers the unit passes in processing order (Q ring), `ul` is the unit's position in the CTA's range.
-struct Fx2Job {
+// `img` lists the biased images first (nb of them), then the unbiased ones.  Groups: np = min(nb, nu) PAIR groups (biased
+// image img[g] + unbiased image img[nb + g], tiles * 2H units: tile-major, then head, biased unit before unbiased), then
+// the SOLO groups of the images without a partner (tiles * H units).  A CTA takes a contiguous range of this order, so it
+// gets the same number of biased and unbiased units (+-1) whatever the image order of the batch, and stays inside one or
+// two images.
+struct FxUnit {
   int b, h, tile, biased, gi;
+};
+struct FxWalk {
+  int B, H, tiles, nb, np;
+  const int* img;
+  int gi, tile, j;
+  __host__ __device__ __forceinline__ FxWalk() {}
+  __host__ __device__ __forceinline__ FxWalk(int u, int B_, int H_, int tiles_, int nb_, const int* img_)
+      : B(B_), H(H_), tiles(tiles_), nb(nb_), img(img_) {
+    const int nu = B - nb;
+    np = nb < nu ? nb : nu;
+    const int per_pair = tiles * 2 * H;
+    if (u < np * per_pair) {
+      gi = u / per_pair;
+      const int r = u - gi * per_pair;
+      tile = r / (2 * H);
+      j = r - tile * 2 * H;
+    } else {
+      u -= np * per_pair;
+      const int per_solo = tiles * H;
+      const int s = u / per_solo;
+      gi = np + s;
+      const int r = u - s * per_solo;
+      tile = r / H;
+      j = r - tile * H;
+    }
+  }
+  __host__ __device__ __forceinline__ void next() {
+    const int gsize = gi < np ? 2 * H : H;
+    if (++j == gsize) {
+      j = 0;
+      if (++tile == tiles) { tile = 0; ++gi; }
+    }
+  }
+  __host__ __device__ __forceinline__ FxUnit get() const {
+    FxUnit r;
+    r.tile = tile;
+    r.gi = gi;
+    if (gi < np) {
+      r.h = j >> 1;
+      r.biased = (j & 1) ^ 1;
+      r.b = r.biased ? img[gi] : img[nb + gi];
+    } else {
+      r.h = j;
+      r.biased = (2 * nb > B) ? 1 : 0;
+      r.b = r.biased ? img[gi] : img[nb + gi];
+    }
+    return r;
+  }
+};
+// 32-bit arithmetic on purpose: a 64-bit division is ~100 SASS instructions and this is inlined at every membership test
+// (it was 28 % of the grouped-head kernel's code); the host checks units * grid < 2^32 (fused_units_ok).
+__host__ __device__ __forceinline__ void fx_range(int cta, int grid, int units, int& u0, int& u1) {
+  u0 = (int)((unsigned)cta * (unsigned)units / (unsigned)grid);
+  u1 = (int)((unsigned)(cta + 1) * (unsigned)units / (unsigned)grid);
+}
+inline bool fused_units_ok(long long units, int grid) { return units > 0 && units * (long long)(grid + 1) < (1ll << 32); }
+// Does CTA `cta` own at least one unit of the BIASED image at list position `pos` (== its group index)?
+__host__ __device__ __forceinline__ bool fx_cta_has_image(int cta, int grid, int units, int pos, int H, int tiles, int np) {
+  int lo, hi;
+  fx_range(cta, grid, units, lo, hi);
+  const int per_pair = tiles * 2 * H, per_solo = tiles * H;
+  const bool pair = pos < np;
+  const int base = pair ? pos * per_pair : np * per_pair + (pos - np) * per_solo;
+  const int len = pair ? per_pair : per_solo;
+  const int a = lo > base ? lo : base, b = hi < base + len ? hi : base + len;
+  if (a >= b) return false;
+  if (!pair) return true;
+  return (b - a >= 2) || (((a - base) & 1) == 0);        // biased units sit at even offsets of a pair group
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// job lists (shared by the kernel and the host replay)
+// ------------------------------------------------------------------------------------------------------------------
+// Units are walked with FxWalk, "heads" being head GROUPS (hg = ceil(H / G) of them); a unit expands into one job per
+// head of its group.  A CTA runs three passes over its contiguous unit range: statistic jobs of the biased units,
+// softmax jobs of the unbiased units, softmax jobs of the biased units.
+struct Fx2Job {
+  int b, h, tile, biased;
   int kind;     // 0 = stat, 1 = main
-  int i;        // job index (score slot = i % NS, softmax group = i % 2, K stage = i % NK)
-  int m;        // main-job index (V stage = m % NV), -1 for stat jobs
+  int i;        // job index
   int li;       // local index of the biased image inside this CTA's range (biased jobs)
-  int up, ul;   // unit pass / local unit
-  int first, last;   // first / last job of its unit pass
 };
 struct Fx2Jobs {
   FxWalk w;
   int u0, n_units, B, H, HG, G, tiles, nb;
   const int* img;
-  int it, phase, i, m, li, lastb, up;
+  int it, phase, i, li, lastb;
   FxUnit cur;
-  int cur_ul, cur_up, cur_li, hl, nh;
+  int cur_li, hl, nh;
   bool have;
   __host__ __device__ __forceinline__ Fx2Jobs(int u0_, int n_units_, int B_, int H_, int G_, int tiles_, int nb_,
                                               const int* img_)
       : u0(u0_), n_units(n_units_), B(B_), H(H_), G(G_), tiles(tiles_), nb(nb_), img(img_) {
     HG = (H + G - 1) / G;
     phase = nb > 0 ? 0 : 1;
-    i = 0; m = 0; up = 0;
+    i = 0;
     rewind();
   }
   __host__ __device__ __forceinline__ void rewind() {
@@ -87,24 +181,21 @@ struct Fx2Jobs {
   __host__ __device__ __forceinline__ bool next(Fx2Job& jb) {
     for (;;) {
       if (have) {
-        jb.b = cur.b; jb.h = cur.h * G + hl; jb.tile = cur.tile; jb.biased = cur.biased; jb.gi = cur.gi;
+        jb.b = cur.b; jb.h = cur.h * G + hl; jb.tile = cur.tile; jb.biased = cur.biased;
         jb.kind = phase == 0 ? 0 : 1;
         jb.i = i++;
-        jb.m = phase == 0 ? -1 : m++;
         jb.li = cur.biased ? cur_li : -1;
-        jb.up = cur_up; jb.ul = cur_ul;
-        jb.first = hl == 0; jb.last = hl == nh - 1;
         if (++hl == nh) have = false;
         return true;
       }
       while (it < n_units) {
         const FxUnit u = w.get();
         w.next();
-        const int ul = it++;
+        ++it;
         if (u.biased && u.b != lastb) { ++li; lastb = u.b; }
         const bool want = (phase == 1) ? !u.biased : (u.biased != 0);
         if (!want) continue;
-        cur = u; cur_ul = ul; cur_li = li; cur_up = up++;
+        cur = u; cur_li = li;
         hl = 0;
         nh = H - u.h * G < G ? H - u.h * G : G;
         have = true;
@@ -126,7 +217,7 @@ struct Fx2Jobs {
 //   s_jobs[i].x = b | h << 8 | tile << 16          s_jobs[i].y = flags, see the JF_* masks
 constexpr int kMaxUnits = 64;        // units per CTA (host-checked: the C ABI splits larger batches)
 constexpr int kMaxJobs = 512;        // kMaxUnits * G heads * 2 passes
-constexpr uint32_t JF_MAIN = 1u, JF_BIASED = 2u, JF_FIRST = 4u, JF_LAST = 8u;   // | li << 4 (2 bits) | ul << 8 (8 bits)
+constexpr uint32_t JF_MAIN = 1u, JF_BIASED = 2u;   // | li << 4 (2 bits)
 
 // Order-preserving map float -> unsigned (0 is below every real number: a zero-filled workspace reads as -infinity).
 __device__ __forceinline__ unsigned f32_key(float f) {
@@ -141,7 +232,7 @@ template <int D, int KC>
 __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const FxParams fp) {
   using C = core::Tile<D>;
   using CF = Cfg2<D, KC>;
-  constexpr int CW = kTP * KC;                     // cidx columns: token 77 c + j of chunk c at column 80 c + j
+  constexpr int CW = core::kTP * KC;                    // cidx columns: token 77 c + j of chunk c at column 80 c + j
   const XattnParams& p = fp.x;
   extern __shared__ __align__(128) unsigned char smem[];
   const uint32_t smem0 = ptx::smem_u32(smem);
@@ -223,7 +314,7 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
       const unsigned base_x = (r.x & 0xffu) | (r.x & 0xffff0000u);
       for (unsigned hl = 0; hl < nh; ++hl) {
         const unsigned x = base_x | ((hg * CF::G + hl) << 8);
-        const unsigned fl = (hl == 0 ? JF_FIRST : 0u) | (hl == nh - 1 ? JF_LAST : 0u) | (li << 4) | ((unsigned)(ul & 0xff) << 8);
+        const unsigned fl = li << 4;
         if (bi) {
           s_jobs[r.z + hl] = make_uint2(x, fl | JF_BIASED);
           s_jobs[ns + nuj + r.z + hl] = make_uint2(x, fl | JF_BIASED | JF_MAIN);
@@ -270,7 +361,7 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
   } else if (warp == 2) {
     for (int idx = lane; idx < nl * CW && idx < kMaxLocal * CW; idx += 32) {
       const int l = idx / CW, t = idx - l * CW;
-      const bool real = KC == 1 ? t < T : t % kTP < core::kChunk;
+      const bool real = t % core::kTP < core::chunk_keys<KC>(T);
       s_cidx[l][t] = real ? fp.cidx[(int64_t)s_widx[s_lb[l]] * CW + t] : (signed char)-1;
     }
   }
@@ -282,18 +373,11 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
     const int b = r.x & 0xff, h = (r.x >> 8) & 0xff, tile = r.x >> 16;
     const bool is_main = (r.y & JF_MAIN) != 0, biased = (r.y & JF_BIASED) != 0;
     const uint32_t st = smem0 + stage(i);
-    const int rows = p.N - tile * kBM < kBM ? p.N - tile * kBM : kBM;
-    core::load_rows<D>(st, p.q + (int64_t)b * p.q_bs + (int64_t)tile * kBM * p.q_rs + h * D, p.q_rs, kBM, rows);
-    const int kv = KC == 1 ? T : core::kChunk;
-#pragma unroll 1
-    for (int c = 0; c < KC; ++c) {
-      const int64_t off = (int64_t)b * p.k_bs + (int64_t)c * core::kChunk * p.k_rs + h * D;
-      core::load_rows<D>(st + C::QBYTES + c * C::KBYTES, p.k + off, p.k_rs, kTP, kv);
-      if (is_main) core::load_rows<D>(st + C::QBYTES + (KC + c) * C::KBYTES, p.v + off, p.k_rs, kTP, kv);
-    }
+    core::load_operands<D, KC>(st, p, b, h, tile, is_main);
     if (is_main && biased) {
-      const __half* mp = reinterpret_cast<const __half*>(fp.mpack) + (int64_t)s_widx[b] * fp.mpack_bs + (int64_t)tile * kBM * kMW;
-      for (int idx = threadIdx.x; idx < kBM * (kMW / 8); idx += blockDim.x) {
+      const int rows = p.N - tile * core::kBM;
+      const __half* mp = reinterpret_cast<const __half*>(fp.mpack) + (int64_t)s_widx[b] * fp.mpack_bs + (int64_t)tile * core::kBM * kMW;
+      for (int idx = threadIdx.x; idx < core::kBM * (kMW / 8); idx += blockDim.x) {
         const int rr = idx >> 2, c = idx & 3;
         const bool ok = rr < rows;
         ptx::cp_async16(st + CF::OFF_M + (uint32_t)(rr * kMW + c * 8) * 2u, ok ? (const void*)(mp + rr * kMW + c * 8) : fp.mpack,
@@ -311,12 +395,7 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
   auto flush = [&]() {
     if (cur_li < 0) return;
     double m = vmax, a = dsum, q = dsq;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
-      a += __shfl_xor_sync(0xffffffffu, a, o);
-      q += __shfl_xor_sync(0xffffffffu, q, o);
-    }
+    core::warp_reduce_stat(m, a, q);
     if (lane == 0 && cur_li < kMaxLocal) {
       StatPartial sp;
       sp.vmax = m; sp.sum = a; sp.sumsq = q; sp.pad = 1.0;
@@ -398,22 +477,10 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
                 a += __ldcg(&pp->sum);
                 q += __ldcg(&pp->sumsq);
               }
-#pragma unroll 1
-            for (int o = 16; o > 0; o >>= 1) {
-              a += __shfl_xor_sync(0xffffffffu, a, o);
-              q += __shfl_xor_sync(0xffffffffu, q, o);
-            }
+            core::warp_reduce_stat(m, a, q);
           }
           if (lane == 0) {
-            const double cnt = (double)p.H * (double)p.N * (double)p.T;
-            double rr;
-            if (is_max) {
-              rr = m;
-            } else {
-              const double var = (q - a * a / cnt) / (cnt - 1.0);
-              rr = sqrt(var > 0.0 ? var : 0.0);
-            }
-            const float st16 = round_to_f16((float)rr);         // qk.max() / qk.std() return fp16 in the reference
+            const float st16 = core::stat_value(p, is_max, m, a, q);
             s_coef[l] = (p.g_sigma != nullptr ? image_g(p, bl) : 0.f) * st16;
             if (p.stats_out != nullptr) p.stats_out[bl] = st16;   // every CTA of the image writes the same value
           }
@@ -428,81 +495,48 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
     const bool is_main = (r.y & JF_MAIN) != 0, biased = (r.y & JF_BIASED) != 0;
     const int li = (r.y >> 4) & 3;
     const uint32_t st = smem0 + stage(i);
-    const int row0 = tile * kBM + warp * 16;
-    if constexpr (KC > 1) {
-      const uint32_t qs = st + (uint32_t)(warp * 16 * C::LD) * 2u;
-      if (!is_main) {
-        if (li != cur_li) { flush(); cur_li = li; }
-        float sum = 0.f, sumsq = 0.f;
-#pragma unroll 1
-        for (int c = 0; c < KC; ++c) {              // the real tokens of every chunk
-          float s[10][4];
-          core::warp_qk<D>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
-          core::warp_stat(s, core::kChunk, p.N - row0, lane, s_ismax[li], vmax, sum, sumsq);
-        }
-        dsum += (double)sum;
-        dsq += (double)sumsq;
-        if (i == ns - 1) flush();
-      } else {
-        const float x = biased ? s_coef[li] : 0.f;
-        const __half* mrow = reinterpret_cast<const __half*>(smem + stage(i) + CF::OFF_M) + (warp * 16 + (lane >> 2)) * kMW;
-        float o[C::NT][4], m0, m1, l0, l1;
-        core::warp_online_begin<D>(o, m0, m1, l0, l1);
-#pragma unroll 1
-        for (int c = 0; c < KC; ++c) {
-          float s[10][4];
-          core::warp_qk<D>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
-          if (biased) {
-            const signed char* ci = s_cidx[li] + c * kTP;
-#pragma unroll
-            for (int j = 0; j < 10; ++j)
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const int cc = ci[core::tok(j, e, lane)];
-                if (cc >= 0) {
-                  const __half* mr = mrow + (e >> 1) * 8 * kMW;
-                  s[j][e] = fmaf(x, __half2float(mr[cc]) + __half2float(mr[kRC + cc]), s[j][e]);
-                }
-              }
-          }
-          core::warp_online_chunk<D>(s, sl2, st + C::QBYTES + (KC + c) * C::KBYTES, lane, o, m0, m1, l0, l1);
-        }
-        core::warp_online_end<D>(o, l0, l1);
-        core::warp_store<D>(o, smem + stage(i) + warp * 16 * C::LD * 2, lane, p.out + (int64_t)b * p.o_bs + h * D, p.o_rs,
-                            row0, p.N);
-      }
-      __syncthreads();
-      continue;
-    }
-    float s[10][4];
-    core::warp_qk<D>(st + (uint32_t)(warp * 16 * C::LD) * 2u, st + C::QBYTES, lane, s);
+    const uint32_t qs = st + (uint32_t)(warp * 16 * C::LD) * 2u;
+    const int row0 = tile * core::kBM + warp * 16;
+    const int kv = core::chunk_keys<KC>(T);
     if (!is_main) {
       if (li != cur_li) { flush(); cur_li = li; }
       float sum = 0.f, sumsq = 0.f;
-      core::warp_stat(s, T, p.N - row0, lane, s_ismax[li], vmax, sum, sumsq);
+#pragma unroll 1
+      for (int c = 0; c < KC; ++c) {                // the real tokens of every chunk
+        float s[10][4];
+        core::warp_qk<D>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
+        core::warp_stat(s, kv, p.N - row0, lane, s_ismax[li], vmax, sum, sumsq);
+      }
       dsum += (double)sum;
       dsq += (double)sumsq;
       if (i == ns - 1) flush();
     } else {
-      if (biased) {
-        const float x = s_coef[li];
-        const signed char* ci = s_cidx[li];
-        const __half* mrow = reinterpret_cast<const __half*>(smem + (i & 1) * CF::STAGE + CF::OFF_M) + (warp * 16 + (lane >> 2)) * kMW;
+      const float x = biased ? s_coef[li] : 0.f;
+      const __half* mrow = reinterpret_cast<const __half*>(smem + stage(i) + CF::OFF_M) + (warp * 16 + (lane >> 2)) * kMW;
+      float o[C::NT][4], m0, m1, l0, l1;
+      core::warp_online_begin<D>(o, m0, m1, l0, l1);
+#pragma unroll 1
+      for (int c = 0; c < KC; ++c) {
+        float s[10][4];
+        core::warp_qk<D>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
+        if (biased) {
+          const signed char* ci = s_cidx[li] + c * core::kTP;
 #pragma unroll
-        for (int j = 0; j < 10; ++j)
+          for (int j = 0; j < 10; ++j)
 #pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int c = ci[core::tok(j, e, lane)];
-            if (c >= 0) {
-              const __half* mr = mrow + (e >> 1) * 8 * kMW;
-              s[j][e] = fmaf(x, __half2float(mr[c]) + __half2float(mr[kRC + c]), s[j][e]);
+            for (int e = 0; e < 4; ++e) {
+              const int cc = ci[core::tok(j, e, lane)];
+              if (cc >= 0) {
+                const __half* mr = mrow + (e >> 1) * 8 * kMW;
+                s[j][e] = fmaf(x, __half2float(mr[cc]) + __half2float(mr[kRC + cc]), s[j][e]);
+              }
             }
-          }
+        }
+        core::warp_online_chunk<D>(s, kv, sl2, st + C::QBYTES + (KC + c) * C::KBYTES, lane, o, m0, m1, l0, l1);
       }
-      float o[C::NT][4];
-      core::warp_softmax_pv<D>(s, T, sl2, st + C::QBYTES + C::KBYTES, lane, o);
-      core::warp_store<D>(o, smem + (i & 1) * CF::STAGE + warp * 16 * C::LD * 2, lane, p.out + (int64_t)b * p.o_bs + h * D,
-                          p.o_rs, row0, p.N);
+      core::warp_online_end<D>(o, l0, l1);
+      core::warp_store<D>(o, smem + stage(i) + warp * 16 * C::LD * 2, lane, p.out + (int64_t)b * p.o_bs + h * D, p.o_rs,
+                          row0, p.N);
     }
     __syncthreads();
   }
@@ -524,6 +558,38 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
 // ------------------------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------------------------
+inline unsigned*& debug_jobs_dump() {   // test infrastructure: device buffer the grouped-head kernel copies its job tables to
+  static unsigned* p = nullptr;
+  return p;
+}
+inline int& debug_grid() {          // test infrastructure: cap the persistent grid (0 = number of SMs)
+  static int g = 0;
+  return g;
+}
+inline int fused_grid(int units) {
+  int g = tc::num_sms();
+  if (debug_grid() > 0 && debug_grid() < g) g = debug_grid();
+  return units < g ? units : g;
+}
+// A CTA range may touch at most kMaxLocal biased images (partial slots in shared memory).
+inline bool fused_range_ok(int B, int H, int tiles, int grid) {
+  const long long units = (long long)B * H * tiles;
+  const long long per_cta = (units + grid - 1) / grid;
+  return per_cta <= (long long)(kMaxLocal - 1) * tiles * H;
+}
+inline size_t fused_workspace_bytes() {
+  return 512 + (size_t)kMaxBatch * 2048 * sizeof(StatPartial) / 8;   // counters | per-image maxima | [32][256] partial slots
+}
+
+inline int fused_cta_has_image_host(int cta, int grid, int B, int H, int tiles, const int* wmap_index, int b) {
+  int nb = 0, pos = -1;
+  for (int i = 0; i < B; ++i)
+    if (wmap_index[i] >= 0) { if (i == b) pos = nb; ++nb; }
+  if (pos < 0) return 0;
+  const int nu = B - nb, np = nb < nu ? nb : nu;
+  return fx_cta_has_image(cta, grid, B * H * tiles, pos, H, tiles, np) ? 1 : 0;
+}
+
 // A launch fits when every CTA's unit range touches at most kMaxLocal biased images and holds at most kMaxUnits units
 // (job table in shared memory); the C ABI halves the images per launch until it does.
 inline bool fused2_fits(int B, int hg, int tiles, int grid) {
@@ -540,7 +606,7 @@ cudaError_t launch_fused2(const XattnParams& x, const void* mpack, int64_t mpack
   fp.cidx = cidx;
   fp.mpack = mpack;
   fp.mpack_bs = mpack_bs;
-  fp.tiles = ceil_div(x.N, kBM);
+  fp.tiles = ceil_div(x.N, core::kBM);
   fp.hg = ceil_div(x.H, CF::G);
   fp.units = x.B * fp.tiles * fp.hg;
   fp.grid = fused_grid(fp.units);
@@ -566,8 +632,8 @@ cudaError_t launch_fused2(const XattnParams& x, const void* mpack, int64_t mpack
   return cudaLaunchKernelEx(&cfg, xattn_fused2_kernel<D, KC>, fp);
 }
 
-// Host replay of the job lists (test infrastructure): out[job] = {cta, i, kind, m, b, h, tile, biased, li, gi, up, ul,
-// first, last} for every job of every CTA; returns the number of jobs written.
+// Host replay of the job lists (test infrastructure): out[job] = {cta, i, kind, b, h, tile, biased, li} for every job of
+// every CTA; returns the number of jobs written.
 inline int fused2_schedule_host(int B, int H, int G, int tiles, int grid, const int* wmap_index, int* out, int max_jobs) {
   if (B <= 0 || B > kMaxBatch || H <= 0 || G <= 0 || tiles <= 0 || grid <= 0) return -1;
   int img[kMaxBatch];
@@ -585,13 +651,12 @@ inline int fused2_schedule_host(int B, int H, int G, int tiles, int grid, const 
     Fx2Job jb;
     while (jobs.next(jb)) {
       if (row >= max_jobs) return -2;
-      int* o = out + 14 * (row++);
-      o[0] = cta; o[1] = jb.i; o[2] = jb.kind; o[3] = jb.m; o[4] = jb.b; o[5] = jb.h; o[6] = jb.tile; o[7] = jb.biased;
-      o[8] = jb.li; o[9] = jb.gi; o[10] = jb.up; o[11] = jb.ul; o[12] = jb.first; o[13] = jb.last;
+      int* o = out + 8 * (row++);
+      o[0] = cta; o[1] = jb.i; o[2] = jb.kind; o[3] = jb.b; o[4] = jb.h; o[5] = jb.tile; o[6] = jb.biased; o[7] = jb.li;
     }
   }
   return row;
 }
 
-}  // namespace fx2
+}  // namespace fx
 }  // namespace pww

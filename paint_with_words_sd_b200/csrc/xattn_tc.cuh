@@ -61,32 +61,25 @@ struct UnitIter {
     }
   }
 };
-// Forward-kernel unit order.  Units are tile-major; inside a row tile the images are visited in GROUPS that share one
-// [128 x T] mask tile:
+// Forward-kernel unit order.  Units are tile-major; inside a row tile the images are visited in groups:
 //   * pair group: one biased image A (has a weight map) and one unbiased image U (classifier-free guidance puts as many
-//     of each in the batch).  2H units, head h = j/2, in the order  U A | A U | U A | ...  so that (1) biased and
-//     unbiased units alternate at the finest grain -- every CTA's contiguous range gets the same mix, whatever the image
-//     order in the batch -- (2) A's mask tile is reused by all H heads (it stays in L2), and (3) the group ends with its
-//     mask no longer needed.
+//     of each in the batch).  2H units, head h = j/2, in the order  U A | A U | U A | ...  so that biased and unbiased
+//     units alternate at the finest grain: every CTA's contiguous range gets the same mix, whatever the image order in
+//     the batch, and all H heads of A read its row tile of the map while it is in L2.
 //   * solo group: an image without a partner (all-biased or all-unbiased batches), H units head-minor.
 // s_img lists the biased images first (nb of them), then the unbiased ones.
 struct FwdUnit {
   int b, h, tile;
-  int j, gsize;       // position inside the group, units in the group
-  int jl;             // last position whose unit reads the mask (gsize-1 when the group has no mask)
-  int mask_b;         // image whose mask tile the group uses, -1 = none
 };
 // Walks a CTA's contiguous unit range in that order; divisions only in the constructor.
 struct FwdWalk {
-  int B, H, nb, np, ng, jl_pair;
+  int B, H, nb, np, ng;
   const int* img;
   int tile, gi, j;    // row tile, group inside the tile (pair groups first, then solo groups), position in the group
   __host__ __device__ __forceinline__ FwdWalk(int u, int B_, int H_, int nb_, const int* img_) : B(B_), H(H_), nb(nb_), img(img_) {
     const int nu = B - nb;
     np = nb < nu ? nb : nu;
     ng = B - np;
-    const int jlast = 2 * H - 1;
-    jl_pair = ((((jlast ^ (jlast >> 1)) & 1) ^ 1) == 0) ? jlast : jlast - 1;
     const int per_tile = B * H;
     tile = u / per_tile;
     int q = u - tile * per_tile;
@@ -110,34 +103,17 @@ struct FwdWalk {
   __host__ __device__ __forceinline__ FwdUnit get() const {
     FwdUnit r;
     r.tile = tile;
-    r.j = j;
     if (gi < np) {
-      r.gsize = 2 * H;
       r.h = j >> 1;
       const int unb = ((j ^ (j >> 1)) & 1) ^ 1;          // 1 = the unbiased image's unit
       r.b = unb ? img[nb + gi] : img[gi];
-      r.mask_b = img[gi];
-      r.jl = jl_pair;
     } else {
-      r.gsize = H;
       r.h = j;
-      r.jl = H - 1;
-      if (2 * nb > B) { r.b = img[gi]; r.mask_b = r.b; }          // biased image without a partner
-      else { r.b = img[nb + gi]; r.mask_b = -1; }                 // unbiased image without a partner
+      r.b = (2 * nb > B) ? img[gi] : img[nb + gi];       // the biased or the unbiased image without a partner
     }
     return r;
   }
 };
-// Position (inside its group) of the last unit of the CTA's range that reads the group's mask tile: the last
-// mask-reading unit if the CTA's range [it - j_lo .., it + rest] contains it, else the last unit of the group in range.
-__host__ __device__ __forceinline__ int mask_release_pos(const FwdUnit& f, int it, int n_it) {
-  const int j_lo = f.j > it ? f.j - it : 0;
-  int j_hi = f.j + (n_it - 1 - it);
-  if (j_hi > f.gsize - 1) j_hi = f.gsize - 1;
-  return (f.jl >= j_lo && f.jl <= j_hi) ? f.jl : j_hi;
-}
-// First unit of a mask group inside a CTA's range.
-__host__ __device__ __forceinline__ bool mask_group_starts_here(const FwdUnit& f, int it) { return f.j == 0 || it == 0; }
 __device__ __forceinline__ void cta_range(int units, int& u0, int& u1) {
   u0 = (int)((long long)blockIdx.x * units / gridDim.x);
   u1 = (int)((long long)(blockIdx.x + 1) * units / gridDim.x);
@@ -145,22 +121,6 @@ __device__ __forceinline__ void cta_range(int units, int& u0, int& u1) {
 __device__ __forceinline__ int image_widx(const XattnParams& p, int b) {
   if (p.wmap == nullptr) return -1;
   return p.wmap_index ? p.wmap_index[b] : b;
-}
-
-// Copies of one unit's operands into a stage: Q rows of the tile, K (and V) rows of the head, one 80-row tile per chunk.
-template <int D, int KC>
-__device__ __forceinline__ void load_unit(uint32_t st, const XattnParams& p, int b, int h, int tile, bool with_v) {
-  using C = core::Tile<D>;
-  const int rows = p.N - tile * kBM;
-  core::load_rows<D>(st, p.q + (int64_t)b * p.q_bs + (int64_t)tile * kBM * p.q_rs + h * D, p.q_rs, kBM, rows < kBM ? rows : kBM);
-  const int kv = KC == 1 ? p.T : core::kChunk;
-#pragma unroll 1
-  for (int c = 0; c < KC; ++c) {
-    const int64_t off = (int64_t)b * p.k_bs + (int64_t)c * core::kChunk * p.k_rs + h * D;
-    core::load_rows<D>(st + C::QBYTES + c * C::KBYTES, p.k + off, p.k_rs, kTP, kv);
-    if (with_v) core::load_rows<D>(st + C::QBYTES + (KC + c) * C::KBYTES, p.v + off, p.k_rs, kTP, kv);
-  }
-  ptx::cp_async_commit();
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -211,20 +171,25 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_fwd_kernel(const TcParams t
   const float sl2 = p.scale * 1.4426950408889634f;
   FwdWalk w(u0, p.B, p.H, s_nb, s_img);
   FwdUnit nxt = w.get();
-  load_unit<D, KC>(smem0, p, nxt.b, nxt.h, nxt.tile, true);
+  core::load_operands<D, KC>(smem0, p, nxt.b, nxt.h, nxt.tile, true);
+  ptx::cp_async_commit();
   for (int it = 0; it < n_it; ++it) {
     const FwdUnit f = nxt;
     if constexpr (CF::NST == 2) {
       if (it + 1 < n_it) {
         w.next();
         nxt = w.get();
-        load_unit<D, KC>(smem0 + ((it + 1) & 1) * CF::STAGE, p, nxt.b, nxt.h, nxt.tile, true);
+        core::load_operands<D, KC>(smem0 + ((it + 1) & 1) * CF::STAGE, p, nxt.b, nxt.h, nxt.tile, true);
+        ptx::cp_async_commit();
         ptx::cp_async_wait<1>();
       } else {
         ptx::cp_async_wait<0>();
       }
     } else {                                       // one stage: refilled once the previous unit is done with it
-      if (it > 0) load_unit<D, KC>(smem0, p, f.b, f.h, f.tile, true);
+      if (it > 0) {
+        core::load_operands<D, KC>(smem0, p, f.b, f.h, f.tile, true);
+        ptx::cp_async_commit();
+      }
       ptx::cp_async_wait<0>();
       if (it + 1 < n_it) { w.next(); nxt = w.get(); }
     }
@@ -233,48 +198,28 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_fwd_kernel(const TcParams t
     const uint32_t qs = st + (uint32_t)(warp * 16 * C::LD) * 2u;
     const int row0 = f.tile * kBM + warp * 16;
     const int widx = s_widx[f.b];
-    if constexpr (KC > 1) {
-      float o[C::NT][4], m0, m1, l0, l1;
-      core::warp_online_begin<D>(o, m0, m1, l0, l1);
+    const int kv = core::chunk_keys<KC>(p.T);
+    float o[C::NT][4], m0, m1, l0, l1;
+    core::warp_online_begin<D>(o, m0, m1, l0, l1);
 #pragma unroll 1
-      for (int c = 0; c < KC; ++c) {
-        float s[10][4];
-        core::warp_qk<D>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
-        if (widx >= 0) {
-          const float x = s_coef[f.b];
-          const float* wm = p.wmap + (int64_t)widx * p.wmap_bs + c * core::kChunk;   // chunk c, slot t = column 77 c + t
+    for (int c = 0; c < KC; ++c) {
+      float s[10][4];
+      core::warp_qk<D>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
+      if (widx >= 0) {
+        const float x = s_coef[f.b];
+        const float* wm = p.wmap + (int64_t)widx * p.wmap_bs + c * core::kChunk;   // chunk c, slot t = column 77 c + t
 #pragma unroll
-          for (int j = 0; j < 10; ++j)
+        for (int j = 0; j < 10; ++j)
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int t = core::tok(j, e, lane), r = row0 + (lane >> 2) + (e >> 1) * 8;
-              if (t < core::kChunk && r < p.N) s[j][e] = fmaf(x, __ldg(wm + (int64_t)r * p.T + t), s[j][e]);
-            }
-        }
-        core::warp_online_chunk<D>(s, sl2, st + C::QBYTES + (KC + c) * C::KBYTES, lane, o, m0, m1, l0, l1);
+          for (int e = 0; e < 4; ++e) {
+            const int t = core::tok(j, e, lane), r = row0 + (lane >> 2) + (e >> 1) * 8;
+            if (t < kv && r < p.N) s[j][e] = fmaf(x, __ldg(wm + (int64_t)r * p.T + t), s[j][e]);
+          }
       }
-      core::warp_online_end<D>(o, l0, l1);
-      core::warp_store<D>(o, smem + (st - smem0) + warp * 16 * C::LD * 2, lane, p.out + (int64_t)f.b * p.o_bs + f.h * D, p.o_rs, row0, p.N);
-      __syncthreads();
-      continue;
+      core::warp_online_chunk<D>(s, kv, sl2, st + C::QBYTES + (KC + c) * C::KBYTES, lane, o, m0, m1, l0, l1);
     }
-    float s[10][4];
-    core::warp_qk<D>(qs, st + C::QBYTES, lane, s);
-    if (widx >= 0) {
-      const float x = s_coef[f.b];
-      const float* wm = p.wmap + (int64_t)widx * p.wmap_bs;
-#pragma unroll
-      for (int j = 0; j < 10; ++j)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int t = core::tok(j, e, lane), r = row0 + (lane >> 2) + (e >> 1) * 8;
-          if (t < p.T && r < p.N) s[j][e] = fmaf(x, __ldg(wm + (int64_t)r * p.T + t), s[j][e]);
-        }
-    }
-    float o[C::NT][4];
-    core::warp_softmax_pv<D>(s, p.T, sl2, st + C::QBYTES + C::KBYTES, lane, o);
-    core::warp_store<D>(o, smem + (it & 1) * CF::STAGE + warp * 16 * C::LD * 2, lane,
-                        p.out + (int64_t)f.b * p.o_bs + f.h * D, p.o_rs, row0, p.N);
+    core::warp_online_end<D>(o, l0, l1);
+    core::warp_store<D>(o, smem + (st - smem0) + warp * 16 * C::LD * 2, lane, p.out + (int64_t)f.b * p.o_bs + f.h * D, p.o_rs, row0, p.N);
     __syncthreads();
   }
 }
@@ -317,12 +262,7 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams
     auto flush = [&]() {
       if (cur_b < 0) return;
       double m = vmax, a = dsum, q = dsq;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
-        a += __shfl_xor_sync(0xffffffffu, a, o);
-        q += __shfl_xor_sync(0xffffffffu, q, o);
-      }
+      core::warp_reduce_stat(m, a, q);
       if (lane == 0) {
         StatPartial sp;
         sp.vmax = m; sp.sum = a; sp.sumsq = q; sp.pad = 1.0;
@@ -335,15 +275,22 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams
     int it_n = 0;
     auto advance = [&]() { while (it_n < n_it && skip(nxt.b)) { nxt.next(); ++it_n; } };
     advance();
-    if (it_n < n_it) load_unit<D, KC>(smem0, p, nxt.b, nxt.h, nxt.tile, false);
+    if (it_n < n_it) {
+      core::load_operands<D, KC>(smem0, p, nxt.b, nxt.h, nxt.tile, false);
+      ptx::cp_async_commit();
+    }
     for (int k = 0; it_n < n_it; ++k) {
       const int b = nxt.b, h = nxt.h, tile = nxt.tile;
-      if (CF::NST == 1 && k > 0) load_unit<D, KC>(smem0, p, b, h, tile, false);   // one stage: refilled here
+      if (CF::NST == 1 && k > 0) {                  // one stage: refilled here
+        core::load_operands<D, KC>(smem0, p, b, h, tile, false);
+        ptx::cp_async_commit();
+      }
       nxt.next();
       ++it_n;
       advance();
       if (CF::NST == 2 && it_n < n_it) {
-        load_unit<D, KC>(smem0 + ((k + 1) & 1) * CF::STAGE, p, nxt.b, nxt.h, nxt.tile, false);
+        core::load_operands<D, KC>(smem0 + ((k + 1) & 1) * CF::STAGE, p, nxt.b, nxt.h, nxt.tile, false);
+        ptx::cp_async_commit();
         ptx::cp_async_wait<1>();
       } else {
         ptx::cp_async_wait<0>();
@@ -357,7 +304,7 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams
       for (int c = 0; c < KC; ++c) {                // the real tokens of every chunk
         float s[10][4];
         core::warp_qk<D>(st + (uint32_t)(warp * 16 * C::LD) * 2u, st + C::QBYTES + c * C::KBYTES, lane, s);
-        core::warp_stat(s, KC == 1 ? p.T : core::kChunk, p.N - tile * kBM - warp * 16, lane, is_max, vmax, sum, sumsq);
+        core::warp_stat(s, core::chunk_keys<KC>(p.T), p.N - tile * kBM - warp * 16, lane, is_max, vmax, sum, sumsq);
       }
       dsum += (double)sum;
       dsq += (double)sumsq;
@@ -406,23 +353,8 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams
         q += __ldcg(&pp->sumsq);
       }
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
-      a += __shfl_xor_sync(0xffffffffu, a, o);
-      q += __shfl_xor_sync(0xffffffffu, q, o);
-    }
-    if (lane == 0) {
-      const double cnt = (double)p.H * (double)p.N * (double)p.T;
-      double r;
-      if (s_ismax[b]) {
-        r = m;
-      } else {
-        const double var = (q - a * a / cnt) / (cnt - 1.0);
-        r = sqrt(var > 0.0 ? var : 0.0);
-      }
-      p.stats_out[b] = round_to_f16((float)r);
-    }
+    core::warp_reduce_stat(m, a, q);
+    if (lane == 0) p.stats_out[b] = core::stat_value(p, s_ismax[b], m, a, q);
   }
   if (threadIdx.x == 0) p.counters[0] = 0u;
 }
@@ -452,10 +384,8 @@ inline int num_sms() {
 
 inline int stats_grid(int units) { return units < num_sms() ? units : num_sms(); }
 
-// Host replay of the forward kernel's unit schedule (test infrastructure): the same FwdWalk / cta_range /
-// mask_release_pos / mask_group_starts_here code, executed on the CPU.  out[u] = {cta, it, b, h, tile, group_id, mask_b,
-// flags} for every unit in launch order of each CTA; flags bit 0 = last unit of the group in the CTA's range that reads
-// the mask tile, bit 1 = first unit of a mask group in the CTA's range.
+// Host replay of the forward kernel's unit schedule (test infrastructure): the same FwdWalk / cta_range code, executed
+// on the CPU.  out[u] = {cta, it, b, h, tile} for every unit in launch order of each CTA.
 inline int fwd_schedule_host(int B, int H, int tiles, int grid, const int* wmap_index, int* out) {
   if (B <= 0 || B > kMaxBatch || H <= 0 || tiles <= 0 || grid <= 0) return -1;
   int img[kMaxBatch];
@@ -470,13 +400,10 @@ inline int fwd_schedule_host(int B, int H, int tiles, int grid, const int* wmap_
     const int n_it = u1 - u0;
     if (n_it == 0) continue;
     FwdWalk w(u0, B, H, nb, img);
-    int grp = -1;
     for (int it = 0; it < n_it; ++it, w.next()) {
       const FwdUnit f = w.get();
-      if (f.j == 0 || it == 0) ++grp;
-      int* o = out + 8 * (row++);
-      o[0] = cta; o[1] = it; o[2] = f.b; o[3] = f.h; o[4] = f.tile; o[5] = grp; o[6] = f.mask_b;
-      o[7] = ((f.j == mask_release_pos(f, it, n_it)) ? 1 : 0) | (mask_group_starts_here(f, it) ? 2 : 0);
+      int* o = out + 5 * (row++);
+      o[0] = cta; o[1] = it; o[2] = f.b; o[3] = f.h; o[4] = f.tile;
     }
   }
   return row;

@@ -15,9 +15,14 @@
  * negative pww_status_t; nothing throws.  Unsupported (D, T) combinations return
  * PWW_ERR_UNSUPPORTED -- there is no fallback path inside or outside the library.
  *
- * Tensor layouts (fp16 = IEEE binary16):
- *   q, out : [B, N, H*D] fp16, element (b,n,h,d) at  b*q_batch_stride + n*q_row_stride + h*D + d
- *   k, v   : [B, T, H*D] fp16, element (b,t,h,d) at  b*k_batch_stride + t*k_row_stride + h*D + d
+ * Element types: every activation entry point exists as an `_f16` (IEEE binary16) and a `_bf16` (bfloat16) twin with
+ * the same arguments, validation and return codes; q, k, v, out, x, y, ... are of the twin's type.  Everything else
+ * keeps its type in both: weight maps, statistics and G(sigma) are fp32, the packed map `mpack` is fp16 (it is a
+ * host-built encoding of the fp32 map, not an activation) and `cidx` is int8.
+ *
+ * Tensor layouts (elem = fp16 or bf16):
+ *   q, out : [B, N, H*D] elem, element (b,n,h,d) at  b*q_batch_stride + n*q_row_stride + h*D + d
+ *   k, v   : [B, T, H*D] elem, element (b,t,h,d) at  b*k_batch_stride + t*k_row_stride + h*D + d
  *            (strides in ELEMENTS; the head slice of a row is contiguous -- no head permute/copy,
  *             unlike paint_with_words.py:83-85,118)
  *   wmap   : [Bw, N, T] fp32 dense weight maps, the reference's CROSS_ATTENTION_WEIGHT_{N} tensors
@@ -69,8 +74,12 @@ size_t pww_xattn_workspace_bytes(int B, int H, int N, int T, int D);
 /*
  * Per-image statistic of the UNSCALED score tensor S[b] = Q_h K_h^T over all heads, pixels and tokens
  * (one scalar per image per call -- what `qk.max()` / `qk.std()` evaluate to inside the reference's
- * weight_function, paint_with_words.py:87,106,402-405).  S is rounded to fp16 before the reduction, as
- * the reference's autocast matmul does; the result is rounded to fp16 and stored as float.
+ * weight_function, paint_with_words.py:87,106,402-405).  S is rounded to the element type before the std sums, as
+ * the reference's autocast matmul does; the maximum is taken over S and rounded once (rounding is monotonic); the
+ * result is rounded to the element type and stored as float.  For bf16 this is what qk.max() / qk.std() return when the
+ * reference's op sequence runs under a bf16 autocast; bf16 has fp32's exponent range, so a statistic above 65504
+ * (inf in fp16) stays finite.
+ * _bf16: the same with bf16 q / k.
  * Images with wmap_index[b] < 0 are skipped (stats[b] = 0).  wmap_index may be NULL (= all images).
  */
 int pww_xattn_stats_f16(const void* q, const void* k,
@@ -80,6 +89,13 @@ int pww_xattn_stats_f16(const void* q, const void* k,
                         int stat, const int32_t* wmap_index,
                         float* stats /* [B] out */,
                         void* workspace, size_t workspace_bytes, void* stream);
+int pww_xattn_stats_bf16(const void* q, const void* k,
+                         int B, int H, int N, int T, int D,
+                         int64_t q_batch_stride, int64_t q_row_stride,
+                         int64_t k_batch_stride, int64_t k_row_stride,
+                         int stat, const int32_t* wmap_index,
+                         float* stats /* [B] out */,
+                         void* workspace, size_t workspace_bytes, void* stream);
 
 /*
  * Fused cross-attention with the Paint-with-Words bias (paint_with_words.py:87-118):
@@ -89,6 +105,7 @@ int pww_xattn_stats_f16(const void* q, const void* k,
  * scalar so a captured CUDA graph can be replayed with a new sigma).  wmap/wmap_index/stats/g_sigma may
  * all be NULL: plain cross-attention (tensor context, paint_with_words.py:67-69,107-108).
  * Requires T <= 80 or T = 154 / 231 (see "Key lengths" above; wmap stays [Bw, N, T], no padding columns).
+ * P is rounded to the element type before P.V and the row sum is the sum of the rounded P; out is stored in it.
  */
 int pww_xattn_fwd_f16(const void* q, const void* k, const void* v, void* out,
                       int B, int H, int N, int T, int D,
@@ -97,6 +114,13 @@ int pww_xattn_fwd_f16(const void* q, const void* k, const void* v, void* out,
                       int64_t o_batch_stride, int64_t o_row_stride,
                       const float* wmap, int64_t wmap_batch_stride, const int32_t* wmap_index,
                       const float* stats, const float* g_sigma, float scale, void* stream);
+int pww_xattn_fwd_bf16(const void* q, const void* k, const void* v, void* out,
+                       int B, int H, int N, int T, int D,
+                       int64_t q_batch_stride, int64_t q_row_stride,
+                       int64_t k_batch_stride, int64_t k_row_stride,
+                       int64_t o_batch_stride, int64_t o_row_stride,
+                       const float* wmap, int64_t wmap_batch_stride, const int32_t* wmap_index,
+                       const float* stats, const float* g_sigma, float scale, void* stream);
 
 /*
  * ONE-LAUNCH Paint-with-Words cross-attention: statistic + bias + softmax + P.V (paint_with_words.py:87-118 with the
@@ -116,11 +140,12 @@ int pww_xattn_fwd_f16(const void* q, const void* k, const void* v, void* out,
  * `paint_with_words_sd_b200.conditioning.pack_weight_map` builds both, bit-exactly reversible to the dense map.
  * Maps with more than 10 distinct columns use the two-launch dense path above.
  *
- *   stats [B] out : the per-image statistic (fp16-rounded, as float; 0 for images without a map); may be NULL
+ *   stats [B] out : the per-image statistic (rounded to the element type as for pww_xattn_stats_f16 / _bf16, as
+ *                   float; 0 for images without a map); may be NULL
  *   workspace     : pww_xattn_fused_workspace_bytes() bytes, zero-filled ONCE after allocation (self-cleaning)
  * mpack == NULL (or every wmap_index[b] < 0): plain cross-attention, workspace may be NULL.
  * Requires T <= 80 or T = 154 / 231, B <= 32 per launch (larger batches are split internally), 16-byte aligned `out`
- * strides.
+ * strides.  _bf16: bf16 q / k / v / out; mpack stays fp16.
  */
 size_t pww_xattn_fused_workspace_bytes(void);
 int pww_xattn_fused_f16(const void* q, const void* k, const void* v, void* out,
@@ -131,6 +156,14 @@ int pww_xattn_fused_f16(const void* q, const void* k, const void* v, void* out,
                         const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
                         const int32_t* wmap_index, int stat, const float* g_sigma, float scale,
                         float* stats, void* workspace, size_t workspace_bytes, void* stream);
+int pww_xattn_fused_bf16(const void* q, const void* k, const void* v, void* out,
+                         int B, int H, int N, int T, int D,
+                         int64_t q_batch_stride, int64_t q_row_stride,
+                         int64_t k_batch_stride, int64_t k_row_stride,
+                         int64_t o_batch_stride, int64_t o_row_stride,
+                         const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+                         const int32_t* wmap_index, int stat, const float* g_sigma, float scale,
+                         float* stats, void* workspace, size_t workspace_bytes, void* stream);
 
 /*
  * Per-image settings: the three calls above with a statistic kind and a G(sigma) for EACH image, so one launch serves a
@@ -141,7 +174,8 @@ int pww_xattn_fused_f16(const void* q, const void* k, const void* v, void* out,
  *   g_sigma : [B] fp32 device array instead of one element; entry b is image b's G(sigma).
  * Entry b belongs to image b of the call; entries of images with wmap_index[b] < 0 are ignored.  A NULL `stat` or
  * `g_sigma` array where a map is given returns PWW_ERR_BAD_ARG (pww_xattn_stats_multi_f16 always needs `stat`).
- * With every kind equal and every G equal, the results are bit-identical to the twin's.
+ * With every kind equal and every G equal, the results are bit-identical to the twin's.  The _multi_bf16 calls are the
+ * same with bf16 activations.
  */
 int pww_xattn_stats_multi_f16(const void* q, const void* k,
                               int B, int H, int N, int T, int D,
@@ -165,6 +199,28 @@ int pww_xattn_fused_multi_f16(const void* q, const void* k, const void* v, void*
                               const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
                               const int32_t* wmap_index, const int32_t* stat, const float* g_sigma, float scale,
                               float* stats, void* workspace, size_t workspace_bytes, void* stream);
+int pww_xattn_stats_multi_bf16(const void* q, const void* k,
+                               int B, int H, int N, int T, int D,
+                               int64_t q_batch_stride, int64_t q_row_stride,
+                               int64_t k_batch_stride, int64_t k_row_stride,
+                               const int32_t* stat, const int32_t* wmap_index,
+                               float* stats /* [B] out */,
+                               void* workspace, size_t workspace_bytes, void* stream);
+int pww_xattn_fwd_multi_bf16(const void* q, const void* k, const void* v, void* out,
+                             int B, int H, int N, int T, int D,
+                             int64_t q_batch_stride, int64_t q_row_stride,
+                             int64_t k_batch_stride, int64_t k_row_stride,
+                             int64_t o_batch_stride, int64_t o_row_stride,
+                             const float* wmap, int64_t wmap_batch_stride, const int32_t* wmap_index,
+                             const float* stats, const float* g_sigma, float scale, void* stream);
+int pww_xattn_fused_multi_bf16(const void* q, const void* k, const void* v, void* out,
+                               int B, int H, int N, int T, int D,
+                               int64_t q_batch_stride, int64_t q_row_stride,
+                               int64_t k_batch_stride, int64_t k_row_stride,
+                               int64_t o_batch_stride, int64_t o_row_stride,
+                               const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+                               const int32_t* wmap_index, const int32_t* stat, const float* g_sigma, float scale,
+                               float* stats, void* workspace, size_t workspace_bytes, void* stream);
 
 /*
  * Self-attention through the same patched function (context=None, paint_with_words.py:71-72):
@@ -175,10 +231,16 @@ int pww_attn_fwd_f16(const void* q, const void* k, const void* v, void* out,
                      int64_t qkv_batch_stride, int64_t qkv_row_stride,
                      int64_t o_batch_stride, int64_t o_row_stride,
                      float scale, void* stream);
+int pww_attn_fwd_bf16(const void* q, const void* k, const void* v, void* out,
+                      int B, int H, int N, int D,
+                      int64_t qkv_batch_stride, int64_t qkv_row_stride,
+                      int64_t o_batch_stride, int64_t o_row_stride,
+                      float scale, void* stream);
 
 /*
  * Fused memory-bound ops of the UNet that calls the attention path (the reference gets them from diffusers/ATen as
- * separate eager launches): channels-last fp16 activations, deterministic reductions.
+ * separate eager launches): channels-last fp16 (_f16) or bf16 (_bf16) activations, parameters and `add` of the same
+ * type, fp32 arithmetic, deterministic reductions.
  *
  * GroupNorm over [B, HW, C] (channels last) with G groups:  y = act((x + add[b,c] - mean) * rstd * gamma + beta),
  * `add` ([B, C] with row stride `add_batch_stride`, may be NULL) is the ResNet block's time-embedding term (added before normalisation), act = SiLU when
@@ -190,15 +252,22 @@ int pww_groupnorm_nhwc_f16(const void* x, const void* add, int64_t add_batch_str
                            const void* gamma, const void* beta, void* y,
                            int B, int HW, int C, int G, float eps, int silu,
                            void* workspace, size_t workspace_bytes, void* stream);
+int pww_groupnorm_nhwc_bf16(const void* x, const void* add, int64_t add_batch_stride /* elements */,
+                            const void* gamma, const void* beta, void* y,
+                            int B, int HW, int C, int G, float eps, int silu,
+                            void* workspace, size_t workspace_bytes, void* stream);
 
 /* GEGLU: out[m, i] = in[m, i] * gelu(in[m, I + i]) for in [M, 2*I], out [M, I] (exact erf GELU); I % 8 == 0. */
 int pww_geglu_f16(const void* in, void* out, int64_t M, int I, void* stream);
+int pww_geglu_bf16(const void* in, void* out, int64_t M, int I, void* stream);
 
 /* Residual add + LayerNorm over the last dim of [M, C]:  s = x + res (res may be NULL);  sum_out = s (may be NULL);
  * y = LayerNorm(s) * gamma + beta.  The transformer block's "x = attn(...) + x; h = norm(x)" pair in one pass.
  * C % 8 == 0, C <= 2048. */
 int pww_add_layernorm_f16(const void* x, const void* res, const void* gamma, const void* beta, void* sum_out, void* y,
                           int64_t M, int C, float eps, void* stream);
+int pww_add_layernorm_bf16(const void* x, const void* res, const void* gamma, const void* beta, void* sum_out, void* y,
+                           int64_t M, int C, float eps, void* stream);
 
 /*
  * The sampler step around the UNet (LMS, Euler, Euler ancestral, DPM++ 2M), two launches per denoising step.
@@ -217,10 +286,12 @@ int pww_add_layernorm_f16(const void* x, const void* res, const void* gamma, con
  * form a [6] device array: form = {alpha, a, b, gamma, slot, row}.  All arithmetic is fp32, rounded after every
  * operation in the order written; a == 0 gives q = b eps and alpha == 1 gives x + (...).
  * Both return PWW_ERR_BAD_ARG for null pointers or bad sizes and PWW_ERR_UNSUPPORTED for other dtypes, before any
- * CUDA call.
+ * CUDA call.  Dtype codes: 0 fp32, 1 fp16, 4 bf16.  Codes 2 and 3 are not assigned: releases up to 0.3.0 returned
+ * PWW_ERR_UNSUPPORTED for them, and they keep doing so, so a caller that relied on that answer sees no change.
  */
 #define PWW_DTYPE_F32 0
 #define PWW_DTYPE_F16 1
+#define PWW_DTYPE_BF16 4
 int pww_sampler_input(const float* latents, const float* scale, const float* extra, void* out, int out_dtype,
                       int m, int channels, int height, int width, void* stream);
 int pww_sampler_update(const void* eps, int eps_dtype, int64_t eps_batch_stride, int64_t eps_channel_stride,

@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("PWW_B200_LIB", os.path.join(_HERE, "libpww_b200.so"))
 
 PWW_STAT_MAX, PWW_STAT_STD = 0, 1
-PWW_DTYPE_F32, PWW_DTYPE_F16 = 0, 1
+PWW_DTYPE_F32, PWW_DTYPE_F16, PWW_DTYPE_BF16 = 0, 1, 4     # 2 and 3 are unassigned (unsupported, as before bf16)
 
 EXPORTS = (
     "pww_version", "pww_status_str", "pww_last_cuda_error", "pww_device_supported",
@@ -22,6 +22,9 @@ EXPORTS = (
     "pww_xattn_stats_multi_f16", "pww_xattn_fwd_multi_f16", "pww_xattn_fused_multi_f16",
     "pww_groupnorm_workspace_bytes", "pww_groupnorm_nhwc_f16", "pww_geglu_f16", "pww_add_layernorm_f16",
     "pww_sampler_input", "pww_sampler_update",
+    "pww_xattn_stats_bf16", "pww_xattn_fwd_bf16", "pww_xattn_fused_bf16",
+    "pww_xattn_stats_multi_bf16", "pww_xattn_fwd_multi_bf16", "pww_xattn_fused_multi_bf16",
+    "pww_attn_fwd_bf16", "pww_groupnorm_nhwc_bf16", "pww_geglu_bf16", "pww_add_layernorm_bf16",
 )
 
 
@@ -81,6 +84,12 @@ def lib() -> ctypes.CDLL:
     L.pww_geglu_f16.argtypes = [c_vp, c_vp, c_i64, c_i, c_vp]
     L.pww_add_layernorm_f16.restype = c_i
     L.pww_add_layernorm_f16.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i, c_f, c_vp]
+    # every _bf16 entry point takes its _f16 twin's arguments
+    for name in EXPORTS:
+        if name.endswith("_bf16"):
+            twin = getattr(L, name[:-len("_bf16")] + "_f16")
+            fn = getattr(L, name)
+            fn.restype, fn.argtypes = twin.restype, list(twin.argtypes)
     L.pww_sampler_input.restype = c_i
     L.pww_sampler_input.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i, c_i, c_i, c_i, c_i, c_vp]
     L.pww_sampler_update.restype = c_i

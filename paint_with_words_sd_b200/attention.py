@@ -18,6 +18,10 @@ bias from the packed weight map, softmax, PV).  Maps with more than 10 distinct 
 There is no PyTorch/CPU fallback for the cross-attention path: unsupported shapes or weight functions
 raise.
 
+Element type: a call runs in bf16 (the `_bf16` entry points) when q is bf16 and in fp16 otherwise; k and v are cast to
+q's type and the output has it.  `inj_forward` runs the projections under a bf16 autocast when the module's weights are
+bf16 and under an fp16 autocast otherwise, so a bf16 UNet keeps a bf16 residual stream.
+
 Extensions beyond the reference (which is hard-wired to batch 1, paint_with_words.py:445):
   * B > 1 with per-image statistics -- each image's max/std is its own, so results do not depend on
     how images are batched or sharded across GPUs;
@@ -127,10 +131,25 @@ def resolve_weight_map(context: dict, n: int, device):
         return w
 
 
-def _rows(t: torch.Tensor) -> torch.Tensor:
-    """[B,L,C] fp16 with unit channel stride and 16-byte friendly strides."""
-    if t.dtype != torch.float16:
-        t = t.to(torch.float16)
+def _elem_dtype(q: torch.Tensor) -> torch.dtype:
+    """The element type the kernels run in for query q: bf16 for a bf16 q, fp16 for anything else."""
+    return torch.bfloat16 if q.dtype == torch.bfloat16 else torch.float16
+
+
+def _entry(name: str, dtype: torch.dtype):
+    """The C entry point `name` (without its type suffix) for element type `dtype`."""
+    return getattr(_native.lib(), name + ("_bf16" if dtype == torch.bfloat16 else "_f16"))
+
+
+def _autocast_dtype(module) -> torch.dtype:
+    """bf16 for a module with bf16 weights, fp16 otherwise (fp32 modules keep the reference's fp16 autocast)."""
+    return torch.bfloat16 if module.to_q.weight.dtype == torch.bfloat16 else torch.float16
+
+
+def _rows(t: torch.Tensor, dtype: torch.dtype = torch.float16) -> torch.Tensor:
+    """[B,L,C] of `dtype` with unit channel stride and 16-byte friendly strides."""
+    if t.dtype != dtype:
+        t = t.to(dtype)
     if t.stride(-1) != 1 or (t.stride(0) % 8) or (t.stride(1) % 8) or (t.data_ptr() % 16):
         t = t.contiguous()
     return t
@@ -155,9 +174,10 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
     every image (an int) with `g_sigma` a 1-element fp32 device tensor holding G(sigma), or per-image settings: an int32
     [B] device tensor of kinds with `g_sigma` an fp32 [B] device tensor (entry b = image b; the `_multi` entry points).
     `stats_out` / `workspace` let a caller that captures CUDA graphs own the scratch (defaults: per-device scratch of
-    this module)."""
+    this module).  The call runs in bf16 when q is bf16 and in fp16 otherwise (see the module docstring)."""
     L = _native.lib()
-    q, k, v = _rows(q), _rows(k), _rows(v)
+    dt = _elem_dtype(q)
+    q, k, v = _rows(q, dt), _rows(k, dt), _rows(v, dt)
     B, N, C = q.shape
     T = k.shape[1]
     D = C // heads
@@ -166,7 +186,7 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
         k = k.contiguous()
     st = _state(q.device)
     with torch.cuda.device(q.device):               # native launches go to q's device whatever the current one is
-        out = torch.empty((B, N, C), dtype=torch.float16, device=q.device)
+        out = torch.empty((B, N, C), dtype=dt, device=q.device)
         stream = torch.cuda.current_stream(q.device).cuda_stream
         biased = wmap is not None or packed is not None
         if wmap is not None:
@@ -209,7 +229,7 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                 mp_ptr, ci_ptr, idx_ptr = mpack.data_ptr(), cidx.data_ptr(), wmap_index.data_ptr()
                 g_ptr, st_ptr, ws_ptr = g_sigma.data_ptr(), stats.data_ptr(), ws.data_ptr()
                 mp_bs, bw, ws_bytes = mpack.stride(0), mpack.shape[0], ws.numel()
-            fn = L.pww_xattn_fused_multi_f16 if per_image else L.pww_xattn_fused_f16
+            fn = _entry("pww_xattn_fused_multi" if per_image else "pww_xattn_fused", dt)
             rc = fn(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, heads, N, T, D,
                     q.stride(0), q.stride(1), k.stride(0), k.stride(1), out.stride(0), out.stride(1),
                     mp_ptr, mp_bs, bw, ci_ptr, idx_ptr, kind_ptr if per_image else stat, g_ptr, float(scale), st_ptr,
@@ -227,7 +247,7 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                 ws_bytes = L.pww_xattn_workspace_bytes(B, heads, N, T, D)
                 st.ensure(B, ws_bytes)
                 stats = st.stats if stats_out is None else stats_out
-                fn = L.pww_xattn_stats_multi_f16 if per_image else L.pww_xattn_stats_f16
+                fn = _entry("pww_xattn_stats_multi" if per_image else "pww_xattn_stats", dt)
                 rc = fn(q.data_ptr(), k.data_ptr(), B, heads, N, T, D, q.stride(0), q.stride(1), k.stride(0),
                         k.stride(1), kind_ptr if per_image else stat, wmap_index.data_ptr(), stats.data_ptr(),
                         st.workspace.data_ptr(), st.workspace.numel(), stream)
@@ -235,7 +255,7 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                 _native.launch_count += 1
                 stats_ptr, g_ptr = stats.data_ptr(), g_sigma.data_ptr()
                 w_ptr, idx_ptr, w_bs = wmap.data_ptr(), wmap_index.data_ptr(), wmap.stride(0)
-            fn = L.pww_xattn_fwd_multi_f16 if per_image else L.pww_xattn_fwd_f16
+            fn = _entry("pww_xattn_fwd_multi" if per_image else "pww_xattn_fwd", dt)
             rc = fn(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, heads, N, T, D,
                     q.stride(0), q.stride(1), k.stride(0), k.stride(1), out.stride(0), out.stride(1),
                     w_ptr, w_bs, idx_ptr, stats_ptr, g_ptr, float(scale), stream)
@@ -259,16 +279,17 @@ def self_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int
     B, N, C = q.shape
     D = C // heads
     if SELF_ATTN_IMPL == "native" or (SELF_ATTN_IMPL == "auto" and N <= SELF_ATTN_NATIVE_MAX_KEYS):
-        L = _native.lib()
-        q, k, v = _rows(q), _rows(k), _rows(v)
+        dt = _elem_dtype(q)
+        fn = _entry("pww_attn_fwd", dt)
+        q, k, v = _rows(q, dt), _rows(k, dt), _rows(v, dt)
         if not (q.stride() == k.stride() == v.stride()):
             q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
         with torch.cuda.device(q.device):
-            out = torch.empty((B, N, C), dtype=torch.float16, device=q.device)
-            rc = L.pww_attn_fwd_f16(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, heads, N, D,
-                                    q.stride(0), q.stride(1), out.stride(0), out.stride(1), float(scale),
-                                    torch.cuda.current_stream(q.device).cuda_stream)
-        _native.check(rc, "pww_attn_fwd_f16")
+            out = torch.empty((B, N, C), dtype=dt, device=q.device)
+            rc = fn(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, heads, N, D,
+                    q.stride(0), q.stride(1), out.stride(0), out.stride(1), float(scale),
+                    torch.cuda.current_stream(q.device).cuda_stream)
+        _native.check(rc, fn.__name__)
         _native.launch_count += 1
         return out
     qh = q.reshape(B, N, heads, D).transpose(1, 2)
@@ -297,8 +318,8 @@ def refresh_kv_cache(context: dict) -> None:
     if not cache:
         return
     ctx = context["CONTEXT_TENSOR"]
-    with torch.autocast("cuda", dtype=torch.float16):
-        for module, kv in cache.values():
+    for module, kv in cache.values():
+        with torch.autocast("cuda", dtype=_autocast_dtype(module)):
             kv.copy_(F.linear(ctx, _fused_weight(module, "_pww_wkv", ("to_k", "to_v"))))
 
 
@@ -313,7 +334,8 @@ def inj_forward(self, hidden_states, context=None, mask=None):
         ctx = context["CONTEXT_TENSOR"] if is_dict else context
 
     C = self.to_q.weight.shape[0]
-    with torch.autocast("cuda", dtype=torch.float16):
+    act = _autocast_dtype(self)
+    with torch.autocast("cuda", dtype=act):
         if context is None:
             # one [C -> 3C] GEMM; q/k/v are column views of its output (row stride 3C) -- the kernels take strides
             qkv = F.linear(hidden_states, _fused_weight(self, "_pww_wqkv", ("to_q", "to_k", "to_v")))
@@ -367,7 +389,7 @@ def inj_forward(self, hidden_states, context=None, mask=None):
         o = cross_attention(q, k, v, self.heads, self.scale, wmap, wmap_index, stat, g_dev, packed=packed,
                             stats_out=scratch[0], workspace=scratch[1])
 
-    with torch.autocast("cuda", dtype=torch.float16):
+    with torch.autocast("cuda", dtype=act):
         o = self.to_out[0](o)
         o = self.to_out[1](o)
     return o

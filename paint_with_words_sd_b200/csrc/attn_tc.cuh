@@ -6,7 +6,7 @@
 // are in flight while tile j is computed):
 //     S = Q K_j^T     mma.m16n8k16, 8 n-tiles per warp, fp32 accumulators in registers
 //     online softmax: running row max m and row sum l; O and l are rescaled by 2^(m_old - m_new) when the max moves
-//     O += P V_j      P packed to fp16 straight from the S accumulators (the C layout of two n-tiles is the A layout of one
+//     O += P V_j      P packed to E (fp16 or bf16, the element type of q / k / v / out) straight from the S accumulators (the C layout of two n-tiles is the A layout of one
 //                     k-step), V fragments by ldmatrix.trans
 // Padding (d >= D, key >= N, row >= N) is zero-filled by the copies; padded keys of the last tile are masked to -inf.
 #pragma once
@@ -31,19 +31,26 @@ struct Cfg {
   static_assert(SMEM <= 232448, "shared memory budget");
 };
 
+template <typename E>
 struct Params {
-  const __half* q;
-  const __half* k;
-  const __half* v;
-  __half* out;
+  const E* q;
+  const E* k;
+  const E* v;
+  E* out;
   int B, H, N;
   int64_t bs, rs;          // q/k/v element strides (batch, row)
   int64_t o_bs, o_rs;
   float scale;
 };
 
-template <int D>
-__global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const Params p) {
+// Minimum CTAs per SM of the launch bound (0 = none).  Unbounded, ptxas fits the bf16 head-dim-80 instance into 128
+// registers (two CTAs per SM) and spills 24 bytes; its fp16 twin takes 137 registers, one CTA per SM.  A bound of one
+// CTA gives the bf16 instance that same occupancy without spills.  Every other instance keeps the unbounded choice.
+template <int D, typename E>
+constexpr int kMinBlocks = (D == 80 && std::is_same_v<E, __nv_bfloat16>) ? 1 : 0;
+
+template <int D, typename E>
+__global__ void __launch_bounds__(kThreads, kMinBlocks<D, E>) attn_fwd_kernel(const Params<E> p) {
   using C = core::Tile<D>;
   using CF = Cfg<D>;
   extern __shared__ __align__(128) unsigned char smem[];
@@ -53,9 +60,9 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const Params p) {
   const int bh = blockIdx.x / qtiles, qt = blockIdx.x - bh * qtiles;
   const int b = bh / p.H, h = bh - b * p.H;
   const int row_base = qt * kBM;
-  const __half* qb = p.q + (int64_t)b * p.bs + h * D;
-  const __half* kb = p.k + (int64_t)b * p.bs + h * D;
-  const __half* vb = p.v + (int64_t)b * p.bs + h * D;
+  const E* qb = p.q + (int64_t)b * p.bs + h * D;
+  const E* kb = p.k + (int64_t)b * p.bs + h * D;
+  const E* vb = p.v + (int64_t)b * p.bs + h * D;
   const int ntiles = (p.N + kBN - 1) / kBN;
   auto issue_kv = [&](int j) {
     const uint32_t st = smem0 + CF::OFF_KV + (j & 1) * 2 * CF::KVBYTES;
@@ -101,8 +108,8 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const Params p) {
         const int t = 16 * jp + (lane & 7) + ((lane >> 4) << 3), d = kk * 16 + ((lane >> 3) & 1) * 8;
         uint32_t b0, b1, b2, b3;
         ptx::ldsm_x4(ks + (uint32_t)(t * C::LD + d) * 2u, b0, b1, b2, b3);
-        ptx::mma16816(s[2 * jp], qa[kk], b0, b1);
-        ptx::mma16816(s[2 * jp + 1], qa[kk], b2, b3);
+        ptx::mma16816<E>(s[2 * jp], qa[kk], b0, b1);
+        ptx::mma16816<E>(s[2 * jp + 1], qa[kk], b2, b3);
       }
     }
     const int valid = p.N - jt * kBN;              // keys of this tile that exist
@@ -126,9 +133,9 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const Params p) {
     float r0 = 0.f, r1 = 0.f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      const uint32_t p01 = ptx::pack_h2(ptx::ex2(fmaf(s[j][0], sl2, n0)), ptx::ex2(fmaf(s[j][1], sl2, n0)));
-      const uint32_t p23 = ptx::pack_h2(ptx::ex2(fmaf(s[j][2], sl2, n1)), ptx::ex2(fmaf(s[j][3], sl2, n1)));
-      const float2 f01 = ptx::unpack_h2(p01), f23 = ptx::unpack_h2(p23);
+      const uint32_t p01 = ptx::pack2<E>(ptx::ex2(fmaf(s[j][0], sl2, n0)), ptx::ex2(fmaf(s[j][1], sl2, n0)));
+      const uint32_t p23 = ptx::pack2<E>(ptx::ex2(fmaf(s[j][2], sl2, n1)), ptx::ex2(fmaf(s[j][3], sl2, n1)));
+      const float2 f01 = ptx::unpack2<E>(p01), f23 = ptx::unpack2<E>(p23);
       r0 += f01.x + f01.y;
       r1 += f23.x + f23.y;
       pa[j >> 1][(j & 1) * 2] = p01;
@@ -147,13 +154,13 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const Params p) {
       for (int jp = 0; jp < C::NT / 2; ++jp) {
         uint32_t b0, b1, b2, b3;
         ptx::ldsm_x4_t(vs + (uint32_t)(t * C::LD + 16 * jp + (lane >> 4) * 8) * 2u, b0, b1, b2, b3);
-        ptx::mma16816(o[2 * jp], pa[kk], b0, b1);
-        ptx::mma16816(o[2 * jp + 1], pa[kk], b2, b3);
+        ptx::mma16816<E>(o[2 * jp], pa[kk], b0, b1);
+        ptx::mma16816<E>(o[2 * jp + 1], pa[kk], b2, b3);
       }
       if constexpr (C::NT & 1) {
         uint32_t b0, b1;
         ptx::ldsm_x2_t(vs + (uint32_t)(t * C::LD + 8 * (C::NT - 1)) * 2u, b0, b1);
-        ptx::mma16816(o[C::NT - 1], pa[kk], b0, b1);
+        ptx::mma16816<E>(o[C::NT - 1], pa[kk], b0, b1);
       }
     }
     __syncthreads();                               // stage jt & 1 is refilled by the copies issued next iteration
@@ -171,22 +178,22 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const Params p) {
                       row_base + warp * 16, p.N);
 }
 
-template <int D>
+template <int D, typename E>
 cudaError_t launch(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int64_t bs, int64_t rs,
                    int64_t o_bs, int64_t o_rs, float scale, cudaStream_t s) {
   using CF = Cfg<D>;
-  Params p;
-  p.q = (const __half*)q; p.k = (const __half*)k; p.v = (const __half*)v; p.out = (__half*)out;
+  Params<E> p;
+  p.q = (const E*)q; p.k = (const E*)k; p.v = (const E*)v; p.out = (E*)out;
   p.B = B; p.H = H; p.N = N; p.bs = bs; p.rs = rs; p.o_bs = o_bs; p.o_rs = o_rs; p.scale = scale;
   static bool attr_set[tc::kMaxDevices] = {false};
   if (!attr_set[tc::cur_device()]) {
-    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, CF::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<D, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, CF::SMEM);
     if (e != cudaSuccess) return e;
     attr_set[tc::cur_device()] = true;
   }
   const long long grid = (long long)B * H * ((N + kBM - 1) / kBM);
   if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
-  attn_fwd_kernel<D><<<(unsigned)grid, kThreads, CF::SMEM, s>>>(p);
+  attn_fwd_kernel<D, E><<<(unsigned)grid, kThreads, CF::SMEM, s>>>(p);
   return cudaGetLastError();
 }
 

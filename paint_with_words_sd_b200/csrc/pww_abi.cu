@@ -107,8 +107,9 @@ size_t pww_xattn_workspace_bytes(int B, int H, int N, int T, int D) {
 
 namespace {
 
-// The statistics launches of pww_xattn_stats_f16 (kinds == NULL: `stat` for every image) and of
-// pww_xattn_stats_multi_f16 (per_image: kinds[b] for image b).
+// The statistics launches of pww_xattn_stats_{f16,bf16} (kinds == NULL: `stat` for every image) and of
+// pww_xattn_stats_multi_{f16,bf16} (per_image: kinds[b] for image b); E = __half or __nv_bfloat16.
+template <typename E>
 int xattn_stats(const void* q, const void* k, int B, int H, int N, int T, int D, int64_t q_batch_stride,
                 int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int stat, const int32_t* kinds,
                 bool per_image, const int32_t* wmap_index, float* stats, void* workspace, size_t workspace_bytes,
@@ -118,9 +119,9 @@ int xattn_stats(const void* q, const void* k, int B, int H, int N, int T, int D,
   if (!stats || !workspace) return PWW_ERR_BAD_ARG;
   if (per_image ? !kinds : (stat != PWW_STAT_MAX && stat != PWW_STAT_STD)) return PWW_ERR_BAD_ARG;
   if (workspace_bytes < pww_xattn_workspace_bytes(B, H, N, T, D)) return PWW_ERR_WORKSPACE;
-  pww::XattnParams p;
+  pww::XattnParams<E> p;
   memset(&p, 0, sizeof(p));
-  p.q = (const __half*)q; p.k = (const __half*)k;
+  p.q = (const E*)q; p.k = (const E*)k;
   p.B = B; p.H = H; p.N = N; p.T = T; p.D = D;
   p.q_bs = q_batch_stride; p.q_rs = q_row_stride; p.k_bs = k_batch_stride; p.k_rs = k_row_stride;
   p.wmap_index = wmap_index; p.stat = stat; p.stat_kind = per_image ? kinds : nullptr; p.stats_out = stats;
@@ -130,7 +131,7 @@ int xattn_stats(const void* q, const void* k, int B, int H, int N, int T, int D,
   {
     if (pww::tc::stats_slots() > stats_slots_per_image(H, N)) return PWW_ERR_WORKSPACE;
     for (int b0 = 0; b0 < B; b0 += pww::tc::kMaxBatch) {          // <= 256 images per launch
-      pww::XattnParams c = p;
+      pww::XattnParams<E> c = p;
       c.B = (B - b0) < pww::tc::kMaxBatch ? (B - b0) : pww::tc::kMaxBatch;
       c.q = p.q + (int64_t)b0 * p.q_bs;
       c.k = p.k + (int64_t)b0 * p.k_bs;
@@ -144,8 +145,9 @@ int xattn_stats(const void* q, const void* k, int B, int H, int N, int T, int D,
   }
 }
 
-// The forward launches of pww_xattn_fwd_f16 (g_stride 0: g_sigma[0] for every image) and of pww_xattn_fwd_multi_f16
-// (g_stride 1: g_sigma[b] for image b).
+// The forward launches of pww_xattn_fwd_{f16,bf16} (g_stride 0: g_sigma[0] for every image) and of
+// pww_xattn_fwd_multi_{f16,bf16} (g_stride 1: g_sigma[b] for image b).
+template <typename E>
 int xattn_fwd(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
               int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
               int64_t o_batch_stride, int64_t o_row_stride, const float* wmap, int64_t wmap_batch_stride,
@@ -156,9 +158,9 @@ int xattn_fwd(const void* q, const void* k, const void* v, void* out, int B, int
   if (!v || !out || !aligned16(v) || !aligned16(out)) return PWW_ERR_BAD_ARG;
   if ((o_batch_stride | o_row_stride) & 7 || o_row_stride < (int64_t)H * D) return PWW_ERR_BAD_ARG;
   if (wmap && (!stats || !g_sigma)) return PWW_ERR_BAD_ARG;
-  pww::XattnParams p;
+  pww::XattnParams<E> p;
   memset(&p, 0, sizeof(p));
-  p.q = (const __half*)q; p.k = (const __half*)k; p.v = (const __half*)v; p.out = (__half*)out;
+  p.q = (const E*)q; p.k = (const E*)k; p.v = (const E*)v; p.out = (E*)out;
   p.B = B; p.H = H; p.N = N; p.T = T; p.D = D;
   p.q_bs = q_batch_stride; p.q_rs = q_row_stride; p.k_bs = k_batch_stride; p.k_rs = k_row_stride;
   p.o_bs = o_batch_stride; p.o_rs = o_row_stride;
@@ -167,7 +169,7 @@ int xattn_fwd(const void* q, const void* k, const void* v, void* out, int B, int
   cudaStream_t s = (cudaStream_t)stream;
   {
     for (int b0 = 0; b0 < B; b0 += pww::tc::kMaxBatch) {          // <= 256 images per launch
-      pww::XattnParams c = p;
+      pww::XattnParams<E> c = p;
       c.B = (B - b0) < pww::tc::kMaxBatch ? (B - b0) : pww::tc::kMaxBatch;
       c.q = p.q + (int64_t)b0 * p.q_bs;
       c.k = p.k + (int64_t)b0 * p.k_bs;
@@ -184,8 +186,9 @@ int xattn_fwd(const void* q, const void* k, const void* v, void* out, int B, int
   }
 }
 
-// The one launch of pww_xattn_fused_f16 (one `stat` and g_sigma[0] for every image) and of pww_xattn_fused_multi_f16
-// (per_image: kinds[b] and g_sigma[b] for image b).
+// The one launch of pww_xattn_fused_{f16,bf16} (one `stat` and g_sigma[0] for every image) and of
+// pww_xattn_fused_multi_{f16,bf16} (per_image: kinds[b] and g_sigma[b] for image b).  mpack is fp16 for both E.
+template <typename E>
 int xattn_fused(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
                 int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
                 int64_t o_batch_stride, int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw,
@@ -202,9 +205,9 @@ int xattn_fused(const void* q, const void* k, const void* v, void* out, int B, i
     if (per_image ? !kinds : (stat != PWW_STAT_MAX && stat != PWW_STAT_STD)) return PWW_ERR_BAD_ARG;
     if (workspace_bytes < pww_xattn_fused_workspace_bytes()) return PWW_ERR_WORKSPACE;
   }
-  pww::XattnParams p;
+  pww::XattnParams<E> p;
   memset(&p, 0, sizeof(p));
-  p.q = (const __half*)q; p.k = (const __half*)k; p.v = (const __half*)v; p.out = (__half*)out;
+  p.q = (const E*)q; p.k = (const E*)k; p.v = (const E*)v; p.out = (E*)out;
   p.B = B; p.H = H; p.N = N; p.T = T; p.D = D;
   p.q_bs = q_batch_stride; p.q_rs = q_row_stride; p.k_bs = k_batch_stride; p.k_rs = k_row_stride;
   p.o_bs = o_batch_stride; p.o_rs = o_row_stride;
@@ -225,7 +228,7 @@ int xattn_fused(const void* q, const void* k, const void* v, void* out, int B, i
     }
   }
   for (int b0 = 0; b0 < B; b0 += chunk) {
-    pww::XattnParams c = p;
+    pww::XattnParams<E> c = p;
     c.B = (B - b0) < chunk ? (B - b0) : chunk;
     c.q = p.q + (int64_t)b0 * p.q_bs;
     c.k = p.k + (int64_t)b0 * p.k_bs;
@@ -252,85 +255,19 @@ int xattn_fused(const void* q, const void* k, const void* v, void* out, int B, i
   return PWW_OK;
 }
 
-}  // namespace
-
-extern "C" {
-
-int pww_xattn_stats_f16(const void* q, const void* k, int B, int H, int N, int T, int D, int64_t q_batch_stride,
-                        int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int stat,
-                        const int32_t* wmap_index, float* stats, void* workspace, size_t workspace_bytes,
-                        void* stream) {
-  return xattn_stats(q, k, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride, stat, nullptr,
-                     false, wmap_index, stats, workspace, workspace_bytes, stream);
-}
-
-int pww_xattn_stats_multi_f16(const void* q, const void* k, int B, int H, int N, int T, int D, int64_t q_batch_stride,
-                              int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, const int32_t* stat,
-                              const int32_t* wmap_index, float* stats, void* workspace, size_t workspace_bytes,
-                              void* stream) {
-  return xattn_stats(q, k, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride, PWW_STAT_MAX,
-                     stat, true, wmap_index, stats, workspace, workspace_bytes, stream);
-}
-
-int pww_xattn_fwd_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
-                      int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
-                      int64_t o_batch_stride, int64_t o_row_stride, const float* wmap, int64_t wmap_batch_stride,
-                      const int32_t* wmap_index, const float* stats, const float* g_sigma, float scale,
-                      void* stream) {
-  return xattn_fwd(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
-                   o_batch_stride, o_row_stride, wmap, wmap_batch_stride, wmap_index, stats, g_sigma, 0, scale, stream);
-}
-
-int pww_xattn_fwd_multi_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
-                            int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
-                            int64_t o_batch_stride, int64_t o_row_stride, const float* wmap, int64_t wmap_batch_stride,
-                            const int32_t* wmap_index, const float* stats, const float* g_sigma, float scale,
-                            void* stream) {
-  return xattn_fwd(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
-                   o_batch_stride, o_row_stride, wmap, wmap_batch_stride, wmap_index, stats, g_sigma, 1, scale, stream);
-}
-
-size_t pww_xattn_fused_workspace_bytes(void) { return pww::fx::fused_workspace_bytes(); }
-
-int pww_xattn_fused_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
-                        int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
-                        int64_t o_batch_stride, int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride,
-                        int Bw, const int8_t* cidx, const int32_t* wmap_index, int stat, const float* g_sigma,
-                        float scale, float* stats, void* workspace, size_t workspace_bytes, void* stream) {
-  return xattn_fused(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
-                     o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, stat, nullptr,
-                     false, g_sigma, scale, stats, workspace, workspace_bytes, stream);
-}
-
-int pww_xattn_fused_multi_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
-                              int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride,
-                              int64_t k_row_stride, int64_t o_batch_stride, int64_t o_row_stride, const void* mpack,
-                              int64_t mpack_batch_stride, int Bw, const int8_t* cidx, const int32_t* wmap_index,
-                              const int32_t* stat, const float* g_sigma, float scale, float* stats, void* workspace,
-                              size_t workspace_bytes, void* stream) {
-  return xattn_fused(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
-                     o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, PWW_STAT_MAX, stat,
-                     true, g_sigma, scale, stats, workspace, workspace_bytes, stream);
-}
-
-size_t pww_groupnorm_workspace_bytes(int B, int HW, int G) {
-  if (B <= 0 || HW <= 0 || G <= 0) return 0;
-  return align_up((size_t)B * sizeof(unsigned int), 256) + align_up((size_t)B * G * 2 * sizeof(float), 256) +
-         (size_t)B * pww::uops::gn_chunks(HW) * G * 2 * sizeof(float);
-}
-
-int pww_groupnorm_nhwc_f16(const void* x, const void* add, int64_t add_batch_stride, const void* gamma, const void* beta,
-                           void* y, int B, int HW, int C, int G, float eps, int silu, void* workspace,
-                           size_t workspace_bytes, void* stream) {
+template <typename E>
+int groupnorm_nhwc(const void* x, const void* add, int64_t add_batch_stride, const void* gamma, const void* beta, void* y,
+                   int B, int HW, int C, int G, float eps, int silu, void* workspace, size_t workspace_bytes,
+                   void* stream) {
   if (!x || !gamma || !beta || !y || !workspace || B <= 0 || HW <= 0 || C <= 0 || G <= 0) return PWW_ERR_BAD_ARG;
   if (!aligned16(x) || !aligned16(y) || !aligned16(gamma) || !aligned16(beta) || (add && !aligned16(add)))
     return PWW_ERR_BAD_ARG;
   if ((C & 7) || (C % G) || G > 64 || (C >> 3) > 1024) return PWW_ERR_UNSUPPORTED;
   if (add && ((add_batch_stride & 7) || add_batch_stride < C)) return PWW_ERR_BAD_ARG;
   if (workspace_bytes < pww_groupnorm_workspace_bytes(B, HW, G)) return PWW_ERR_WORKSPACE;
-  pww::uops::GnParams p;
-  p.x = (const __half*)x; p.add = (const __half*)add; p.add_bs = add_batch_stride; p.gamma = (const __half*)gamma; p.beta = (const __half*)beta;
-  p.y = (__half*)y;
+  pww::uops::GnParams<E> p;
+  p.x = (const E*)x; p.add = (const E*)add; p.add_bs = add_batch_stride; p.gamma = (const E*)gamma; p.beta = (const E*)beta;
+  p.y = (E*)y;
   char* w = (char*)workspace;
   p.counters = (unsigned int*)w;
   w += align_up((size_t)B * sizeof(unsigned int), 256);
@@ -345,30 +282,32 @@ int pww_groupnorm_nhwc_f16(const void* x, const void* add, int64_t add_batch_str
   const int rpp = nvec >= 256 ? 1 : 256 / nvec;
   const size_t smem1 = (size_t)rpp * C * 2 * sizeof(float);
   if (smem1 > 48 * 1024) return PWW_ERR_UNSUPPORTED;
-  pww::uops::gn_stats_kernel<<<dim3(p.chunks, B), nvec * rpp, smem1, s>>>(p);
+  pww::uops::gn_stats_kernel<E><<<dim3(p.chunks, B), nvec * rpp, smem1, s>>>(p);
   // enough row chunks to fill the machine even at 8x8 resolution
   int rows_per_block = (int)(((long long)HW * B + 2 * pww::tc::num_sms() - 1) / (2 * pww::tc::num_sms()));
   if (rows_per_block < rpp) rows_per_block = rpp;
   if (rows_per_block > 32) rows_per_block = 32;
-  pww::uops::gn_apply_kernel<<<dim3((HW + rows_per_block - 1) / rows_per_block, B), nvec * rpp, 0, s>>>(p, rows_per_block);
+  pww::uops::gn_apply_kernel<E><<<dim3((HW + rows_per_block - 1) / rows_per_block, B), nvec * rpp, 0, s>>>(p, rows_per_block);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 
-int pww_geglu_f16(const void* in, void* out, int64_t M, int I, void* stream) {
+template <typename E>
+int geglu(const void* in, void* out, int64_t M, int I, void* stream) {
   if (!in || !out || M <= 0 || I <= 0 || !aligned16(in) || !aligned16(out)) return PWW_ERR_BAD_ARG;
   if (I & 7) return PWW_ERR_UNSUPPORTED;
   const long long total = (long long)M * (I >> 3);
   long long blocks = (total + 255) / 256;
   const long long cap = (long long)pww::tc::num_sms() * 16;
   if (blocks > cap) blocks = cap;
-  pww::uops::geglu_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>((const __half*)in, (__half*)out, M, I);
+  pww::uops::geglu_kernel<E><<<(int)blocks, 256, 0, (cudaStream_t)stream>>>((const E*)in, (E*)out, M, I);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 
-int pww_add_layernorm_f16(const void* x, const void* res, const void* gamma, const void* beta, void* sum_out, void* y,
-                          int64_t M, int C, float eps, void* stream) {
+template <typename E>
+int add_layernorm(const void* x, const void* res, const void* gamma, const void* beta, void* sum_out, void* y, int64_t M,
+                  int C, float eps, void* stream) {
   if (!x || !gamma || !beta || !y || M <= 0 || C <= 0) return PWW_ERR_BAD_ARG;
   if (!aligned16(x) || !aligned16(y) || !aligned16(gamma) || !aligned16(beta) || (res && !aligned16(res)) ||
       (sum_out && !aligned16(sum_out)))
@@ -378,21 +317,200 @@ int pww_add_layernorm_f16(const void* x, const void* res, const void* gamma, con
   const int warps = 8;
   const unsigned grid = (unsigned)((M + warps - 1) / warps);
   cudaStream_t s = (cudaStream_t)stream;
-  const __half *xp = (const __half*)x, *rp = (const __half*)res, *gp = (const __half*)gamma, *bp = (const __half*)beta;
-  __half *sp = (__half*)sum_out, *yp = (__half*)y;
+  const E *xp = (const E*)x, *rp = (const E*)res, *gp = (const E*)gamma, *bp = (const E*)beta;
+  E *sp = (E*)sum_out, *yp = (E*)y;
   switch (vpl) {
-    case 1: pww::uops::add_layernorm_kernel<1><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
-    case 2: pww::uops::add_layernorm_kernel<2><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
-    case 3: pww::uops::add_layernorm_kernel<3><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
-    case 4: pww::uops::add_layernorm_kernel<4><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
-    case 5: pww::uops::add_layernorm_kernel<5><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
-    case 6: pww::uops::add_layernorm_kernel<6><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
-    case 7: pww::uops::add_layernorm_kernel<7><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
-    case 8: pww::uops::add_layernorm_kernel<8><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
+    case 1: pww::uops::add_layernorm_kernel<E, 1><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
+    case 2: pww::uops::add_layernorm_kernel<E, 2><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
+    case 3: pww::uops::add_layernorm_kernel<E, 3><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
+    case 4: pww::uops::add_layernorm_kernel<E, 4><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
+    case 5: pww::uops::add_layernorm_kernel<E, 5><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
+    case 6: pww::uops::add_layernorm_kernel<E, 6><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
+    case 7: pww::uops::add_layernorm_kernel<E, 7><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
+    case 8: pww::uops::add_layernorm_kernel<E, 8><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
     default: return PWW_ERR_UNSUPPORTED;
   }
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
+}
+
+template <typename E>
+int attn_fwd(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int D, int64_t qkv_batch_stride,
+             int64_t qkv_row_stride, int64_t o_batch_stride, int64_t o_row_stride, float scale, void* stream) {
+  if (!q || !k || !v || !out || B <= 0 || H <= 0 || N <= 0 || D <= 0) return PWW_ERR_BAD_ARG;
+  if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out)) return PWW_ERR_BAD_ARG;
+  if ((qkv_batch_stride | qkv_row_stride | o_batch_stride | o_row_stride) & 7) return PWW_ERR_BAD_ARG;
+  if (qkv_row_stride < (int64_t)H * D || o_row_stride < (int64_t)H * D) return PWW_ERR_BAD_ARG;
+  if (!supported_head_dim(D)) return PWW_ERR_UNSUPPORTED;
+  cudaStream_t s = (cudaStream_t)stream;
+  cudaError_t e = cudaErrorInvalidValue;
+  const int64_t bs = qkv_batch_stride, rs = qkv_row_stride, obs = o_batch_stride, ors = o_row_stride;
+  switch (D) {
+    case 40: e = pww::fa::launch<40, E>(q, k, v, out, B, H, N, bs, rs, obs, ors, scale, s); break;
+    case 64: e = pww::fa::launch<64, E>(q, k, v, out, B, H, N, bs, rs, obs, ors, scale, s); break;
+    case 80: e = pww::fa::launch<80, E>(q, k, v, out, B, H, N, bs, rs, obs, ors, scale, s); break;
+    case 160: e = pww::fa::launch<160, E>(q, k, v, out, B, H, N, bs, rs, obs, ors, scale, s); break;
+  }
+  return e == cudaSuccess ? PWW_OK : cuda_fail(e);
+}
+
+}  // namespace
+
+extern "C" {
+
+// Every _f16 / _bf16 pair below is one templated body above, instantiated for __half / __nv_bfloat16.
+int pww_xattn_stats_f16(const void* q, const void* k, int B, int H, int N, int T, int D, int64_t q_batch_stride,
+    int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int stat, const int32_t* wmap_index,
+    float* stats, void* workspace, size_t workspace_bytes, void* stream) {
+  return xattn_stats<__half>(
+      q, k, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride, stat, nullptr, false,
+      wmap_index, stats, workspace, workspace_bytes, stream);
+}
+int pww_xattn_stats_bf16(const void* q, const void* k, int B, int H, int N, int T, int D, int64_t q_batch_stride,
+    int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int stat, const int32_t* wmap_index,
+    float* stats, void* workspace, size_t workspace_bytes, void* stream) {
+  return xattn_stats<__nv_bfloat16>(
+      q, k, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride, stat, nullptr, false,
+      wmap_index, stats, workspace, workspace_bytes, stream);
+}
+
+int pww_xattn_stats_multi_f16(const void* q, const void* k, int B, int H, int N, int T, int D, int64_t q_batch_stride,
+    int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, const int32_t* stat, const int32_t* wmap_index,
+    float* stats, void* workspace, size_t workspace_bytes, void* stream) {
+  return xattn_stats<__half>(
+      q, k, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride, PWW_STAT_MAX, stat, true,
+      wmap_index, stats, workspace, workspace_bytes, stream);
+}
+int pww_xattn_stats_multi_bf16(const void* q, const void* k, int B, int H, int N, int T, int D, int64_t q_batch_stride,
+    int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, const int32_t* stat, const int32_t* wmap_index,
+    float* stats, void* workspace, size_t workspace_bytes, void* stream) {
+  return xattn_stats<__nv_bfloat16>(
+      q, k, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride, PWW_STAT_MAX, stat, true,
+      wmap_index, stats, workspace, workspace_bytes, stream);
+}
+
+int pww_xattn_fwd_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+    int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int64_t o_batch_stride,
+    int64_t o_row_stride, const float* wmap, int64_t wmap_batch_stride, const int32_t* wmap_index, const float* stats,
+    const float* g_sigma, float scale, void* stream) {
+  return xattn_fwd<__half>(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+      o_batch_stride, o_row_stride, wmap, wmap_batch_stride, wmap_index, stats, g_sigma, 0, scale, stream);
+}
+int pww_xattn_fwd_bf16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+    int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int64_t o_batch_stride,
+    int64_t o_row_stride, const float* wmap, int64_t wmap_batch_stride, const int32_t* wmap_index, const float* stats,
+    const float* g_sigma, float scale, void* stream) {
+  return xattn_fwd<__nv_bfloat16>(
+      q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+      o_batch_stride, o_row_stride, wmap, wmap_batch_stride, wmap_index, stats, g_sigma, 0, scale, stream);
+}
+
+int pww_xattn_fwd_multi_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+    int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int64_t o_batch_stride,
+    int64_t o_row_stride, const float* wmap, int64_t wmap_batch_stride, const int32_t* wmap_index, const float* stats,
+    const float* g_sigma, float scale, void* stream) {
+  return xattn_fwd<__half>(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+      o_batch_stride, o_row_stride, wmap, wmap_batch_stride, wmap_index, stats, g_sigma, 1, scale, stream);
+}
+int pww_xattn_fwd_multi_bf16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+    int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int64_t o_batch_stride,
+    int64_t o_row_stride, const float* wmap, int64_t wmap_batch_stride, const int32_t* wmap_index, const float* stats,
+    const float* g_sigma, float scale, void* stream) {
+  return xattn_fwd<__nv_bfloat16>(
+      q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+      o_batch_stride, o_row_stride, wmap, wmap_batch_stride, wmap_index, stats, g_sigma, 1, scale, stream);
+}
+
+size_t pww_xattn_fused_workspace_bytes(void) { return pww::fx::fused_workspace_bytes(); }
+
+int pww_xattn_fused_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+    int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int64_t o_batch_stride,
+    int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+    const int32_t* wmap_index, int stat, const float* g_sigma, float scale, float* stats, void* workspace,
+    size_t workspace_bytes, void* stream) {
+  return xattn_fused<__half>(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+      o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, stat, nullptr, false,
+      g_sigma, scale, stats, workspace, workspace_bytes, stream);
+}
+int pww_xattn_fused_bf16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+    int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int64_t o_batch_stride,
+    int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+    const int32_t* wmap_index, int stat, const float* g_sigma, float scale, float* stats, void* workspace,
+    size_t workspace_bytes, void* stream) {
+  return xattn_fused<__nv_bfloat16>(
+      q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+      o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, stat, nullptr, false,
+      g_sigma, scale, stats, workspace, workspace_bytes, stream);
+}
+
+int pww_xattn_fused_multi_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+    int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int64_t o_batch_stride,
+    int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+    const int32_t* wmap_index, const int32_t* stat, const float* g_sigma, float scale, float* stats, void* workspace,
+    size_t workspace_bytes, void* stream) {
+  return xattn_fused<__half>(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+      o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, PWW_STAT_MAX, stat, true,
+      g_sigma, scale, stats, workspace, workspace_bytes, stream);
+}
+int pww_xattn_fused_multi_bf16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+    int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int64_t o_batch_stride,
+    int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+    const int32_t* wmap_index, const int32_t* stat, const float* g_sigma, float scale, float* stats, void* workspace,
+    size_t workspace_bytes, void* stream) {
+  return xattn_fused<__nv_bfloat16>(
+      q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+      o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, PWW_STAT_MAX, stat, true,
+      g_sigma, scale, stats, workspace, workspace_bytes, stream);
+}
+
+int pww_attn_fwd_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int D,
+    int64_t qkv_batch_stride, int64_t qkv_row_stride, int64_t o_batch_stride, int64_t o_row_stride, float scale,
+    void* stream) {
+  return attn_fwd<__half>(
+      q, k, v, out, B, H, N, D, qkv_batch_stride, qkv_row_stride, o_batch_stride, o_row_stride, scale, stream);
+}
+int pww_attn_fwd_bf16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int D,
+    int64_t qkv_batch_stride, int64_t qkv_row_stride, int64_t o_batch_stride, int64_t o_row_stride, float scale,
+    void* stream) {
+  return attn_fwd<__nv_bfloat16>(
+      q, k, v, out, B, H, N, D, qkv_batch_stride, qkv_row_stride, o_batch_stride, o_row_stride, scale, stream);
+}
+
+size_t pww_groupnorm_workspace_bytes(int B, int HW, int G) {
+  if (B <= 0 || HW <= 0 || G <= 0) return 0;
+  return align_up((size_t)B * sizeof(unsigned int), 256) + align_up((size_t)B * G * 2 * sizeof(float), 256) +
+         (size_t)B * pww::uops::gn_chunks(HW) * G * 2 * sizeof(float);
+}
+
+int pww_groupnorm_nhwc_f16(const void* x, const void* add, int64_t add_batch_stride, const void* gamma,
+    const void* beta, void* y, int B, int HW, int C, int G, float eps, int silu, void* workspace, size_t workspace_bytes,
+    void* stream) {
+  return groupnorm_nhwc<__half>(
+      x, add, add_batch_stride, gamma, beta, y, B, HW, C, G, eps, silu, workspace, workspace_bytes,
+      stream);
+}
+int pww_groupnorm_nhwc_bf16(const void* x, const void* add, int64_t add_batch_stride, const void* gamma,
+    const void* beta, void* y, int B, int HW, int C, int G, float eps, int silu, void* workspace, size_t workspace_bytes,
+    void* stream) {
+  return groupnorm_nhwc<__nv_bfloat16>(
+      x, add, add_batch_stride, gamma, beta, y, B, HW, C, G, eps, silu, workspace, workspace_bytes,
+      stream);
+}
+
+int pww_geglu_f16(const void* in, void* out, int64_t M, int I, void* stream) {
+  return geglu<__half>(in, out, M, I, stream);
+}
+int pww_geglu_bf16(const void* in, void* out, int64_t M, int I, void* stream) {
+  return geglu<__nv_bfloat16>(in, out, M, I, stream);
+}
+
+int pww_add_layernorm_f16(const void* x, const void* res, const void* gamma, const void* beta, void* sum_out, void* y,
+    int64_t M, int C, float eps, void* stream) {
+  return add_layernorm<__half>(x, res, gamma, beta, sum_out, y, M, C, eps, stream);
+}
+int pww_add_layernorm_bf16(const void* x, const void* res, const void* gamma, const void* beta, void* sum_out, void* y,
+    int64_t M, int C, float eps, void* stream) {
+  return add_layernorm<__nv_bfloat16>(x, res, gamma, beta, sum_out, y, M, C, eps, stream);
 }
 
 int pww_sampler_input(const float* latents, const float* scale, const float* extra, void* out, int out_dtype, int m,
@@ -400,13 +518,14 @@ int pww_sampler_input(const float* latents, const float* scale, const float* ext
   if (!latents || !scale || !out || m <= 0 || height <= 0 || width <= 0) return PWW_ERR_BAD_ARG;
   if (channels != 4 && channels != 9) return PWW_ERR_BAD_ARG;
   if ((channels == 9) != (extra != nullptr)) return PWW_ERR_BAD_ARG;
-  if (out_dtype != PWW_DTYPE_F32 && out_dtype != PWW_DTYPE_F16) return PWW_ERR_UNSUPPORTED;
+  if (out_dtype != PWW_DTYPE_F32 && out_dtype != PWW_DTYPE_F16 && out_dtype != PWW_DTYPE_BF16) return PWW_ERR_UNSUPPORTED;
   pww::smp::InputArgs a;
   a.lat = latents; a.scale = scale; a.extra = extra; a.out = out; a.m = m; a.C = channels; a.hw = height * width;
   const bool px4 = (a.hw % 4) == 0 && aligned16(latents) && (!extra || aligned16(extra)) && aligned16(out);
   cudaStream_t s = (cudaStream_t)stream;
-  const cudaError_t e = out_dtype == PWW_DTYPE_F16 ? pww::smp::launch_input<__half>(a, px4, s)
-                                                   : pww::smp::launch_input<float>(a, px4, s);
+  const cudaError_t e = out_dtype == PWW_DTYPE_F16    ? pww::smp::launch_input<__half>(a, px4, s)
+                        : out_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_input<__nv_bfloat16>(a, px4, s)
+                                                      : pww::smp::launch_input<float>(a, px4, s);
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 
@@ -416,21 +535,22 @@ int pww_sampler_update(const void* eps, int eps_dtype, int64_t eps_batch_stride,
                        int height, int width, void* stream) {
   if (!eps || !latents || !history || !guidance || !beta || !form) return PWW_ERR_BAD_ARG;
   if (m <= 0 || height <= 0 || width <= 0 || history_len < 1 || history_len > 4) return PWW_ERR_BAD_ARG;
-  if (eps_dtype != PWW_DTYPE_F32 && eps_dtype != PWW_DTYPE_F16) return PWW_ERR_UNSUPPORTED;
+  if (eps_dtype != PWW_DTYPE_F32 && eps_dtype != PWW_DTYPE_F16 && eps_dtype != PWW_DTYPE_BF16) return PWW_ERR_UNSUPPORTED;
   pww::smp::UpdateArgs a;
   a.eps = eps; a.e_sn = eps_batch_stride; a.e_sc = eps_channel_stride; a.e_sh = eps_row_stride; a.e_sw = eps_col_stride;
   a.lat = latents; a.hist = history; a.noise = noise; a.gscale = guidance; a.beta = beta; a.form = form;
   a.m = m; a.h = height; a.w = width; a.nh = history_len;
   const int64_t hw = (int64_t)height * width;
-  const size_t es = eps_dtype == PWW_DTYPE_F16 ? 2 : 4;
+  const size_t es = eps_dtype == PWW_DTYPE_F32 ? 4 : 2;
   const bool px4 = (hw % 4) == 0 && aligned16(latents) && aligned16(history) && (!noise || aligned16(noise));
-  // channels-last packed rows: pixel p's 4 channels at 4p (8 bytes per pixel in fp16, 16 in fp32)
+  // channels-last packed rows: pixel p's 4 channels at 4p (8 bytes per pixel in fp16 / bf16, 16 in fp32)
   const size_t need = px4 ? 16 : 4 * es;
   const bool cl = eps_channel_stride == 1 && eps_col_stride == 4 && eps_row_stride == 4 * (int64_t)width &&
                   (reinterpret_cast<uintptr_t>(eps) % need) == 0 && ((size_t)eps_batch_stride * es) % need == 0;
   cudaStream_t s = (cudaStream_t)stream;
-  const cudaError_t e = eps_dtype == PWW_DTYPE_F16 ? pww::smp::launch_update<__half>(a, px4, cl, s)
-                                                   : pww::smp::launch_update<float>(a, px4, cl, s);
+  const cudaError_t e = eps_dtype == PWW_DTYPE_F16    ? pww::smp::launch_update<__half>(a, px4, cl, s)
+                        : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_update<__nv_bfloat16>(a, px4, cl, s)
+                                                      : pww::smp::launch_update<float>(a, px4, cl, s);
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 
@@ -463,25 +583,6 @@ int pww_debug_set_fused_jobs_dump(void* device_buffer) {
 int pww_debug_fused_cta_has_image(int cta, int grid, int B, int H, int tiles, const int* wmap_index, int b) {
   if (!wmap_index) return PWW_ERR_BAD_ARG;
   return pww::fx::fused_cta_has_image_host(cta, grid, B, H, tiles, wmap_index, b);
-}
-
-int pww_attn_fwd_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int D,
-                     int64_t qkv_batch_stride, int64_t qkv_row_stride, int64_t o_batch_stride, int64_t o_row_stride,
-                     float scale, void* stream) {
-  if (!q || !k || !v || !out || B <= 0 || H <= 0 || N <= 0 || D <= 0) return PWW_ERR_BAD_ARG;
-  if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out)) return PWW_ERR_BAD_ARG;
-  if ((qkv_batch_stride | qkv_row_stride | o_batch_stride | o_row_stride) & 7) return PWW_ERR_BAD_ARG;
-  if (qkv_row_stride < (int64_t)H * D || o_row_stride < (int64_t)H * D) return PWW_ERR_BAD_ARG;
-  if (!supported_head_dim(D)) return PWW_ERR_UNSUPPORTED;
-  cudaStream_t s = (cudaStream_t)stream;
-  cudaError_t e = cudaErrorInvalidValue;
-  switch (D) {
-    case 40: e = pww::fa::launch<40>(q, k, v, out, B, H, N, qkv_batch_stride, qkv_row_stride, o_batch_stride, o_row_stride, scale, s); break;
-    case 64: e = pww::fa::launch<64>(q, k, v, out, B, H, N, qkv_batch_stride, qkv_row_stride, o_batch_stride, o_row_stride, scale, s); break;
-    case 80: e = pww::fa::launch<80>(q, k, v, out, B, H, N, qkv_batch_stride, qkv_row_stride, o_batch_stride, o_row_stride, scale, s); break;
-    case 160: e = pww::fa::launch<160>(q, k, v, out, B, H, N, qkv_batch_stride, qkv_row_stride, o_batch_stride, o_row_stride, scale, s); break;
-  }
-  return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 
 }  // extern "C"

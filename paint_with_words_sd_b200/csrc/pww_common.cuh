@@ -1,5 +1,6 @@
 // Shared host/device helpers for libpww_b200.so (sm_90a).
 #pragma once
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -8,19 +9,39 @@
 
 namespace pww {
 
+// Element type of the activations: __half (fp16) or __nv_bfloat16 (bf16).  Every kernel family is instantiated for
+// both; the conversions below are the only place the two differ outside the MMA instruction (mma_sm90.cuh).  Both
+// are 2-byte types, so copies, strides and shared-memory layouts are the same.
+template <typename E> struct Elem;
+template <> struct Elem<__half> {
+  using E2 = __half2;
+  static __device__ __forceinline__ float to_float(__half x) { return __half2float(x); }
+  static __device__ __forceinline__ __half from_float(float x) { return __float2half_rn(x); }
+  static __device__ __forceinline__ float2 to_float2(__half2 x) { return __half22float2(x); }
+  static __device__ __forceinline__ __half2 from_float2(float lo, float hi) { return __floats2half2_rn(lo, hi); }
+};
+template <> struct Elem<__nv_bfloat16> {
+  using E2 = __nv_bfloat162;
+  static __device__ __forceinline__ float to_float(__nv_bfloat16 x) { return __bfloat162float(x); }
+  static __device__ __forceinline__ __nv_bfloat16 from_float(float x) { return __float2bfloat16_rn(x); }
+  static __device__ __forceinline__ float2 to_float2(__nv_bfloat162 x) { return __bfloat1622float2(x); }
+  static __device__ __forceinline__ __nv_bfloat162 from_float2(float lo, float hi) { return __floats2bfloat162_rn(lo, hi); }
+};
+
 // Per-image partial of the score statistic written by one CTA of the stats kernel.
 struct StatPartial {
-  double vmax;   // max of fp16-rounded scores seen by the CTA
-  double sum;    // sum of fp16-rounded scores
+  double vmax;   // max of the scores seen by the CTA
+  double sum;    // sum of the element-type-rounded scores
   double sumsq;  // sum of squares
   double pad;
 };
 
+template <typename E>
 struct XattnParams {
-  const __half* q;
-  const __half* k;
-  const __half* v;
-  __half* out;
+  const E* q;
+  const E* k;
+  const E* v;
+  E* out;
   int B, H, N, T, D;
   int64_t q_bs, q_rs, k_bs, k_rs, o_bs, o_rs;  // element strides
   const float* wmap;
@@ -40,13 +61,17 @@ struct XattnParams {
 
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
-__device__ __forceinline__ float round_to_f16(float x) { return __half2float(__float2half_rn(x)); }
+// x rounded to the nearest value of element type E.
+template <typename E>
+__device__ __forceinline__ float round_to(float x) { return Elem<E>::to_float(Elem<E>::from_float(x)); }
 
 // Statistic kind of image b: max unless the image's kind (per-image array, else the launch's `stat`) is PWW_STAT_STD.
-__device__ __forceinline__ bool image_is_max(const XattnParams& p, int b) {
+template <typename E>
+__device__ __forceinline__ bool image_is_max(const XattnParams<E>& p, int b) {
   return p.stat_kind != nullptr ? __ldg(p.stat_kind + b) != PWW_STAT_STD : p.stat != PWW_STAT_STD;
 }
 // G(sigma) of image b.
-__device__ __forceinline__ float image_g(const XattnParams& p, int b) { return __ldg(p.g_sigma + (int64_t)b * p.g_stride); }
+template <typename E>
+__device__ __forceinline__ float image_g(const XattnParams<E>& p, int b) { return __ldg(p.g_sigma + (int64_t)b * p.g_stride); }
 
 }  // namespace pww

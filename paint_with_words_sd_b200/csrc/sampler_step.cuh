@@ -36,14 +36,19 @@ struct InputArgs {
   int m, C, hw;
 };
 
-template <typename T> __device__ __forceinline__ float to_f(T v);
-template <> __device__ __forceinline__ float to_f<float>(float v) { return v; }
-template <> __device__ __forceinline__ float to_f<__half>(__half v) { return __half2float(v); }
+// T = float, __half or __nv_bfloat16 (the UNet's dtype)
+template <typename T>
+__device__ __forceinline__ float to_f(T v) {
+  if constexpr (sizeof(T) == 4) return v;
+  else return Elem<T>::to_float(v);
+}
 
-__device__ __forceinline__ float2 h2_to_f2(unsigned u) {
-  __half2 h;
+// Two 2-byte elements packed in one 32-bit word.
+template <typename T>
+__device__ __forceinline__ float2 pair_to_f2(unsigned u) {
+  typename Elem<T>::E2 h;
   memcpy(&h, &u, sizeof(h));
-  return __half22float2(h);
+  return Elem<T>::to_float2(h);
 }
 
 // PX consecutive fp32 values (PX = 4: one 16-byte access).
@@ -81,13 +86,13 @@ __device__ __forceinline__ void load_eps(const T* base, const UpdateArgs& a, int
 #pragma unroll
     for (int k = 0; k < 2; ++k) {                 // one 16-byte access = two pixels
       const uint4 t = __ldg(s + k);
-      const float2 a0 = h2_to_f2(t.x), a1 = h2_to_f2(t.y), b0 = h2_to_f2(t.z), b1 = h2_to_f2(t.w);
+      const float2 a0 = pair_to_f2<T>(t.x), a1 = pair_to_f2<T>(t.y), b0 = pair_to_f2<T>(t.z), b1 = pair_to_f2<T>(t.w);
       e[0][2 * k] = a0.x; e[1][2 * k] = a0.y; e[2][2 * k] = a1.x; e[3][2 * k] = a1.y;
       e[0][2 * k + 1] = b0.x; e[1][2 * k + 1] = b0.y; e[2][2 * k + 1] = b1.x; e[3][2 * k + 1] = b1.y;
     }
-  } else if constexpr (CL) {                      // fp16, one pixel: one 8-byte access
+  } else if constexpr (CL) {                      // 2-byte types, one pixel: one 8-byte access
     const uint2 t = __ldg(reinterpret_cast<const uint2*>(base + (int64_t)p0 * 4));
-    const float2 a0 = h2_to_f2(t.x), a1 = h2_to_f2(t.y);
+    const float2 a0 = pair_to_f2<T>(t.x), a1 = pair_to_f2<T>(t.y);
     e[0][0] = a0.x; e[1][0] = a0.y; e[2][0] = a1.x; e[3][0] = a1.y;
   } else {
 #pragma unroll
@@ -160,18 +165,18 @@ __global__ void __launch_bounds__(kThreads) sampler_update_kernel(const UpdateAr
   }
 }
 
-template <int PX>
-__device__ __forceinline__ void store_out(float* p, const float (&v)[PX]) { store_px<PX>(p, v); }
-template <int PX>
-__device__ __forceinline__ void store_out(__half* p, const float (&v)[PX]) {
-  if constexpr (PX == 4) {
-    const __half2 lo = __floats2half2_rn(v[0], v[1]), hi = __floats2half2_rn(v[2], v[3]);
+template <typename T, int PX>
+__device__ __forceinline__ void store_out(T* p, const float (&v)[PX]) {
+  if constexpr (sizeof(T) == 4) {
+    store_px<PX>(p, v);
+  } else if constexpr (PX == 4) {
+    const typename Elem<T>::E2 lo = Elem<T>::from_float2(v[0], v[1]), hi = Elem<T>::from_float2(v[2], v[3]);
     uint2 u;
     memcpy(&u.x, &lo, 4);
     memcpy(&u.y, &hi, 4);
     *reinterpret_cast<uint2*>(p) = u;
   } else {
-    *p = __float2half_rn(v[0]);
+    *p = Elem<T>::from_float(v[0]);
   }
 }
 
@@ -194,8 +199,8 @@ __global__ void __launch_bounds__(kThreads) sampler_input_kernel(const InputArgs
     load_px<PX>(a.extra + ((int64_t)i * (a.C - 4) + (c - 4)) * a.hw + p0, v);
   }
   T* out = static_cast<T*>(a.out);
-  store_out<PX>(out + ((int64_t)i * a.C + c) * a.hw + p0, v);
-  store_out<PX>(out + ((int64_t)(i + a.m) * a.C + c) * a.hw + p0, v);
+  store_out<T, PX>(out + ((int64_t)i * a.C + c) * a.hw + p0, v);
+  store_out<T, PX>(out + ((int64_t)(i + a.m) * a.C + c) * a.hw + p0, v);
 }
 
 inline unsigned blocks_for(int64_t threads) { return (unsigned)((threads + kThreads - 1) / kThreads); }

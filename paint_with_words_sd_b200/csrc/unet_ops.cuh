@@ -1,20 +1,22 @@
 // Memory-bound fused ops of the UNet that CALLS the attention path (SURVEY.md 8f-1): GroupNorm(+per-channel add)(+SiLU)
-// and GEGLU on channels-last fp16 activations.  Each replaces 3-6 eager PyTorch launches and, together with
-// channels-last convolutions, removes every NCHW<->NHWC conversion from the step.  Both are HBM-bound streaming
-// kernels: 16-byte vector loads/stores, one pass for statistics + one pass to apply, deterministic reductions.
+// and GEGLU on channels-last activations of element type E (fp16 or bf16).  Each replaces 3-6 eager PyTorch launches
+// and, together with channels-last convolutions, removes every NCHW<->NHWC conversion from the step.  Both are HBM-bound
+// streaming kernels: 16-byte vector loads/stores, one pass for statistics + one pass to apply, deterministic reductions.
+// Arithmetic is fp32 in both types; only the loads' conversion and the stores' rounding depend on E.
 #pragma once
 #include "pww_common.cuh"
 
 namespace pww {
 namespace uops {
 
+template <typename E>
 struct GnParams {
-  const __half* x;      // [B, HW, C] channels-last activations
-  const __half* add;    // [B, C] (row stride add_bs) or nullptr: per-image per-channel value added BEFORE normalisation
+  const E* x;      // [B, HW, C] channels-last activations
+  const E* add;    // [B, C] (row stride add_bs) or nullptr: per-image per-channel value added BEFORE normalisation
   long long add_bs;
-  const __half* gamma;  // [C]
-  const __half* beta;   // [C]
-  __half* y;            // [B, HW, C]
+  const E* gamma;  // [C]
+  const E* beta;   // [C]
+  E* y;            // [B, HW, C]
   float* partial;       // [B, chunks, G, 2] (sum, sumsq) scratch
   float* stats;         // [B, G, 2] (mean, rstd), written by the last stats block of each image
   unsigned int* counters;  // [B] arrival counters (zero on entry, zero on exit)
@@ -23,7 +25,10 @@ struct GnParams {
 };
 
 // pass 1: per (image, row chunk) partial sums per group.  block = nvec * rpp threads (nvec = C/8 vectors per row)
-__global__ void gn_stats_kernel(GnParams p) {
+template <typename E>
+__global__ void gn_stats_kernel(GnParams<E> p) {
+  using X = Elem<E>;
+  using E2 = typename X::E2;
   extern __shared__ float sm[];                 // [rpp][C][2] staging for the cross-row reduction, then [G][2]
   const int nvec = p.C >> 3;
   const int rpp = blockDim.x / nvec;
@@ -35,11 +40,11 @@ __global__ void gn_stats_kernel(GnParams p) {
   for (int i = 0; i < 8; ++i) { s[i] = 0.f; q[i] = 0.f; a[i] = 0.f; }
   if (p.add) {
     const uint4 av = *reinterpret_cast<const uint4*>(p.add + (size_t)b * p.add_bs + v * 8);
-    const __half2* ah = reinterpret_cast<const __half2*>(&av);
+    const E2* ah = reinterpret_cast<const E2*>(&av);
 #pragma unroll
-    for (int i = 0; i < 4; ++i) { float2 f = __half22float2(ah[i]); a[2 * i] = f.x; a[2 * i + 1] = f.y; }
+    for (int i = 0; i < 4; ++i) { float2 f = X::to_float2(ah[i]); a[2 * i] = f.x; a[2 * i + 1] = f.y; }
   }
-  const __half* xb = p.x + (size_t)b * p.HW * p.C;
+  const E* xb = p.x + (size_t)b * p.HW * p.C;
   // 4 independent 16-byte loads in flight per thread
   for (int r = r0 + rl; r < r1; r += 4 * rpp) {
     uint4 xv[4];
@@ -51,10 +56,10 @@ __global__ void gn_stats_kernel(GnParams p) {
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       if (r + u * rpp < r1) {
-        const __half2* xh = reinterpret_cast<const __half2*>(&xv[u]);
+        const E2* xh = reinterpret_cast<const E2*>(&xv[u]);
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-          float2 f = __half22float2(xh[i]);
+          float2 f = X::to_float2(xh[i]);
           const float x0 = f.x + a[2 * i], x1 = f.y + a[2 * i + 1];
           s[2 * i] += x0; q[2 * i] = fmaf(x0, x0, q[2 * i]);
           s[2 * i + 1] += x1; q[2 * i + 1] = fmaf(x1, x1, q[2 * i + 1]);
@@ -111,7 +116,10 @@ __global__ void gn_stats_kernel(GnParams p) {
 
 // pass 2: y = act((x + add - mean) * rstd * gamma + beta).  grid (row chunks, B); block = nvec * rpp threads: a thread
 // keeps ONE 8-channel vector column, so its scale/shift live in registers and the row loop is pure streaming.
-__global__ void gn_apply_kernel(GnParams p, int rows_per_block) {
+template <typename E>
+__global__ void gn_apply_kernel(GnParams<E> p, int rows_per_block) {
+  using X = Elem<E>;
+  using E2 = typename X::E2;
   const int nvec = p.C >> 3;
   const int rpp = blockDim.x / nvec;
   const int v = threadIdx.x % nvec, rl = threadIdx.x / nvec;
@@ -123,41 +131,44 @@ __global__ void gn_apply_kernel(GnParams p, int rows_per_block) {
     const uint4 bv = __ldg(reinterpret_cast<const uint4*>(p.beta) + v);
     uint4 av = make_uint4(0, 0, 0, 0);
     if (p.add) av = __ldg(reinterpret_cast<const uint4*>(p.add + (size_t)b * p.add_bs) + v);
-    const __half* gh = reinterpret_cast<const __half*>(&gv);
-    const __half* bh = reinterpret_cast<const __half*>(&bv);
-    const __half* ah = reinterpret_cast<const __half*>(&av);
+    const E* gh = reinterpret_cast<const E*>(&gv);
+    const E* bh = reinterpret_cast<const E*>(&bv);
+    const E* ah = reinterpret_cast<const E*>(&av);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int g = (v * 8 + i) / cg;
       const float mean = __ldg(p.stats + ((size_t)b * p.G + g) * 2), rstd = __ldg(p.stats + ((size_t)b * p.G + g) * 2 + 1);
-      sc[i] = rstd * __half2float(gh[i]);
-      sh[i] = __half2float(bh[i]) + (__half2float(ah[i]) - mean) * sc[i];
+      sc[i] = rstd * X::to_float(gh[i]);
+      sh[i] = X::to_float(bh[i]) + (X::to_float(ah[i]) - mean) * sc[i];
     }
   }
   const int r0 = blockIdx.x * rows_per_block, r1 = min(p.HW, r0 + rows_per_block);
-  const __half* xb = p.x + (size_t)b * p.HW * p.C;
-  __half* yb = p.y + (size_t)b * p.HW * p.C;
+  const E* xb = p.x + (size_t)b * p.HW * p.C;
+  E* yb = p.y + (size_t)b * p.HW * p.C;
   for (int r = r0 + rl; r < r1; r += rpp) {
     const uint4 xv = __ldg(reinterpret_cast<const uint4*>(xb + (size_t)r * p.C) + v);
-    const __half2* xh = reinterpret_cast<const __half2*>(&xv);
-    __align__(16) __half2 o[4];
+    const E2* xh = reinterpret_cast<const E2*>(&xv);
+    __align__(16) E2 o[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const float2 f = __half22float2(xh[k]);
+      const float2 f = X::to_float2(xh[k]);
       float y0 = fmaf(f.x, sc[2 * k], sh[2 * k]);
       float y1 = fmaf(f.y, sc[2 * k + 1], sh[2 * k + 1]);
       if (p.silu) {
         y0 = __fdividef(y0, 1.f + __expf(-y0));
         y1 = __fdividef(y1, 1.f + __expf(-y1));
       }
-      o[k] = __floats2half2_rn(y0, y1);
+      o[k] = X::from_float2(y0, y1);
     }
     reinterpret_cast<uint4*>(yb + (size_t)r * p.C)[v] = *reinterpret_cast<const uint4*>(o);
   }
 }
 
 // GEGLU: out[m, i] = in[m, i] * gelu(in[m, I + i])   (exact erf GELU, like torch.nn.functional.gelu)
-__global__ void geglu_kernel(const __half* __restrict__ in, __half* __restrict__ out, long long M, int I) {
+template <typename E>
+__global__ void geglu_kernel(const E* __restrict__ in, E* __restrict__ out, long long M, int I) {
+  using X = Elem<E>;
+  using E2 = typename X::E2;
   const int nvec = I >> 3;
   const long long total = M * nvec;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -165,15 +176,15 @@ __global__ void geglu_kernel(const __half* __restrict__ in, __half* __restrict__
     const int v = (int)(i % nvec);
     const uint4 av = __ldg(reinterpret_cast<const uint4*>(in + m * 2 * I) + v);
     const uint4 gv = __ldg(reinterpret_cast<const uint4*>(in + m * 2 * I + I) + v);
-    const __half2* ah = reinterpret_cast<const __half2*>(&av);
-    const __half2* gh = reinterpret_cast<const __half2*>(&gv);
-    __align__(16) __half2 o[4];
+    const E2* ah = reinterpret_cast<const E2*>(&av);
+    const E2* gh = reinterpret_cast<const E2*>(&gv);
+    __align__(16) E2 o[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const float2 a = __half22float2(ah[k]), g = __half22float2(gh[k]);
+      const float2 a = X::to_float2(ah[k]), g = X::to_float2(gh[k]);
       const float g0 = 0.5f * g.x * (1.f + erff(g.x * 0.70710678118654752f));
       const float g1 = 0.5f * g.y * (1.f + erff(g.y * 0.70710678118654752f));
-      o[k] = __floats2half2_rn(a.x * g0, a.y * g1);
+      o[k] = X::from_float2(a.x * g0, a.y * g1);
     }
     reinterpret_cast<uint4*>(out + m * I)[v] = *reinterpret_cast<const uint4*>(o);
   }
@@ -181,10 +192,12 @@ __global__ void geglu_kernel(const __half* __restrict__ in, __half* __restrict__
 
 // Fused residual add + LayerNorm over the last dim: s = x (+ res); sum_out = s (optional); y = LN(s) * gamma + beta.
 // One warp per row; a lane keeps its 16-byte vectors of the row in registers (C <= 2048), two-pass mean/variance.
-template <int VPL>   // vectors per lane
-__global__ void add_layernorm_kernel(const __half* __restrict__ x, const __half* __restrict__ res,
-                                     const __half* __restrict__ gamma, const __half* __restrict__ beta,
-                                     __half* __restrict__ sum_out, __half* __restrict__ y, long long M, int C, float eps) {
+template <typename E, int VPL>   // vectors per lane
+__global__ void add_layernorm_kernel(const E* __restrict__ x, const E* __restrict__ res,
+                                     const E* __restrict__ gamma, const E* __restrict__ beta,
+                                     E* __restrict__ sum_out, E* __restrict__ y, long long M, int C, float eps) {
+  using X = Elem<E>;
+  using E2 = typename X::E2;
   const int lane = threadIdx.x & 31;
   const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= M) return;
@@ -196,17 +209,17 @@ __global__ void add_layernorm_kernel(const __half* __restrict__ x, const __half*
     const int vi = lane + i * 32;
     if (vi < nvec) {
       const uint4 xv = __ldg(reinterpret_cast<const uint4*>(x + row * C) + vi);
-      const __half2* xh = reinterpret_cast<const __half2*>(&xv);
+      const E2* xh = reinterpret_cast<const E2*>(&xv);
       uint4 rv = make_uint4(0, 0, 0, 0);
       if (res) rv = __ldg(reinterpret_cast<const uint4*>(res + row * C) + vi);
-      const __half2* rh = reinterpret_cast<const __half2*>(&rv);
-      __align__(16) __half2 so[4];
+      const E2* rh = reinterpret_cast<const E2*>(&rv);
+      __align__(16) E2 so[4];
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        const float2 a = __half22float2(xh[k]), b = __half22float2(rh[k]);
-        // the residual stream is fp16 in the eager model too: round the sum once, then normalise the rounded value
-        so[k] = __floats2half2_rn(a.x + b.x, a.y + b.y);
-        const float2 f = __half22float2(so[k]);
+        const float2 a = X::to_float2(xh[k]), b = X::to_float2(rh[k]);
+        // the residual stream is E in the eager model too: round the sum once, then normalise the rounded value
+        so[k] = X::from_float2(a.x + b.x, a.y + b.y);
+        const float2 f = X::to_float2(so[k]);
         v[i][2 * k] = f.x; v[i][2 * k + 1] = f.y;
         sum += f.x + f.y;
       }
@@ -236,13 +249,13 @@ __global__ void add_layernorm_kernel(const __half* __restrict__ x, const __half*
     if (vi < nvec) {
       const uint4 gv = __ldg(reinterpret_cast<const uint4*>(gamma) + vi);
       const uint4 bv = __ldg(reinterpret_cast<const uint4*>(beta) + vi);
-      const __half2* gh = reinterpret_cast<const __half2*>(&gv);
-      const __half2* bh = reinterpret_cast<const __half2*>(&bv);
-      __align__(16) __half2 o[4];
+      const E2* gh = reinterpret_cast<const E2*>(&gv);
+      const E2* bh = reinterpret_cast<const E2*>(&bv);
+      __align__(16) E2 o[4];
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        const float2 g = __half22float2(gh[k]), b = __half22float2(bh[k]);
-        o[k] = __floats2half2_rn((v[i][2 * k] - mean) * rstd * g.x + b.x, (v[i][2 * k + 1] - mean) * rstd * g.y + b.y);
+        const float2 g = X::to_float2(gh[k]), b = X::to_float2(bh[k]);
+        o[k] = X::from_float2((v[i][2 * k] - mean) * rstd * g.x + b.x, (v[i][2 * k + 1] - mean) * rstd * g.y + b.y);
       }
       reinterpret_cast<uint4*>(y + row * C)[vi] = *reinterpret_cast<const uint4*>(o);
     }

@@ -1,13 +1,15 @@
 // Warp-level building blocks of the attention kernels on Hopper tensor cores.
 //
 // A CTA of 8 warps works on one [128-row x head] tile at a time; warp w owns query rows [16 w, 16 w + 16).  Operands are
-// staged in shared memory by 16-byte cp.async copies (rows of LD = DP + 8 halfs: the 16-byte pad makes every ldmatrix
-// phase hit 8 distinct bank groups), read into registers with ldmatrix and multiplied with mma.m16n8k16 (fp16 in, fp32
-// accumulate).  Cross-attention, per chunk of at most 80 keys (the softmax streams over 1, 2 or 3 chunks, below):
+// staged in shared memory by 16-byte cp.async copies (rows of LD = DP + 8 elements: the 16-byte pad makes every ldmatrix
+// phase hit 8 distinct bank groups), read into registers with ldmatrix and multiplied with mma.m16n8k16 (E in, fp32
+// accumulate).  E, the element type of q / k / v / out, is fp16 (__half) or bf16 (__nv_bfloat16); both are 2-byte types,
+// so only the MMA, the packing of P and O and the rounding of the statistic depend on it.  Cross-attention, per chunk
+// of at most 80 keys (the softmax streams over 1, 2 or 3 chunks, below):
 //     S = Q K^T   16 x 80 per warp, DP / 16 k-steps      accumulators: 10 n-tiles x 4 fp32 per thread
-//     P = 2^(log2e * scale * (S + bias - rowmax))        in registers; packed to fp16 it is the A operand of
+//     P = 2^(log2e * scale * (S + bias - rowmax))        in registers; packed to E it is the A operand of
 //     O = P V     16 x D per warp, 5 k-steps over the 80 padded keys, V fragments by ldmatrix.trans
-// and O is divided by the row sum of the fp16 P that was multiplied.  Padding (d >= D, token >= T, row >= N) is zero-filled
+// and O is divided by the row sum of the E-rounded P that was multiplied.  Padding (d >= D, token >= T, row >= N) is zero-filled
 // by the copies; padded tokens are masked to -inf before the softmax.
 #pragma once
 #include "mma_sm90.cuh"
@@ -25,17 +27,17 @@ template <int D>
 struct Tile {
   static_assert(D == 40 || D == 64 || D == 80 || D == 160, "head dims of SD1.5 (40 / 80 / 160) and SD2.x (64)");
   static constexpr int DP = (D + 15) / 16 * 16;    // k extent of Q K^T
-  static constexpr int LD = DP + 8;                // shared-memory row stride in halfs
+  static constexpr int LD = DP + 8;                // shared-memory row stride in (2-byte) elements
   static constexpr int KS = DP / 16;
   static constexpr int NT = D / 8;                 // n-tiles of P V
   static constexpr uint32_t QBYTES = kBM * LD * 2;
   static constexpr uint32_t KBYTES = kTP * LD * 2;
 };
 
-// Block-cooperative copy of rows [0, nrows) of a [rows x D] fp16 head slice (row stride rs elements) into shared rows of
-// LD halfs.  Rows >= valid and columns D .. DP-1 are zero-filled.
-template <int D>
-__device__ __forceinline__ void load_rows(uint32_t dst, const __half* src, int64_t rs, int nrows, int valid) {
+// Block-cooperative copy of rows [0, nrows) of a [rows x D] head slice (row stride rs elements) into shared rows of
+// LD elements.  Rows >= valid and columns D .. DP-1 are zero-filled.
+template <int D, typename E>
+__device__ __forceinline__ void load_rows(uint32_t dst, const E* src, int64_t rs, int nrows, int valid) {
   using C = Tile<D>;
   constexpr int CH = C::DP / 8, DCH = D / 8;
   for (int idx = threadIdx.x; idx < nrows * CH; idx += blockDim.x) {
@@ -47,7 +49,7 @@ __device__ __forceinline__ void load_rows(uint32_t dst, const __half* src, int64
 }
 
 // S (16 x 80) of the warp's rows: qs = shared address of the warp's first Q row, ks = the K tile.
-template <int D>
+template <int D, typename E>
 __device__ __forceinline__ void warp_qk(uint32_t qs, uint32_t ks, int lane, float (&s)[10][4]) {
   using C = Tile<D>;
 #pragma unroll
@@ -61,8 +63,8 @@ __device__ __forceinline__ void warp_qk(uint32_t qs, uint32_t ks, int lane, floa
       const int t = 16 * jp + (lane & 7) + ((lane >> 4) << 3), d = kk * 16 + ((lane >> 3) & 1) * 8;
       uint32_t b0, b1, b2, b3;
       ptx::ldsm_x4(ks + (uint32_t)(t * C::LD + d) * 2u, b0, b1, b2, b3);
-      ptx::mma16816(s[2 * jp], a, b0, b1);
-      ptx::mma16816(s[2 * jp + 1], a, b2, b3);
+      ptx::mma16816<E>(s[2 * jp], a, b0, b1);
+      ptx::mma16816<E>(s[2 * jp + 1], a, b2, b3);
     }
   }
 }
@@ -70,18 +72,18 @@ __device__ __forceinline__ void warp_qk(uint32_t qs, uint32_t ks, int lane, floa
 // Token of accumulator element e of n-tile j for this lane; the row is lane / 4 (+ 8 for e >= 2).
 __device__ __forceinline__ int tok(int j, int e, int lane) { return 8 * j + 2 * (lane & 3) + (e & 1); }
 
-// Normalised O of the warp's 16 rows -> fp16 in global memory: staged over the warp's own Q rows in shared memory (dead
+// Normalised O of the warp's 16 rows -> E in global memory: staged over the warp's own Q rows in shared memory (dead
 // once S exists), then written as whole 16-byte pieces of each row.  Rows >= N are dropped.
-template <int D>
-__device__ __forceinline__ void warp_store(const float (&o)[Tile<D>::NT][4], unsigned char* stage, int lane, __half* out,
+template <int D, typename E>
+__device__ __forceinline__ void warp_store(const float (&o)[Tile<D>::NT][4], unsigned char* stage, int lane, E* out,
                                            int64_t o_rs, int row0, int N) {
   using C = Tile<D>;
   __syncwarp();
   const int g = lane >> 2, q = lane & 3;
 #pragma unroll
   for (int j = 0; j < C::NT; ++j) {
-    *reinterpret_cast<uint32_t*>(stage + (g * C::LD + 8 * j + 2 * q) * 2) = ptx::pack_h2(o[j][0], o[j][1]);
-    *reinterpret_cast<uint32_t*>(stage + ((g + 8) * C::LD + 8 * j + 2 * q) * 2) = ptx::pack_h2(o[j][2], o[j][3]);
+    *reinterpret_cast<uint32_t*>(stage + (g * C::LD + 8 * j + 2 * q) * 2) = ptx::pack2<E>(o[j][0], o[j][1]);
+    *reinterpret_cast<uint32_t*>(stage + ((g + 8) * C::LD + 8 * j + 2 * q) * 2) = ptx::pack2<E>(o[j][2], o[j][3]);
   }
   __syncwarp();
   for (int idx = lane; idx < 16 * C::NT; idx += 32) {
@@ -96,7 +98,7 @@ __device__ __forceinline__ void warp_store(const float (&o)[Tile<D>::NT][4], uns
 // ---- key chunks: T <= 80 is one chunk of T keys; T = 154, 231 are 2 / 3 CLIP chunks of 77 ----
 // Chunk c (keys 77 c .. 77 c + kv - 1) is staged as its own 80-row K / V tile, rows kv .. 79 zero-filled and masked to
 // -inf, so warp_qk runs unchanged on every chunk.  The softmax streams over the chunks (running row max and sum, O
-// rescaled when the max moves, as in attn_tc.cuh); P is packed to fp16 and the row sum is the sum of the fp16 P values
+// rescaled when the max moves, as in attn_tc.cuh); P is packed to E and the row sum is the sum of the E-rounded P values
 // that were multiplied, rescaled in fp32.  The first chunk's rescale factor is ex2(-inf * scale) = 0 (scale > 0), so a
 // single chunk gives exactly the one-pass softmax.
 constexpr int kChunk = 77;      // keys per CLIP chunk
@@ -112,8 +114,8 @@ __host__ __device__ __forceinline__ constexpr int chunk_keys(int T) { return KC 
 
 // Copies of one job's operands into a stage: Q rows of the tile, then K (and V) rows of head h, one 80-row tile per
 // chunk with chunk_keys<KC>(T) real rows.  The caller commits the group.
-template <int D, int KC>
-__device__ __forceinline__ void load_operands(uint32_t st, const XattnParams& p, int b, int h, int tile, bool with_v) {
+template <int D, int KC, typename E>
+__device__ __forceinline__ void load_operands(uint32_t st, const XattnParams<E>& p, int b, int h, int tile, bool with_v) {
   using C = Tile<D>;
   const int rows = p.N - tile * kBM;
   load_rows<D>(st, p.q + (int64_t)b * p.q_bs + (int64_t)tile * kBM * p.q_rs + h * D, p.q_rs, kBM, rows < kBM ? rows : kBM);
@@ -136,7 +138,7 @@ __device__ __forceinline__ void warp_online_begin(float (&o)[Tile<D>::NT][4], fl
 
 // One chunk: s holds S + bias of the chunk's 80 padded keys, of which the first kv are real; vs is its V tile.  l0 / l1
 // are per-thread partial row sums.
-template <int D>
+template <int D, typename E>
 __device__ __forceinline__ void warp_online_chunk(float (&s)[10][4], int kv, float sl2, uint32_t vs, int lane,
                                                   float (&o)[Tile<D>::NT][4], float& m0, float& m1, float& l0, float& l1) {
   using C = Tile<D>;
@@ -160,9 +162,9 @@ __device__ __forceinline__ void warp_online_chunk(float (&s)[10][4], int kv, flo
   float r0 = 0.f, r1 = 0.f;
 #pragma unroll
   for (int j = 0; j < 10; ++j) {
-    const uint32_t p01 = ptx::pack_h2(ptx::ex2(fmaf(s[j][0], sl2, n0)), ptx::ex2(fmaf(s[j][1], sl2, n0)));
-    const uint32_t p23 = ptx::pack_h2(ptx::ex2(fmaf(s[j][2], sl2, n1)), ptx::ex2(fmaf(s[j][3], sl2, n1)));
-    const float2 f01 = ptx::unpack_h2(p01), f23 = ptx::unpack_h2(p23);    // sum exactly what the MMA multiplies
+    const uint32_t p01 = ptx::pack2<E>(ptx::ex2(fmaf(s[j][0], sl2, n0)), ptx::ex2(fmaf(s[j][1], sl2, n0)));
+    const uint32_t p23 = ptx::pack2<E>(ptx::ex2(fmaf(s[j][2], sl2, n1)), ptx::ex2(fmaf(s[j][3], sl2, n1)));
+    const float2 f01 = ptx::unpack2<E>(p01), f23 = ptx::unpack2<E>(p23);    // sum exactly what the MMA multiplies
     r0 += f01.x + f01.y;
     r1 += f23.x + f23.y;
     pa[j >> 1][(j & 1) * 2] = p01;
@@ -181,13 +183,13 @@ __device__ __forceinline__ void warp_online_chunk(float (&s)[10][4], int kv, flo
     for (int jp = 0; jp < C::NT / 2; ++jp) {
       uint32_t b0, b1, b2, b3;
       ptx::ldsm_x4_t(vs + (uint32_t)(t * C::LD + 16 * jp + (lane >> 4) * 8) * 2u, b0, b1, b2, b3);
-      ptx::mma16816(o[2 * jp], pa[kk], b0, b1);
-      ptx::mma16816(o[2 * jp + 1], pa[kk], b2, b3);
+      ptx::mma16816<E>(o[2 * jp], pa[kk], b0, b1);
+      ptx::mma16816<E>(o[2 * jp + 1], pa[kk], b2, b3);
     }
     if constexpr (C::NT & 1) {
       uint32_t b0, b1;
       ptx::ldsm_x2_t(vs + (uint32_t)(t * C::LD + 8 * (C::NT - 1)) * 2u, b0, b1);
-      ptx::mma16816(o[C::NT - 1], pa[kk], b0, b1);
+      ptx::mma16816<E>(o[C::NT - 1], pa[kk], b0, b1);
     }
   }
 }
@@ -206,8 +208,9 @@ __device__ __forceinline__ void warp_online_end(float (&o)[Tile<D>::NT][4], floa
   }
 }
 
-// Statistic partials of S over the warp's valid elements (row < N, token < T): running max of S (rounding to fp16 is
-// monotonic, so the maximum is rounded once at the end) or sum / sum of squares of fp16(S).
+// Statistic partials of S over the warp's valid elements (row < N, token < T): running max of S (rounding to E is
+// monotonic, so the maximum is rounded once at the end) or sum / sum of squares of E(S).
+template <typename E>
 __device__ __forceinline__ void warp_stat(const float (&s)[10][4], int T, int rows_left, int lane, bool is_max, float& vmax,
                                           float& sum, float& sumsq) {
   const int g = lane >> 2;
@@ -219,7 +222,7 @@ __device__ __forceinline__ void warp_stat(const float (&s)[10][4], int T, int ro
       if (is_max) {
         if (ok) vmax = fmaxf(vmax, s[j][e]);
       } else if (ok) {
-        const float h = round_to_f16(s[j][e]);
+        const float h = round_to<E>(s[j][e]);
         sum += h;
         sumsq = fmaf(h, h, sumsq);
       }
@@ -237,8 +240,9 @@ __device__ __forceinline__ void warp_reduce_stat(double& m, double& a, double& q
 }
 
 // The statistic of an image from its totals over all H * N * T scores: the maximum, or the unbiased standard deviation
-// (variance clamped at 0), rounded to fp16 as qk.max() / qk.std() return it in the reference.
-__device__ __forceinline__ float stat_value(const XattnParams& p, bool is_max, double m, double a, double q) {
+// (variance clamped at 0), rounded to E as qk.max() / qk.std() return it in the reference's op sequence under an E autocast.
+template <typename E>
+__device__ __forceinline__ float stat_value(const XattnParams<E>& p, bool is_max, double m, double a, double q) {
   const double cnt = (double)p.H * (double)p.N * (double)p.T;
   double r;
   if (is_max) {
@@ -247,7 +251,7 @@ __device__ __forceinline__ float stat_value(const XattnParams& p, bool is_max, d
     const double var = (q - a * a / cnt) / (cnt - 1.0);
     r = sqrt(var > 0.0 ? var : 0.0);
   }
-  return round_to_f16((float)r);
+  return round_to<E>((float)r);
 }
 
 }  // namespace core

@@ -9,7 +9,8 @@
 //        summed by the waiters in CTA order -- deterministic for a given grid);
 //     2. softmax jobs of the unbiased units: they need no statistic and overlap the other CTAs' statistic pass;
 //     3. grid barrier (per biased image, only the CTAs that publish for it), then the softmax jobs of the biased units
-//        with the bias x * W, x = g(sigma) * fp16(statistic), W rebuilt from the packed map (below).
+//        with the bias x * W, x = g(sigma) * E(statistic), W rebuilt from the packed map (below).  E, the element type
+//        of q / k / v / out, is fp16 or bf16; the packed map is fp16 whatever E is.
 // The statistic kind and g(sigma) are per image when the launch carries per-image arrays (XattnParams::stat_kind,
 // g_stride = 1), else one kind and one g(sigma) for every image; each CTA keeps the kind of its local biased images in
 // shared memory, so the statistic jobs, the publish step and the finalise step branch per image.
@@ -42,8 +43,9 @@ constexpr int kMaxLocal = 4;      // biased images one CTA's unit range may touc
 constexpr int kMW = 32;           // packed-map columns per row (64 bytes)
 constexpr int kRC = 10;           // dictionary capacity (distinct non-zero columns)
 
+template <typename E>
 struct FxParams {
-  XattnParams x;            // q/k/v/out, strides, wmap_index, g_sigma, scale, stat, stats_out, counters, partials
+  XattnParams<E> x;            // q/k/v/out, strides, wmap_index, g_sigma, scale, stat, stats_out, counters, partials
   const int8_t* cidx;       // [Bw, 80 k] dictionary column per token (k key chunks; token 77 c + j at 80 c + j), -1 = none
   const void* mpack;        // [Bw, N, 32] fp16 packed maps (see above)
   int64_t mpack_bs;         // elements
@@ -228,12 +230,12 @@ __device__ __forceinline__ float key_f32(unsigned k) {
   return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
 }
 
-template <int D, int KC>
-__global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const FxParams fp) {
+template <int D, int KC, typename E>
+__global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const FxParams<E> fp) {
   using C = core::Tile<D>;
   using CF = Cfg2<D, KC>;
   constexpr int CW = core::kTP * KC;                    // cidx columns: token 77 c + j of chunk c at column 80 c + j
-  const XattnParams& p = fp.x;
+  const XattnParams<E>& p = fp.x;
   extern __shared__ __align__(128) unsigned char smem[];
   const uint32_t smem0 = ptx::smem_u32(smem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -480,9 +482,9 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
             core::warp_reduce_stat(m, a, q);
           }
           if (lane == 0) {
-            const float st16 = core::stat_value(p, is_max, m, a, q);
-            s_coef[l] = (p.g_sigma != nullptr ? image_g(p, bl) : 0.f) * st16;
-            if (p.stats_out != nullptr) p.stats_out[bl] = st16;   // every CTA of the image writes the same value
+            const float stv = core::stat_value(p, is_max, m, a, q);
+            s_coef[l] = (p.g_sigma != nullptr ? image_g(p, bl) : 0.f) * stv;
+            if (p.stats_out != nullptr) p.stats_out[bl] = stv;   // every CTA of the image writes the same value
           }
         }
         __syncwarp();
@@ -504,8 +506,8 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
 #pragma unroll 1
       for (int c = 0; c < KC; ++c) {                // the real tokens of every chunk
         float s[10][4];
-        core::warp_qk<D>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
-        core::warp_stat(s, kv, p.N - row0, lane, s_ismax[li], vmax, sum, sumsq);
+        core::warp_qk<D, E>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
+        core::warp_stat<E>(s, kv, p.N - row0, lane, s_ismax[li], vmax, sum, sumsq);
       }
       dsum += (double)sum;
       dsq += (double)sumsq;
@@ -518,7 +520,7 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
 #pragma unroll 1
       for (int c = 0; c < KC; ++c) {
         float s[10][4];
-        core::warp_qk<D>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
+        core::warp_qk<D, E>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
         if (biased) {
           const signed char* ci = s_cidx[li] + c * core::kTP;
 #pragma unroll
@@ -532,7 +534,7 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
               }
             }
         }
-        core::warp_online_chunk<D>(s, kv, sl2, st + C::QBYTES + (KC + c) * C::KBYTES, lane, o, m0, m1, l0, l1);
+        core::warp_online_chunk<D, E>(s, kv, sl2, st + C::QBYTES + (KC + c) * C::KBYTES, lane, o, m0, m1, l0, l1);
       }
       core::warp_online_end<D>(o, l0, l1);
       core::warp_store<D>(o, smem + stage(i) + warp * 16 * C::LD * 2, lane, p.out + (int64_t)b * p.o_bs + h * D, p.o_rs,
@@ -597,10 +599,10 @@ inline bool fused2_fits(int B, int hg, int tiles, int grid) {
   return fused_range_ok(B, hg, tiles, grid) && fused_units_ok(units, grid) && (units + grid - 1) / grid + 1 <= kMaxUnits;
 }
 
-template <int D, int KC>
-cudaError_t launch_fused2(const XattnParams& x, const void* mpack, int64_t mpack_bs, const int8_t* cidx, cudaStream_t s) {
+template <int D, int KC, typename E>
+cudaError_t launch_fused2(const XattnParams<E>& x, const void* mpack, int64_t mpack_bs, const int8_t* cidx, cudaStream_t s) {
   using CF = Cfg2<D, KC>;
-  FxParams fp;
+  FxParams<E> fp;
   memset(&fp, 0, sizeof(fp));
   fp.x = x;
   fp.cidx = cidx;
@@ -614,7 +616,7 @@ cudaError_t launch_fused2(const XattnParams& x, const void* mpack, int64_t mpack
   if (!fused2_fits(x.B, fp.hg, fp.tiles, fp.grid)) return cudaErrorInvalidConfiguration;
   static bool attr_set[tc::kMaxDevices] = {false};
   if (!attr_set[tc::cur_device()]) {
-    cudaError_t e = cudaFuncSetAttribute(xattn_fused2_kernel<D, KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, CF::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(xattn_fused2_kernel<D, KC, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, CF::SMEM);
     if (e != cudaSuccess) return e;
     attr_set[tc::cur_device()] = true;
   }
@@ -629,7 +631,7 @@ cudaError_t launch_fused2(const XattnParams& x, const void* mpack, int64_t mpack
   attr[0].val.cooperative = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, xattn_fused2_kernel<D, KC>, fp);
+  return cudaLaunchKernelEx(&cfg, xattn_fused2_kernel<D, KC, E>, fp);
 }
 
 // Host replay of the job lists (test infrastructure): out[job] = {cta, i, kind, b, h, tile, biased, li} for every job of

@@ -4,7 +4,7 @@
 // 80-row K / V tile of the stage, and the softmax streams over them (xattn_core.cuh).
 //
 // Fused region of the reference's inj_forward (paint_with_words.py:87-118), per image b / head h / 128-row tile:
-//     statistics kernel:  per-image max / (sum, sumsq) of fp16(Q_h K_h^T) over all heads, rows and tokens
+//     statistics kernel:  per-image max / (sum, sumsq) of E(Q_h K_h^T) over all heads, rows and tokens (E = fp16 / bf16)
 //     forward kernel:     S = Q_h K_h^T;  P = softmax(scale * (S + g[b] * M_b * w[b]));  O = P V_h
 // The statistic kind and g are one value for the launch or one per image (XattnParams::stat_kind, g_stride).
 // with the warp-level MMA tiles of xattn_core.cuh.  Work unit = (image, row tile, head); every CTA of the persistent grid
@@ -39,8 +39,9 @@ struct Cfg {
   static_assert(SMEM <= 232448 - 8192, "shared memory budget (dynamic + static tables)");
 };
 
+template <typename E>
 struct TcParams {
-  XattnParams x;
+  XattnParams<E> x;
   int tiles;        // row tiles per image
   int units;        // B * tiles * H
 };
@@ -118,7 +119,8 @@ __device__ __forceinline__ void cta_range(int units, int& u0, int& u1) {
   u0 = (int)((long long)blockIdx.x * units / gridDim.x);
   u1 = (int)((long long)(blockIdx.x + 1) * units / gridDim.x);
 }
-__device__ __forceinline__ int image_widx(const XattnParams& p, int b) {
+template <typename E>
+__device__ __forceinline__ int image_widx(const XattnParams<E>& p, int b) {
   if (p.wmap == nullptr) return -1;
   return p.wmap_index ? p.wmap_index[b] : b;
 }
@@ -126,11 +128,11 @@ __device__ __forceinline__ int image_widx(const XattnParams& p, int b) {
 // ---------------------------------------------------------------------------------------------------------
 // forward kernel
 // ---------------------------------------------------------------------------------------------------------
-template <int D, int KC>
-__global__ void __launch_bounds__(kThreads, 1) xattn_fwd_kernel(const TcParams tp) {
+template <int D, int KC, typename E>
+__global__ void __launch_bounds__(kThreads, 1) xattn_fwd_kernel(const TcParams<E> tp) {
   using C = core::Tile<D>;
   using CF = Cfg<D, KC>;
-  const XattnParams& p = tp.x;
+  const XattnParams<E>& p = tp.x;
   extern __shared__ __align__(128) unsigned char smem[];
   const uint32_t smem0 = ptx::smem_u32(smem);
   __shared__ int s_img[kMaxBatch];
@@ -204,7 +206,7 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_fwd_kernel(const TcParams t
 #pragma unroll 1
     for (int c = 0; c < KC; ++c) {
       float s[10][4];
-      core::warp_qk<D>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
+      core::warp_qk<D, E>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
       if (widx >= 0) {
         const float x = s_coef[f.b];
         const float* wm = p.wmap + (int64_t)widx * p.wmap_bs + c * core::kChunk;   // chunk c, slot t = column 77 c + t
@@ -216,7 +218,7 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_fwd_kernel(const TcParams t
             if (t < kv && r < p.N) s[j][e] = fmaf(x, __ldg(wm + (int64_t)r * p.T + t), s[j][e]);
           }
       }
-      core::warp_online_chunk<D>(s, kv, sl2, st + C::QBYTES + (KC + c) * C::KBYTES, lane, o, m0, m1, l0, l1);
+      core::warp_online_chunk<D, E>(s, kv, sl2, st + C::QBYTES + (KC + c) * C::KBYTES, lane, o, m0, m1, l0, l1);
     }
     core::warp_online_end<D>(o, l0, l1);
     core::warp_store<D>(o, smem + (st - smem0) + warp * 16 * C::LD * 2, lane, p.out + (int64_t)f.b * p.o_bs + f.h * D, p.o_rs, row0, p.N);
@@ -225,13 +227,13 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_fwd_kernel(const TcParams t
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// statistics kernel: per-image max / (sum, sumsq) of fp16(S) over all heads, rows and tokens
+// statistics kernel: per-image max / (sum, sumsq) of E(S) over all heads, rows and tokens
 // ---------------------------------------------------------------------------------------------------------
-template <int D, int KC>
-__global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams tp) {
+template <int D, int KC, typename E>
+__global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams<E> tp) {
   using C = core::Tile<D>;
   using CF = Cfg<D, KC>;
-  const XattnParams& p = tp.x;
+  const XattnParams<E>& p = tp.x;
   extern __shared__ __align__(128) unsigned char smem[];
   const uint32_t smem0 = ptx::smem_u32(smem);
   __shared__ StatPartial s_part[core::kWarps][kMaxLocal];     // [warp][local image]
@@ -303,8 +305,8 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams
 #pragma unroll 1
       for (int c = 0; c < KC; ++c) {                // the real tokens of every chunk
         float s[10][4];
-        core::warp_qk<D>(st + (uint32_t)(warp * 16 * C::LD) * 2u, st + C::QBYTES + c * C::KBYTES, lane, s);
-        core::warp_stat(s, core::chunk_keys<KC>(p.T), p.N - tile * kBM - warp * 16, lane, is_max, vmax, sum, sumsq);
+        core::warp_qk<D, E>(st + (uint32_t)(warp * 16 * C::LD) * 2u, st + C::QBYTES + c * C::KBYTES, lane, s);
+        core::warp_stat<E>(s, core::chunk_keys<KC>(p.T), p.N - tile * kBM - warp * 16, lane, is_max, vmax, sum, sumsq);
       }
       dsum += (double)sum;
       dsq += (double)sumsq;
@@ -417,30 +419,30 @@ cudaError_t set_smem(const void* fn, uint32_t bytes, bool (&done)[kMaxDevices]) 
   return e;
 }
 
-template <int D, int KC>
-cudaError_t launch_fwd(const XattnParams& x, cudaStream_t s) {
-  TcParams tp;
+template <int D, int KC, typename E>
+cudaError_t launch_fwd(const XattnParams<E>& x, cudaStream_t s) {
+  TcParams<E> tp;
   tp.x = x;
   tp.tiles = ceil_div(x.N, kBM);
   tp.units = x.B * tp.tiles * x.H;
   static bool attr_set[kMaxDevices] = {false};
-  cudaError_t e = set_smem<D>((const void*)xattn_fwd_kernel<D, KC>, Cfg<D, KC>::SMEM, attr_set);
+  cudaError_t e = set_smem<D>((const void*)xattn_fwd_kernel<D, KC, E>, Cfg<D, KC>::SMEM, attr_set);
   if (e != cudaSuccess) return e;
   const int grid = tp.units < num_sms() ? tp.units : num_sms();
-  xattn_fwd_kernel<D, KC><<<grid, kThreads, Cfg<D, KC>::SMEM, s>>>(tp);
+  xattn_fwd_kernel<D, KC, E><<<grid, kThreads, Cfg<D, KC>::SMEM, s>>>(tp);
   return cudaGetLastError();
 }
 
-template <int D, int KC>
-cudaError_t launch_stats(const XattnParams& x, cudaStream_t s) {
-  TcParams tp;
+template <int D, int KC, typename E>
+cudaError_t launch_stats(const XattnParams<E>& x, cudaStream_t s) {
+  TcParams<E> tp;
   tp.x = x;
   tp.tiles = ceil_div(x.N, kBM);
   tp.units = x.B * tp.tiles * x.H;
   static bool attr_set[kMaxDevices] = {false};
-  cudaError_t e = set_smem<D>((const void*)xattn_stats_kernel<D, KC>, Cfg<D, KC>::SMEM, attr_set);
+  cudaError_t e = set_smem<D>((const void*)xattn_stats_kernel<D, KC, E>, Cfg<D, KC>::SMEM, attr_set);
   if (e != cudaSuccess) return e;
-  xattn_stats_kernel<D, KC><<<stats_grid(tp.units), kThreads, Cfg<D, KC>::SMEM, s>>>(tp);
+  xattn_stats_kernel<D, KC, E><<<stats_grid(tp.units), kThreads, Cfg<D, KC>::SMEM, s>>>(tp);
   return cudaGetLastError();
 }
 

@@ -1,7 +1,8 @@
 """Python wrappers for the fused channels-last UNet ops of libpww_b200 (GroupNorm[+add][+SiLU], GEGLU).
 
-Used by `unet.py` on CUDA fp16 activations; the CPU/fp32 route of the same modules stays plain PyTorch (it is what the
-CPU reference arm runs).  No fallback on CUDA: a non-zero status raises.
+Used by `unet.py` on CUDA fp16 or bf16 activations (the `_f16` / `_bf16` entry points, picked from x.dtype); the
+CPU/fp32 route of the same modules stays plain PyTorch (it is what the CPU reference arm runs).  No fallback on CUDA: a
+non-zero status raises.
 """
 from __future__ import annotations
 
@@ -33,12 +34,18 @@ ENABLED = True     # bench.py's eager-PyTorch comparison leg turns the fused UNe
 
 
 def is_fast(x: torch.Tensor) -> bool:
-    return ENABLED and x.is_cuda and x.dtype == torch.float16
+    return ENABLED and x.is_cuda and x.dtype in (torch.float16, torch.bfloat16)
+
+
+def _entry(name: str, x: torch.Tensor):
+    """The C entry point `name` (without its type suffix) for x's element type."""
+    return getattr(_native.lib(), name + ("_bf16" if x.dtype == torch.bfloat16 else "_f16"))
 
 
 def group_norm_nhwc(x: torch.Tensor, gn: torch.nn.GroupNorm, add: Optional[torch.Tensor] = None,
                     silu: bool = True) -> torch.Tensor:
-    """x: [B,C,H,W] fp16 in channels-last memory.  Returns act(GroupNorm(x + add[:, :, None, None])), channels last."""
+    """x: [B,C,H,W] fp16 or bf16 in channels-last memory, gn's parameters of the same type.  Returns
+    act(GroupNorm(x + add[:, :, None, None])), channels last; `add` is cast to x's type."""
     if not x.is_contiguous(memory_format=torch.channels_last):
         x = x.contiguous(memory_format=torch.channels_last)
     B, C, H, W = x.shape
@@ -48,35 +55,37 @@ def group_norm_nhwc(x: torch.Tensor, gn: torch.nn.GroupNorm, add: Optional[torch
     ws = _workspace(x.device, nbytes)
     add_bs = 0
     if add is not None:
-        if add.dtype != torch.float16 or add.stride(-1) != 1 or (add.stride(0) % 8) or (add.data_ptr() % 16):
-            add = add.to(torch.float16).contiguous()
+        if add.dtype != x.dtype or add.stride(-1) != 1 or (add.stride(0) % 8) or (add.data_ptr() % 16):
+            add = add.to(x.dtype).contiguous()
         add_bs = add.stride(0)
+    fn = _entry("pww_groupnorm_nhwc", x)
     with torch.cuda.device(x.device):
-        rc = L.pww_groupnorm_nhwc_f16(x.data_ptr(), None if add is None else add.data_ptr(), add_bs, gn.weight.data_ptr(),
-                                      gn.bias.data_ptr(), y.data_ptr(), B, H * W, C, gn.num_groups, float(gn.eps),
-                                      1 if silu else 0, ws.data_ptr(), ws.numel(),
-                                      torch.cuda.current_stream(x.device).cuda_stream)
-    _native.check(rc, "pww_groupnorm_nhwc_f16")
+        rc = fn(x.data_ptr(), None if add is None else add.data_ptr(), add_bs, gn.weight.data_ptr(),
+                gn.bias.data_ptr(), y.data_ptr(), B, H * W, C, gn.num_groups, float(gn.eps),
+                1 if silu else 0, ws.data_ptr(), ws.numel(), torch.cuda.current_stream(x.device).cuda_stream)
+    _native.check(rc, fn.__name__)
     _native.launch_count += 2
     return y
 
 
 def geglu(h: torch.Tensor) -> torch.Tensor:
-    """h: [..., 2*I] fp16 contiguous -> [..., I] = h[..., :I] * gelu(h[..., I:])."""
+    """h: [..., 2*I] fp16 or bf16 contiguous -> [..., I] = h[..., :I] * gelu(h[..., I:])."""
     if not h.is_contiguous():
         h = h.contiguous()
     I = h.shape[-1] // 2
     M = h.numel() // h.shape[-1]
     out = torch.empty(h.shape[:-1] + (I,), dtype=h.dtype, device=h.device)
+    fn = _entry("pww_geglu", h)
     with torch.cuda.device(h.device):
-        rc = _native.lib().pww_geglu_f16(h.data_ptr(), out.data_ptr(), M, I, torch.cuda.current_stream(h.device).cuda_stream)
-    _native.check(rc, "pww_geglu_f16")
+        rc = fn(h.data_ptr(), out.data_ptr(), M, I, torch.cuda.current_stream(h.device).cuda_stream)
+    _native.check(rc, fn.__name__)
     _native.launch_count += 1
     return out
 
 
 def add_layer_norm(x: torch.Tensor, res: Optional[torch.Tensor], ln: torch.nn.LayerNorm, want_sum: bool = True):
-    """(s, y) with s = x + res (s is x itself when res is None) and y = LayerNorm(s); x, res: [..., C] fp16."""
+    """(s, y) with s = x + res (s is x itself when res is None) and y = LayerNorm(s); x, res: [..., C] fp16 or bf16
+    (both of one type, ln's parameters too)."""
     if not x.is_contiguous():
         x = x.contiguous()
     if res is not None and not res.is_contiguous():
@@ -85,11 +94,11 @@ def add_layer_norm(x: torch.Tensor, res: Optional[torch.Tensor], ln: torch.nn.La
     M = x.numel() // C
     y = torch.empty_like(x)
     s = torch.empty_like(x) if (res is not None and want_sum) else None
+    fn = _entry("pww_add_layernorm", x)
     with torch.cuda.device(x.device):
-        rc = _native.lib().pww_add_layernorm_f16(x.data_ptr(), None if res is None else res.data_ptr(),
-                                                 ln.weight.data_ptr(), ln.bias.data_ptr(),
-                                                 None if s is None else s.data_ptr(), y.data_ptr(), M, C,
-                                                 float(ln.eps), torch.cuda.current_stream(x.device).cuda_stream)
-    _native.check(rc, "pww_add_layernorm_f16")
+        rc = fn(x.data_ptr(), None if res is None else res.data_ptr(), ln.weight.data_ptr(), ln.bias.data_ptr(),
+                None if s is None else s.data_ptr(), y.data_ptr(), M, C, float(ln.eps),
+                torch.cuda.current_stream(x.device).cuda_stream)
+    _native.check(rc, fn.__name__)
     _native.launch_count += 1
     return (x if res is None else s), y

@@ -54,14 +54,16 @@ _SYNTHETIC_CONFIGS = {
 
 def pww_load_tools(device: str = "cuda:0", scheduler_type=LMSDiscreteScheduler,
                    local_model_path: Optional[str] = None, hf_model_path: Optional[str] = None,
-                   model_token: Optional[str] = None, seed: int = 0):
+                   model_token: Optional[str] = None, seed: int = 0, torch_dtype: Optional[torch.dtype] = None):
     """paint_with_words.py:128-204: returns (vae, unet, text_encoder, tokenizer, scheduler) with the
     attention of `unet` patched.  `"synthetic:<sd15|sd15-inpaint|sd21|tiny>"` model paths build seeded
     random-weight stand-ins (no weights or network exist in this environment); any other path is
-    loaded with diffusers/transformers when those are installed."""
+    loaded with diffusers/transformers when those are installed.
+    `torch_dtype`: the UNet's (and VAE's) dtype; None keeps the reference's rule (fp16, fp32 on mps), and
+    torch.bfloat16 runs every native kernel in bf16."""
     assert local_model_path or hf_model_path, "either local_model_path or hf_model_path must be provided"
     model_path = local_model_path if local_model_path is not None else hf_model_path
-    dtype = torch.float16 if device != "mps" else torch.float32
+    dtype = torch_dtype if torch_dtype is not None else (torch.float16 if device != "mps" else torch.float32)
     if model_path in _SYNTHETIC_CONFIGS:
         cfg = _SYNTHETIC_CONFIGS[model_path]()
         unet = build_unet(cfg, seed=seed, dtype=dtype, device=device)
@@ -88,8 +90,9 @@ def pww_load_tools(device: str = "cuda:0", scheduler_type=LMSDiscreteScheduler,
 
 
 def _dtype_code(dtype) -> int:
-    """The C ABI's dtype code; -1 (rejected by the kernels as unsupported) for anything but fp16 / fp32."""
-    return {torch.float32: _native.PWW_DTYPE_F32, torch.float16: _native.PWW_DTYPE_F16}.get(dtype, -1)
+    """The C ABI's dtype code; -1 (rejected by the kernels as unsupported) for anything but fp32 / fp16 / bf16."""
+    return {torch.float32: _native.PWW_DTYPE_F32, torch.float16: _native.PWW_DTYPE_F16,
+            torch.bfloat16: _native.PWW_DTYPE_BF16}.get(dtype, -1)
 
 
 def _module_dtype(module, default=torch.float32):
@@ -436,14 +439,17 @@ def paint_with_words(
     strength: float = 0.5,
     return_latents: bool = False,
     max_prompt_chunks: int = 1,
+    torch_dtype: Optional[torch.dtype] = None,
 ):
     """paint_with_words.py:391-510.  Returns one PIL.Image (or the final latents with return_latents).
     `max_prompt_chunks` (1 .. 3): a prompt longer than 75 tokens fills up to that many 77-token CLIP chunks instead of
-    being truncated (conditioning.chunk_prompt); 1 is the reference's behaviour."""
+    being truncated (conditioning.chunk_prompt); 1 is the reference's behaviour.
+    `torch_dtype` is passed to `pww_load_tools` when this call loads the models (torch.bfloat16 for a bf16 UNet); with
+    `preloaded_utils` the UNet's own dtype decides."""
     width, height = color_map_image.size
     vae, unet, text_encoder, tokenizer, scheduler = (
         pww_load_tools(device, scheduler_type, local_model_path=local_model_path, hf_model_path=hf_model_path,
-                       model_token=model_token)
+                       model_token=model_token, torch_dtype=torch_dtype)
         if preloaded_utils is None else preloaded_utils)
     extra_seeds, seperated_word_contexts, cond, uncond = _encode_text_color_inputs(
         text_encoder, tokenizer, device, color_map_image, color_context, input_prompt, unconditional_input_prompt,
@@ -520,6 +526,7 @@ def paint_with_words_batch(
     model_token: Optional[str] = None,
     max_batch_size: int = 8,
     return_latents: bool = False,
+    torch_dtype: Optional[torch.dtype] = None,
 ):
     """Many images, each with its own settings, in as few samplers as possible.  `settings[i]` is a dict of the
     per-image keyword arguments of `paint_with_words` (BATCH_SETTING_KEYS: color_context, color_map_image, input_prompt,
@@ -530,13 +537,14 @@ def paint_with_words_batch(
     Entries of the same latent size and text length run in one `PwWSampler` of at most `max_batch_size` images (a
     2 * max_batch_size UNet batch with CFG), whatever their weight functions and guidance scales.  The default of 8 gave
     the most images/s of k = 1, 2, 4, 8 at 512x512 (BASELINE.md section 4) and bounds memory.  Sizes that are not multiples of 64 need the single-image weight-map fallback and
-    run one image per sampler.  img2img (init_image / strength) is not batched."""
+    run one image per sampler.  img2img (init_image / strength) is not batched.  `torch_dtype` as in
+    `paint_with_words`."""
     entries = _batch_settings(settings)
     if max_batch_size < 1:
         raise ValueError("max_batch_size must be >= 1")
     vae, unet, text_encoder, tokenizer, scheduler = (
         pww_load_tools(device, scheduler_type, local_model_path=local_model_path, hf_model_path=hf_model_path,
-                       model_token=model_token)
+                       model_token=model_token, torch_dtype=torch_dtype)
         if preloaded_utils is None else preloaded_utils)
     scheduler.set_timesteps(num_inference_steps)
     encoded, keys = [], []
@@ -614,12 +622,13 @@ def paint_with_words_inpaint(
     strength: float = 1.0,
     return_latents: bool = False,
     max_prompt_chunks: int = 1,
+    torch_dtype: Optional[torch.dtype] = None,
 ):
     """paint_with_words_inpaint.py:137-270: 9-channel UNet input cat[latents, mask, masked-image latents].
-    `max_prompt_chunks` as in `paint_with_words`."""
+    `max_prompt_chunks` and `torch_dtype` as in `paint_with_words`."""
     vae, unet, text_encoder, tokenizer, scheduler = (
         pww_load_tools(device, scheduler_type, local_model_path=local_model_path, hf_model_path=hf_model_path,
-                       model_token=model_token)
+                       model_token=model_token, torch_dtype=torch_dtype)
         if preloaded_utils is None else preloaded_utils)
     width, height = init_image.size
     color_map_image = color_map_image.resize((width, height), Image.NEAREST)
@@ -683,8 +692,10 @@ class PaintWithWord_StableDiffusionPipeline:
         self.plugin_cross_attention()
 
     @classmethod
-    def from_pretrained(cls, save_dir, device: str = "cuda:0", **kwargs):
-        vae, unet, text_encoder, tokenizer, scheduler = pww_load_tools(device, local_model_path=save_dir)
+    def from_pretrained(cls, save_dir, device: str = "cuda:0", torch_dtype: Optional[torch.dtype] = None, **kwargs):
+        """`torch_dtype` as in `pww_load_tools` (torch.bfloat16 for a bf16 UNet)."""
+        vae, unet, text_encoder, tokenizer, scheduler = pww_load_tools(device, local_model_path=save_dir,
+                                                                       torch_dtype=torch_dtype)
         return cls(vae=vae, text_encoder=text_encoder, tokenizer=tokenizer, unet=unet, scheduler=scheduler)
 
     def plugin_cross_attention(self):
@@ -735,8 +746,10 @@ class PaintWithWord_StableDiffusionInpaintPipeline(PaintWithWord_StableDiffusion
     """paint_with_words_inpaint.py:273-575: `__call__(prompt, image, mask_image, color_map_image, color_context, ...)`."""
 
     @classmethod
-    def from_pretrained(cls, save_dir, device: str = "cuda:0", **kwargs):
-        vae, unet, text_encoder, tokenizer, scheduler = pww_load_tools(device, local_model_path=save_dir)
+    def from_pretrained(cls, save_dir, device: str = "cuda:0", torch_dtype: Optional[torch.dtype] = None, **kwargs):
+        """`torch_dtype` as in `pww_load_tools` (torch.bfloat16 for a bf16 UNet)."""
+        vae, unet, text_encoder, tokenizer, scheduler = pww_load_tools(device, local_model_path=save_dir,
+                                                                       torch_dtype=torch_dtype)
         return cls(vae=vae, text_encoder=text_encoder, tokenizer=tokenizer, unet=unet, scheduler=scheduler)
 
     @torch.no_grad()

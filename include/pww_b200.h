@@ -300,6 +300,23 @@ int pww_sampler_update(const void* eps, int eps_dtype, int64_t eps_batch_stride,
                        const float* guidance, const float* beta, const float* form,
                        int m, int height, int width, void* stream);
 
+/*
+ * ControlNet residual injection: n (1..16) residuals added in place into n activations, in one launch.
+ *   dst_k[b] = E( dst_k[b] + E( s[k, b] * res_k[b] ) )        k < n, b < rows
+ * dst[k] points at a [B, elems_per_image[k]] tensor and res[k] at a [rows, elems_per_image[k]] one, both dense (a
+ * channels-last activation is); only the first `rows` images of each dst are touched (rows = B is the ordinary case,
+ * rows = B / 2 guess mode, where only the cond half gets the residuals).  `scales` is a device fp32 [n, rows] array, or
+ * NULL for a scale of 1.  The arithmetic is fp32, the product rounded to E before the add, so the result is bitwise
+ * torch's `skip + (r * s)` with the product in E.  dst, res and elems_per_image are HOST arrays of n entries; the
+ * table travels in the kernel parameters, so a captured CUDA graph carries it.
+ * Returns PWW_ERR_BAD_ARG, before any CUDA call, for n outside 1..16, rows < 1, an elems_per_image entry that is not a
+ * positive multiple of 8, or a null or not 16-byte-aligned pointer.
+ */
+int pww_control_inject_f16(int n, void* const* dst, const void* const* res, const int64_t* elems_per_image, int rows,
+                           const float* scales, void* stream);
+int pww_control_inject_bf16(int n, void* const* dst, const void* const* res, const int64_t* elems_per_image, int rows,
+                            const float* scales, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

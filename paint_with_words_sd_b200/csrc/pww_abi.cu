@@ -8,6 +8,7 @@
 #include "attn_tc.cuh"
 #include "unet_ops.cuh"
 #include "sampler_step.cuh"
+#include "control_inject.cuh"
 #include <stdlib.h>
 
 namespace {
@@ -354,6 +355,34 @@ int attn_fwd(const void* q, const void* k, const void* v, void* out, int B, int 
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 
+template <typename E>
+int control_inject(int n, void* const* dst, const void* const* res, const int64_t* elems_per_image, int rows,
+                   const float* scales, void* stream) {
+  if (n < 1 || n > pww::ctl::kMaxLevels || rows < 1 || !dst || !res || !elems_per_image) return PWW_ERR_BAD_ARG;
+  pww::ctl::InjectArgs a;
+  a.off[0] = 0;
+  for (int k = 0; k < n; ++k) {
+    const int64_t e = elems_per_image[k];
+    if (e <= 0 || (e % pww::ctl::kVec) != 0) return PWW_ERR_BAD_ARG;
+    if (!dst[k] || !res[k] || !aligned16(dst[k]) || !aligned16(res[k])) return PWW_ERR_BAD_ARG;
+    a.dst[k] = dst[k];
+    a.res[k] = res[k];
+    a.vec_per_image[k] = e / pww::ctl::kVec;
+    a.off[k + 1] = a.off[k] + (int64_t)rows * a.vec_per_image[k];
+  }
+  for (int k = n; k < pww::ctl::kMaxLevels; ++k) {
+    a.dst[k] = nullptr;
+    a.res[k] = nullptr;
+    a.vec_per_image[k] = 0;
+    a.off[k + 1] = a.off[n];
+  }
+  a.scales = scales;
+  a.n = n;
+  a.rows = rows;
+  const cudaError_t e = pww::ctl::launch_inject<E>(a, (int64_t)pww::tc::num_sms() * 8, (cudaStream_t)stream);
+  return e == cudaSuccess ? PWW_OK : cuda_fail(e);
+}
+
 }  // namespace
 
 extern "C" {
@@ -552,6 +581,15 @@ int pww_sampler_update(const void* eps, int eps_dtype, int64_t eps_batch_stride,
                         : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_update<__nv_bfloat16>(a, px4, cl, s)
                                                       : pww::smp::launch_update<float>(a, px4, cl, s);
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
+}
+
+int pww_control_inject_f16(int n, void* const* dst, const void* const* res, const int64_t* elems_per_image, int rows,
+                           const float* scales, void* stream) {
+  return control_inject<__half>(n, dst, res, elems_per_image, rows, scales, stream);
+}
+int pww_control_inject_bf16(int n, void* const* dst, const void* const* res, const int64_t* elems_per_image, int rows,
+                            const float* scales, void* stream) {
+  return control_inject<__nv_bfloat16>(n, dst, res, elems_per_image, rows, scales, stream);
 }
 
 // Test infrastructure (not declared in the public header): replay the forward kernel's unit schedule on the host.

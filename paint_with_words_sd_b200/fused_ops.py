@@ -1,4 +1,5 @@
-"""Python wrappers for the fused channels-last UNet ops of libpww_b200 (GroupNorm[+add][+SiLU], GEGLU).
+"""Python wrappers for the fused channels-last UNet ops of libpww_b200 (GroupNorm[+add][+SiLU], GEGLU, add+LayerNorm)
+and the ControlNet residual injection.
 
 Used by `unet.py` on CUDA fp16 or bf16 activations (the `_f16` / `_bf16` entry points, picked from x.dtype); the
 CPU/fp32 route of the same modules stays plain PyTorch (it is what the CPU reference arm runs).  No fallback on CUDA: a
@@ -6,6 +7,7 @@ non-zero status raises.
 """
 from __future__ import annotations
 
+import ctypes
 from typing import Dict, Optional
 
 import torch
@@ -102,3 +104,39 @@ def add_layer_norm(x: torch.Tensor, res: Optional[torch.Tensor], ln: torch.nn.La
     _native.check(rc, fn.__name__)
     _native.launch_count += 1
     return (x if res is None else s), y
+
+
+def _same_dense_layout(a: torch.Tensor, b: torch.Tensor) -> bool:
+    """Both channels-last contiguous or both contiguous: element j of image i is at i * C*h*w + j in both."""
+    cl = torch.channels_last
+    return (a.is_contiguous(memory_format=cl) and b.is_contiguous(memory_format=cl)) or (a.is_contiguous()
+                                                                                         and b.is_contiguous())
+
+
+def control_inject(dst, res, scales: Optional[torch.Tensor] = None) -> None:
+    """dst_k[:rows] += (res_k * scales[k, :, None, None, None]) in place for every k, in ONE launch
+    (`pww_control_inject_*`); rows = res_k.shape[0] <= dst_k.shape[0], the product rounded to dst's type before the add.
+    dst_k and res_k: [B, C, h, w] / [rows, C, h, w] of one element type and one memory format (channels-last in the
+    UNet).  `scales`: fp32 [n, rows] on dst's device, or None for a scale of 1."""
+    n = len(dst)
+    if n != len(res) or n < 1:
+        raise ValueError(f"control_inject needs as many residuals as targets (got {len(res)} for {n})")
+    rows = int(res[0].shape[0])
+    for k, (d, r) in enumerate(zip(dst, res)):
+        if (tuple(r.shape[1:]) != tuple(d.shape[1:]) or r.shape[0] != rows or rows > d.shape[0] or r.dtype != d.dtype
+                or r.device != d.device or not _same_dense_layout(d, r)):
+            raise ValueError(f"residual {k} {tuple(r.shape)} {r.dtype} does not match its target {tuple(d.shape)} "
+                             f"{d.dtype} (same type, format, channels and size, at most as many images)")
+    if scales is not None and (scales.dtype != torch.float32 or tuple(scales.shape) != (n, rows)
+                               or not scales.is_contiguous() or scales.device != dst[0].device):
+        raise ValueError(f"control scales must be a contiguous fp32 [{n}, {rows}] tensor on {dst[0].device}")
+    d0 = dst[0]
+    fn = _entry("pww_control_inject", d0)
+    ptrs = (ctypes.c_void_p * n)(*[d.data_ptr() for d in dst])
+    rptrs = (ctypes.c_void_p * n)(*[r.data_ptr() for r in res])
+    elems = (ctypes.c_int64 * n)(*[d[0].numel() for d in dst])
+    with torch.cuda.device(d0.device):
+        rc = fn(n, ptrs, rptrs, elems, rows, None if scales is None else scales.data_ptr(),
+                torch.cuda.current_stream(d0.device).cuda_stream)
+    _native.check(rc, fn.__name__)
+    _native.launch_count += 1

@@ -153,6 +153,32 @@ def _per_image(value, m: int, name: str, is_one) -> list:
     return vals
 
 
+# guess mode scales ControlNet residual k (0..12, the mid residual last) by 0.825 ** (12 - k) (hook_pww.py:132)
+GUESS_MODE_DECAY = 0.825
+
+
+def control_scales(conditioning_scales: Sequence[float], guess_mode: bool, levels: int = 13) -> torch.Tensor:
+    """CONTROL_SCALES for m images with these ControlNet weights: fp32 [levels, rows].  Plain: rows = 2m, column i and
+    column m + i both hold weight_i (the cond and uncond image share the residual's weight).  Guess mode: rows = m
+    (only the cond half gets residuals), entry [k, i] = weight_i * 0.825 ** (levels - 1 - k)."""
+    w = torch.tensor([float(s) for s in conditioning_scales], dtype=torch.float64)
+    if guess_mode:
+        decay = torch.tensor([GUESS_MODE_DECAY ** float(levels - 1 - k) for k in range(levels)], dtype=torch.float64)
+        return (decay[:, None] * w[None, :]).to(torch.float32)
+    return torch.cat([w, w]).to(torch.float32)[None, :].repeat(levels, 1)
+
+
+def control_step_active(i: int, n: int, start: float, end: float) -> bool:
+    """Is the ControlNet applied at step i (0-based) of n?  hook_pww.py:23-26: iff start <= i / n <= end."""
+    return start <= i / n <= end
+
+
+def control_image_tensor(image: Image.Image) -> torch.Tensor:
+    """A hint image as the ControlNet takes it: HWC RGB -> float / 255 -> [1, 3, H, W] in [0, 1] (no [-1, 1] remap)."""
+    arr = np.asarray(image.convert("RGB"), dtype=np.float32) / 255.0
+    return torch.from_numpy(arr.transpose(2, 0, 1).copy())[None]
+
+
 class PwWSampler:
     """Denoising loop for a group of images on ONE GPU (paint_with_words.py:471-506 semantics per image).
 
@@ -169,13 +195,26 @@ class PwWSampler:
     one float or m floats: images made with different settings share the sampler, and every cross-attention call is
     still one launch (per-image statistic kind and G(sigma) on the device).  An identically-zero function leaves its
     image unbiased.
+
+    ControlNet (`controlnet`, a `controlnet.ControlNetModel` built for the UNet's config): `control_image` is one
+    [1, 3, 8h, 8w] tensor in [0, 1] per image (one tensor for every image, or m), `controlnet_conditioning_scale` one
+    weight or m.  At set-up every image's hint is embedded once (it does not depend on the step) and the weights become
+    the UNet's CONTROL_SCALES table.  A step then runs the ControlNet on the first 4 channels of the UNet input with the
+    plain text context (the reference builds the PwW dict only afterwards, hook_pww.py:113-149), and the UNet adds its
+    13 residuals in one native launch.  `guess_mode`: the ControlNet sees only the m cond images, residual k is weighted
+    by 0.825 ** (12 - k) and only the cond half gets them (hook_pww.py:28-61, 128-132).  Step i of n is controlled iff
+    `control_guidance_start <= i / n <= control_guidance_end`; the other steps replay a second graph without the
+    ControlNet, captured only when some step needs it.
     """
 
     def __init__(self, unet, scheduler: LMSDiscreteScheduler, cond_ctxs: Sequence[dict], uncond_ctxs: Sequence[dict],
                  latents: torch.Tensor, weight_function: Union[Callable, Sequence[Callable]],
                  guidance_scale: Union[float, Sequence[float]] = 7.5,
                  extra_input: Optional[torch.Tensor] = None, use_graph: bool = True, timesteps=None,
-                 noise_seed: Union[None, int, Sequence[int]] = None):
+                 noise_seed: Union[None, int, Sequence[int]] = None, controlnet=None,
+                 control_image: Union[None, torch.Tensor, Sequence[torch.Tensor]] = None,
+                 controlnet_conditioning_scale: Union[float, Sequence[float]] = 1.0, guess_mode: bool = False,
+                 control_guidance_start: float = 0.0, control_guidance_end: float = 1.0):
         if not isinstance(scheduler, SIGMA_SCHEDULERS):
             raise TypeError(f"PwWSampler does not support {type(scheduler).__name__}; use one of "
                             + ", ".join(c.__name__ for c in SIGMA_SCHEDULERS))
@@ -200,8 +239,10 @@ class PwWSampler:
                             extra_input.to(self.device, torch.float32, memory_format=torch.contiguous_format))
         self.use_graph = use_graph and latents.is_cuda
         self._graph = None
+        self._plain_graph = None           # the step without the ControlNet, for steps outside its window
         self._kv_graph = None
         self.native_launches_per_step = None
+        self.native_launches_per_step_without_control = None
         self._probed = []
         for i, f in enumerate(self._fns):
             try:
@@ -238,6 +279,63 @@ class PwWSampler:
         self._unet_in = torch.empty((2 * m, channels) + tuple(self.latents.shape[2:]), dtype=self._unet_dtype,
                                     device=dev)
         self._step_no = 0
+        self.controlnet = controlnet
+        self.guess_mode = bool(guess_mode)
+        self._control_active = [False] * len(self.timesteps)
+        if controlnet is None:
+            if control_image is not None:
+                raise ValueError("control_image is given but controlnet is None")
+        else:
+            self._set_up_control(control_image, controlnet_conditioning_scale, control_guidance_start,
+                                 control_guidance_end)
+
+    def _set_up_control(self, control_image, conditioning_scale, start: float, end: float):
+        """Validate the ControlNet arguments; embed the hints, build CONTROL_SCALES and the ControlNet's context."""
+        from .controlnet import ControlNetModel
+        net, unet, m = self.controlnet, self.unet, self.m
+        if not isinstance(net, ControlNetModel):
+            raise TypeError(f"controlnet must be a paint_with_words_sd_b200.controlnet.ControlNetModel, got "
+                            f"{type(net).__name__}")
+        params = inspect.signature(unet.forward).parameters
+        if "down_block_additional_residuals" not in params or "mid_block_additional_residual" not in params:
+            raise TypeError(f"the UNet ({type(unet).__name__}) does not take down_block_additional_residuals / "
+                            "mid_block_additional_residual, so it cannot take a controlnet")
+        ucfg, ccfg = getattr(unet, "config", None), net.config
+        for name in ("block_out_channels", "layers_per_block", "cross_attention_dim"):
+            if getattr(ucfg, name, None) != getattr(ccfg, name):
+                raise ValueError(f"controlnet config {name} = {getattr(ccfg, name)} does not match the UNet's "
+                                 f"{getattr(ucfg, name, None)}")
+        if ccfg.in_channels != 4:
+            raise ValueError(f"controlnet config in_channels = {ccfg.in_channels}: a ControlNet takes the 4 latent "
+                             "channels")
+        if not start <= end:
+            raise ValueError(f"control_guidance_start ({start}) must not exceed control_guidance_end ({end})")
+        if control_image is None:
+            raise ValueError("controlnet needs a control_image (one [1, 3, H, W] tensor per image)")
+        images = _per_image(control_image, m, "control_image", torch.is_tensor)
+        h, w = self.latents.shape[-2:]
+        for i, img in enumerate(images):
+            if tuple(img.shape) != (1, 3, 8 * h, 8 * w):
+                raise ValueError(f"control_image {i} is {tuple(img.shape)}; expected (1, 3, {8 * h}, {8 * w}): 8x the "
+                                 f"latent size {h}x{w}")
+        weights = _per_image(conditioning_scale, m, "controlnet_conditioning_scale",
+                             lambda s: isinstance(s, (int, float)) and not isinstance(s, bool))
+        n = len(self.timesteps)
+        self._control_active = [control_step_active(i, n, start, end) for i in range(n)]
+        dev = self.device
+        with torch.no_grad():
+            emb = net.embed_condition(torch.cat([img.to(dev) for img in images], 0))     # once: step-invariant
+        if not self.guess_mode:
+            emb = torch.cat([emb, emb], 0)                                            # rows i and m + i share image i
+        self._hint = emb.contiguous(memory_format=torch.channels_last) if emb.is_cuda else emb
+        levels = len(net.controlnet_down_blocks) + 1
+        self._ctx["CONTROL_SCALES"] = control_scales(weights, self.guess_mode, levels).to(dev)
+        # the ControlNet's own dict: the plain text context (cond rows only in guess mode), no weight maps, so every
+        # cross-attention call is unbiased; its K/V are staged once like the UNet's
+        text = self._ctx["CONTEXT_TENSOR"]
+        self._control_ctx = {"CONTEXT_TENSOR": text[:m] if self.guess_mode else text,
+                             "CROSS_ATTENTION_WEIGHT_ORIG": 0, "WEIGHT_FUNCTION": _zero_weight_function,
+                             "SIGMA": 0.0, "KV_CACHE": {}}
 
     def step_forms(self) -> List[tuple]:
         """float64 (alpha, a, b, [beta0..beta3], gamma) of every step of this run (`scheduler.step_form`); the run's
@@ -305,7 +403,7 @@ class PwWSampler:
         return ctx
 
     # -- one step, expressed only with device tensors / device scalars --------------------------
-    def _step_body(self):
+    def _step_body(self, control: bool = False):
         m, (h, w) = self.m, self.latents.shape[-2:]
         L = _native.lib()
         stream = torch.cuda.current_stream(self.device).cuda_stream
@@ -316,7 +414,15 @@ class PwWSampler:
                                           None if self.extra_input is None else self.extra_input.data_ptr(),
                                           self._unet_in.data_ptr(), _dtype_code(self._unet_in.dtype), m,
                                           self._unet_in.shape[1], h, w, stream), "pww_sampler_input")
-        eps = self.unet(self._unet_in, self._params[2:3], encoder_hidden_states=self._ctx).sample
+        residuals = {}
+        if control:
+            # the ControlNet sees the 4 latent channels of the UNet input (hook_pww.py:113-119), only the cond rows in
+            # guess mode (the uncond rows' residuals would be discarded)
+            x = self._unet_in[:m, :4] if self.guess_mode else self._unet_in[:, :4]
+            down, mid = self.controlnet(x, self._params[2:3], encoder_hidden_states=self._control_ctx,
+                                        controlnet_cond_embedding=self._hint, return_dict=False)
+            residuals = {"down_block_additional_residuals": down, "mid_block_additional_residual": mid}
+        eps = self.unet(self._unet_in, self._params[2:3], encoder_hidden_states=self._ctx, **residuals).sample
         if tuple(eps.shape) != (2 * m, 4, h, w) or eps.device != self.device:
             raise ValueError(f"the UNet returned {tuple(eps.shape)} on {eps.device}; expected {(2 * m, 4, h, w)}")
         # CFG with the per-image scale, then the step form; eps is read in place through its strides
@@ -354,19 +460,25 @@ class PwWSampler:
             dev[k].copy_(h, non_blocking=True)
             n += h.numel() * h.element_size()
         if "CONTEXT_TENSOR" in pinned and self._ctx.get("KV_CACHE"):
-            # the cached K/V follow the new context: 16 small GEMMs, replayed as one CUDA graph
+            # the cached K/V follow the new context: 16 small GEMMs, replayed as one CUDA graph (the ControlNet's
+            # context is a view of the same tensor, so its cached K/V are refreshed too)
+            ctxs = [self._ctx] + ([self._control_ctx] if self.controlnet is not None else [])
+
+            def refresh():
+                for c in ctxs:
+                    _attention.refresh_kv_cache(c)
             if not self.use_graph:
-                _attention.refresh_kv_cache(self._ctx)
+                refresh()
             else:
                 if self._kv_graph is None:
                     s = torch.cuda.Stream(device=self.device)
                     s.wait_stream(torch.cuda.current_stream(self.device))
                     with torch.cuda.stream(s):
-                        _attention.refresh_kv_cache(self._ctx)
+                        refresh()
                     torch.cuda.current_stream(self.device).wait_stream(s)
                     self._kv_graph = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(self._kv_graph):
-                        _attention.refresh_kv_cache(self._ctx)
+                        refresh()
                 self._kv_graph.replay()
         return n
 
@@ -383,33 +495,40 @@ class PwWSampler:
         i = self._step_no
         step_index = self.scheduler.step_index_of(self.timesteps[i])
         self._set_step_scalars(i, step_index)
+        control = self._control_active[i]
         if not self.use_graph:
-            self._step_body()
-        elif self._graph is None:
-            # warm-up on a side stream (allocator + cuDNN/cuBLAS autotune), then capture
-            self._capture()
-            self._graph.replay()
+            self._step_body(control)
         else:
-            self._graph.replay()
+            # the step with the ControlNet (or the only step, without one) is `_graph`; a ControlNet's steps outside its
+            # window replay `_plain_graph`.  Each is captured at its first step: warm-up on a side stream (allocator +
+            # cuDNN/cuBLAS autotune), then capture
+            g = self._graph if control or self.controlnet is None else self._plain_graph
+            if g is None:
+                g = self._capture(control)
+            g.replay()
         self._step_no += 1
 
-    def _capture(self):
+    def _capture(self, control: bool = False) -> "torch.cuda.CUDAGraph":
         snap = (self.latents.clone(), self._derivs.clone())
         s = torch.cuda.Stream(device=self.device)
         s.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(s):
             for _ in range(2):
-                self._step_body()
+                self._step_body(control)
         torch.cuda.current_stream(self.device).wait_stream(s)
         self.latents.copy_(snap[0]); self._derivs.copy_(snap[1])
         g = torch.cuda.CUDAGraph()
         from . import _native
         before = _native.launch_count
         with torch.cuda.graph(g):
-            self._step_body()
-        self.native_launches_per_step = _native.launch_count - before
+            self._step_body(control)
+        launches = _native.launch_count - before
         self.latents.copy_(snap[0]); self._derivs.copy_(snap[1])
-        self._graph = g
+        if control or self.controlnet is None:
+            self._graph, self.native_launches_per_step = g, launches
+        else:
+            self._plain_graph, self.native_launches_per_step_without_control = g, launches
+        return g
 
     def run(self, num_steps: Optional[int] = None) -> torch.Tensor:
         n = len(self.timesteps) - self._step_no if num_steps is None else num_steps
@@ -440,13 +559,23 @@ def paint_with_words(
     return_latents: bool = False,
     max_prompt_chunks: int = 1,
     torch_dtype: Optional[torch.dtype] = None,
+    controlnet=None,
+    control_image: Optional[Image.Image] = None,
+    controlnet_conditioning_scale: float = 1.0,
+    guess_mode: bool = False,
+    control_guidance_start: float = 0.0,
+    control_guidance_end: float = 1.0,
 ):
     """paint_with_words.py:391-510.  Returns one PIL.Image (or the final latents with return_latents).
     `max_prompt_chunks` (1 .. 3): a prompt longer than 75 tokens fills up to that many 77-token CLIP chunks instead of
     being truncated (conditioning.chunk_prompt); 1 is the reference's behaviour.
     `torch_dtype` is passed to `pww_load_tools` when this call loads the models (torch.bfloat16 for a bf16 UNet); with
-    `preloaded_utils` the UNet's own dtype decides."""
+    `preloaded_utils` the UNet's own dtype decides.
+    ControlNet (the reference's PwW + ControlNet extension): `controlnet` from `pww_load_controlnet`, `control_image`
+    a PIL image of the colour map's size (scribble, edges, pose, ...) that fixes the layout while the colour map says
+    which words go where; `controlnet_conditioning_scale`, `guess_mode` and the guidance window as in `PwWSampler`."""
     width, height = color_map_image.size
+    control = _control_arguments(controlnet, control_image, (width, height), "color_map_image")
     vae, unet, text_encoder, tokenizer, scheduler = (
         pww_load_tools(device, scheduler_type, local_model_path=local_model_path, hf_model_path=hf_model_path,
                        model_token=model_token, torch_dtype=torch_dtype)
@@ -471,16 +600,34 @@ def paint_with_words(
         latents = scheduler.add_noise(init_latents, noise, timesteps[:1])
 
     sampler = PwWSampler(unet, scheduler, [cond], [uncond], latents, weight_function, guidance_scale,
-                         timesteps=timesteps, noise_seed=seed)
+                         timesteps=timesteps, noise_seed=seed,
+                         **control, controlnet_conditioning_scale=controlnet_conditioning_scale,
+                         guess_mode=guess_mode, control_guidance_start=control_guidance_start,
+                         control_guidance_end=control_guidance_end)
     latents = sampler.run()
     if return_latents:
         return latents
     return _pil_from_latents(vae, latents)[0]
 
 
+def _control_arguments(controlnet, control_image, size: Tuple[int, int], size_of: str) -> dict:
+    """PwWSampler's controlnet / control_image from the public arguments; the hint image must be `size` (W, H)."""
+    if controlnet is None:
+        if control_image is not None:
+            raise ValueError("control_image is given but controlnet is None")
+        return {}
+    if not isinstance(control_image, Image.Image):
+        raise ValueError(f"controlnet needs a control_image (a PIL image of the {size_of} size {size}), got "
+                         f"{type(control_image).__name__}")
+    if control_image.size != tuple(size):
+        raise ValueError(f"control_image is {control_image.size}; it must have the {size_of} size {tuple(size)}")
+    return {"controlnet": controlnet, "control_image": control_image_tensor(control_image)}
+
+
 # the per-image keyword arguments of paint_with_words that paint_with_words_batch takes per entry
 BATCH_SETTING_KEYS = ("color_context", "color_map_image", "input_prompt", "unconditional_input_prompt", "seed",
-                      "weight_function", "guidance_scale", "max_prompt_chunks")
+                      "weight_function", "guidance_scale", "max_prompt_chunks", "control_image",
+                      "controlnet_conditioning_scale")
 
 
 def _batch_settings(settings) -> List[dict]:
@@ -527,12 +674,18 @@ def paint_with_words_batch(
     max_batch_size: int = 8,
     return_latents: bool = False,
     torch_dtype: Optional[torch.dtype] = None,
+    controlnet=None,
+    guess_mode: bool = False,
+    control_guidance_start: float = 0.0,
+    control_guidance_end: float = 1.0,
 ):
     """Many images, each with its own settings, in as few samplers as possible.  `settings[i]` is a dict of the
     per-image keyword arguments of `paint_with_words` (BATCH_SETTING_KEYS: color_context, color_map_image, input_prompt,
-    unconditional_input_prompt, seed, weight_function, guidance_scale, max_prompt_chunks); missing keys take
-    paint_with_words's defaults.  Returns a list of PIL images (or [1,4,h,w] latents) in input order; image i equals
-    `paint_with_words(**settings[i])` up to fp16 noise.
+    unconditional_input_prompt, seed, weight_function, guidance_scale, max_prompt_chunks, control_image,
+    controlnet_conditioning_scale); missing keys take paint_with_words's defaults.  Returns a list of PIL images (or
+    [1,4,h,w] latents) in input order; image i equals `paint_with_words(**settings[i])` up to fp16 noise.
+    With `controlnet` (one for the batch, with `guess_mode` and the guidance window) every entry needs a
+    `control_image` of its colour map's size; its `controlnet_conditioning_scale` is its own.
 
     Entries of the same latent size and text length run in one `PwWSampler` of at most `max_batch_size` images (a
     2 * max_batch_size UNet batch with CFG), whatever their weight functions and guidance scales.  The default of 8 gave
@@ -542,6 +695,11 @@ def paint_with_words_batch(
     entries = _batch_settings(settings)
     if max_batch_size < 1:
         raise ValueError("max_batch_size must be >= 1")
+    for i, e in enumerate(entries):
+        try:
+            _control_arguments(controlnet, e["control_image"], e["color_map_image"].size, "color_map_image")
+        except ValueError as err:
+            raise ValueError(f"settings[{i}]: {err}") from err
     vae, unet, text_encoder, tokenizer, scheduler = (
         pww_load_tools(device, scheduler_type, local_model_path=local_model_path, hf_model_path=hf_model_path,
                        model_token=model_token, torch_dtype=torch_dtype)
@@ -560,10 +718,17 @@ def paint_with_words_batch(
         keys.append(None if solo else (height // 8, width // 8, int(cond["CONTEXT_TENSOR"].shape[1])))
     results: List[Optional[torch.Tensor]] = [None] * len(entries)
     for idx in batch_groups(keys, max_batch_size):
+        control = {}
+        if controlnet is not None:
+            control = dict(controlnet=controlnet,
+                           control_image=[control_image_tensor(entries[i]["control_image"]) for i in idx],
+                           controlnet_conditioning_scale=[entries[i]["controlnet_conditioning_scale"] for i in idx],
+                           guess_mode=guess_mode, control_guidance_start=control_guidance_start,
+                           control_guidance_end=control_guidance_end)
         sampler = PwWSampler(unet, scheduler, [encoded[i][0] for i in idx], [encoded[i][1] for i in idx],
                              torch.cat([encoded[i][2] for i in idx], 0),
                              [entries[i]["weight_function"] for i in idx], [entries[i]["guidance_scale"] for i in idx],
-                             timesteps=scheduler.timesteps, noise_seed=[entries[i]["seed"] for i in idx])
+                             timesteps=scheduler.timesteps, noise_seed=[entries[i]["seed"] for i in idx], **control)
         latents = sampler.run()
         for j, i in enumerate(idx):
             results[i] = latents[j:j + 1].clone()
@@ -623,14 +788,23 @@ def paint_with_words_inpaint(
     return_latents: bool = False,
     max_prompt_chunks: int = 1,
     torch_dtype: Optional[torch.dtype] = None,
+    controlnet=None,
+    control_image: Optional[Image.Image] = None,
+    controlnet_conditioning_scale: float = 1.0,
+    guess_mode: bool = False,
+    control_guidance_start: float = 0.0,
+    control_guidance_end: float = 1.0,
 ):
     """paint_with_words_inpaint.py:137-270: 9-channel UNet input cat[latents, mask, masked-image latents].
-    `max_prompt_chunks` and `torch_dtype` as in `paint_with_words`."""
+    `max_prompt_chunks`, `torch_dtype` and the ControlNet arguments as in `paint_with_words`; the colour map is resized
+    to the init image, so `control_image` has the init image's size.  The ControlNet sees the 4 latent channels of
+    the UNet input (hook_pww.py:113-119)."""
+    width, height = init_image.size
+    control = _control_arguments(controlnet, control_image, (width, height), "init_image (and resized color_map_image)")
     vae, unet, text_encoder, tokenizer, scheduler = (
         pww_load_tools(device, scheduler_type, local_model_path=local_model_path, hf_model_path=hf_model_path,
                        model_token=model_token, torch_dtype=torch_dtype)
         if preloaded_utils is None else preloaded_utils)
-    width, height = init_image.size
     color_map_image = color_map_image.resize((width, height), Image.NEAREST)
     mask_image = mask_image.resize((width, height), Image.NEAREST)
     _, _, cond, uncond = _encode_text_color_inputs(
@@ -661,7 +835,9 @@ def paint_with_words_inpaint(
             f"num_channels_masked_image: {masked_image_latents.shape[1]} = {total}.")
     sampler = PwWSampler(unet, scheduler, [cond], [uncond], latents, weight_function, guidance_scale,
                          extra_input=torch.cat([mask, masked_image_latents], 1).float(), timesteps=timesteps,
-                         noise_seed=seed)
+                         noise_seed=seed, **control, controlnet_conditioning_scale=controlnet_conditioning_scale,
+                         guess_mode=guess_mode, control_guidance_start=control_guidance_start,
+                         control_guidance_end=control_guidance_end)
     latents = sampler.run()
     if return_latents:
         return latents
@@ -684,9 +860,11 @@ class PaintWithWord_StableDiffusionPipeline:
     it always uses its own LMS scheduler (paint_with_words.py:534-539) and has no regional blur (:574)."""
 
     def __init__(self, vae, text_encoder, tokenizer, unet, scheduler=None, safety_checker=None, feature_extractor=None,
-                 requires_safety_checker: bool = False):
+                 requires_safety_checker: bool = False, controlnet=None):
+        """`controlnet`: a `ControlNetModel` (`pww_load_controlnet`) every call that passes a `control_image` uses."""
         self.vae, self.text_encoder, self.tokenizer, self.unet = vae, text_encoder, tokenizer, unet
         self.safety_checker, self.feature_extractor = safety_checker, feature_extractor
+        self.controlnet = controlnet
         self.scheduler = LMSDiscreteScheduler(beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear",
                                               num_train_timesteps=1000)
         self.plugin_cross_attention()
@@ -696,7 +874,8 @@ class PaintWithWord_StableDiffusionPipeline:
         """`torch_dtype` as in `pww_load_tools` (torch.bfloat16 for a bf16 UNet)."""
         vae, unet, text_encoder, tokenizer, scheduler = pww_load_tools(device, local_model_path=save_dir,
                                                                        torch_dtype=torch_dtype)
-        return cls(vae=vae, text_encoder=text_encoder, tokenizer=tokenizer, unet=unet, scheduler=scheduler)
+        return cls(vae=vae, text_encoder=text_encoder, tokenizer=tokenizer, unet=unet, scheduler=scheduler,
+                   controlnet=kwargs.get("controlnet"))
 
     def plugin_cross_attention(self):
         """paint_with_words.py:556-559."""
@@ -734,12 +913,22 @@ class PaintWithWord_StableDiffusionPipeline:
                  height=None, width=None, num_inference_steps: int = 30, guidance_scale: float = 7.5, negative_prompt="",
                  num_images_per_prompt: int = 1, eta: float = 0.5, seed: int = 0, generator=None, image=None, latents=None,
                  output_type: str = "pil", return_dict: bool = True, callback=None, callback_steps: int = 1,
-                 max_prompt_chunks: int = 1):
+                 max_prompt_chunks: int = 1, control_image=None, controlnet_conditioning_scale: float = 1.0,
+                 guess_mode: bool = False, control_guidance_start: float = 0.0, control_guidance_end: float = 1.0):
         extra = {} if image is None else {"init_image": image, "strength": eta}
         extra["max_prompt_chunks"] = max_prompt_chunks
+        extra.update(self._control(control_image, controlnet_conditioning_scale, guess_mode, control_guidance_start,
+                                   control_guidance_end))
         return self._run(paint_with_words, prompt, color_map_image, dict(color_context), weight_function,
                          num_inference_steps, guidance_scale, negative_prompt, seed, output_type, return_dict, callback,
                          callback_steps, **extra)
+
+    def _control(self, control_image, scale, guess_mode, start, end) -> dict:
+        """The ControlNet keyword arguments of a call: none when it passes no control_image."""
+        if control_image is None:
+            return {}
+        return dict(controlnet=self.controlnet, control_image=control_image, controlnet_conditioning_scale=scale,
+                    guess_mode=guess_mode, control_guidance_start=start, control_guidance_end=end)
 
 
 class PaintWithWord_StableDiffusionInpaintPipeline(PaintWithWord_StableDiffusionPipeline):
@@ -750,7 +939,8 @@ class PaintWithWord_StableDiffusionInpaintPipeline(PaintWithWord_StableDiffusion
         """`torch_dtype` as in `pww_load_tools` (torch.bfloat16 for a bf16 UNet)."""
         vae, unet, text_encoder, tokenizer, scheduler = pww_load_tools(device, local_model_path=save_dir,
                                                                        torch_dtype=torch_dtype)
-        return cls(vae=vae, text_encoder=text_encoder, tokenizer=tokenizer, unet=unet, scheduler=scheduler)
+        return cls(vae=vae, text_encoder=text_encoder, tokenizer=tokenizer, unet=unet, scheduler=scheduler,
+                   controlnet=kwargs.get("controlnet"))
 
     @torch.no_grad()
     def __call__(self, prompt, image=None, mask_image=None, color_map_image=None, color_context={},
@@ -758,8 +948,11 @@ class PaintWithWord_StableDiffusionInpaintPipeline(PaintWithWord_StableDiffusion
                  num_inference_steps: int = 30, guidance_scale: float = 7.5, negative_prompt="",
                  num_images_per_prompt: int = 1, eta: float = 1.0, seed: int = 0, generator=None, latents=None,
                  output_type: str = "pil", return_dict: bool = True, callback=None, callback_steps: int = 1,
-                 max_prompt_chunks: int = 1):
+                 max_prompt_chunks: int = 1, control_image=None, controlnet_conditioning_scale: float = 1.0,
+                 guess_mode: bool = False, control_guidance_start: float = 0.0, control_guidance_end: float = 1.0):
         return self._run(paint_with_words_inpaint, prompt, color_map_image, dict(color_context), weight_function,
                          num_inference_steps, guidance_scale, negative_prompt, seed, output_type, return_dict, callback,
                          callback_steps, mask_image=mask_image, init_image=image, strength=eta,
-                         max_prompt_chunks=max_prompt_chunks)
+                         max_prompt_chunks=max_prompt_chunks,
+                         **self._control(control_image, controlnet_conditioning_scale, guess_mode,
+                                         control_guidance_start, control_guidance_end))

@@ -337,7 +337,15 @@ class UNet2DConditionModel(nn.Module):
         self.conv_norm_out = nn.GroupNorm(g, ch[0], eps=1e-5)
         self.conv_out = nn.Conv2d(ch[0], cfg.out_channels, 3, padding=1)
 
-    def forward(self, sample, timestep, encoder_hidden_states=None):
+    def forward(self, sample, timestep, encoder_hidden_states=None, down_block_additional_residuals=None,
+                mid_block_additional_residual=None):
+        """`down_block_additional_residuals` (one per skip) and `mid_block_additional_residual` are a ControlNet's
+        outputs, as in diffusers: residual k is added to skip k before the decoder concatenates it, the mid residual to
+        the mid-block output.  Residuals of fewer images than the batch go into its first images (guess mode: the cond
+        half).  A context dict may carry "CONTROL_SCALES", an fp32 [len(skips) + 1, rows] device tensor: residual k of
+        image b is multiplied by CONTROL_SCALES[k, b] first (absent: 1, diffusers' plain add)."""
+        if (down_block_additional_residuals is None) != (mid_block_additional_residual is None):
+            raise ValueError("down_block_additional_residuals and mid_block_additional_residual go together")
         if not torch.is_tensor(timestep):
             timestep = torch.tensor([timestep], dtype=torch.float32, device=sample.device)
         elif timestep.dim() == 0:
@@ -357,6 +365,15 @@ class UNet2DConditionModel(nn.Module):
             x, outs = blk(x, temb, encoder_hidden_states)
             skips.extend(outs)
         x = self.mid_block(x, temb, encoder_hidden_states)
+        if mid_block_additional_residual is not None:
+            residuals = list(down_block_additional_residuals) + [mid_block_additional_residual]
+            if len(residuals) != len(skips) + 1:
+                raise ValueError(f"{len(residuals) - 1} down-block residuals for {len(skips)} skips")
+            scales = encoder_hidden_states.get("CONTROL_SCALES") if isinstance(encoder_hidden_states, dict) else None
+            if fast:
+                fused_ops.control_inject(skips + [x], residuals, scales)   # one launch, in place
+            else:
+                *skips, x = add_control_residuals(skips + [x], residuals, scales)
         for blk in self.up_blocks:
             x = blk(x, skips, temb, encoder_hidden_states)
         if fast:
@@ -364,6 +381,21 @@ class UNet2DConditionModel(nn.Module):
         else:
             x = self.conv_out(F.silu(self.conv_norm_out(x)))
         return _Sample(x)
+
+
+def add_control_residuals(targets: Sequence[torch.Tensor], residuals: Sequence[torch.Tensor],
+                          scales: Optional[torch.Tensor] = None) -> List[torch.Tensor]:
+    """The torch statement of `pww_control_inject`: target_k[:rows] + (residual_k * scales[k]) with the product
+    rounded to the target's type (rows = residual_k.shape[0]; scales an fp32 [n, rows] tensor or None for 1)."""
+    out = []
+    for k, (d, r) in enumerate(zip(targets, residuals)):
+        rows = r.shape[0]
+        if tuple(r.shape[1:]) != tuple(d.shape[1:]) or rows > d.shape[0]:
+            raise ValueError(f"residual {k} {tuple(r.shape)} does not match its target {tuple(d.shape)}")
+        p = r if scales is None else r * scales[k].to(r.device).view(rows, 1, 1, 1)
+        p = p.to(d.dtype)
+        out.append(d + p if rows == d.shape[0] else torch.cat([d[:rows] + p, d[rows:]], 0))
+    return out
 
 
 def _resnets(unet: nn.Module):

@@ -179,6 +179,16 @@ def control_image_tensor(image: Image.Image) -> torch.Tensor:
     return torch.from_numpy(arr.transpose(2, 0, 1).copy())[None]
 
 
+# Columns of a step row.  PwWSampler tabulates one row per step at set-up (`_rows`) and a step copies its row into
+# `_params` (one D2D copy), so a captured graph reads new values through the same device pointers:
+_SIGMA = 0    # sigma
+_SCALE = 1    # 1/sqrt(sigma^2 + 1): pww_sampler_input's `scale`
+_T = 2        # the timestep: the UNet's and the ControlNet's `timestep`
+_BETA = 3     # beta0..beta3: pww_sampler_update's `beta`
+_G = 7        # G_0(sigma) .. G_{m-1}(sigma), then m zeros for the uncond images: the attention's G_SIGMA
+# after them, at _G + 2m, scheduler.FORM_COLUMNS (alpha, a, b, gamma, slot, row): pww_sampler_update's `form`
+
+
 class PwWSampler:
     """Denoising loop for a group of images on ONE GPU (paint_with_words.py:471-506 semantics per image).
 
@@ -238,11 +248,8 @@ class PwWSampler:
         self.extra_input = (None if extra_input is None else     # inpaint: [m,5,h,w] (mask + masked-image latents)
                             extra_input.to(self.device, torch.float32, memory_format=torch.contiguous_format))
         self.use_graph = use_graph and latents.is_cuda
-        self._graph = None
-        self._plain_graph = None           # the step without the ControlNet, for steps outside its window
+        self._graphs = {}                  # "the step runs the ControlNet" -> (captured step, its native launches)
         self._kv_graph = None
-        self.native_launches_per_step = None
-        self.native_launches_per_step_without_control = None
         self._probed = []
         for i, f in enumerate(self._fns):
             try:
@@ -251,23 +258,17 @@ class PwWSampler:
                 if callable(weight_function):
                     raise
                 raise UnsupportedWeightFunction(f"weight_function of image {i}: {e}") from e
-        up = next(iter(unet.parameters()), None)
-        self._unet_dtype = up.dtype if up is not None else torch.float32
         self._ctx = self._merge_contexts(cond_ctxs, uncond_ctxs)
         dev = self.device
-        # Per-step scalars are tabulated once on the host and uploaded; a step copies its row into `_params` (one D2D
-        # copy), so a captured graph sees new values and the host never feeds the stream mid-loop.  A row is
-        #   [sigma, 1/sqrt(sigma^2+1), t, beta0..beta3, G_0(sigma) .. G_{m-1}(sigma), 0 x m, alpha, a, b, gamma, slot, row]
-        # (`_table` is its first 7 + m columns; FORM_COLUMNS names the last six).  G_SIGMA holds one value per image of
-        # the UNet batch: the m zeros leave the uncond images unbiased.
+        # the step rows (column layout above); `_table` is the columns up to the images' G, without the uncond zeros
         m = self.m
-        table = self._build_step_table()
         self._hist_len = history_length(scheduler)
-        self._rows = torch.cat([table, torch.zeros(table.shape[0], m), self._build_form_table()], 1).to(dev)
-        self._table = self._rows[:, :7 + m]
+        self._form = _G + 2 * m                # the step form's first column
+        self._rows = self._build_rows().to(dev)
+        self._table = self._rows[:, :_G + m]
         self._params = torch.zeros(self._rows.shape[1], dtype=torch.float32, device=dev)
         self._derivs = torch.zeros((self._hist_len,) + tuple(self.latents.shape), dtype=torch.float32, device=dev)
-        self._ctx["G_SIGMA"] = self._params[7:7 + 2 * m]
+        self._ctx["G_SIGMA"] = self._params[_G:self._form]
         self._gscale = torch.tensor(scales, dtype=torch.float32, device=dev).view(m, 1, 1, 1)
         self._noise = None
         if isinstance(scheduler, EulerAncestralDiscreteScheduler):
@@ -276,7 +277,7 @@ class PwWSampler:
             seeds = _per_image(noise_seed, m, "noise_seed", lambda v: isinstance(v, (int, np.integer)))
             self._noise = ancestral_noise(seeds, tuple(self.latents.shape[1:]), len(self.timesteps)).to(dev)
         channels = 4 + (0 if self.extra_input is None else int(self.extra_input.shape[1]))
-        self._unet_in = torch.empty((2 * m, channels) + tuple(self.latents.shape[2:]), dtype=self._unet_dtype,
+        self._unet_in = torch.empty((2 * m, channels) + tuple(self.latents.shape[2:]), dtype=_module_dtype(unet),
                                     device=dev)
         self._step_no = 0
         self.controlnet = controlnet
@@ -343,20 +344,18 @@ class PwWSampler:
         sch = self.scheduler
         return [step_form(sch, sch.step_index_of(t), first=(i == 0)) for i, t in enumerate(self.timesteps)]
 
-    def _build_step_table(self) -> torch.Tensor:
-        sch = self.scheduler
+    def _build_rows(self) -> torch.Tensor:
+        """[steps, _G + 2m + 6] fp32: every step's row.  The step form ends with the history slot this step writes and
+        the noise row it reads."""
+        sch, zeros = self.scheduler, [0.0] * self.m
         rows = []
-        for t, (_, _, _, beta, _) in zip(self.timesteps, self.step_forms()):
+        for i, (t, (alpha, a, b, beta, gamma)) in enumerate(zip(self.timesteps, self.step_forms())):
             si = sch.step_index_of(t)
             sigma = float(sch.sigmas[si])
             gs = [g_of_sigma(f, pr, sch.sigmas[si]) for f, pr in zip(self._fns, self._probed)]
-            rows.append([sigma, 1.0 / math.sqrt(sigma * sigma + 1.0), float(t), *beta, *gs])
+            rows.append([sigma, 1.0 / math.sqrt(sigma * sigma + 1.0), float(t), *beta, *gs, *zeros,
+                         alpha, a, b, gamma, float(i % self._hist_len), float(i)])
         return torch.tensor(rows, dtype=torch.float32)
-
-    def _build_form_table(self) -> torch.Tensor:
-        """[steps, 6] = FORM_COLUMNS: alpha, a, b, gamma, the history slot this step writes, the noise row it reads."""
-        return torch.tensor([[alpha, a, b, gamma, float(i % self._hist_len), float(i)]
-                             for i, (alpha, a, b, _, gamma) in enumerate(self.step_forms())], dtype=torch.float32)
 
     def _merge_contexts(self, conds, unconds) -> dict:
         """Batch the per-image dicts: CONTEXT_TENSOR -> [2m,T,Dc]; weight maps -> [m,N,T] stacks;
@@ -396,7 +395,6 @@ class PwWSampler:
         ctx["KV_CACHE"] = {}       # to_k/to_v of the text context are step-invariant: computed at the first step
         # scratch of the attention launches, owned by this sampler: its captured graphs never see a buffer that another
         # sampler or a later, larger call replaced
-        from . import _native
         ctx["PWW_SCRATCH"] = (torch.zeros(max(64, 2 * m), dtype=torch.float32, device=self.device),
                               torch.zeros(_native.lib().pww_xattn_fused_workspace_bytes(), dtype=torch.uint8,
                                           device=self.device))
@@ -407,31 +405,31 @@ class PwWSampler:
         m, (h, w) = self.m, self.latents.shape[-2:]
         L = _native.lib()
         stream = torch.cuda.current_stream(self.device).cuda_stream
-        f32 = self._params.element_size()
+        p = self._params
         # the UNet input in the UNet's own dtype (the reference runs under autocast): [2m, C, h, w], rows i and m + i
         # both fp16(latents_i / sqrt(sigma^2 + 1)) [+ the inpaint channels]
-        _native.check(L.pww_sampler_input(self.latents.data_ptr(), self._params.data_ptr() + f32,
+        _native.check(L.pww_sampler_input(self.latents.data_ptr(), p[_SCALE:].data_ptr(),
                                           None if self.extra_input is None else self.extra_input.data_ptr(),
                                           self._unet_in.data_ptr(), _dtype_code(self._unet_in.dtype), m,
                                           self._unet_in.shape[1], h, w, stream), "pww_sampler_input")
+        t = p[_T:_T + 1]
         residuals = {}
         if control:
             # the ControlNet sees the 4 latent channels of the UNet input (hook_pww.py:113-119), only the cond rows in
             # guess mode (the uncond rows' residuals would be discarded)
             x = self._unet_in[:m, :4] if self.guess_mode else self._unet_in[:, :4]
-            down, mid = self.controlnet(x, self._params[2:3], encoder_hidden_states=self._control_ctx,
+            down, mid = self.controlnet(x, t, encoder_hidden_states=self._control_ctx,
                                         controlnet_cond_embedding=self._hint, return_dict=False)
             residuals = {"down_block_additional_residuals": down, "mid_block_additional_residual": mid}
-        eps = self.unet(self._unet_in, self._params[2:3], encoder_hidden_states=self._ctx, **residuals).sample
+        eps = self.unet(self._unet_in, t, encoder_hidden_states=self._ctx, **residuals).sample
         if tuple(eps.shape) != (2 * m, 4, h, w) or eps.device != self.device:
             raise ValueError(f"the UNet returned {tuple(eps.shape)} on {eps.device}; expected {(2 * m, 4, h, w)}")
         # CFG with the per-image scale, then the step form; eps is read in place through its strides
-        form = self._params.data_ptr() + (7 + 2 * m) * f32
         _native.check(L.pww_sampler_update(eps.data_ptr(), _dtype_code(eps.dtype), *eps.stride(),
                                            self.latents.data_ptr(), self._derivs.data_ptr(), self._hist_len,
                                            None if self._noise is None else self._noise.data_ptr(),
-                                           self._gscale.data_ptr(), self._params.data_ptr() + 3 * f32, form, m, h, w,
-                                           stream), "pww_sampler_update")
+                                           self._gscale.data_ptr(), p[_BETA:].data_ptr(), p[self._form:].data_ptr(),
+                                           m, h, w, stream), "pww_sampler_update")
         _native.launch_count += 2
 
     def _set_step_scalars(self, i: int, step_index: int):
@@ -471,14 +469,7 @@ class PwWSampler:
                 refresh()
             else:
                 if self._kv_graph is None:
-                    s = torch.cuda.Stream(device=self.device)
-                    s.wait_stream(torch.cuda.current_stream(self.device))
-                    with torch.cuda.stream(s):
-                        refresh()
-                    torch.cuda.current_stream(self.device).wait_stream(s)
-                    self._kv_graph = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(self._kv_graph):
-                        refresh()
+                    self._kv_graph, _ = self._capture(refresh, warmup=1)
                 self._kv_graph.replay()
         return n
 
@@ -499,36 +490,39 @@ class PwWSampler:
         if not self.use_graph:
             self._step_body(control)
         else:
-            # the step with the ControlNet (or the only step, without one) is `_graph`; a ControlNet's steps outside its
-            # window replay `_plain_graph`.  Each is captured at its first step: warm-up on a side stream (allocator +
-            # cuDNN/cuBLAS autotune), then capture
-            g = self._graph if control or self.controlnet is None else self._plain_graph
-            if g is None:
-                g = self._capture(control)
-            g.replay()
+            # one graph for the steps with the ControlNet and one for those without, each captured at the first step
+            # that needs it; its two warm-up steps are undone, so the replay below is this step
+            if control not in self._graphs:
+                snap = (self.latents.clone(), self._derivs.clone())
+                self._graphs[control] = self._capture(lambda: self._step_body(control), warmup=2)
+                self.latents.copy_(snap[0]); self._derivs.copy_(snap[1])
+            self._graphs[control][0].replay()
         self._step_no += 1
 
-    def _capture(self, control: bool = False) -> "torch.cuda.CUDAGraph":
-        snap = (self.latents.clone(), self._derivs.clone())
+    def _capture(self, fn: Callable[[], None], warmup: int) -> Tuple["torch.cuda.CUDAGraph", int]:
+        """`fn` captured in a CUDA graph after `warmup` eager runs on a side stream (allocator, cuDNN / cuBLAS
+        autotuning); returns the graph and the native launches it holds."""
         s = torch.cuda.Stream(device=self.device)
         s.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(s):
-            for _ in range(2):
-                self._step_body(control)
+            for _ in range(warmup):
+                fn()
         torch.cuda.current_stream(self.device).wait_stream(s)
-        self.latents.copy_(snap[0]); self._derivs.copy_(snap[1])
         g = torch.cuda.CUDAGraph()
-        from . import _native
         before = _native.launch_count
         with torch.cuda.graph(g):
-            self._step_body(control)
-        launches = _native.launch_count - before
-        self.latents.copy_(snap[0]); self._derivs.copy_(snap[1])
-        if control or self.controlnet is None:
-            self._graph, self.native_launches_per_step = g, launches
-        else:
-            self._plain_graph, self.native_launches_per_step_without_control = g, launches
-        return g
+            fn()
+        return g, _native.launch_count - before
+
+    @property
+    def native_launches_per_step(self) -> Optional[int]:
+        """Native launches of the captured step (the step with the ControlNet, if there is one); None until captured."""
+        return self._graphs.get(self.controlnet is not None, (None, None))[1]
+
+    @property
+    def native_launches_per_step_without_control(self) -> Optional[int]:
+        """Native launches of a ControlNet's captured step outside its window; None until captured or without one."""
+        return self._graphs.get(False, (None, None))[1] if self.controlnet is not None else None
 
     def run(self, num_steps: Optional[int] = None) -> torch.Tensor:
         n = len(self.timesteps) - self._step_no if num_steps is None else num_steps
@@ -574,44 +568,71 @@ def paint_with_words(
     ControlNet (the reference's PwW + ControlNet extension): `controlnet` from `pww_load_controlnet`, `control_image`
     a PIL image of the colour map's size (scribble, edges, pose, ...) that fixes the layout while the colour map says
     which words go where; `controlnet_conditioning_scale`, `guess_mode` and the guidance window as in `PwWSampler`."""
+    control = _control_arguments(controlnet, control_image, color_map_image.size, "color_map_image",
+                                 controlnet_conditioning_scale, guess_mode, control_guidance_start,
+                                 control_guidance_end)
+    tools = _tools(preloaded_utils, device, scheduler_type, local_model_path, hf_model_path, model_token, torch_dtype)
+    vae, unet, text_encoder, tokenizer, scheduler = tools
+    scheduler.set_timesteps(num_inference_steps)
+    if init_image is None:
+        cond, uncond, latents = _txt2img_inputs(tools, device, color_map_image, color_context, input_prompt,
+                                                unconditional_input_prompt, seed, max_prompt_chunks)
+        timesteps = scheduler.timesteps
+    else:
+        _, _, cond, uncond = _encode_text_color_inputs(
+            text_encoder, tokenizer, device, color_map_image, color_context, input_prompt, unconditional_input_prompt,
+            max_prompt_chunks=max_prompt_chunks)
+        # the reference draws img2img's noise from the global RNG as it stands: unseeded here
+        latents, timesteps = _img2img_latents(vae, scheduler, init_image, num_inference_steps, strength, device)
+    sampler = PwWSampler(unet, scheduler, [cond], [uncond], latents, weight_function, guidance_scale,
+                         timesteps=timesteps, noise_seed=seed, **control)
+    return _result(vae, sampler.run(), return_latents)
+
+
+def _tools(preloaded_utils, device, scheduler_type, local_model_path, hf_model_path, model_token, torch_dtype):
+    """The caller's (vae, unet, text_encoder, tokenizer, scheduler), or `pww_load_tools`'s when it passes none."""
+    if preloaded_utils is not None:
+        return preloaded_utils
+    return pww_load_tools(device, scheduler_type, local_model_path=local_model_path, hf_model_path=hf_model_path,
+                          model_token=model_token, torch_dtype=torch_dtype)
+
+
+def _txt2img_inputs(tools, device, color_map_image, color_context, input_prompt, unconditional_input_prompt, seed,
+                    max_prompt_chunks) -> Tuple[dict, dict, torch.Tensor]:
+    """One txt2img image's (cond, uncond, latents): its text and colour contexts, and its seeded initial noise scaled
+    by the scheduler's initial sigma (so `scheduler.set_timesteps` comes first)."""
+    _, unet, text_encoder, tokenizer, scheduler = tools
     width, height = color_map_image.size
-    control = _control_arguments(controlnet, control_image, (width, height), "color_map_image")
-    vae, unet, text_encoder, tokenizer, scheduler = (
-        pww_load_tools(device, scheduler_type, local_model_path=local_model_path, hf_model_path=hf_model_path,
-                       model_token=model_token, torch_dtype=torch_dtype)
-        if preloaded_utils is None else preloaded_utils)
     extra_seeds, seperated_word_contexts, cond, uncond = _encode_text_color_inputs(
         text_encoder, tokenizer, device, color_map_image, color_context, input_prompt, unconditional_input_prompt,
         max_prompt_chunks=max_prompt_chunks)
-
-    scheduler.set_timesteps(num_inference_steps)
-    timesteps = scheduler.timesteps
-    if init_image is None:
-        latents = initial_latents((1, unet.in_channels, height // 8, width // 8), seed, extra_seeds,
-                                  seperated_word_contexts).to(device)
-        latents = latents * scheduler.init_noise_sigma
-    else:
-        init_timestep = min(int(num_inference_steps * strength), num_inference_steps)
-        t_start = max(num_inference_steps - init_timestep, 0)
-        timesteps = scheduler.timesteps[t_start:]
-        image = preprocess(init_image).to(device=device)
-        init_latents = 0.18215 * vae.encode(image.to(_module_dtype(vae, image.dtype))).latent_dist.sample().float()
-        noise = torch.randn(init_latents.shape).to(device)
-        latents = scheduler.add_noise(init_latents, noise, timesteps[:1])
-
-    sampler = PwWSampler(unet, scheduler, [cond], [uncond], latents, weight_function, guidance_scale,
-                         timesteps=timesteps, noise_seed=seed,
-                         **control, controlnet_conditioning_scale=controlnet_conditioning_scale,
-                         guess_mode=guess_mode, control_guidance_start=control_guidance_start,
-                         control_guidance_end=control_guidance_end)
-    latents = sampler.run()
-    if return_latents:
-        return latents
-    return _pil_from_latents(vae, latents)[0]
+    latents = initial_latents((1, unet.in_channels, height // 8, width // 8), seed, extra_seeds,
+                              seperated_word_contexts).to(device)
+    return cond, uncond, latents * scheduler.init_noise_sigma
 
 
-def _control_arguments(controlnet, control_image, size: Tuple[int, int], size_of: str) -> dict:
-    """PwWSampler's controlnet / control_image from the public arguments; the hint image must be `size` (W, H)."""
+def _img2img_latents(vae, scheduler, init_image, num_inference_steps: int, strength: float, device,
+                     generator: Optional[torch.Generator] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(latents, timesteps) of an img2img run: the last `strength` of the schedule, and the init image's VAE latents
+    noised to its first timestep with noise from `generator` (None: the global RNG)."""
+    init_timestep = min(int(num_inference_steps * strength), num_inference_steps)
+    t_start = max(num_inference_steps - init_timestep, 0)
+    timesteps = scheduler.timesteps[t_start:]
+    image = preprocess(init_image).to(device=device)
+    init_latents = 0.18215 * vae.encode(image.to(_module_dtype(vae, image.dtype))).latent_dist.sample().float()
+    noise = torch.randn(init_latents.shape, generator=generator).to(device)
+    return scheduler.add_noise(init_latents, noise, timesteps[:1]), timesteps
+
+
+def _result(vae, latents: torch.Tensor, return_latents: bool):
+    """What the public functions return for one image: its final latents, or the PIL image they decode to."""
+    return latents if return_latents else _pil_from_latents(vae, latents)[0]
+
+
+def _control_arguments(controlnet, control_image, size: Tuple[int, int], size_of: str, conditioning_scale,
+                       guess_mode: bool, start: float, end: float) -> dict:
+    """PwWSampler's ControlNet keyword arguments from the public ones, {} without a controlnet; the hint image must be
+    `size` (W, H)."""
     if controlnet is None:
         if control_image is not None:
             raise ValueError("control_image is given but controlnet is None")
@@ -621,7 +642,9 @@ def _control_arguments(controlnet, control_image, size: Tuple[int, int], size_of
                          f"{type(control_image).__name__}")
     if control_image.size != tuple(size):
         raise ValueError(f"control_image is {control_image.size}; it must have the {size_of} size {tuple(size)}")
-    return {"controlnet": controlnet, "control_image": control_image_tensor(control_image)}
+    return dict(controlnet=controlnet, control_image=control_image_tensor(control_image),
+                controlnet_conditioning_scale=conditioning_scale, guess_mode=guess_mode, control_guidance_start=start,
+                control_guidance_end=end)
 
 
 # the per-image keyword arguments of paint_with_words that paint_with_words_batch takes per entry
@@ -652,9 +675,8 @@ def _batch_settings(settings) -> List[dict]:
 
 def batch_groups(keys: Sequence, max_batch_size: int) -> List[List[int]]:
     """Indices of the entries grouped by key (groups in order of first appearance, input order inside a group), each
-    group cut into runs of at most `max_batch_size`: one sampler per run.  A key of None is never shared."""
-    if max_batch_size < 1:
-        raise ValueError("max_batch_size must be >= 1")
+    group cut into runs of at most `max_batch_size` (>= 1: paint_with_words_batch checks it before it loads any
+    model): one sampler per run.  A key of None is never shared."""
     groups: Dict[object, List[int]] = {}
     for i, key in enumerate(keys):
         groups.setdefault(("solo", i) if key is None else key, []).append(i)
@@ -695,36 +717,32 @@ def paint_with_words_batch(
     entries = _batch_settings(settings)
     if max_batch_size < 1:
         raise ValueError("max_batch_size must be >= 1")
+    controls = []
     for i, e in enumerate(entries):
         try:
-            _control_arguments(controlnet, e["control_image"], e["color_map_image"].size, "color_map_image")
+            controls.append(_control_arguments(controlnet, e["control_image"], e["color_map_image"].size,
+                                               "color_map_image", e["controlnet_conditioning_scale"], guess_mode,
+                                               control_guidance_start, control_guidance_end))
         except ValueError as err:
             raise ValueError(f"settings[{i}]: {err}") from err
-    vae, unet, text_encoder, tokenizer, scheduler = (
-        pww_load_tools(device, scheduler_type, local_model_path=local_model_path, hf_model_path=hf_model_path,
-                       model_token=model_token, torch_dtype=torch_dtype)
-        if preloaded_utils is None else preloaded_utils)
+    tools = _tools(preloaded_utils, device, scheduler_type, local_model_path, hf_model_path, model_token, torch_dtype)
+    vae, unet, _, _, scheduler = tools
     scheduler.set_timesteps(num_inference_steps)
     encoded, keys = [], []
     for e in entries:
+        cond, uncond, latents = _txt2img_inputs(tools, device, e["color_map_image"], dict(e["color_context"]),
+                                                e["input_prompt"], e["unconditional_input_prompt"], e["seed"],
+                                                e["max_prompt_chunks"])
+        encoded.append((cond, uncond, latents))
         width, height = e["color_map_image"].size
-        extra_seeds, seperated_word_contexts, cond, uncond = _encode_text_color_inputs(
-            text_encoder, tokenizer, device, e["color_map_image"], dict(e["color_context"]), e["input_prompt"],
-            e["unconditional_input_prompt"], max_prompt_chunks=e["max_prompt_chunks"])
-        latents = initial_latents((1, unet.in_channels, height // 8, width // 8), e["seed"], extra_seeds,
-                                  seperated_word_contexts).to(device)
-        encoded.append((cond, uncond, latents * scheduler.init_noise_sigma))
         solo = width % 64 != 0 or height % 64 != 0
         keys.append(None if solo else (height // 8, width // 8, int(cond["CONTEXT_TENSOR"].shape[1])))
     results: List[Optional[torch.Tensor]] = [None] * len(entries)
     for idx in batch_groups(keys, max_batch_size):
-        control = {}
-        if controlnet is not None:
-            control = dict(controlnet=controlnet,
-                           control_image=[control_image_tensor(entries[i]["control_image"]) for i in idx],
-                           controlnet_conditioning_scale=[entries[i]["controlnet_conditioning_scale"] for i in idx],
-                           guess_mode=guess_mode, control_guidance_start=control_guidance_start,
-                           control_guidance_end=control_guidance_end)
+        control = controls[idx[0]]
+        if control:       # the batch's ControlNet and window, each image's own hint and weight
+            control = dict(control, control_image=[controls[i]["control_image"] for i in idx],
+                           controlnet_conditioning_scale=[controls[i]["controlnet_conditioning_scale"] for i in idx])
         sampler = PwWSampler(unet, scheduler, [encoded[i][0] for i in idx], [encoded[i][1] for i in idx],
                              torch.cat([encoded[i][2] for i in idx], 0),
                              [entries[i]["weight_function"] for i in idx], [entries[i]["guidance_scale"] for i in idx],
@@ -733,9 +751,7 @@ def paint_with_words_batch(
         for j, i in enumerate(idx):
             results[i] = latents[j:j + 1].clone()
         del sampler
-    if return_latents:
-        return results
-    return [_pil_from_latents(vae, lat)[0] for lat in results]
+    return [_result(vae, lat, return_latents) for lat in results]
 
 
 def prepare_mask_and_masked_image(image, mask):
@@ -800,11 +816,11 @@ def paint_with_words_inpaint(
     to the init image, so `control_image` has the init image's size.  The ControlNet sees the 4 latent channels of
     the UNet input (hook_pww.py:113-119)."""
     width, height = init_image.size
-    control = _control_arguments(controlnet, control_image, (width, height), "init_image (and resized color_map_image)")
-    vae, unet, text_encoder, tokenizer, scheduler = (
-        pww_load_tools(device, scheduler_type, local_model_path=local_model_path, hf_model_path=hf_model_path,
-                       model_token=model_token, torch_dtype=torch_dtype)
-        if preloaded_utils is None else preloaded_utils)
+    control = _control_arguments(controlnet, control_image, (width, height), "init_image (and resized color_map_image)",
+                                 controlnet_conditioning_scale, guess_mode, control_guidance_start,
+                                 control_guidance_end)
+    vae, unet, text_encoder, tokenizer, scheduler = _tools(preloaded_utils, device, scheduler_type, local_model_path,
+                                                           hf_model_path, model_token, torch_dtype)
     color_map_image = color_map_image.resize((width, height), Image.NEAREST)
     mask_image = mask_image.resize((width, height), Image.NEAREST)
     _, _, cond, uncond = _encode_text_color_inputs(
@@ -813,15 +829,9 @@ def paint_with_words_inpaint(
     mask, masked_image = prepare_mask_and_masked_image(init_image, mask_image)
 
     scheduler.set_timesteps(num_inference_steps)
-    init_timestep = min(int(num_inference_steps * strength), num_inference_steps)
-    t_start = max(num_inference_steps - init_timestep, 0)
-    timesteps = scheduler.timesteps[t_start:]
-
-    generator = torch.manual_seed(seed)
-    image = preprocess(init_image).to(device=device)
-    init_latents = 0.18215 * vae.encode(image.to(_module_dtype(vae, image.dtype))).latent_dist.sample().float()
-    noise = torch.randn(init_latents.shape, generator=generator).to(device)
-    latents = scheduler.add_noise(init_latents, noise, timesteps[:1])
+    # seeded before the VAE encode, which draws from the same (global) generator
+    latents, timesteps = _img2img_latents(vae, scheduler, init_image, num_inference_steps, strength, device,
+                                          generator=torch.manual_seed(seed))
 
     mask = F.interpolate(mask, size=(height // 8, width // 8)).to(device=device, dtype=latents.dtype)
     masked_image_latents = 0.18215 * vae.encode(masked_image.to(device=device, dtype=_module_dtype(vae, latents.dtype))).latent_dist.sample().float()
@@ -835,13 +845,8 @@ def paint_with_words_inpaint(
             f"num_channels_masked_image: {masked_image_latents.shape[1]} = {total}.")
     sampler = PwWSampler(unet, scheduler, [cond], [uncond], latents, weight_function, guidance_scale,
                          extra_input=torch.cat([mask, masked_image_latents], 1).float(), timesteps=timesteps,
-                         noise_seed=seed, **control, controlnet_conditioning_scale=controlnet_conditioning_scale,
-                         guess_mode=guess_mode, control_guidance_start=control_guidance_start,
-                         control_guidance_end=control_guidance_end)
-    latents = sampler.run()
-    if return_latents:
-        return latents
-    return _pil_from_latents(vae, latents)[0]
+                         noise_seed=seed, **control)
+    return _result(vae, sampler.run(), return_latents)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -933,14 +938,6 @@ class PaintWithWord_StableDiffusionPipeline:
 
 class PaintWithWord_StableDiffusionInpaintPipeline(PaintWithWord_StableDiffusionPipeline):
     """paint_with_words_inpaint.py:273-575: `__call__(prompt, image, mask_image, color_map_image, color_context, ...)`."""
-
-    @classmethod
-    def from_pretrained(cls, save_dir, device: str = "cuda:0", torch_dtype: Optional[torch.dtype] = None, **kwargs):
-        """`torch_dtype` as in `pww_load_tools` (torch.bfloat16 for a bf16 UNet)."""
-        vae, unet, text_encoder, tokenizer, scheduler = pww_load_tools(device, local_model_path=save_dir,
-                                                                       torch_dtype=torch_dtype)
-        return cls(vae=vae, text_encoder=text_encoder, tokenizer=tokenizer, unet=unet, scheduler=scheduler,
-                   controlnet=kwargs.get("controlnet"))
 
     @torch.no_grad()
     def __call__(self, prompt, image=None, mask_image=None, color_map_image=None, color_context={},

@@ -9,6 +9,8 @@ import ctypes
 import os
 from typing import Optional
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("PWW_B200_LIB", os.path.join(_HERE, "libpww_b200.so"))
 
@@ -102,6 +104,12 @@ def lib() -> ctypes.CDLL:
                                      c_i, c_i, c_i, c_vp]
     _lib = L
     return L
+
+
+def entry(name: str, dtype):
+    """The C entry point `name` (without its type suffix) for element type `dtype`: `_bf16` for torch.bfloat16, else
+    `_f16`."""
+    return getattr(lib(), name + ("_bf16" if dtype == torch.bfloat16 else "_f16"))
 
 
 def check(status: int, what: str) -> None:

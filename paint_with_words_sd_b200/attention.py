@@ -136,11 +136,6 @@ def _elem_dtype(q: torch.Tensor) -> torch.dtype:
     return torch.bfloat16 if q.dtype == torch.bfloat16 else torch.float16
 
 
-def _entry(name: str, dtype: torch.dtype):
-    """The C entry point `name` (without its type suffix) for element type `dtype`."""
-    return getattr(_native.lib(), name + ("_bf16" if dtype == torch.bfloat16 else "_f16"))
-
-
 def _autocast_dtype(module) -> torch.dtype:
     """bf16 for a module with bf16 weights, fp16 otherwise (fp32 modules keep the reference's fp16 autocast)."""
     return torch.bfloat16 if module.to_q.weight.dtype == torch.bfloat16 else torch.float16
@@ -229,7 +224,7 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                 mp_ptr, ci_ptr, idx_ptr = mpack.data_ptr(), cidx.data_ptr(), wmap_index.data_ptr()
                 g_ptr, st_ptr, ws_ptr = g_sigma.data_ptr(), stats.data_ptr(), ws.data_ptr()
                 mp_bs, bw, ws_bytes = mpack.stride(0), mpack.shape[0], ws.numel()
-            fn = _entry("pww_xattn_fused_multi" if per_image else "pww_xattn_fused", dt)
+            fn = _native.entry("pww_xattn_fused_multi" if per_image else "pww_xattn_fused", dt)
             rc = fn(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, heads, N, T, D,
                     q.stride(0), q.stride(1), k.stride(0), k.stride(1), out.stride(0), out.stride(1),
                     mp_ptr, mp_bs, bw, ci_ptr, idx_ptr, kind_ptr if per_image else stat, g_ptr, float(scale), st_ptr,
@@ -247,7 +242,7 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                 ws_bytes = L.pww_xattn_workspace_bytes(B, heads, N, T, D)
                 st.ensure(B, ws_bytes)
                 stats = st.stats if stats_out is None else stats_out
-                fn = _entry("pww_xattn_stats_multi" if per_image else "pww_xattn_stats", dt)
+                fn = _native.entry("pww_xattn_stats_multi" if per_image else "pww_xattn_stats", dt)
                 rc = fn(q.data_ptr(), k.data_ptr(), B, heads, N, T, D, q.stride(0), q.stride(1), k.stride(0),
                         k.stride(1), kind_ptr if per_image else stat, wmap_index.data_ptr(), stats.data_ptr(),
                         st.workspace.data_ptr(), st.workspace.numel(), stream)
@@ -255,7 +250,7 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                 _native.launch_count += 1
                 stats_ptr, g_ptr = stats.data_ptr(), g_sigma.data_ptr()
                 w_ptr, idx_ptr, w_bs = wmap.data_ptr(), wmap_index.data_ptr(), wmap.stride(0)
-            fn = _entry("pww_xattn_fwd_multi" if per_image else "pww_xattn_fwd", dt)
+            fn = _native.entry("pww_xattn_fwd_multi" if per_image else "pww_xattn_fwd", dt)
             rc = fn(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, heads, N, T, D,
                     q.stride(0), q.stride(1), k.stride(0), k.stride(1), out.stride(0), out.stride(1),
                     w_ptr, w_bs, idx_ptr, stats_ptr, g_ptr, float(scale), stream)
@@ -280,7 +275,7 @@ def self_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int
     D = C // heads
     if SELF_ATTN_IMPL == "native" or (SELF_ATTN_IMPL == "auto" and N <= SELF_ATTN_NATIVE_MAX_KEYS):
         dt = _elem_dtype(q)
-        fn = _entry("pww_attn_fwd", dt)
+        fn = _native.entry("pww_attn_fwd", dt)
         q, k, v = _rows(q, dt), _rows(k, dt), _rows(v, dt)
         if not (q.stride() == k.stride() == v.stride()):
             q, k, v = q.contiguous(), k.contiguous(), v.contiguous()

@@ -8,12 +8,12 @@
 //     online softmax: running row max m and row sum l; O and l are rescaled by 2^(m_old - m_new) when the max moves
 //     O += P V_j      P packed to E (fp16 or bf16, the element type of q / k / v / out) straight from the S accumulators (the C layout of two n-tiles is the A layout of one
 //                     k-step), V fragments by ldmatrix.trans
+// The softmax and P V are the cross-attention kernels' block (core::warp_online_*, xattn_core.cuh) at 8 n-tiles per tile.
 // Padding (d >= D, key >= N, row >= N) is zero-filled by the copies; padded keys of the last tile are masked to -inf.
 #pragma once
 #include "mma_sm90.cuh"
 #include "pww_common.cuh"
 #include "xattn_core.cuh"
-#include "xattn_tc.cuh"   // num_sms, cur_device
 
 namespace pww {
 namespace fa {
@@ -77,10 +77,8 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks<D, E>) attn_fwd_kernel(co
   }
   issue_kv(0);                                     // one group: Q and the first key tile
   uint32_t qa[C::KS][4];
-  float o[C::NT][4];
-#pragma unroll
-  for (int j = 0; j < C::NT; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
-  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+  float o[C::NT][4], m0, m1, l0, l1;
+  core::warp_online_begin<D>(o, m0, m1, l0, l1);
   const float sl2 = p.scale * 1.4426950408889634f;
   const uint32_t qs = smem0 + (uint32_t)(warp * 16 * C::LD) * 2u;
 #pragma unroll 1
@@ -98,13 +96,13 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks<D, E>) attn_fwd_kernel(co
         ptx::ldsm_x4(qs + (uint32_t)((lane & 15) * C::LD + kk * 16 + (lane >> 4) * 8) * 2u, qa[kk][0], qa[kk][1], qa[kk][2], qa[kk][3]);
     }
     const uint32_t ks = smem0 + CF::OFF_KV + (jt & 1) * 2 * CF::KVBYTES, vs = ks + CF::KVBYTES;
-    float s[8][4];
+    float s[kBN / 8][4];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
+    for (int j = 0; j < kBN / 8; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
 #pragma unroll
     for (int kk = 0; kk < C::KS; ++kk) {
 #pragma unroll
-      for (int jp = 0; jp < 4; ++jp) {
+      for (int jp = 0; jp < kBN / 16; ++jp) {
         const int t = 16 * jp + (lane & 7) + ((lane >> 4) << 3), d = kk * 16 + ((lane >> 3) & 1) * 8;
         uint32_t b0, b1, b2, b3;
         ptx::ldsm_x4(ks + (uint32_t)(t * C::LD + d) * 2u, b0, b1, b2, b3);
@@ -112,68 +110,10 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks<D, E>) attn_fwd_kernel(co
         ptx::mma16816<E>(s[2 * jp + 1], qa[kk], b2, b3);
       }
     }
-    const int valid = p.N - jt * kBN;              // keys of this tile that exist
-    float t0 = -INFINITY, t1 = -INFINITY;
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        if (core::tok(j, e, lane) >= valid) s[j][e] = -INFINITY;
-        if (e < 2) t0 = fmaxf(t0, s[j][e]); else t1 = fmaxf(t1, s[j][e]);
-      }
-    t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, 1));
-    t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, 2));
-    t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, 1));
-    t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, 2));
-    const float mn0 = fmaxf(m0, t0), mn1 = fmaxf(m1, t1);
-    const float a0 = ptx::ex2((m0 - mn0) * sl2), a1 = ptx::ex2((m1 - mn1) * sl2);   // 0 on the first tile (m = -inf)
-    m0 = mn0; m1 = mn1;
-    const float n0 = -mn0 * sl2, n1 = -mn1 * sl2;
-    uint32_t pa[4][4];
-    float r0 = 0.f, r1 = 0.f;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const uint32_t p01 = ptx::pack2<E>(ptx::ex2(fmaf(s[j][0], sl2, n0)), ptx::ex2(fmaf(s[j][1], sl2, n0)));
-      const uint32_t p23 = ptx::pack2<E>(ptx::ex2(fmaf(s[j][2], sl2, n1)), ptx::ex2(fmaf(s[j][3], sl2, n1)));
-      const float2 f01 = ptx::unpack2<E>(p01), f23 = ptx::unpack2<E>(p23);
-      r0 += f01.x + f01.y;
-      r1 += f23.x + f23.y;
-      pa[j >> 1][(j & 1) * 2] = p01;
-      pa[j >> 1][(j & 1) * 2 + 1] = p23;
-    }
-    l0 = l0 * a0 + r0;                             // per-thread partial row sums; reduced over the quad at the end
-    l1 = l1 * a1 + r1;
-#pragma unroll
-    for (int j = 0; j < C::NT; ++j) {
-      o[j][0] *= a0; o[j][1] *= a0; o[j][2] *= a1; o[j][3] *= a1;
-    }
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      const int t = 16 * kk + (lane & 7) + ((lane >> 3) & 1) * 8;
-#pragma unroll
-      for (int jp = 0; jp < C::NT / 2; ++jp) {
-        uint32_t b0, b1, b2, b3;
-        ptx::ldsm_x4_t(vs + (uint32_t)(t * C::LD + 16 * jp + (lane >> 4) * 8) * 2u, b0, b1, b2, b3);
-        ptx::mma16816<E>(o[2 * jp], pa[kk], b0, b1);
-        ptx::mma16816<E>(o[2 * jp + 1], pa[kk], b2, b3);
-      }
-      if constexpr (C::NT & 1) {
-        uint32_t b0, b1;
-        ptx::ldsm_x2_t(vs + (uint32_t)(t * C::LD + 8 * (C::NT - 1)) * 2u, b0, b1);
-        ptx::mma16816<E>(o[C::NT - 1], pa[kk], b0, b1);
-      }
-    }
+    core::warp_online_chunk<D, E>(s, p.N - jt * kBN, sl2, vs, lane, o, m0, m1, l0, l1);
     __syncthreads();                               // stage jt & 1 is refilled by the copies issued next iteration
   }
-  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
-  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
-  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-  const float i0 = 1.f / l0, i1 = 1.f / l1;
-#pragma unroll
-  for (int j = 0; j < C::NT; ++j) {
-    o[j][0] *= i0; o[j][1] *= i0; o[j][2] *= i1; o[j][3] *= i1;
-  }
+  core::warp_online_end<D>(o, l0, l1);
   core::warp_store<D>(o, smem + warp * 16 * C::LD * 2, lane, p.out + (int64_t)b * p.o_bs + h * D, p.o_rs,
                       row_base + warp * 16, p.N);
 }
@@ -185,12 +125,8 @@ cudaError_t launch(const void* q, const void* k, const void* v, void* out, int B
   Params<E> p;
   p.q = (const E*)q; p.k = (const E*)k; p.v = (const E*)v; p.out = (E*)out;
   p.B = B; p.H = H; p.N = N; p.bs = bs; p.rs = rs; p.o_bs = o_bs; p.o_rs = o_rs; p.scale = scale;
-  static bool attr_set[tc::kMaxDevices] = {false};
-  if (!attr_set[tc::cur_device()]) {
-    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<D, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, CF::SMEM);
-    if (e != cudaSuccess) return e;
-    attr_set[tc::cur_device()] = true;
-  }
+  const cudaError_t e = allow_dynamic_smem<attn_fwd_kernel<D, E>>(CF::SMEM);
+  if (e != cudaSuccess) return e;
   const long long grid = (long long)B * H * ((N + kBM - 1) / kBM);
   if (grid > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
   attn_fwd_kernel<D, E><<<(unsigned)grid, kThreads, CF::SMEM, s>>>(p);

@@ -10,6 +10,8 @@
 #include "sampler_step.cuh"
 #include "control_inject.cuh"
 #include <stdlib.h>
+#include <algorithm>
+#include <type_traits>
 
 namespace {
 
@@ -56,17 +58,54 @@ cudaError_t with_shape(int D, int T, F&& f) {
   return cudaErrorInvalidValue;
 }
 
+// f(std::integral_constant<int, v>{}) for lo <= v <= hi.
+template <int lo, int hi, typename F>
+void with_int(int v, F&& f) {
+  if constexpr (lo < hi)
+    if (v != lo) return with_int<lo + 1, hi>(v, f);
+  f(std::integral_constant<int, lo>{});
+}
+
 size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// Partial slots reserved per image (one per CTA of the persistent grid; device independent upper bound so the size
-// can be computed without a GPU).
-int stats_slots_per_image(int, int) { return 2048; }
+// Partial slots the statistics workspace reserves per image: one per CTA of the persistent grid, a device-independent
+// upper bound so that the size can be computed without a GPU.
+constexpr int kStatSlotsPerImage = 2048;
 
 int cuda_fail(cudaError_t e) {
-  snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "%s: %s %s", cudaGetErrorName(e), cudaGetErrorString(e),
-           pww::tc::tc_error_buf());
-  pww::tc::tc_error_buf()[0] = 0;
+  snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "%s: %s ", cudaGetErrorName(e), cudaGetErrorString(e));
   return PWW_ERR_CUDA;
+}
+
+// The XattnParams fields every cross-attention launch takes from its arguments; the others start at zero.
+template <typename E>
+pww::XattnParams<E> xattn_params(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+                                 int64_t q_bs, int64_t q_rs, int64_t k_bs, int64_t k_rs, int64_t o_bs, int64_t o_rs) {
+  pww::XattnParams<E> p;
+  memset(&p, 0, sizeof(p));
+  p.q = (const E*)q; p.k = (const E*)k; p.v = (const E*)v; p.out = (E*)out;
+  p.B = B; p.H = H; p.N = N; p.T = T; p.D = D;
+  p.q_bs = q_bs; p.q_rs = q_rs; p.k_bs = k_bs; p.k_rs = k_rs; p.o_bs = o_bs; p.o_rs = o_rs;
+  return p;
+}
+
+// p restricted to images [b0, b0 + n): every per-image pointer that is set starts at image b0.  The workspace
+// (counters, partials) is shared by the launches, and the weight maps are reached through wmap_index; a caller that maps
+// image b to map b without an index offsets its maps itself.
+template <typename E>
+pww::XattnParams<E> images(const pww::XattnParams<E>& p, int b0, int n) {
+  pww::XattnParams<E> c = p;
+  c.B = n;
+  c.q += (int64_t)b0 * p.q_bs;
+  c.k += (int64_t)b0 * p.k_bs;
+  if (c.v) c.v += (int64_t)b0 * p.k_bs;
+  if (c.out) c.out += (int64_t)b0 * p.o_bs;
+  if (c.wmap_index) c.wmap_index += b0;
+  if (c.stat_kind) c.stat_kind += b0;
+  if (c.stats) c.stats += b0;
+  if (c.stats_out) c.stats_out += b0;
+  if (c.g_sigma) c.g_sigma += (int64_t)b0 * p.g_stride;
+  return c;
 }
 
 }  // namespace
@@ -101,7 +140,7 @@ size_t pww_xattn_workspace_bytes(int B, int H, int N, int T, int D) {
   (void)T; (void)D;
   if (B <= 0 || H <= 0 || N <= 0) return 0;
   return align_up((size_t)B * sizeof(unsigned int), 256) +
-         (size_t)B * stats_slots_per_image(H, N) * sizeof(pww::StatPartial);
+         (size_t)B * kStatSlotsPerImage * sizeof(pww::StatPartial);
 }
 
 }  // extern "C"
@@ -120,30 +159,19 @@ int xattn_stats(const void* q, const void* k, int B, int H, int N, int T, int D,
   if (!stats || !workspace) return PWW_ERR_BAD_ARG;
   if (per_image ? !kinds : (stat != PWW_STAT_MAX && stat != PWW_STAT_STD)) return PWW_ERR_BAD_ARG;
   if (workspace_bytes < pww_xattn_workspace_bytes(B, H, N, T, D)) return PWW_ERR_WORKSPACE;
-  pww::XattnParams<E> p;
-  memset(&p, 0, sizeof(p));
-  p.q = (const E*)q; p.k = (const E*)k;
-  p.B = B; p.H = H; p.N = N; p.T = T; p.D = D;
-  p.q_bs = q_batch_stride; p.q_rs = q_row_stride; p.k_bs = k_batch_stride; p.k_rs = k_row_stride;
+  if (pww::num_sms() > kStatSlotsPerImage) return PWW_ERR_WORKSPACE;
+  pww::XattnParams<E> p = xattn_params<E>(q, k, nullptr, nullptr, B, H, N, T, D, q_batch_stride, q_row_stride,
+                                          k_batch_stride, k_row_stride, 0, 0);
   p.wmap_index = wmap_index; p.stat = stat; p.stat_kind = per_image ? kinds : nullptr; p.stats_out = stats;
   p.counters = (unsigned int*)workspace;
   p.partials = (pww::StatPartial*)((char*)workspace + align_up((size_t)B * sizeof(unsigned int), 256));
-  cudaStream_t s = (cudaStream_t)stream;
-  {
-    if (pww::tc::stats_slots() > stats_slots_per_image(H, N)) return PWW_ERR_WORKSPACE;
-    for (int b0 = 0; b0 < B; b0 += pww::tc::kMaxBatch) {          // <= 256 images per launch
-      pww::XattnParams<E> c = p;
-      c.B = (B - b0) < pww::tc::kMaxBatch ? (B - b0) : pww::tc::kMaxBatch;
-      c.q = p.q + (int64_t)b0 * p.q_bs;
-      c.k = p.k + (int64_t)b0 * p.k_bs;
-      c.wmap_index = p.wmap_index ? p.wmap_index + b0 : nullptr;
-      c.stat_kind = p.stat_kind ? p.stat_kind + b0 : nullptr;
-      c.stats_out = p.stats_out + b0;
-      const cudaError_t e = with_shape(D, T, [&](auto k) { return pww::tc::launch_stats<k.D, k.KC>(c, s); });
-      if (e != cudaSuccess) return cuda_fail(e);
-    }
-    return PWW_OK;
+  for (int b0 = 0; b0 < B; b0 += pww::tc::kMaxBatch) {
+    const pww::XattnParams<E> c = images(p, b0, std::min(B - b0, pww::tc::kMaxBatch));
+    const cudaError_t e =
+        with_shape(D, T, [&](auto k) { return pww::tc::launch_stats<k.D, k.KC>(c, (cudaStream_t)stream); });
+    if (e != cudaSuccess) return cuda_fail(e);
   }
+  return PWW_OK;
 }
 
 // The forward launches of pww_xattn_fwd_{f16,bf16} (g_stride 0: g_sigma[0] for every image) and of
@@ -159,32 +187,18 @@ int xattn_fwd(const void* q, const void* k, const void* v, void* out, int B, int
   if (!v || !out || !aligned16(v) || !aligned16(out)) return PWW_ERR_BAD_ARG;
   if ((o_batch_stride | o_row_stride) & 7 || o_row_stride < (int64_t)H * D) return PWW_ERR_BAD_ARG;
   if (wmap && (!stats || !g_sigma)) return PWW_ERR_BAD_ARG;
-  pww::XattnParams<E> p;
-  memset(&p, 0, sizeof(p));
-  p.q = (const E*)q; p.k = (const E*)k; p.v = (const E*)v; p.out = (E*)out;
-  p.B = B; p.H = H; p.N = N; p.T = T; p.D = D;
-  p.q_bs = q_batch_stride; p.q_rs = q_row_stride; p.k_bs = k_batch_stride; p.k_rs = k_row_stride;
-  p.o_bs = o_batch_stride; p.o_rs = o_row_stride;
-  p.wmap = wmap; p.wmap_bs = wmap_batch_stride; p.wmap_index = wmap_index;
+  pww::XattnParams<E> p = xattn_params<E>(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride,
+                                          k_row_stride, o_batch_stride, o_row_stride);
+  p.wmap = wmap; p.wmap_bs = wmap_batch_stride; p.wmap_index = wmap ? wmap_index : nullptr;
   p.stats = stats; p.g_sigma = g_sigma; p.g_stride = g_stride; p.scale = scale;
-  cudaStream_t s = (cudaStream_t)stream;
-  {
-    for (int b0 = 0; b0 < B; b0 += pww::tc::kMaxBatch) {          // <= 256 images per launch
-      pww::XattnParams<E> c = p;
-      c.B = (B - b0) < pww::tc::kMaxBatch ? (B - b0) : pww::tc::kMaxBatch;
-      c.q = p.q + (int64_t)b0 * p.q_bs;
-      c.k = p.k + (int64_t)b0 * p.k_bs;
-      c.v = p.v + (int64_t)b0 * p.k_bs;
-      c.out = p.out + (int64_t)b0 * p.o_bs;
-      c.wmap_index = (p.wmap && p.wmap_index) ? p.wmap_index + b0 : nullptr;
-      c.stats = p.stats ? p.stats + b0 : nullptr;
-      c.g_sigma = p.g_sigma ? p.g_sigma + (int64_t)b0 * p.g_stride : nullptr;
-      if (p.wmap && !p.wmap_index) c.wmap = p.wmap + (int64_t)b0 * p.wmap_bs;   // identity mapping
-      const cudaError_t e = with_shape(D, T, [&](auto k) { return pww::tc::launch_fwd<k.D, k.KC>(c, s); });
-      if (e != cudaSuccess) return cuda_fail(e);
-    }
-    return PWW_OK;
+  for (int b0 = 0; b0 < B; b0 += pww::tc::kMaxBatch) {
+    pww::XattnParams<E> c = images(p, b0, std::min(B - b0, pww::tc::kMaxBatch));
+    if (wmap && !wmap_index) c.wmap += (int64_t)b0 * wmap_batch_stride;   // identity mapping: image b uses map b
+    const cudaError_t e =
+        with_shape(D, T, [&](auto k) { return pww::tc::launch_fwd<k.D, k.KC>(c, (cudaStream_t)stream); });
+    if (e != cudaSuccess) return cuda_fail(e);
   }
+  return PWW_OK;
 }
 
 // The one launch of pww_xattn_fused_{f16,bf16} (one `stat` and g_sigma[0] for every image) and of
@@ -206,50 +220,35 @@ int xattn_fused(const void* q, const void* k, const void* v, void* out, int B, i
     if (per_image ? !kinds : (stat != PWW_STAT_MAX && stat != PWW_STAT_STD)) return PWW_ERR_BAD_ARG;
     if (workspace_bytes < pww_xattn_fused_workspace_bytes()) return PWW_ERR_WORKSPACE;
   }
-  pww::XattnParams<E> p;
-  memset(&p, 0, sizeof(p));
-  p.q = (const E*)q; p.k = (const E*)k; p.v = (const E*)v; p.out = (E*)out;
-  p.B = B; p.H = H; p.N = N; p.T = T; p.D = D;
-  p.q_bs = q_batch_stride; p.q_rs = q_row_stride; p.k_bs = k_batch_stride; p.k_rs = k_row_stride;
-  p.o_bs = o_batch_stride; p.o_rs = o_row_stride;
+  pww::XattnParams<E> p = xattn_params<E>(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride,
+                                          k_row_stride, o_batch_stride, o_row_stride);
   p.g_sigma = g_sigma; p.g_stride = per_image ? 1 : 0; p.scale = scale; p.stat = stat;
-  p.stat_kind = per_image ? kinds : nullptr;
+  p.stat_kind = per_image ? kinds : nullptr; p.stats_out = stats;
+  // image b is biased iff it has a packed map: with mpack == NULL the kernel takes every index as -1
+  p.wmap_index = mpack ? wmap_index : nullptr;
   p.counters = (unsigned int*)workspace;
   p.partials = workspace ? (pww::StatPartial*)((char*)workspace + 512) : nullptr;   // header: counters @0, per-image maxima @256
-  cudaStream_t s = (cudaStream_t)stream;
-  // image b is biased iff it has a packed map: with mpack == NULL every index is -1 (the kernel reads wmap_index)
-  int chunk = pww::fx::kMaxBatch;                                  // images per launch
-  {                                                                // job table of <= 64 units per CTA
-    const int tiles = pww::ceil_div(N, pww::core::kBM);
-    const int hg = pww::ceil_div(H, D == 40 ? pww::fx::Cfg2<40>::G : (D == 64 ? pww::fx::Cfg2<64>::G : 1));
-    while (chunk > 1) {
-      const int cb = B < chunk ? B : chunk;
-      if (pww::fx::fused2_fits(cb, hg, tiles, pww::fx::fused_grid(cb * hg * tiles))) break;
-      chunk >>= 1;
-    }
+  // images per launch: halved until every CTA's job table holds at most 64 units
+  int chunk = pww::fx::kMaxBatch;
+  const int tiles = pww::ceil_div(N, pww::core::kBM);
+  const int hg = pww::ceil_div(H, D == 40 ? pww::fx::Cfg2<40>::G : (D == 64 ? pww::fx::Cfg2<64>::G : 1));
+  while (chunk > 1) {
+    const int cb = B < chunk ? B : chunk;
+    if (pww::fx::fused2_fits(cb, hg, tiles, pww::fx::fused_grid(cb * hg * tiles))) break;
+    chunk >>= 1;
   }
   for (int b0 = 0; b0 < B; b0 += chunk) {
-    pww::XattnParams<E> c = p;
-    c.B = (B - b0) < chunk ? (B - b0) : chunk;
-    c.q = p.q + (int64_t)b0 * p.q_bs;
-    c.k = p.k + (int64_t)b0 * p.k_bs;
-    c.v = p.v + (int64_t)b0 * p.k_bs;
-    c.out = p.out + (int64_t)b0 * p.o_bs;
-    c.stats_out = stats ? stats + b0 : nullptr;
-    c.stat_kind = p.stat_kind ? p.stat_kind + b0 : nullptr;
-    c.g_sigma = p.g_sigma ? p.g_sigma + (int64_t)b0 * p.g_stride : nullptr;
+    pww::XattnParams<E> c = images(p, b0, std::min(B - b0, chunk));
     const void* mp = mpack;
     const int8_t* ci = cidx;
-    if (mpack && wmap_index) {
-      c.wmap_index = wmap_index + b0;
-    } else if (mpack) {                                            // identity mapping: image b uses map b
-      c.wmap_index = nullptr;
+    if (mpack && !wmap_index) {                                    // identity mapping: image b uses map b
       mp = (const __half*)mpack + (int64_t)b0 * mpack_batch_stride;
       ci = cidx + (int64_t)b0 * pww::core::kTP * pww::core::chunks_of(T);   // [Bw, 80 k]
     }
-    c.wmap = mpack ? (const float*)mp : nullptr;                   // non-null marks "maps present" for the kernel
-    const cudaError_t e =
-        with_shape(D, T, [&](auto k) { return pww::fx::launch_fused2<k.D, k.KC>(c, mp, mpack_batch_stride, ci, s); });
+    c.wmap = (const float*)mp;                                     // non-null marks "maps present" for the kernel
+    const cudaError_t e = with_shape(D, T, [&](auto k) {
+      return pww::fx::launch_fused2<k.D, k.KC>(c, mp, mpack_batch_stride, ci, (cudaStream_t)stream);
+    });
     if (e == cudaErrorInvalidConfiguration) return PWW_ERR_UNSUPPORTED;
     if (e != cudaSuccess) return cuda_fail(e);
   }
@@ -285,7 +284,7 @@ int groupnorm_nhwc(const void* x, const void* add, int64_t add_batch_stride, con
   if (smem1 > 48 * 1024) return PWW_ERR_UNSUPPORTED;
   pww::uops::gn_stats_kernel<E><<<dim3(p.chunks, B), nvec * rpp, smem1, s>>>(p);
   // enough row chunks to fill the machine even at 8x8 resolution
-  int rows_per_block = (int)(((long long)HW * B + 2 * pww::tc::num_sms() - 1) / (2 * pww::tc::num_sms()));
+  int rows_per_block = (int)(((long long)HW * B + 2 * pww::num_sms() - 1) / (2 * pww::num_sms()));
   if (rows_per_block < rpp) rows_per_block = rpp;
   if (rows_per_block > 32) rows_per_block = 32;
   pww::uops::gn_apply_kernel<E><<<dim3((HW + rows_per_block - 1) / rows_per_block, B), nvec * rpp, 0, s>>>(p, rows_per_block);
@@ -299,7 +298,7 @@ int geglu(const void* in, void* out, int64_t M, int I, void* stream) {
   if (I & 7) return PWW_ERR_UNSUPPORTED;
   const long long total = (long long)M * (I >> 3);
   long long blocks = (total + 255) / 256;
-  const long long cap = (long long)pww::tc::num_sms() * 16;
+  const long long cap = (long long)pww::num_sms() * 16;
   if (blocks > cap) blocks = cap;
   pww::uops::geglu_kernel<E><<<(int)blocks, 256, 0, (cudaStream_t)stream>>>((const E*)in, (E*)out, M, I);
   cudaError_t e = cudaGetLastError();
@@ -314,23 +313,13 @@ int add_layernorm(const void* x, const void* res, const void* gamma, const void*
       (sum_out && !aligned16(sum_out)))
     return PWW_ERR_BAD_ARG;
   if ((C & 7) || C > 2048) return PWW_ERR_UNSUPPORTED;
-  const int vpl = ((C >> 3) + 31) / 32;
   const int warps = 8;
   const unsigned grid = (unsigned)((M + warps - 1) / warps);
-  cudaStream_t s = (cudaStream_t)stream;
-  const E *xp = (const E*)x, *rp = (const E*)res, *gp = (const E*)gamma, *bp = (const E*)beta;
-  E *sp = (E*)sum_out, *yp = (E*)y;
-  switch (vpl) {
-    case 1: pww::uops::add_layernorm_kernel<E, 1><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
-    case 2: pww::uops::add_layernorm_kernel<E, 2><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
-    case 3: pww::uops::add_layernorm_kernel<E, 3><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
-    case 4: pww::uops::add_layernorm_kernel<E, 4><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
-    case 5: pww::uops::add_layernorm_kernel<E, 5><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
-    case 6: pww::uops::add_layernorm_kernel<E, 6><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
-    case 7: pww::uops::add_layernorm_kernel<E, 7><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
-    case 8: pww::uops::add_layernorm_kernel<E, 8><<<grid, warps * 32, 0, s>>>(xp, rp, gp, bp, sp, yp, M, C, eps); break;
-    default: return PWW_ERR_UNSUPPORTED;
-  }
+  // 16-byte vectors per lane: 1 .. 8 for C <= 2048
+  with_int<1, 8>(((C >> 3) + 31) / 32, [&](auto vpl) {
+    pww::uops::add_layernorm_kernel<E, vpl><<<grid, warps * 32, 0, (cudaStream_t)stream>>>(
+        (const E*)x, (const E*)res, (const E*)gamma, (const E*)beta, (E*)sum_out, (E*)y, M, C, eps);
+  });
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
@@ -343,15 +332,11 @@ int attn_fwd(const void* q, const void* k, const void* v, void* out, int B, int 
   if ((qkv_batch_stride | qkv_row_stride | o_batch_stride | o_row_stride) & 7) return PWW_ERR_BAD_ARG;
   if (qkv_row_stride < (int64_t)H * D || o_row_stride < (int64_t)H * D) return PWW_ERR_BAD_ARG;
   if (!supported_head_dim(D)) return PWW_ERR_UNSUPPORTED;
-  cudaStream_t s = (cudaStream_t)stream;
-  cudaError_t e = cudaErrorInvalidValue;
-  const int64_t bs = qkv_batch_stride, rs = qkv_row_stride, obs = o_batch_stride, ors = o_row_stride;
-  switch (D) {
-    case 40: e = pww::fa::launch<40, E>(q, k, v, out, B, H, N, bs, rs, obs, ors, scale, s); break;
-    case 64: e = pww::fa::launch<64, E>(q, k, v, out, B, H, N, bs, rs, obs, ors, scale, s); break;
-    case 80: e = pww::fa::launch<80, E>(q, k, v, out, B, H, N, bs, rs, obs, ors, scale, s); break;
-    case 160: e = pww::fa::launch<160, E>(q, k, v, out, B, H, N, bs, rs, obs, ors, scale, s); break;
-  }
+  // self-attention has no key chunks: T = 1 picks the one-chunk shape of the head dim
+  const cudaError_t e = with_shape(D, 1, [&](auto sh) {
+    return pww::fa::launch<sh.D, E>(q, k, v, out, B, H, N, qkv_batch_stride, qkv_row_stride, o_batch_stride,
+                                    o_row_stride, scale, (cudaStream_t)stream);
+  });
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 
@@ -379,7 +364,7 @@ int control_inject(int n, void* const* dst, const void* const* res, const int64_
   a.scales = scales;
   a.n = n;
   a.rows = rows;
-  const cudaError_t e = pww::ctl::launch_inject<E>(a, (int64_t)pww::tc::num_sms() * 8, (cudaStream_t)stream);
+  const cudaError_t e = pww::ctl::launch_inject<E>(a, (int64_t)pww::num_sms() * 8, (cudaStream_t)stream);
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 

@@ -74,4 +74,39 @@ __device__ __forceinline__ bool image_is_max(const XattnParams<E>& p, int b) {
 template <typename E>
 __device__ __forceinline__ float image_g(const XattnParams<E>& p, int b) { return __ldg(p.g_sigma + (int64_t)b * p.g_stride); }
 
+// ---- host side of the launchers: per-device state, keyed by the current device (the Python shim makes the tensors'
+// device current) ----
+constexpr int kMaxDevices = 64;
+inline int cur_device() {
+  int dev = 0;
+  cudaGetDevice(&dev);
+  return (dev >= 0 && dev < kMaxDevices) ? dev : 0;
+}
+inline int num_sms() {
+  static int n[kMaxDevices] = {0};
+  const int dev = cur_device();
+  if (!n[dev]) cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev);
+  return n[dev];
+}
+// Lets Kernel take `bytes` of dynamic shared memory; the attribute is set once per device.
+template <auto Kernel>
+cudaError_t allow_dynamic_smem(uint32_t bytes) {
+  static bool done[kMaxDevices] = {false};
+  const int dev = cur_device();
+  if (done[dev]) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  if (e == cudaSuccess) done[dev] = true;
+  return e;
+}
+
+// The image order of the host schedule replays: img[0, nb) = the images with a weight map (wmap_index[b] >= 0), then
+// img[nb, B) = the others, each in batch order.  Returns nb.  The kernels build the same order with warp ballots.
+inline int partition_images(int B, const int* wmap_index, int* img) {
+  int nb = 0;
+  for (int b = 0; b < B; ++b) if (wmap_index[b] >= 0) img[nb++] = b;
+  int nu = 0;
+  for (int b = 0; b < B; ++b) if (wmap_index[b] < 0) img[nb + nu++] = b;
+  return nb;
+}
+
 }  // namespace pww

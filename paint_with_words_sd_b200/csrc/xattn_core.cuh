@@ -98,8 +98,8 @@ __device__ __forceinline__ void warp_store(const float (&o)[Tile<D>::NT][4], uns
 // ---- key chunks: T <= 80 is one chunk of T keys; T = 154, 231 are 2 / 3 CLIP chunks of 77 ----
 // Chunk c (keys 77 c .. 77 c + kv - 1) is staged as its own 80-row K / V tile, rows kv .. 79 zero-filled and masked to
 // -inf, so warp_qk runs unchanged on every chunk.  The softmax streams over the chunks (running row max and sum, O
-// rescaled when the max moves, as in attn_tc.cuh); P is packed to E and the row sum is the sum of the E-rounded P values
-// that were multiplied, rescaled in fp32.  The first chunk's rescale factor is ex2(-inf * scale) = 0 (scale > 0), so a
+// rescaled when the max moves; attn_tc.cuh streams its 64-key tiles through the same block); P is packed to E and the row
+// sum is the sum of the E-rounded P values that were multiplied, rescaled in fp32.  The first chunk's rescale factor is ex2(-inf * scale) = 0 (scale > 0), so a
 // single chunk gives exactly the one-pass softmax.
 constexpr int kChunk = 77;      // keys per CLIP chunk
 constexpr int kMaxChunks = 3;
@@ -136,15 +136,16 @@ __device__ __forceinline__ void warp_online_begin(float (&o)[Tile<D>::NT][4], fl
   l0 = l1 = 0.f;
 }
 
-// One chunk: s holds S + bias of the chunk's 80 padded keys, of which the first kv are real; vs is its V tile.  l0 / l1
-// are per-thread partial row sums.
-template <int D, typename E>
-__device__ __forceinline__ void warp_online_chunk(float (&s)[10][4], int kv, float sl2, uint32_t vs, int lane,
+// One key tile of NJ n-tiles (10: a cross-attention chunk of 80 padded keys; 8: a self-attention tile of 64): s holds
+// S (+ bias) of the tile, of which the first kv keys are real; vs is its V tile.  l0 / l1 are per-thread partial row sums.
+template <int D, typename E, int NJ>
+__device__ __forceinline__ void warp_online_chunk(float (&s)[NJ][4], int kv, float sl2, uint32_t vs, int lane,
                                                   float (&o)[Tile<D>::NT][4], float& m0, float& m1, float& l0, float& l1) {
+  static_assert(NJ % 2 == 0, "P V takes two n-tiles of P per k-step");
   using C = Tile<D>;
   float t0 = -INFINITY, t1 = -INFINITY;
 #pragma unroll
-  for (int j = 0; j < 10; ++j)
+  for (int j = 0; j < NJ; ++j)
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       if (tok(j, e, lane) >= kv) s[j][e] = -INFINITY;
@@ -158,10 +159,10 @@ __device__ __forceinline__ void warp_online_chunk(float (&s)[10][4], int kv, flo
   const float a0 = ptx::ex2((m0 - mn0) * sl2), a1 = ptx::ex2((m1 - mn1) * sl2);   // 0 on the first chunk (m = -inf)
   m0 = mn0; m1 = mn1;
   const float n0 = -mn0 * sl2, n1 = -mn1 * sl2;
-  uint32_t pa[5][4];
+  uint32_t pa[NJ / 2][4];
   float r0 = 0.f, r1 = 0.f;
 #pragma unroll
-  for (int j = 0; j < 10; ++j) {
+  for (int j = 0; j < NJ; ++j) {
     const uint32_t p01 = ptx::pack2<E>(ptx::ex2(fmaf(s[j][0], sl2, n0)), ptx::ex2(fmaf(s[j][1], sl2, n0)));
     const uint32_t p23 = ptx::pack2<E>(ptx::ex2(fmaf(s[j][2], sl2, n1)), ptx::ex2(fmaf(s[j][3], sl2, n1)));
     const float2 f01 = ptx::unpack2<E>(p01), f23 = ptx::unpack2<E>(p23);    // sum exactly what the MMA multiplies
@@ -177,7 +178,7 @@ __device__ __forceinline__ void warp_online_chunk(float (&s)[10][4], int kv, flo
     o[j][0] *= a0; o[j][1] *= a0; o[j][2] *= a1; o[j][3] *= a1;
   }
 #pragma unroll
-  for (int kk = 0; kk < 5; ++kk) {
+  for (int kk = 0; kk < NJ / 2; ++kk) {
     const int t = 16 * kk + (lane & 7) + ((lane >> 3) & 1) * 8;
 #pragma unroll
     for (int jp = 0; jp < C::NT / 2; ++jp) {

@@ -30,10 +30,12 @@
 // 64 bytes per row instead of 308).  The kernel rebuilds W[n, t] = hi + lo in fp32 (exact to 2^-22 relative) from the row
 // tile's 8 KB of packed map in shared memory and adds x * W to the fp32 scores.
 #pragma once
+#include <algorithm>
+#include <vector>
+
 #include "mma_sm90.cuh"
 #include "pww_common.cuh"
 #include "xattn_core.cuh"
-#include "xattn_tc.cuh"      // num_sms, cur_device, tc_error_buf
 
 namespace pww {
 namespace fx {
@@ -569,7 +571,7 @@ inline int& debug_grid() {          // test infrastructure: cap the persistent g
   return g;
 }
 inline int fused_grid(int units) {
-  int g = tc::num_sms();
+  int g = num_sms();
   if (debug_grid() > 0 && debug_grid() < g) g = debug_grid();
   return units < g ? units : g;
 }
@@ -584,10 +586,10 @@ inline size_t fused_workspace_bytes() {
 }
 
 inline int fused_cta_has_image_host(int cta, int grid, int B, int H, int tiles, const int* wmap_index, int b) {
-  int nb = 0, pos = -1;
-  for (int i = 0; i < B; ++i)
-    if (wmap_index[i] >= 0) { if (i == b) pos = nb; ++nb; }
-  if (pos < 0) return 0;
+  std::vector<int> img(B > 0 ? B : 0);
+  const int nb = partition_images(B, wmap_index, img.data());
+  const int pos = (int)(std::find(img.begin(), img.begin() + nb, b) - img.begin());   // b's place among the biased images
+  if (pos == nb) return 0;
   const int nu = B - nb, np = nb < nu ? nb : nu;
   return fx_cta_has_image(cta, grid, B * H * tiles, pos, H, tiles, np) ? 1 : 0;
 }
@@ -614,12 +616,8 @@ cudaError_t launch_fused2(const XattnParams<E>& x, const void* mpack, int64_t mp
   fp.grid = fused_grid(fp.units);
   fp.jobs_dump = debug_jobs_dump();
   if (!fused2_fits(x.B, fp.hg, fp.tiles, fp.grid)) return cudaErrorInvalidConfiguration;
-  static bool attr_set[tc::kMaxDevices] = {false};
-  if (!attr_set[tc::cur_device()]) {
-    cudaError_t e = cudaFuncSetAttribute(xattn_fused2_kernel<D, KC, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, CF::SMEM);
-    if (e != cudaSuccess) return e;
-    attr_set[tc::cur_device()] = true;
-  }
+  const cudaError_t e = allow_dynamic_smem<xattn_fused2_kernel<D, KC, E>>(CF::SMEM);
+  if (e != cudaSuccess) return e;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(fp.grid);
@@ -639,10 +637,7 @@ cudaError_t launch_fused2(const XattnParams<E>& x, const void* mpack, int64_t mp
 inline int fused2_schedule_host(int B, int H, int G, int tiles, int grid, const int* wmap_index, int* out, int max_jobs) {
   if (B <= 0 || B > kMaxBatch || H <= 0 || G <= 0 || tiles <= 0 || grid <= 0) return -1;
   int img[kMaxBatch];
-  int nb = 0;
-  for (int b = 0; b < B; ++b) if (wmap_index[b] >= 0) img[nb++] = b;
-  int nu = 0;
-  for (int b = 0; b < B; ++b) if (wmap_index[b] < 0) img[nb + nu++] = b;
+  const int nb = partition_images(B, wmap_index, img);
   const int hg = (H + G - 1) / G;
   const int units = B * hg * tiles;
   int row = 0;

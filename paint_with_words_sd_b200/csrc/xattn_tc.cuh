@@ -364,37 +364,12 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams
 // ---------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------
-// Diagnostics of the last host-side failure in the launchers (read by pww_abi.cu into pww_last_cuda_error()).
-inline char* tc_error_buf() {
-  static thread_local char buf[256] = "";
-  return buf;
-}
-
-// Per-device host state: the current device decides (the Python shim makes the tensors' device current).
-constexpr int kMaxDevices = 64;
-inline int cur_device() {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  return (dev >= 0 && dev < kMaxDevices) ? dev : 0;
-}
-inline int num_sms() {
-  static int n[kMaxDevices] = {0};
-  const int dev = cur_device();
-  if (!n[dev]) cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev);
-  return n[dev];
-}
-
-inline int stats_grid(int units) { return units < num_sms() ? units : num_sms(); }
-
 // Host replay of the forward kernel's unit schedule (test infrastructure): the same FwdWalk / cta_range code, executed
 // on the CPU.  out[u] = {cta, it, b, h, tile} for every unit in launch order of each CTA.
 inline int fwd_schedule_host(int B, int H, int tiles, int grid, const int* wmap_index, int* out) {
   if (B <= 0 || B > kMaxBatch || H <= 0 || tiles <= 0 || grid <= 0) return -1;
   int img[kMaxBatch];
-  int nb = 0;
-  for (int b = 0; b < B; ++b) if (wmap_index[b] >= 0) img[nb++] = b;
-  int nu = 0;
-  for (int b = 0; b < B; ++b) if (wmap_index[b] < 0) img[nb + nu++] = b;
+  const int nb = partition_images(B, wmap_index, img);
   const long long units = (long long)B * H * tiles;
   int row = 0;
   for (int cta = 0; cta < grid; ++cta) {
@@ -411,43 +386,23 @@ inline int fwd_schedule_host(int B, int H, int tiles, int grid, const int* wmap_
   return row;
 }
 
-template <int D>
-cudaError_t set_smem(const void* fn, uint32_t bytes, bool (&done)[kMaxDevices]) {
-  if (done[cur_device()]) return cudaSuccess;
-  cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-  if (e == cudaSuccess) done[cur_device()] = true;
-  return e;
-}
-
-template <int D, int KC, typename E>
-cudaError_t launch_fwd(const XattnParams<E>& x, cudaStream_t s) {
+// One persistent launch of either kernel of the pair: a CTA per SM, or per unit when there are fewer units.
+template <auto Kernel, int D, int KC, typename E>
+cudaError_t launch(const XattnParams<E>& x, cudaStream_t s) {
   TcParams<E> tp;
   tp.x = x;
   tp.tiles = ceil_div(x.N, kBM);
   tp.units = x.B * tp.tiles * x.H;
-  static bool attr_set[kMaxDevices] = {false};
-  cudaError_t e = set_smem<D>((const void*)xattn_fwd_kernel<D, KC, E>, Cfg<D, KC>::SMEM, attr_set);
+  const cudaError_t e = allow_dynamic_smem<Kernel>(Cfg<D, KC>::SMEM);
   if (e != cudaSuccess) return e;
   const int grid = tp.units < num_sms() ? tp.units : num_sms();
-  xattn_fwd_kernel<D, KC, E><<<grid, kThreads, Cfg<D, KC>::SMEM, s>>>(tp);
+  Kernel<<<grid, kThreads, Cfg<D, KC>::SMEM, s>>>(tp);
   return cudaGetLastError();
 }
-
 template <int D, int KC, typename E>
-cudaError_t launch_stats(const XattnParams<E>& x, cudaStream_t s) {
-  TcParams<E> tp;
-  tp.x = x;
-  tp.tiles = ceil_div(x.N, kBM);
-  tp.units = x.B * tp.tiles * x.H;
-  static bool attr_set[kMaxDevices] = {false};
-  cudaError_t e = set_smem<D>((const void*)xattn_stats_kernel<D, KC, E>, Cfg<D, KC>::SMEM, attr_set);
-  if (e != cudaSuccess) return e;
-  xattn_stats_kernel<D, KC, E><<<stats_grid(tp.units), kThreads, Cfg<D, KC>::SMEM, s>>>(tp);
-  return cudaGetLastError();
-}
-
-// partial slots the stats kernel writes per image
-inline int stats_slots() { return num_sms(); }
+cudaError_t launch_fwd(const XattnParams<E>& x, cudaStream_t s) { return launch<xattn_fwd_kernel<D, KC, E>, D, KC>(x, s); }
+template <int D, int KC, typename E>
+cudaError_t launch_stats(const XattnParams<E>& x, cudaStream_t s) { return launch<xattn_stats_kernel<D, KC, E>, D, KC>(x, s); }
 
 }  // namespace tc
 }  // namespace pww

@@ -39,11 +39,6 @@ def is_fast(x: torch.Tensor) -> bool:
     return ENABLED and x.is_cuda and x.dtype in (torch.float16, torch.bfloat16)
 
 
-def _entry(name: str, x: torch.Tensor):
-    """The C entry point `name` (without its type suffix) for x's element type."""
-    return getattr(_native.lib(), name + ("_bf16" if x.dtype == torch.bfloat16 else "_f16"))
-
-
 def group_norm_nhwc(x: torch.Tensor, gn: torch.nn.GroupNorm, add: Optional[torch.Tensor] = None,
                     silu: bool = True) -> torch.Tensor:
     """x: [B,C,H,W] fp16 or bf16 in channels-last memory, gn's parameters of the same type.  Returns
@@ -60,7 +55,7 @@ def group_norm_nhwc(x: torch.Tensor, gn: torch.nn.GroupNorm, add: Optional[torch
         if add.dtype != x.dtype or add.stride(-1) != 1 or (add.stride(0) % 8) or (add.data_ptr() % 16):
             add = add.to(x.dtype).contiguous()
         add_bs = add.stride(0)
-    fn = _entry("pww_groupnorm_nhwc", x)
+    fn = _native.entry("pww_groupnorm_nhwc", x.dtype)
     with torch.cuda.device(x.device):
         rc = fn(x.data_ptr(), None if add is None else add.data_ptr(), add_bs, gn.weight.data_ptr(),
                 gn.bias.data_ptr(), y.data_ptr(), B, H * W, C, gn.num_groups, float(gn.eps),
@@ -77,7 +72,7 @@ def geglu(h: torch.Tensor) -> torch.Tensor:
     I = h.shape[-1] // 2
     M = h.numel() // h.shape[-1]
     out = torch.empty(h.shape[:-1] + (I,), dtype=h.dtype, device=h.device)
-    fn = _entry("pww_geglu", h)
+    fn = _native.entry("pww_geglu", h.dtype)
     with torch.cuda.device(h.device):
         rc = fn(h.data_ptr(), out.data_ptr(), M, I, torch.cuda.current_stream(h.device).cuda_stream)
     _native.check(rc, fn.__name__)
@@ -96,7 +91,7 @@ def add_layer_norm(x: torch.Tensor, res: Optional[torch.Tensor], ln: torch.nn.La
     M = x.numel() // C
     y = torch.empty_like(x)
     s = torch.empty_like(x) if (res is not None and want_sum) else None
-    fn = _entry("pww_add_layernorm", x)
+    fn = _native.entry("pww_add_layernorm", x.dtype)
     with torch.cuda.device(x.device):
         rc = fn(x.data_ptr(), None if res is None else res.data_ptr(), ln.weight.data_ptr(), ln.bias.data_ptr(),
                 None if s is None else s.data_ptr(), y.data_ptr(), M, C, float(ln.eps),
@@ -131,7 +126,7 @@ def control_inject(dst, res, scales: Optional[torch.Tensor] = None) -> None:
                                or not scales.is_contiguous() or scales.device != dst[0].device):
         raise ValueError(f"control scales must be a contiguous fp32 [{n}, {rows}] tensor on {dst[0].device}")
     d0 = dst[0]
-    fn = _entry("pww_control_inject", d0)
+    fn = _native.entry("pww_control_inject", d0.dtype)
     ptrs = (ctypes.c_void_p * n)(*[d.data_ptr() for d in dst])
     rptrs = (ctypes.c_void_p * n)(*[r.data_ptr() for r in res])
     elems = (ctypes.c_int64 * n)(*[d[0].numel() for d in dst])

@@ -317,6 +317,25 @@ int pww_control_inject_f16(int n, void* const* dst, const void* const* res, cons
 int pww_control_inject_bf16(int n, void* const* dst, const void* const* res, const int64_t* elems_per_image, int rows,
                             const float* scales, void* stream);
 
+/*
+ * Multi-ControlNet residual combine: the n (1..16) residuals of each of `units` (1..10) ControlNets, scaled and summed
+ * level by level in unit order, in one launch.
+ *   out_k[b] = E( ... E( E(s[0,k,b] * res_{0,k}[b]) + E(s[1,k,b] * res_{1,k}[b]) ) ... + E(s[U-1,k,b] * res_{U-1,k}[b]) )
+ *                                                                                             k < n, b < rows
+ * out[k] and res[u * n + k] (unit-major, units * n entries) point at dense [rows, elems_per_image[k]] tensors.  out[k]
+ * may be the same buffer as any res[u * n + k] (in place into one unit's residuals); partial overlaps are undefined.
+ * `scales` is a device fp32 [units, n, rows] array.  Every product and partial sum is rounded to E, so the result is
+ * bitwise torch's left-to-right sum of `(r * s).to(E)` in E; passing it to pww_control_inject with a NULL scale then
+ * adds it unchanged.  out, res and elems_per_image are HOST arrays; the table travels in the kernel parameters, so a
+ * captured CUDA graph carries it.
+ * Returns PWW_ERR_BAD_ARG, before any CUDA call, for units outside 1..10, n outside 1..16, rows < 1, a NULL scales, an
+ * elems_per_image entry that is not a positive multiple of 8, or a null or not 16-byte-aligned pointer.
+ */
+int pww_control_combine_f16(int units, int n, void* const* out, const void* const* res,
+                            const int64_t* elems_per_image, int rows, const float* scales, void* stream);
+int pww_control_combine_bf16(int units, int n, void* const* out, const void* const* res,
+                             const int64_t* elems_per_image, int rows, const float* scales, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -28,6 +28,7 @@ EXPORTS = (
     "pww_xattn_stats_multi_bf16", "pww_xattn_fwd_multi_bf16", "pww_xattn_fused_multi_bf16",
     "pww_attn_fwd_bf16", "pww_groupnorm_nhwc_bf16", "pww_geglu_bf16", "pww_add_layernorm_bf16",
     "pww_control_inject_f16", "pww_control_inject_bf16",
+    "pww_control_combine_f16", "pww_control_combine_bf16",
 )
 
 
@@ -91,6 +92,10 @@ def lib() -> ctypes.CDLL:
     L.pww_control_inject_f16.restype = c_i
     L.pww_control_inject_f16.argtypes = [c_i, ctypes.POINTER(c_vp), ctypes.POINTER(c_vp), ctypes.POINTER(c_i64), c_i,
                                          c_vp, c_vp]
+    # units, n, out[n], res[units * n], elems_per_image[n] (host arrays), rows, scales (device [units, n, rows]), stream
+    L.pww_control_combine_f16.restype = c_i
+    L.pww_control_combine_f16.argtypes = [c_i, c_i, ctypes.POINTER(c_vp), ctypes.POINTER(c_vp), ctypes.POINTER(c_i64),
+                                          c_i, c_vp, c_vp]
     # every _bf16 entry point takes its _f16 twin's arguments
     for name in EXPORTS:
         if name.endswith("_bf16"):

@@ -9,6 +9,7 @@
 #include "unet_ops.cuh"
 #include "sampler_step.cuh"
 #include "control_inject.cuh"
+#include "control_combine.cuh"
 #include <stdlib.h>
 #include <algorithm>
 #include <type_traits>
@@ -368,6 +369,34 @@ int control_inject(int n, void* const* dst, const void* const* res, const int64_
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 
+template <typename E>
+int control_combine(int units, int n, void* const* out, const void* const* res, const int64_t* elems_per_image,
+                    int rows, const float* scales, void* stream) {
+  if (units < 1 || units > pww::ctl::kMaxUnits || n < 1 || n > pww::ctl::kMaxLevels || rows < 1 || !out || !res ||
+      !elems_per_image || !scales)
+    return PWW_ERR_BAD_ARG;
+  pww::ctl::CombineArgs a = {};
+  for (int k = 0; k < n; ++k) {
+    const int64_t e = elems_per_image[k];
+    if (e <= 0 || (e % pww::ctl::kVec) != 0) return PWW_ERR_BAD_ARG;
+    if (!out[k] || !aligned16(out[k])) return PWW_ERR_BAD_ARG;
+    a.out[k] = out[k];
+    a.vec_per_image[k] = e / pww::ctl::kVec;
+    a.off[k + 1] = a.off[k] + (int64_t)rows * a.vec_per_image[k];
+  }
+  for (int i = 0; i < units * n; ++i) {
+    if (!res[i] || !aligned16(res[i])) return PWW_ERR_BAD_ARG;
+    a.res[i] = res[i];
+  }
+  for (int k = n; k < pww::ctl::kMaxLevels; ++k) a.off[k + 1] = a.off[n];
+  a.scales = scales;
+  a.units = units;
+  a.n = n;
+  a.rows = rows;
+  const cudaError_t e = pww::ctl::launch_combine<E>(a, (int64_t)pww::num_sms() * 8, (cudaStream_t)stream);
+  return e == cudaSuccess ? PWW_OK : cuda_fail(e);
+}
+
 }  // namespace
 
 extern "C" {
@@ -575,6 +604,15 @@ int pww_control_inject_f16(int n, void* const* dst, const void* const* res, cons
 int pww_control_inject_bf16(int n, void* const* dst, const void* const* res, const int64_t* elems_per_image, int rows,
                             const float* scales, void* stream) {
   return control_inject<__nv_bfloat16>(n, dst, res, elems_per_image, rows, scales, stream);
+}
+
+int pww_control_combine_f16(int units, int n, void* const* out, const void* const* res,
+                            const int64_t* elems_per_image, int rows, const float* scales, void* stream) {
+  return control_combine<__half>(units, n, out, res, elems_per_image, rows, scales, stream);
+}
+int pww_control_combine_bf16(int units, int n, void* const* out, const void* const* res,
+                             const int64_t* elems_per_image, int rows, const float* scales, void* stream) {
+  return control_combine<__nv_bfloat16>(units, n, out, res, elems_per_image, rows, scales, stream);
 }
 
 // Test infrastructure (not declared in the public header): replay the forward kernel's unit schedule on the host.

@@ -1,5 +1,5 @@
 """Python wrappers for the fused channels-last UNet ops of libpww_b200 (GroupNorm[+add][+SiLU], GEGLU, add+LayerNorm)
-and the ControlNet residual injection.
+and the ControlNet residual injection and multi-ControlNet combine.
 
 Used by `unet.py` on CUDA fp16 or bf16 activations (the `_f16` / `_bf16` entry points, picked from x.dtype); the
 CPU/fp32 route of the same modules stays plain PyTorch (it is what the CPU reference arm runs).  No fallback on CUDA: a
@@ -135,3 +135,40 @@ def control_inject(dst, res, scales: Optional[torch.Tensor] = None) -> None:
                 torch.cuda.current_stream(d0.device).cuda_stream)
     _native.check(rc, fn.__name__)
     _native.launch_count += 1
+
+
+def control_combine(res_per_unit, scales: torch.Tensor, out=None) -> list:
+    """out_k = sum over units u, in order, of (res_per_unit[u][k] * scales[u, k, :, None, None, None]), each product and
+    partial sum rounded to the residuals' type, for every level k in ONE launch (`pww_control_combine_*`).  Every
+    unit gives n residuals [rows, C_k, h_k, w_k] of one element type and one memory format; `scales` is fp32
+    [units, n, rows] on their device.  `out` (n tensors like unit 0's) defaults to unit 0's residuals: the sum goes
+    in place.  Returns out."""
+    units = len(res_per_unit)
+    first = list(res_per_unit[0]) if units else []
+    n = len(first)
+    out = first if out is None else list(out)
+    if units < 1 or n < 1 or len(out) != n or any(len(r) != n for r in res_per_unit):
+        raise ValueError(f"control_combine needs n >= 1 residuals from each of >= 1 units and n outputs (got "
+                         f"{[len(r) for r in res_per_unit]} residuals, {len(out)} outputs)")
+    rows = int(first[0].shape[0])
+    for k in range(n):
+        ref = first[k]
+        for u, r in enumerate([res_per_unit[u][k] for u in range(units)] + [out[k]]):
+            if (tuple(r.shape) != tuple(ref.shape) or r.shape[0] != rows or r.dtype != ref.dtype
+                    or r.device != ref.device or not _same_dense_layout(ref, r)):
+                what = "output" if u == units else f"unit {u}'s residual"
+                raise ValueError(f"{what} {k} {tuple(r.shape)} {r.dtype} does not match unit 0's {tuple(ref.shape)} "
+                                 f"{ref.dtype} (same type, format, shape and device)")
+    d0 = first[0]
+    if (scales.dtype != torch.float32 or tuple(scales.shape) != (units, n, rows) or not scales.is_contiguous()
+            or scales.device != d0.device):
+        raise ValueError(f"control scales must be a contiguous fp32 [{units}, {n}, {rows}] tensor on {d0.device}")
+    fn = _native.entry("pww_control_combine", d0.dtype)
+    optrs = (ctypes.c_void_p * n)(*[o.data_ptr() for o in out])
+    rptrs = (ctypes.c_void_p * (units * n))(*[r.data_ptr() for unit in res_per_unit for r in unit])
+    elems = (ctypes.c_int64 * n)(*[r[0].numel() for r in first])
+    with torch.cuda.device(d0.device):
+        rc = fn(units, n, optrs, rptrs, elems, rows, scales.data_ptr(), torch.cuda.current_stream(d0.device).cuda_stream)
+    _native.check(rc, fn.__name__)
+    _native.launch_count += 1
+    return out

@@ -25,11 +25,11 @@ from PIL import Image
 
 from . import attention as _attention
 from .conditioning import _encode_text_color_inputs, _get_binary_mask, pack_weight_map, packed_key
-from . import _native
+from . import _native, fused_ops
 from .scheduler import (SIGMA_SCHEDULERS, EulerAncestralDiscreteScheduler, LMSDiscreteScheduler, history_length,
                         step_form)
 from .synthetic import IdentityVAE, RandomTextEncoder, SimpleWordTokenizer
-from .unet import UNet2DConditionModel, UNetConfig, build_unet
+from .unet import UNet2DConditionModel, UNetConfig, build_unet, combine_control_residuals
 from .weight_function import STAT_MAX, UnsupportedWeightFunction, g_of_sigma, probe_weight_function
 
 
@@ -173,6 +173,39 @@ def control_step_active(i: int, n: int, start: float, end: float) -> bool:
     return start <= i / n <= end
 
 
+MAX_CONTROLNET_UNITS = 10      # the reference extension's "Multi ControlNet: Max models amount"
+
+
+def _control_units(controlnet, control_image, conditioning_scale, guess_mode, start, end) -> tuple:
+    """PwWSampler's ControlNet arguments as per-unit lists (nets, images, weights, guesses, starts, ends).  One
+    ControlNetModel is one unit with the arguments as they are.  A list of U (1..10) units takes `control_image` as a
+    list of U entries (each one tensor or one per image), `controlnet_conditioning_scale` as one float or U entries
+    (each one float or one per image), and `guess_mode` and the window each as one value or U values; lists are indexed
+    by unit first."""
+    if not isinstance(controlnet, (list, tuple)):
+        return [controlnet], [control_image], [conditioning_scale], [bool(guess_mode)], [start], [end]
+    U = len(controlnet)
+    if not 1 <= U <= MAX_CONTROLNET_UNITS:
+        raise ValueError(f"controlnet: a list of 1 to {MAX_CONTROLNET_UNITS} ControlNets, got {U}")
+    if not isinstance(control_image, (list, tuple)) or len(control_image) != U:
+        got = f"{len(control_image)} entries" if isinstance(control_image, (list, tuple)) else type(control_image).__name__
+        raise ValueError(f"control_image must be a list of {U} entries, one per ControlNet (each one [1, 3, H, W] "
+                         f"tensor or one per image), got {got}")
+
+    def per_unit(value, name, is_one):
+        if is_one(value):
+            return [value] * U
+        if not isinstance(value, (list, tuple)) or len(value) != U:
+            raise ValueError(f"{name} must be one value or a list of {U} (one per ControlNet), got {value!r}")
+        return list(value)
+    number = lambda v: isinstance(v, (int, float)) and not isinstance(v, bool)   # noqa: E731
+    weights = per_unit(conditioning_scale, "controlnet_conditioning_scale", number)
+    guesses = per_unit(guess_mode, "guess_mode", lambda v: isinstance(v, (bool, np.bool_)))
+    starts = per_unit(start, "control_guidance_start", number)
+    ends = per_unit(end, "control_guidance_end", number)
+    return list(controlnet), list(control_image), weights, [bool(g) for g in guesses], starts, ends
+
+
 def control_image_tensor(image: Image.Image) -> torch.Tensor:
     """A hint image as the ControlNet takes it: HWC RGB -> float / 255 -> [1, 3, H, W] in [0, 1] (no [-1, 1] remap)."""
     arr = np.asarray(image.convert("RGB"), dtype=np.float32) / 255.0
@@ -215,6 +248,14 @@ class PwWSampler:
     by 0.825 ** (12 - k) and only the cond half gets them (hook_pww.py:28-61, 128-132).  Step i of n is controlled iff
     `control_guidance_start <= i / n <= control_guidance_end`; the other steps replay a second graph without the
     ControlNet, captured only when some step needs it.
+
+    Multi-ControlNet (the extension's control units): `controlnet` a list of 1..10 ControlNetModels, `control_image` a
+    list with one entry per unit (each one tensor or m), and `controlnet_conditioning_scale`, `guess_mode` and the window
+    each one value or one per unit (a unit's weight may again be m floats).  A list of one is the single path above.
+    With several, the units active at a step run in unit order, their residuals scaled (0.825 ** (12 - k) for a unit in
+    guess mode) and summed level by level in ONE native combine, and the UNet adds the sum.  If any unit is in guess
+    mode, every unit runs on the m cond rows and only the cond half gets residuals (hook_pww.py:39-53, 199).  Each set
+    of active units over the run has its own captured graph.
     """
 
     def __init__(self, unet, scheduler: LMSDiscreteScheduler, cond_ctxs: Sequence[dict], uncond_ctxs: Sequence[dict],
@@ -282,57 +323,83 @@ class PwWSampler:
         self._step_no = 0
         self.controlnet = controlnet
         self.guess_mode = bool(guess_mode)
+        self._nets: List = []              # the ControlNet units, in unit order
+        self._active_sets = [()] * len(self.timesteps)      # step i -> which units run (one bool per unit)
         self._control_active = [False] * len(self.timesteps)
         if controlnet is None:
             if control_image is not None:
                 raise ValueError("control_image is given but controlnet is None")
         else:
-            self._set_up_control(control_image, controlnet_conditioning_scale, control_guidance_start,
-                                 control_guidance_end)
+            units = _control_units(controlnet, control_image, controlnet_conditioning_scale, guess_mode,
+                                   control_guidance_start, control_guidance_end)
+            if len(units[0]) == 1:
+                self.controlnet = units[0][0]
+            self._set_up_control(*units)
 
-    def _set_up_control(self, control_image, conditioning_scale, start: float, end: float):
-        """Validate the ControlNet arguments; embed the hints, build CONTROL_SCALES and the ControlNet's context."""
+    def _set_up_control(self, nets, images, weights, guesses, starts, ends):
+        """Validate every unit's ControlNet arguments (per-unit lists); embed the hints, build the scale tables and the
+        ControlNets' context.  One unit: CONTROL_SCALES for the UNet's inject.  Several: one [|A|, levels, rows] table
+        per active set A that occurs, for the combine."""
         from .controlnet import ControlNetModel
-        net, unet, m = self.controlnet, self.unet, self.m
-        if not isinstance(net, ControlNetModel):
-            raise TypeError(f"controlnet must be a paint_with_words_sd_b200.controlnet.ControlNetModel, got "
-                            f"{type(net).__name__}")
+        unet, m, U = self.unet, self.m, len(nets)
+        h, w = self.latents.shape[-2:]
         params = inspect.signature(unet.forward).parameters
         if "down_block_additional_residuals" not in params or "mid_block_additional_residual" not in params:
             raise TypeError(f"the UNet ({type(unet).__name__}) does not take down_block_additional_residuals / "
                             "mid_block_additional_residual, so it cannot take a controlnet")
-        ucfg, ccfg = getattr(unet, "config", None), net.config
-        for name in ("block_out_channels", "layers_per_block", "cross_attention_dim"):
-            if getattr(ucfg, name, None) != getattr(ccfg, name):
-                raise ValueError(f"controlnet config {name} = {getattr(ccfg, name)} does not match the UNet's "
-                                 f"{getattr(ucfg, name, None)}")
-        if ccfg.in_channels != 4:
-            raise ValueError(f"controlnet config in_channels = {ccfg.in_channels}: a ControlNet takes the 4 latent "
-                             "channels")
-        if not start <= end:
-            raise ValueError(f"control_guidance_start ({start}) must not exceed control_guidance_end ({end})")
-        if control_image is None:
-            raise ValueError("controlnet needs a control_image (one [1, 3, H, W] tensor per image)")
-        images = _per_image(control_image, m, "control_image", torch.is_tensor)
-        h, w = self.latents.shape[-2:]
-        for i, img in enumerate(images):
-            if tuple(img.shape) != (1, 3, 8 * h, 8 * w):
-                raise ValueError(f"control_image {i} is {tuple(img.shape)}; expected (1, 3, {8 * h}, {8 * w}): 8x the "
-                                 f"latent size {h}x{w}")
-        weights = _per_image(conditioning_scale, m, "controlnet_conditioning_scale",
-                             lambda s: isinstance(s, (int, float)) and not isinstance(s, bool))
+        ucfg = getattr(unet, "config", None)
+        for u, (net, start, end) in enumerate(zip(nets, starts, ends)):
+            def arg(name):           # the argument, with the unit's index when there are several
+                return name if U == 1 else f"{name}[{u}]"
+            if not isinstance(net, ControlNetModel):
+                raise TypeError(f"{arg('controlnet')} must be a paint_with_words_sd_b200.controlnet.ControlNetModel, "
+                                f"got {type(net).__name__}")
+            ccfg = net.config
+            for name in ("block_out_channels", "layers_per_block", "cross_attention_dim"):
+                if getattr(ucfg, name, None) != getattr(ccfg, name):
+                    raise ValueError(f"{arg('controlnet')} config {name} = {getattr(ccfg, name)} does not match the "
+                                     f"UNet's {getattr(ucfg, name, None)}")
+            if ccfg.in_channels != 4:
+                raise ValueError(f"{arg('controlnet')} config in_channels = {ccfg.in_channels}: a ControlNet takes the "
+                                 "4 latent channels")
+            if not start <= end:
+                raise ValueError(f"{arg('control_guidance_start')} ({start}) must not exceed "
+                                 f"{arg('control_guidance_end')} ({end})")
+            if images[u] is None:
+                raise ValueError(f"controlnet needs a {arg('control_image')} (one [1, 3, H, W] tensor per image)")
+            images[u] = _per_image(images[u], m, arg("control_image"), torch.is_tensor)
+            for i, img in enumerate(images[u]):
+                if tuple(img.shape) != (1, 3, 8 * h, 8 * w):
+                    raise ValueError(f"{arg('control_image')} {i} is {tuple(img.shape)}; expected (1, 3, {8 * h}, "
+                                     f"{8 * w}): 8x the latent size {h}x{w}")
+            weights[u] = _per_image(weights[u], m, arg("controlnet_conditioning_scale"),
+                                    lambda s: isinstance(s, (int, float)) and not isinstance(s, bool))
+        # guess-mode routing is global (hook_pww.py:39-53, 199): if any unit is in guess mode, every unit's residuals
+        # go to the cond half only, and every ControlNet runs on the m cond rows
+        self._nets, self.guess_mode = list(nets), any(guesses)
         n = len(self.timesteps)
-        self._control_active = [control_step_active(i, n, start, end) for i in range(n)]
+        self._active_sets = [tuple(control_step_active(i, n, s, e) for s, e in zip(starts, ends)) for i in range(n)]
+        self._control_active = [any(a) for a in self._active_sets]
         dev = self.device
-        with torch.no_grad():
-            emb = net.embed_condition(torch.cat([img.to(dev) for img in images], 0))     # once: step-invariant
-        if not self.guess_mode:
-            emb = torch.cat([emb, emb], 0)                                            # rows i and m + i share image i
-        self._hint = emb.contiguous(memory_format=torch.channels_last) if emb.is_cuda else emb
-        levels = len(net.controlnet_down_blocks) + 1
-        self._ctx["CONTROL_SCALES"] = control_scales(weights, self.guess_mode, levels).to(dev)
-        # the ControlNet's own dict: the plain text context (cond rows only in guess mode), no weight maps, so every
-        # cross-attention call is unbiased; its K/V are staged once like the UNet's
+        self._hints = []
+        for net, imgs in zip(nets, images):
+            with torch.no_grad():
+                emb = net.embed_condition(torch.cat([img.to(dev) for img in imgs], 0))     # once: step-invariant
+            if not self.guess_mode:
+                emb = torch.cat([emb, emb], 0)                                          # rows i and m + i share image i
+            self._hints.append(emb.contiguous(memory_format=torch.channels_last) if emb.is_cuda else emb)
+        rows = m if self.guess_mode else 2 * m
+        tables = [control_scales(wt, g, len(net.controlnet_down_blocks) + 1)[:, :rows]
+                  for net, wt, g in zip(nets, weights, guesses)]
+        if U == 1:
+            self._ctx["CONTROL_SCALES"] = tables[0].to(dev)
+        else:            # the scales are applied in the combine; the UNet adds the sum at scale 1
+            full = torch.stack(tables, 0)
+            self._combine_scales = {a: full[[u for u in range(U) if a[u]]].contiguous().to(dev)
+                                    for a in set(self._active_sets) if any(a)}
+        # the ControlNets' own dict: the plain text context (cond rows only in guess mode), no weight maps, so every
+        # cross-attention call is unbiased; its K/V are staged once like the UNet's (the cache is keyed by module, so
+        # the units share the dict, and a model that appears twice its K/V)
         text = self._ctx["CONTEXT_TENSOR"]
         self._control_ctx = {"CONTEXT_TENSOR": text[:m] if self.guess_mode else text,
                              "CROSS_ATTENTION_WEIGHT_ORIG": 0, "WEIGHT_FUNCTION": _zero_weight_function,
@@ -401,7 +468,12 @@ class PwWSampler:
         return ctx
 
     # -- one step, expressed only with device tensors / device scalars --------------------------
-    def _step_body(self, control: bool = False):
+    @property
+    def _hint(self) -> torch.Tensor:
+        """The single ControlNet's hint embedding (unit 0's with several)."""
+        return self._hints[0]
+
+    def _step_body(self, active: tuple = ()):
         m, (h, w) = self.m, self.latents.shape[-2:]
         L = _native.lib()
         stream = torch.cuda.current_stream(self.device).cuda_stream
@@ -414,12 +486,23 @@ class PwWSampler:
                                           self._unet_in.shape[1], h, w, stream), "pww_sampler_input")
         t = p[_T:_T + 1]
         residuals = {}
-        if control:
-            # the ControlNet sees the 4 latent channels of the UNet input (hook_pww.py:113-119), only the cond rows in
-            # guess mode (the uncond rows' residuals would be discarded)
+        if any(active):
+            # each active ControlNet sees the 4 latent channels of the UNet input (hook_pww.py:113-119), only the cond
+            # rows in guess mode (the uncond rows' residuals would be discarded)
             x = self._unet_in[:m, :4] if self.guess_mode else self._unet_in[:, :4]
-            down, mid = self.controlnet(x, t, encoder_hidden_states=self._control_ctx,
-                                        controlnet_cond_embedding=self._hint, return_dict=False)
+            outs = [net(x, t, encoder_hidden_states=self._control_ctx, controlnet_cond_embedding=hint,
+                        return_dict=False) for net, hint, on in zip(self._nets, self._hints, active) if on]
+            if len(self._nets) == 1:
+                down, mid = outs[0]
+            else:
+                # several units: their scaled residuals summed level by level in unit order (hook_pww.py:136-139), in
+                # place into the first active unit's, then added by the UNet at scale 1
+                per_unit = [list(d) + [md] for d, md in outs]
+                scales = self._combine_scales[active]
+                if fused_ops.is_fast(per_unit[0][0]):
+                    *down, mid = fused_ops.control_combine(per_unit, scales)
+                else:
+                    *down, mid = combine_control_residuals(per_unit, scales)
             residuals = {"down_block_additional_residuals": down, "mid_block_additional_residual": mid}
         eps = self.unet(self._unet_in, t, encoder_hidden_states=self._ctx, **residuals).sample
         if tuple(eps.shape) != (2 * m, 4, h, w) or eps.device != self.device:
@@ -486,17 +569,17 @@ class PwWSampler:
         i = self._step_no
         step_index = self.scheduler.step_index_of(self.timesteps[i])
         self._set_step_scalars(i, step_index)
-        control = self._control_active[i]
+        active = self._active_sets[i]
         if not self.use_graph:
-            self._step_body(control)
+            self._step_body(active)
         else:
-            # one graph for the steps with the ControlNet and one for those without, each captured at the first step
+            # one graph per set of active ControlNets (at most 2U + 1 over a run), each captured at the first step
             # that needs it; its two warm-up steps are undone, so the replay below is this step
-            if control not in self._graphs:
+            if active not in self._graphs:
                 snap = (self.latents.clone(), self._derivs.clone())
-                self._graphs[control] = self._capture(lambda: self._step_body(control), warmup=2)
+                self._graphs[active] = self._capture(lambda: self._step_body(active), warmup=2)
                 self.latents.copy_(snap[0]); self._derivs.copy_(snap[1])
-            self._graphs[control][0].replay()
+            self._graphs[active][0].replay()
         self._step_no += 1
 
     def _capture(self, fn: Callable[[], None], warmup: int) -> Tuple["torch.cuda.CUDAGraph", int]:
@@ -516,13 +599,20 @@ class PwWSampler:
 
     @property
     def native_launches_per_step(self) -> Optional[int]:
-        """Native launches of the captured step (the step with the ControlNet, if there is one); None until captured."""
-        return self._graphs.get(self.controlnet is not None, (None, None))[1]
+        """Native launches of the captured step (the step with every ControlNet, if there are any); None until
+        captured."""
+        return self._graphs.get((True,) * len(self._nets), (None, None))[1]
 
     @property
     def native_launches_per_step_without_control(self) -> Optional[int]:
         """Native launches of a ControlNet's captured step outside its window; None until captured or without one."""
-        return self._graphs.get(False, (None, None))[1] if self.controlnet is not None else None
+        return self._graphs.get((False,) * len(self._nets), (None, None))[1] if self._nets else None
+
+    @property
+    def native_launches_per_active_set(self) -> Dict[tuple, int]:
+        """Native launches of every captured step, keyed by its active set: one bool per ControlNet unit (() without
+        a ControlNet)."""
+        return {a: launches for a, (_, launches) in self._graphs.items()}
 
     def run(self, num_steps: Optional[int] = None) -> torch.Tensor:
         n = len(self.timesteps) - self._step_no if num_steps is None else num_steps
@@ -554,11 +644,11 @@ def paint_with_words(
     max_prompt_chunks: int = 1,
     torch_dtype: Optional[torch.dtype] = None,
     controlnet=None,
-    control_image: Optional[Image.Image] = None,
-    controlnet_conditioning_scale: float = 1.0,
-    guess_mode: bool = False,
-    control_guidance_start: float = 0.0,
-    control_guidance_end: float = 1.0,
+    control_image: Union[None, Image.Image, Sequence[Image.Image]] = None,
+    controlnet_conditioning_scale: Union[float, Sequence] = 1.0,
+    guess_mode: Union[bool, Sequence[bool]] = False,
+    control_guidance_start: Union[float, Sequence[float]] = 0.0,
+    control_guidance_end: Union[float, Sequence[float]] = 1.0,
 ):
     """paint_with_words.py:391-510.  Returns one PIL.Image (or the final latents with return_latents).
     `max_prompt_chunks` (1 .. 3): a prompt longer than 75 tokens fills up to that many 77-token CLIP chunks instead of
@@ -567,7 +657,10 @@ def paint_with_words(
     `preloaded_utils` the UNet's own dtype decides.
     ControlNet (the reference's PwW + ControlNet extension): `controlnet` from `pww_load_controlnet`, `control_image`
     a PIL image of the colour map's size (scribble, edges, pose, ...) that fixes the layout while the colour map says
-    which words go where; `controlnet_conditioning_scale`, `guess_mode` and the guidance window as in `PwWSampler`."""
+    which words go where; `controlnet_conditioning_scale`, `guess_mode` and the guidance window as in `PwWSampler`.
+    Several ControlNets (e.g. pose for the figure, edges for the background): `controlnet` a list of up to 10,
+    `control_image` a list with one such image per ControlNet, and the other four arguments one value or one per
+    ControlNet."""
     control = _control_arguments(controlnet, control_image, color_map_image.size, "color_map_image",
                                  controlnet_conditioning_scale, guess_mode, control_guidance_start,
                                  control_guidance_end)
@@ -632,17 +725,24 @@ def _result(vae, latents: torch.Tensor, return_latents: bool):
 def _control_arguments(controlnet, control_image, size: Tuple[int, int], size_of: str, conditioning_scale,
                        guess_mode: bool, start: float, end: float) -> dict:
     """PwWSampler's ControlNet keyword arguments from the public ones, {} without a controlnet; the hint image must be
-    `size` (W, H)."""
+    `size` (W, H).  With a list of ControlNets, `control_image` is a list of one such image per unit, and the other
+    arguments are one value or one per unit (`_control_units`)."""
     if controlnet is None:
         if control_image is not None:
             raise ValueError("control_image is given but controlnet is None")
         return {}
-    if not isinstance(control_image, Image.Image):
-        raise ValueError(f"controlnet needs a control_image (a PIL image of the {size_of} size {size}), got "
-                         f"{type(control_image).__name__}")
-    if control_image.size != tuple(size):
-        raise ValueError(f"control_image is {control_image.size}; it must have the {size_of} size {tuple(size)}")
-    return dict(controlnet=controlnet, control_image=control_image_tensor(control_image),
+    multi = isinstance(controlnet, (list, tuple))
+    _control_units(controlnet, control_image, conditioning_scale, guess_mode, start, end)     # counts and lengths
+    images = list(control_image) if multi else [control_image]
+    for u, image in enumerate(images):
+        name = f"control_image[{u}]" if multi else "control_image"
+        if not isinstance(image, Image.Image):
+            raise ValueError(f"controlnet needs a {name} (a PIL image of the {size_of} size {size}), got "
+                             f"{type(image).__name__}")
+        if image.size != tuple(size):
+            raise ValueError(f"{name} is {image.size}; it must have the {size_of} size {tuple(size)}")
+    tensors = [control_image_tensor(image) for image in images]
+    return dict(controlnet=controlnet, control_image=tensors if multi else tensors[0],
                 controlnet_conditioning_scale=conditioning_scale, guess_mode=guess_mode, control_guidance_start=start,
                 control_guidance_end=end)
 
@@ -697,9 +797,9 @@ def paint_with_words_batch(
     return_latents: bool = False,
     torch_dtype: Optional[torch.dtype] = None,
     controlnet=None,
-    guess_mode: bool = False,
-    control_guidance_start: float = 0.0,
-    control_guidance_end: float = 1.0,
+    guess_mode: Union[bool, Sequence[bool]] = False,
+    control_guidance_start: Union[float, Sequence[float]] = 0.0,
+    control_guidance_end: Union[float, Sequence[float]] = 1.0,
 ):
     """Many images, each with its own settings, in as few samplers as possible.  `settings[i]` is a dict of the
     per-image keyword arguments of `paint_with_words` (BATCH_SETTING_KEYS: color_context, color_map_image, input_prompt,
@@ -707,7 +807,9 @@ def paint_with_words_batch(
     controlnet_conditioning_scale); missing keys take paint_with_words's defaults.  Returns a list of PIL images (or
     [1,4,h,w] latents) in input order; image i equals `paint_with_words(**settings[i])` up to fp16 noise.
     With `controlnet` (one for the batch, with `guess_mode` and the guidance window) every entry needs a
-    `control_image` of its colour map's size; its `controlnet_conditioning_scale` is its own.
+    `control_image` of its colour map's size; its `controlnet_conditioning_scale` is its own.  With a list of
+    ControlNets (`guess_mode` and the window each one value or one per ControlNet), an entry's `control_image` is a list
+    of one image per ControlNet and its `controlnet_conditioning_scale` one float or one per ControlNet.
 
     Entries of the same latent size and text length run in one `PwWSampler` of at most `max_batch_size` images (a
     2 * max_batch_size UNet batch with CFG), whatever their weight functions and guidance scales.  The default of 8 gave
@@ -740,7 +842,16 @@ def paint_with_words_batch(
     results: List[Optional[torch.Tensor]] = [None] * len(entries)
     for idx in batch_groups(keys, max_batch_size):
         control = controls[idx[0]]
-        if control:       # the batch's ControlNet and window, each image's own hint and weight
+        if control and isinstance(controlnet, (list, tuple)):
+            # per unit u: the images' hints for u and their weights for u (an entry's one float is every unit's)
+            def unit_weight(s, u):
+                return s if isinstance(s, (int, float)) else s[u]
+            units = range(len(controlnet))
+            control = dict(control, control_image=[[controls[i]["control_image"][u] for i in idx] for u in units],
+                           controlnet_conditioning_scale=[
+                               [unit_weight(controls[i]["controlnet_conditioning_scale"], u) for i in idx]
+                               for u in units])
+        elif control:       # the batch's ControlNet and window, each image's own hint and weight
             control = dict(control, control_image=[controls[i]["control_image"] for i in idx],
                            controlnet_conditioning_scale=[controls[i]["controlnet_conditioning_scale"] for i in idx])
         sampler = PwWSampler(unet, scheduler, [encoded[i][0] for i in idx], [encoded[i][1] for i in idx],
@@ -805,11 +916,11 @@ def paint_with_words_inpaint(
     max_prompt_chunks: int = 1,
     torch_dtype: Optional[torch.dtype] = None,
     controlnet=None,
-    control_image: Optional[Image.Image] = None,
-    controlnet_conditioning_scale: float = 1.0,
-    guess_mode: bool = False,
-    control_guidance_start: float = 0.0,
-    control_guidance_end: float = 1.0,
+    control_image: Union[None, Image.Image, Sequence[Image.Image]] = None,
+    controlnet_conditioning_scale: Union[float, Sequence] = 1.0,
+    guess_mode: Union[bool, Sequence[bool]] = False,
+    control_guidance_start: Union[float, Sequence[float]] = 0.0,
+    control_guidance_end: Union[float, Sequence[float]] = 1.0,
 ):
     """paint_with_words_inpaint.py:137-270: 9-channel UNet input cat[latents, mask, masked-image latents].
     `max_prompt_chunks`, `torch_dtype` and the ControlNet arguments as in `paint_with_words`; the colour map is resized
@@ -866,7 +977,8 @@ class PaintWithWord_StableDiffusionPipeline:
 
     def __init__(self, vae, text_encoder, tokenizer, unet, scheduler=None, safety_checker=None, feature_extractor=None,
                  requires_safety_checker: bool = False, controlnet=None):
-        """`controlnet`: a `ControlNetModel` (`pww_load_controlnet`) every call that passes a `control_image` uses."""
+        """`controlnet`: a `ControlNetModel` (`pww_load_controlnet`), or a list of them, that every call passing a
+        `control_image` uses (with a list, `control_image` has one image per ControlNet)."""
         self.vae, self.text_encoder, self.tokenizer, self.unet = vae, text_encoder, tokenizer, unet
         self.safety_checker, self.feature_extractor = safety_checker, feature_extractor
         self.controlnet = controlnet

@@ -398,6 +398,20 @@ def add_control_residuals(targets: Sequence[torch.Tensor], residuals: Sequence[t
     return out
 
 
+def combine_control_residuals(res_per_unit: Sequence[Sequence[torch.Tensor]], scales: torch.Tensor) -> List[torch.Tensor]:
+    """The torch statement of `pww_control_combine`: level k is (res_0k * s[0, k]).to(E) + (res_1k * s[1, k]).to(E) +
+    ..., summed left to right in the residuals' type E (scales an fp32 [units, n, rows] tensor)."""
+    out = []
+    for k in range(len(res_per_unit[0])):
+        total = None
+        for u, unit in enumerate(res_per_unit):
+            r = unit[k]
+            p = (r * scales[u, k].to(r.device).view(r.shape[0], 1, 1, 1)).to(r.dtype)
+            total = p if total is None else total + p
+        out.append(total)
+    return out
+
+
 def _resnets(unet: nn.Module):
     return [m for m in unet.modules() if isinstance(m, ResnetBlock2D)]
 

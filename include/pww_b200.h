@@ -269,6 +269,17 @@ int pww_add_layernorm_f16(const void* x, const void* res, const void* gamma, con
 int pww_add_layernorm_bf16(const void* x, const void* res, const void* gamma, const void* beta, void* sum_out, void* y,
                            int64_t M, int C, float eps, void* stream);
 
+/* ResNet-block residual epilogue over [rows, C] channels-last activations:
+ *   out[r, c] = E( a[r, c] + h[r, c] + bias[c] )
+ * a is the block input (identity shortcut) or the bias-free shortcut conv output, h the bias-free conv2 output, bias an
+ * fp32 [C] array (conv2's bias plus the shortcut's).  fp32 arithmetic with one rounding.  out may be h (in place); it
+ * must not otherwise overlap a or h.  Returns PWW_ERR_BAD_ARG, before any CUDA call, for a null pointer, rows <= 0,
+ * C <= 0, C % 8 != 0 or a pointer that is not 16-byte aligned. */
+int pww_resnet_residual_f16(const void* a, const void* h, const float* bias, void* out, int64_t rows, int C,
+                            void* stream);
+int pww_resnet_residual_bf16(const void* a, const void* h, const float* bias, void* out, int64_t rows, int C,
+                             void* stream);
+
 /*
  * The sampler step around the UNet (LMS, Euler, Euler ancestral, DPM++ 2M), two launches per denoising step.
  * Latents are [m, 4, h, w] fp32 contiguous; dtype codes name the UNet's input / output type.

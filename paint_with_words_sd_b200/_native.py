@@ -29,6 +29,7 @@ EXPORTS = (
     "pww_attn_fwd_bf16", "pww_groupnorm_nhwc_bf16", "pww_geglu_bf16", "pww_add_layernorm_bf16",
     "pww_control_inject_f16", "pww_control_inject_bf16",
     "pww_control_combine_f16", "pww_control_combine_bf16",
+    "pww_resnet_residual_f16", "pww_resnet_residual_bf16",
 )
 
 
@@ -88,6 +89,8 @@ def lib() -> ctypes.CDLL:
     L.pww_geglu_f16.argtypes = [c_vp, c_vp, c_i64, c_i, c_vp]
     L.pww_add_layernorm_f16.restype = c_i
     L.pww_add_layernorm_f16.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i, c_f, c_vp]
+    L.pww_resnet_residual_f16.restype = c_i
+    L.pww_resnet_residual_f16.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i64, c_i, c_vp]
     # n, dst[n], res[n], elems_per_image[n] (host arrays), rows, scales (device [n, rows] fp32 or NULL), stream
     L.pww_control_inject_f16.restype = c_i
     L.pww_control_inject_f16.argtypes = [c_i, ctypes.POINTER(c_vp), ctypes.POINTER(c_vp), ctypes.POINTER(c_i64), c_i,

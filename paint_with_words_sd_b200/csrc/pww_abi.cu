@@ -326,7 +326,21 @@ int add_layernorm(const void* x, const void* res, const void* gamma, const void*
 }
 
 template <typename E>
-int attn_fwd(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int D, int64_t qkv_batch_stride,
+int resnet_residual(const void* a, const void* h, const float* bias, void* out, int64_t rows, int C, void* stream) {
+  if (!a || !h || !bias || !out || rows <= 0 || C <= 0 || (C & 7)) return PWW_ERR_BAD_ARG;
+  if (!aligned16(a) || !aligned16(h) || !aligned16(bias) || !aligned16(out)) return PWW_ERR_BAD_ARG;
+  const long long total = (long long)rows * (C >> 3);
+  long long blocks = (total + 255) / 256;
+  const long long cap = (long long)pww::num_sms() * 16;
+  if (blocks > cap) blocks = cap;
+  pww::uops::resnet_residual_kernel<E><<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(
+      (const E*)a, (const E*)h, bias, (E*)out, total, C >> 3);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? PWW_OK : cuda_fail(e);
+}
+
+template <typename E>
+int attn_fwd(const void* q,const void* k, const void* v, void* out, int B, int H, int N, int D, int64_t qkv_batch_stride,
              int64_t qkv_row_stride, int64_t o_batch_stride, int64_t o_row_stride, float scale, void* stream) {
   if (!q || !k || !v || !out || B <= 0 || H <= 0 || N <= 0 || D <= 0) return PWW_ERR_BAD_ARG;
   if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out)) return PWW_ERR_BAD_ARG;
@@ -554,6 +568,15 @@ int pww_add_layernorm_f16(const void* x, const void* res, const void* gamma, con
 int pww_add_layernorm_bf16(const void* x, const void* res, const void* gamma, const void* beta, void* sum_out, void* y,
     int64_t M, int C, float eps, void* stream) {
   return add_layernorm<__nv_bfloat16>(x, res, gamma, beta, sum_out, y, M, C, eps, stream);
+}
+
+int pww_resnet_residual_f16(const void* a, const void* h, const float* bias, void* out, int64_t rows, int C,
+                            void* stream) {
+  return resnet_residual<__half>(a, h, bias, out, rows, C, stream);
+}
+int pww_resnet_residual_bf16(const void* a, const void* h, const float* bias, void* out, int64_t rows, int C,
+                             void* stream) {
+  return resnet_residual<__nv_bfloat16>(a, h, bias, out, rows, C, stream);
 }
 
 int pww_sampler_input(const float* latents, const float* scale, const float* extra, void* out, int out_dtype, int m,

@@ -262,6 +262,35 @@ __global__ void add_layernorm_kernel(const E* __restrict__ x, const E* __restric
   }
 }
 
+// ResNet-block epilogue: out[r, c] = E(a[r, c] + h[r, c] + bias[c]) over [rows, C] channels-last activations, with
+// a = the block input (identity) or the bias-free shortcut conv output, h = the bias-free conv2 output and bias the fp32
+// sum of conv2's and the shortcut's biases.  fp32 arithmetic, one rounding.  `out` may alias `h` (each thread reads its
+// vector before it writes it), so neither carries __restrict__ or goes through the read-only cache.
+template <typename E>
+__global__ void resnet_residual_kernel(const E* a, const E* h, const float* __restrict__ bias, E* out,
+                                       long long total_vec, int nvec) {
+  using X = Elem<E>;
+  using E2 = typename X::E2;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total_vec;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int v = (int)(i % nvec);
+    const uint4 av = reinterpret_cast<const uint4*>(a)[i];
+    const uint4 hv = reinterpret_cast<const uint4*>(h)[i];
+    const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias) + 2 * v);
+    const float4 b1 = __ldg(reinterpret_cast<const float4*>(bias) + 2 * v + 1);
+    const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+    const E2* ah = reinterpret_cast<const E2*>(&av);
+    const E2* hh = reinterpret_cast<const E2*>(&hv);
+    __align__(16) E2 o[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float2 fa = X::to_float2(ah[k]), fh = X::to_float2(hh[k]);
+      o[k] = X::from_float2(fa.x + fh.x + bb[2 * k], fa.y + fh.y + bb[2 * k + 1]);
+    }
+    reinterpret_cast<uint4*>(out)[i] = *reinterpret_cast<const uint4*>(o);
+  }
+}
+
 inline int gn_chunks(int HW) {
   int rows = HW >= 4096 ? 64 : (HW >= 1024 ? 32 : 16);   // enough blocks to fill the SMs, few enough to finalise fast
   int c = (HW + rows - 1) / rows;

@@ -1,5 +1,5 @@
-"""Python wrappers for the fused channels-last UNet ops of libpww_b200 (GroupNorm[+add][+SiLU], GEGLU, add+LayerNorm)
-and the ControlNet residual injection and multi-ControlNet combine.
+"""Python wrappers for the fused channels-last UNet ops of libpww_b200 (GroupNorm[+add][+SiLU], GEGLU, add+LayerNorm,
+the ResNet residual epilogue) and the ControlNet residual injection and multi-ControlNet combine.
 
 Used by `unet.py` on CUDA fp16 or bf16 activations (the `_f16` / `_bf16` entry points, picked from x.dtype); the
 CPU/fp32 route of the same modules stays plain PyTorch (it is what the CPU reference arm runs).  No fallback on CUDA: a
@@ -99,6 +99,30 @@ def add_layer_norm(x: torch.Tensor, res: Optional[torch.Tensor], ln: torch.nn.La
     _native.check(rc, fn.__name__)
     _native.launch_count += 1
     return (x if res is None else s), y
+
+
+def resnet_residual(a: torch.Tensor, h: torch.Tensor, bias: torch.Tensor, out: Optional[torch.Tensor] = None):
+    """out = (a.float() + h.float() + bias[None, :, None, None]).to(E) in one launch (`pww_resnet_residual_*`): a ResNet
+    block's output from its identity or bias-free shortcut output `a` and its bias-free conv2 output `h`, both [B, C, H,
+    W] of one type E (fp16 or bf16), made channels-last if they are not.  `bias`: fp32 [C] (conv2's bias plus the
+    shortcut's).  `out` (channels-last) defaults to h (in place).  Returns out."""
+    cl = torch.channels_last
+    a, h = a.contiguous(memory_format=cl), h.contiguous(memory_format=cl)
+    out = h if out is None else out
+    C = h.shape[1]
+    if (tuple(a.shape) != tuple(h.shape) or tuple(out.shape) != tuple(h.shape) or a.dtype != h.dtype
+            or out.dtype != h.dtype or not all(t.is_contiguous(memory_format=cl) for t in (a, h, out))):
+        raise ValueError(f"resnet_residual needs a, h and out of one shape and type, channels-last (got "
+                         f"{tuple(a.shape)} {a.dtype}, {tuple(h.shape)} {h.dtype}, {tuple(out.shape)} {out.dtype})")
+    if bias.dtype != torch.float32 or tuple(bias.shape) != (C,) or not bias.is_contiguous() or bias.device != h.device:
+        raise ValueError(f"resnet_residual bias must be a contiguous fp32 [{C}] tensor on {h.device}")
+    fn = _native.entry("pww_resnet_residual", h.dtype)
+    with torch.cuda.device(h.device):
+        rc = fn(a.data_ptr(), h.data_ptr(), bias.data_ptr(), out.data_ptr(), h.numel() // C, C,
+                torch.cuda.current_stream(h.device).cuda_stream)
+    _native.check(rc, fn.__name__)
+    _native.launch_count += 1
+    return out
 
 
 def _same_dense_layout(a: torch.Tensor, b: torch.Tensor) -> bool:

@@ -196,13 +196,19 @@ class ResnetBlock2D(nn.Module):
 
     def forward(self, x, temb):
         if fused_ops.is_fast(x):
-            # GroupNorm+SiLU fused; the time-embedding add rides inside the second GroupNorm
-            h = self.conv1(fused_ops.group_norm_nhwc(x, self.norm1, silu=True))
+            # GroupNorm+SiLU fused; the convolutions run without bias, so no per-channel bias pass touches their outputs:
+            # conv1's bias rides with the time embedding into the second GroupNorm's add, conv2's and the shortcut's go
+            # into the residual epilogue
+            t_bias, res_bias = _block_biases(self)
+            h = self.conv1._conv_forward(fused_ops.group_norm_nhwc(x, self.norm1, silu=True), self.conv1.weight, None)
             t = getattr(self, "_pww_t", None)       # slice of the UNet-wide batched projection, when provided
             if t is None:
-                t = self.time_emb_proj(F.silu(temb))
-            h = self.conv2(fused_ops.group_norm_nhwc(h, self.norm2, add=t, silu=True))
-            return (x if self.conv_shortcut is None else self.conv_shortcut(x)) + h
+                t = F.linear(F.silu(temb), self.time_emb_proj.weight, t_bias)
+            h = self.conv2._conv_forward(fused_ops.group_norm_nhwc(h, self.norm2, add=t, silu=True), self.conv2.weight,
+                                         None)
+            sc = self.conv_shortcut
+            a = x if sc is None else sc._conv_forward(x, sc.weight, None)
+            return fused_ops.resnet_residual(a, h, res_bias)
         h = self.conv1(F.silu(self.norm1(x)))
         h = h + self.time_emb_proj(F.silu(temb))[:, :, None, None]
         h = self.conv2(F.silu(self.norm2(h)))
@@ -416,16 +422,41 @@ def _resnets(unet: nn.Module):
     return [m for m in unet.modules() if isinstance(m, ResnetBlock2D)]
 
 
+def _param_key(params) -> tuple:
+    """Cache key of tensors derived from `params`: their storage and version counters, so an in-place update
+    (load_state_dict, a weight broadcast after a first forward) invalidates the derived tensors."""
+    return tuple((p.data_ptr(), p._version, p.dtype, p.device) for p in params)
+
+
+def _block_biases(block: ResnetBlock2D):
+    """The fast route's biases of one ResNet block: (time_emb_proj.bias + conv1.bias in the parameters' type, the
+    time-embedding projection's bias; conv2.bias + conv_shortcut.bias in fp32, the residual epilogue's).  Each sum is
+    taken in fp32 and rounded once; both are cached on the block, keyed on the biases' storage and version counters."""
+    sc = block.conv_shortcut
+    params = [block.time_emb_proj.bias, block.conv1.bias, block.conv2.bias] + ([] if sc is None else [sc.bias])
+    key = _param_key(params)
+    hit = block.__dict__.get("_pww_biases")
+    if hit is None or hit[0] != key:
+        tb = block.time_emb_proj.bias.float() + block.conv1.bias.float()
+        rb = block.conv2.bias.float() + (0.0 if sc is None else sc.bias.float())
+        hit = (key, tb.to(block.time_emb_proj.bias.dtype).detach(), rb.detach().contiguous())
+        block.__dict__["_pww_biases"] = hit
+    return hit[1], hit[2]
+
+
 def _project_time_embeddings(self, temb):
-    """All 22 ResNet `time_emb_proj(silu(temb))` projections as ONE GEMM; each block reads its column slice."""
-    cache = self.__dict__.get("_pww_temb_w")
+    """All 22 ResNet `time_emb_proj(silu(temb))` projections as ONE GEMM, each block's conv1 bias folded into its
+    projection bias (`_block_biases`); each block reads its column slice.  The concatenated weights and biases are
+    cached, keyed on the parameters' storage and version counters."""
     res = _resnets(self)
-    if cache is None or cache[0].device != temb.device or cache[0].dtype != temb.dtype:
+    key = _param_key([p for r in res for p in (r.time_emb_proj.weight, r.time_emb_proj.bias, r.conv1.bias)])
+    cache = self.__dict__.get("_pww_temb_w")
+    if cache is None or cache[0] != key:
         w = torch.cat([r.time_emb_proj.weight for r in res], 0).detach().contiguous()
-        b = torch.cat([r.time_emb_proj.bias for r in res], 0).detach().contiguous()
-        cache = (w, b)
+        b = torch.cat([_block_biases(r)[0] for r in res], 0).contiguous()
+        cache = (key, w, b)
         self.__dict__["_pww_temb_w"] = cache
-    t_all = F.linear(F.silu(temb), cache[0], cache[1])
+    t_all = F.linear(F.silu(temb), cache[1], cache[2])
     off = 0
     for r in res:
         n = r.time_emb_proj.weight.shape[0]

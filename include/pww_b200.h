@@ -244,8 +244,9 @@ int pww_attn_fwd_bf16(const void* q, const void* k, const void* v, void* out,
  *
  * GroupNorm over [B, HW, C] (channels last) with G groups:  y = act((x + add[b,c] - mean) * rstd * gamma + beta),
  * `add` ([B, C] with row stride `add_batch_stride`, may be NULL) is the ResNet block's time-embedding term (added before normalisation), act = SiLU when
- * `silu` != 0.  Needs C % 8 == 0, C % G == 0, G <= 64 and pww_groupnorm_workspace_bytes() of scratch that was
- * zero-filled once after allocation (self-cleaning arrival counters, like the attention statistics workspace).
+ * `silu` != 0.  Needs C % 8 == 0, C % G == 0, G <= 64 and pww_groupnorm_workspace_bytes() of scratch (any
+ * contents: the statistics launch writes every partial the apply launch reads).  The apply launch is a programmatic
+ * dependent of the statistics launch on `stream`.
  */
 size_t pww_groupnorm_workspace_bytes(int B, int HW, int G);
 int pww_groupnorm_nhwc_f16(const void* x, const void* add, int64_t add_batch_stride /* elements */,

@@ -266,30 +266,38 @@ int groupnorm_nhwc(const void* x, const void* add, int64_t add_batch_stride, con
   if ((C & 7) || (C % G) || G > 64 || (C >> 3) > 1024) return PWW_ERR_UNSUPPORTED;
   if (add && ((add_batch_stride & 7) || add_batch_stride < C)) return PWW_ERR_BAD_ARG;
   if (workspace_bytes < pww_groupnorm_workspace_bytes(B, HW, G)) return PWW_ERR_WORKSPACE;
+  const pww::uops::GnSplit sp = pww::uops::gn_split(HW, C, G);
   pww::uops::GnParams<E> p;
   p.x = (const E*)x; p.add = (const E*)add; p.add_bs = add_batch_stride; p.gamma = (const E*)gamma; p.beta = (const E*)beta;
   p.y = (E*)y;
-  char* w = (char*)workspace;
-  p.counters = (unsigned int*)w;
-  w += align_up((size_t)B * sizeof(unsigned int), 256);
-  p.stats = (float*)w;
-  w += align_up((size_t)B * G * 2 * sizeof(float), 256);
-  p.partial = (float*)w;
-  p.B = B; p.HW = HW; p.C = C; p.G = G; p.eps = eps; p.silu = silu;
-  p.chunks = pww::uops::gn_chunks(HW);
-  p.rows_per_chunk = (HW + p.chunks - 1) / p.chunks;
+  p.partial = (float2*)workspace;
+  p.HW = HW; p.C = C; p.G = G; p.eps = eps; p.silu = silu;
+  p.sv = sp.sv; p.chunks = sp.chunks; p.rows_per_chunk = sp.rows_per_chunk;
   cudaStream_t s = (cudaStream_t)stream;
-  const int nvec = C >> 3;
-  const int rpp = nvec >= 256 ? 1 : 256 / nvec;
-  const size_t smem1 = (size_t)rpp * C * 2 * sizeof(float);
-  if (smem1 > 48 * 1024) return PWW_ERR_UNSUPPORTED;
-  pww::uops::gn_stats_kernel<E><<<dim3(p.chunks, B), nvec * rpp, smem1, s>>>(p);
-  // enough row chunks to fill the machine even at 8x8 resolution
-  int rows_per_block = (int)(((long long)HW * B + 2 * pww::num_sms() - 1) / (2 * pww::num_sms()));
-  if (rows_per_block < rpp) rows_per_block = rpp;
-  if (rows_per_block > 32) rows_per_block = 32;
-  pww::uops::gn_apply_kernel<E><<<dim3((HW + rows_per_block - 1) / rows_per_block, B), nvec * rpp, 0, s>>>(p, rows_per_block);
-  cudaError_t e = cudaGetLastError();
+  // 64 group shifts + per-thread channel sums: 16 KB up to 256-vector slices, 64 KB at most (C = 8192, one group)
+  const size_t smem1 = (64 + (size_t)2 * sp.rpp * sp.sv * 8) * sizeof(float);
+  if (smem1 > 48 * 1024) {
+    const cudaError_t e = pww::allow_dynamic_smem<pww::uops::gn_stats_kernel<E>>(64 * 1024 + 256);
+    if (e != cudaSuccess) return cuda_fail(e);
+  }
+  pww::uops::gn_stats_kernel<E><<<dim3(sp.chunks, sp.slices, B), sp.threads, smem1, s>>>(p);
+  // rows per thread: 4, or fewer until the apply grid has two blocks per SM (the split of the apply pass does not
+  // change any result, so it may depend on B)
+  int rows = 4;
+  while (rows > 1 && (long long)B * sp.slices * pww::ceil_div(HW, sp.rpp * rows) < 2 * pww::num_sms()) rows >>= 1;
+  // Programmatic dependent launch: the apply grid starts while the stats grid runs and waits (griddepcontrol.wait)
+  // only before it reads the partials
+  cudaLaunchAttribute pdl;
+  pdl.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  pdl.val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(pww::ceil_div(HW, sp.rpp * rows), sp.slices, B);
+  cfg.blockDim = dim3(sp.threads);
+  cfg.stream = s;
+  cfg.attrs = &pdl;
+  cfg.numAttrs = 1;
+  cudaError_t e = cudaLaunchKernelEx(&cfg, pww::uops::gn_apply_kernel<E>, p, sp.rpp * rows);
+  if (e == cudaSuccess) e = cudaGetLastError();
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 
@@ -535,8 +543,9 @@ int pww_attn_fwd_bf16(const void* q, const void* k, const void* v, void* out, in
 
 size_t pww_groupnorm_workspace_bytes(int B, int HW, int G) {
   if (B <= 0 || HW <= 0 || G <= 0) return 0;
-  return align_up((size_t)B * sizeof(unsigned int), 256) + align_up((size_t)B * G * 2 * sizeof(float), 256) +
-         (size_t)B * pww::uops::gn_chunks(HW) * G * 2 * sizeof(float);
+  // gn_split never makes more than min(HW, kGnMaxChunks) row chunks, whatever C is
+  const size_t chunks = (size_t)std::min(HW, pww::uops::kGnMaxChunks);
+  return align_up((size_t)B * G * chunks * sizeof(float2), 256);
 }
 
 int pww_groupnorm_nhwc_f16(const void* x, const void* add, int64_t add_batch_stride, const void* gamma,

@@ -9,6 +9,9 @@
 namespace pww {
 namespace uops {
 
+// GroupNorm.  Both passes split an image into channel slices (whole groups AND whole 16-byte vectors: a multiple of
+// lcm(8, C/G) channels) and row chunks; a thread keeps one 8-channel vector column of its slice.  The split is a
+// function of (HW, C, G) only (gn_split), so batching never changes a result.
 template <typename E>
 struct GnParams {
   const E* x;      // [B, HW, C] channels-last activations
@@ -17,137 +20,177 @@ struct GnParams {
   const E* gamma;  // [C]
   const E* beta;   // [C]
   E* y;            // [B, HW, C]
-  float* partial;       // [B, chunks, G, 2] (sum, sumsq) scratch
-  float* stats;         // [B, G, 2] (mean, rstd), written by the last stats block of each image
-  unsigned int* counters;  // [B] arrival counters (zero on entry, zero on exit)
-  int B, HW, C, G, chunks, rows_per_chunk, silu;
+  float2* partial; // [B, G, chunks]: (sum, sum of squares) of x + add - shift over one row chunk
+  int HW, C, G, sv, chunks, rows_per_chunk, silu;   // sv: vectors per channel slice
   float eps;
 };
 
-// pass 1: per (image, row chunk) partial sums per group.  block = nvec * rpp threads (nvec = C/8 vectors per row)
+// The value the sums of group g (first channel c) of image b are taken about: the group's first element.  Shifted
+// sums keep E[d^2] - E[d]^2 accurate when |mean| >> std, where fp32 E[x^2] - mean^2 cancels.
 template <typename E>
-__global__ void gn_stats_kernel(GnParams<E> p) {
+__device__ __forceinline__ float gn_shift(const GnParams<E>& p, int b, int c) {
+  float s = Elem<E>::to_float(p.x[(size_t)b * p.HW * p.C + c]);
+  if (p.add) s += Elem<E>::to_float(p.add[(size_t)b * p.add_bs + c]);
+  return s;
+}
+
+// 16-byte vectors of rows r, r + rpp, r + 2 rpp, r + 3 rpp of one column (zero at and past r1): four loads in flight.
+__device__ __forceinline__ void gn_load4(uint4 (&xv)[4], const uint4* col, int stride_vec, int r, int rpp, int r1) {
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    const int rr = r + u * rpp;
+    xv[u] = rr < r1 ? __ldg(col + (size_t)rr * stride_vec) : make_uint4(0, 0, 0, 0);
+  }
+}
+
+// pass 1: grid (row chunk, channel slice, image).  Per-thread column sums -> shared memory -> one warp per group
+// reduces its rpp x C/G values (lanes in a fixed stride, then a shuffle tree) -> partial[b, g, chunk].
+template <typename E>
+__global__ void __launch_bounds__(1024) gn_stats_kernel(GnParams<E> p) {
   using X = Elem<E>;
   using E2 = typename X::E2;
-  extern __shared__ float sm[];                 // [rpp][C][2] staging for the cross-row reduction, then [G][2]
-  const int nvec = p.C >> 3;
-  const int rpp = blockDim.x / nvec;
-  const int v = threadIdx.x % nvec, rl = threadIdx.x / nvec;
-  const int b = blockIdx.y, chunk = blockIdx.x;
-  const int r0 = chunk * p.rows_per_chunk, r1 = min(p.HW, r0 + p.rows_per_chunk);
-  float s[8], q[8], a[8];
+  // let the apply pass (launched as a programmatic dependent) start its prologue; it waits for this grid's
+  // completion before it reads the partials
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  extern __shared__ float sm[];   // [64] group shifts, then [2][rpp][sv * 8] per-thread channel sums
+  const int cg = p.C / p.G, sv = p.sv, rpp = blockDim.x / sv, b = blockIdx.z;
+  const int v0 = blockIdx.y * sv, nv = min(sv, (p.C >> 3) - v0);   // the last slice may be narrower
+  const int c0 = v0 * 8, ng = nv * 8 / cg;
+  const int v = threadIdx.x % sv, rl = threadIdx.x / sv;
+  const bool lane_on = rl < rpp && v < nv;
+  const int r0 = blockIdx.x * p.rows_per_chunk;
+  const int r1 = lane_on ? min(p.HW, r0 + p.rows_per_chunk) : r0;
+  const uint4* col = reinterpret_cast<const uint4*>(p.x + (size_t)b * p.HW * p.C + c0) + v;
+  const int stride_vec = p.C >> 3;
+  uint4 xv[4];
+  gn_load4(xv, col, stride_vec, r0 + rl, rpp, r1);
+  float* s_shift = sm;
+  float* ss = sm + 64;
+  float* sq = ss + rpp * sv * 8;
+  if (threadIdx.x < ng) s_shift[threadIdx.x] = gn_shift(p, b, c0 + threadIdx.x * cg);
+  float o[8], s[8], q[8];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) { s[i] = 0.f; q[i] = 0.f; a[i] = 0.f; }
-  if (p.add) {
-    const uint4 av = *reinterpret_cast<const uint4*>(p.add + (size_t)b * p.add_bs + v * 8);
+  for (int i = 0; i < 8; ++i) { o[i] = 0.f; s[i] = 0.f; q[i] = 0.f; }
+  if (p.add && lane_on) {
+    const uint4 av = __ldg(reinterpret_cast<const uint4*>(p.add + (size_t)b * p.add_bs + c0) + v);
     const E2* ah = reinterpret_cast<const E2*>(&av);
 #pragma unroll
-    for (int i = 0; i < 4; ++i) { float2 f = X::to_float2(ah[i]); a[2 * i] = f.x; a[2 * i + 1] = f.y; }
+    for (int i = 0; i < 4; ++i) { const float2 f = X::to_float2(ah[i]); o[2 * i] = f.x; o[2 * i + 1] = f.y; }
   }
-  const E* xb = p.x + (size_t)b * p.HW * p.C;
-  // 4 independent 16-byte loads in flight per thread
-  for (int r = r0 + rl; r < r1; r += 4 * rpp) {
-    uint4 xv[4];
+  __syncthreads();
 #pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const int rr = r + u * rpp;
-      xv[u] = rr < r1 ? __ldg(reinterpret_cast<const uint4*>(xb + (size_t)rr * p.C) + v) : make_uint4(0, 0, 0, 0);
-    }
+  for (int i = 0; i < 8; ++i) o[i] -= s_shift[(v * 8 + i) / cg];   // < 64 for every thread: sv * 8 / cg <= G
+  for (int r = r0 + rl; r < r1; r += 4 * rpp) {
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       if (r + u * rpp < r1) {
         const E2* xh = reinterpret_cast<const E2*>(&xv[u]);
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-          float2 f = X::to_float2(xh[i]);
-          const float x0 = f.x + a[2 * i], x1 = f.y + a[2 * i + 1];
-          s[2 * i] += x0; q[2 * i] = fmaf(x0, x0, q[2 * i]);
-          s[2 * i + 1] += x1; q[2 * i + 1] = fmaf(x1, x1, q[2 * i + 1]);
+          const float2 f = X::to_float2(xh[i]);
+          const float d0 = f.x + o[2 * i], d1 = f.y + o[2 * i + 1];
+          s[2 * i] += d0; q[2 * i] = fmaf(d0, d0, q[2 * i]);
+          s[2 * i + 1] += d1; q[2 * i + 1] = fmaf(d1, d1, q[2 * i + 1]);
         }
       }
     }
+    if (r + 4 * rpp < r1) gn_load4(xv, col, stride_vec, r + 4 * rpp, rpp, r1);
   }
-  // per-thread channel sums -> shared [rl][c]
-  float* ss = sm;
-  float* sq = sm + rpp * p.C;
+  const int w8 = sv * 8;
+  if (lane_on) {
 #pragma unroll
-  for (int i = 0; i < 8; ++i) { ss[rl * p.C + v * 8 + i] = s[i]; sq[rl * p.C + v * 8 + i] = q[i]; }
-  __syncthreads();
-  // one thread per group reduces its channels over all row lanes in a fixed order
-  const int cg = p.C / p.G;
-  for (int g = threadIdx.x; g < p.G; g += blockDim.x) {
-    float ts = 0.f, tq = 0.f;
-    for (int r = 0; r < rpp; ++r)
-      for (int c = g * cg; c < (g + 1) * cg; ++c) { ts += ss[r * p.C + c]; tq += sq[r * p.C + c]; }
-    float* out = p.partial + (((size_t)b * p.chunks + chunk) * p.G + g) * 2;
-    out[0] = ts; out[1] = tq;
+    for (int i = 0; i < 8; ++i) { ss[rl * w8 + v * 8 + i] = s[i]; sq[rl * w8 + v * 8 + i] = q[i]; }
   }
-  // the last block of this image reduces the chunk partials in a fixed order -> (mean, rstd) per group
-  __shared__ int is_last;
-  __threadfence();
   __syncthreads();
-  if (threadIdx.x == 0) is_last = (atomicAdd(&p.counters[b], 1u) == (unsigned)p.chunks - 1u) ? 1 : 0;
-  __syncthreads();
-  if (!is_last) return;
-  __threadfence();
-  // only FULL warps finalise (blockDim.x = nvec * rpp need not be a multiple of 32: a trailing partial warp would
-  // alias warp 0's groups and shuffle with lanes that do not exist)
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-  for (int g = warp; warp < nwarps && g < p.G; g += nwarps) {
-    const float* pp = p.partial + ((size_t)b * p.chunks * p.G + g) * 2;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5, n = rpp * cg;
+  for (int lg = warp; lg < ng; lg += nwarps) {
     float ts = 0.f, tq = 0.f;
-    for (int c = lane; c < p.chunks; c += 32) { ts += __ldcg(pp + (size_t)c * p.G * 2); tq += __ldcg(pp + (size_t)c * p.G * 2 + 1); }
+    for (int j = lane; j < n; j += 32) {
+      const int r = j / cg, c = lg * cg + (j - r * cg);
+      ts += ss[r * w8 + c]; tq += sq[r * w8 + c];
+    }
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      ts += __shfl_xor_sync(0xffffffffu, ts, o);
-      tq += __shfl_xor_sync(0xffffffffu, tq, o);
+    for (int m = 16; m > 0; m >>= 1) {
+      ts += __shfl_xor_sync(0xffffffffu, ts, m);
+      tq += __shfl_xor_sync(0xffffffffu, tq, m);
     }
-    if (lane == 0) {
-      const float n = (float)p.HW * (float)cg;
-      const float mean = ts / n;
-      float var = tq / n - mean * mean;
-      var = var < 0.f ? 0.f : var;
-      p.stats[((size_t)b * p.G + g) * 2] = mean;
-      p.stats[((size_t)b * p.G + g) * 2 + 1] = rsqrtf(var + p.eps);
-    }
+    if (lane == 0) p.partial[((size_t)b * p.G + c0 / cg + lg) * p.chunks + blockIdx.x] = make_float2(ts, tq);
   }
-  if (threadIdx.x == 0) p.counters[b] = 0u;
 }
 
-// pass 2: y = act((x + add - mean) * rstd * gamma + beta).  grid (row chunks, B); block = nvec * rpp threads: a thread
-// keeps ONE 8-channel vector column, so its scale/shift live in registers and the row loop is pure streaming.
+// pass 2: y = act((x + add - mean) * rstd * gamma + beta).  grid (row blocks, channel slice, image), the stats pass's
+// block shape, rows_per_block <= 4 rpp.  Launched as a programmatic dependent of the stats grid: a thread first
+// loads its (up to) four rows of one column, all in flight, and its gamma / beta / add, which overlaps the stats
+// grid's tail; after the grid-dependency wait, segments of L lanes (one per group of the slice) fold the group's chunk
+// partials in a fixed order (every block of the slice computes the same bits); then it writes its rows.
 template <typename E>
-__global__ void gn_apply_kernel(GnParams<E> p, int rows_per_block) {
+__global__ void __launch_bounds__(1024) gn_apply_kernel(GnParams<E> p, int rows_per_block) {
   using X = Elem<E>;
   using E2 = typename X::E2;
-  const int nvec = p.C >> 3;
-  const int rpp = blockDim.x / nvec;
-  const int v = threadIdx.x % nvec, rl = threadIdx.x / nvec;
-  const int b = blockIdx.y;
-  const int cg = p.C / p.G;
+  __shared__ float2 s_stat[64];   // (mean, rstd) of the slice's groups
+  const int cg = p.C / p.G, sv = p.sv, rpp = blockDim.x / sv, b = blockIdx.z;
+  const int v0 = blockIdx.y * sv, nv = min(sv, (p.C >> 3) - v0);
+  const int c0 = v0 * 8, ng = nv * 8 / cg;
+  const int v = threadIdx.x % sv, rl = threadIdx.x / sv;
+  const bool lane_on = rl < rpp && v < nv;
+  const int r0 = blockIdx.x * rows_per_block;
+  const int r1 = lane_on ? min(p.HW, r0 + rows_per_block) : r0;
+  const int stride_vec = p.C >> 3;
+  const uint4* __restrict__ xcol = reinterpret_cast<const uint4*>(p.x + (size_t)b * p.HW * p.C + c0) + v;
+  uint4* __restrict__ ycol = reinterpret_cast<uint4*>(p.y + (size_t)b * p.HW * p.C + c0) + v;
+  uint4 xv[4];
+  gn_load4(xv, xcol, stride_vec, r0 + rl, rpp, r1);
   float sc[8], sh[8];
+  uint4 gv = make_uint4(0, 0, 0, 0), bv = gv, av = gv;
+  if (lane_on) {
+    gv = __ldg(reinterpret_cast<const uint4*>(p.gamma + c0) + v);
+    bv = __ldg(reinterpret_cast<const uint4*>(p.beta + c0) + v);
+    if (p.add) av = __ldg(reinterpret_cast<const uint4*>(p.add + (size_t)b * p.add_bs + c0) + v);
+  }
   {
-    const uint4 gv = __ldg(reinterpret_cast<const uint4*>(p.gamma) + v);
-    const uint4 bv = __ldg(reinterpret_cast<const uint4*>(p.beta) + v);
-    uint4 av = make_uint4(0, 0, 0, 0);
-    if (p.add) av = __ldg(reinterpret_cast<const uint4*>(p.add + (size_t)b * p.add_bs) + v);
+    // L lanes per group: a power of two with ng * L <= blockDim.x (>= 4, as ng <= 64), so a segment never
+    // straddles a warp; every load of the fold is issued before the first add
+    int L = 32;
+    while (ng * L > (int)blockDim.x) L >>= 1;
+    const int lg = threadIdx.x / L, j = threadIdx.x % L, g = c0 / cg + lg;
+    float ts = 0.f, tq = 0.f, shift = 0.f;
+    if (lg < ng && j == 0) shift = gn_shift(p, b, g * cg);
+    // everything above reads only this GroupNorm's inputs; the partials are the statistics grid's output
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    if (lg < ng) {
+      const float2* pp = p.partial + ((size_t)b * p.G + g) * p.chunks;
+#pragma unroll 4
+      for (int c = j; c < p.chunks; c += L) { const float2 t = pp[c]; ts += t.x; tq += t.y; }
+    }
+    for (int m = L >> 1; m > 0; m >>= 1) {
+      ts += __shfl_xor_sync(0xffffffffu, ts, m);
+      tq += __shfl_xor_sync(0xffffffffu, tq, m);
+    }
+    if (lg < ng && j == 0) {
+      const float n = (float)p.HW * (float)cg;
+      const float dm = ts / n;
+      float var = tq / n - dm * dm;
+      var = var < 0.f ? 0.f : var;
+      s_stat[lg] = make_float2(shift + dm, rsqrtf(var + p.eps));
+    }
+  }
+  __syncthreads();
+  {
     const E* gh = reinterpret_cast<const E*>(&gv);
     const E* bh = reinterpret_cast<const E*>(&bv);
     const E* ah = reinterpret_cast<const E*>(&av);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      const int g = (v * 8 + i) / cg;
-      const float mean = __ldg(p.stats + ((size_t)b * p.G + g) * 2), rstd = __ldg(p.stats + ((size_t)b * p.G + g) * 2 + 1);
-      sc[i] = rstd * X::to_float(gh[i]);
-      sh[i] = X::to_float(bh[i]) + (X::to_float(ah[i]) - mean) * sc[i];
+      const float2 st = s_stat[(v * 8 + i) / cg];
+      sc[i] = st.y * X::to_float(gh[i]);
+      sh[i] = X::to_float(bh[i]) + (X::to_float(ah[i]) - st.x) * sc[i];
     }
   }
-  const int r0 = blockIdx.x * rows_per_block, r1 = min(p.HW, r0 + rows_per_block);
-  const E* xb = p.x + (size_t)b * p.HW * p.C;
-  E* yb = p.y + (size_t)b * p.HW * p.C;
-  for (int r = r0 + rl; r < r1; r += rpp) {
-    const uint4 xv = __ldg(reinterpret_cast<const uint4*>(xb + (size_t)r * p.C) + v);
-    const E2* xh = reinterpret_cast<const E2*>(&xv);
+  const int r = r0 + rl;
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    if (r + u * rpp >= r1) break;
+    const E2* xh = reinterpret_cast<const E2*>(&xv[u]);
     __align__(16) E2 o[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
@@ -160,7 +203,7 @@ __global__ void gn_apply_kernel(GnParams<E> p, int rows_per_block) {
       }
       o[k] = X::from_float2(y0, y1);
     }
-    reinterpret_cast<uint4*>(yb + (size_t)r * p.C)[v] = *reinterpret_cast<const uint4*>(o);
+    ycol[(size_t)(r + u * rpp) * stride_vec] = *reinterpret_cast<const uint4*>(o);
   }
 }
 
@@ -291,11 +334,34 @@ __global__ void resnet_residual_kernel(const E* a, const E* h, const float* __re
   }
 }
 
-inline int gn_chunks(int HW) {
-  int rows = HW >= 4096 ? 64 : (HW >= 1024 ? 32 : 16);   // enough blocks to fill the SMs, few enough to finalise fast
-  int c = (HW + rows - 1) / rows;
-  return c < 1 ? 1 : (c > 512 ? 512 : c);
+// GroupNorm's work split over one image: a function of (HW, C, G) only.
+constexpr int kGnMaxChunks = 64;             // row chunks of the statistics pass, at most (and at most HW)
+constexpr int kGnStatBlocksPerImage = 128;   // two images fill the H100's 132 SMs about twice
+struct GnSplit {
+  int sv;              // vectors per channel slice: whole lcm(8, C/G)-channel units, about 32 vectors
+  int slices;          // channel slices (the last may be narrower)
+  int threads, rpp;    // threads per block (a multiple of 32, >= 256) and row lanes: threads / sv
+  int chunks, rows_per_chunk;
+};
+inline GnSplit gn_split(int HW, int C, int G) {
+  GnSplit s;
+  const int cg = C / G, nvec = C >> 3;
+  int gcd = cg, t = 8;
+  while (t) { const int r = gcd % t; gcd = t; t = r; }
+  const int uv = cg / gcd;                          // vectors per unit: lcm(8, cg) / 8
+  const int nunits = nvec / uv, want = (nvec + 31) / 32;
+  const int per_slice = (nunits + want - 1) / want;
+  s.sv = per_slice * uv;
+  s.slices = (nunits + per_slice - 1) / per_slice;
+  s.threads = s.sv > 256 ? (s.sv + 31) / 32 * 32 : 256;
+  s.rpp = s.threads / s.sv;
+  int chunks = (kGnStatBlocksPerImage + s.slices - 1) / s.slices;
+  const int most = (HW + s.rpp - 1) / s.rpp;
+  chunks = chunks < most ? chunks : most;
+  chunks = chunks < kGnMaxChunks ? chunks : kGnMaxChunks;
+  s.rows_per_chunk = (HW + chunks - 1) / chunks;
+  s.chunks = (HW + s.rows_per_chunk - 1) / s.rows_per_chunk;
+  return s;
 }
-
 }  // namespace uops
 }  // namespace pww

@@ -24,7 +24,7 @@ def _workspace(device, nbytes: int) -> torch.Tensor:
     if w is None or w.numel() < nbytes:
         if w is not None:
             _WS_KEEP.append(w)
-        w = torch.zeros(max(nbytes, 4 << 20), dtype=torch.uint8, device=device)   # counters must start at zero
+        w = torch.empty(max(nbytes, 4 << 20), dtype=torch.uint8, device=device)
         _WS[device] = w
     return w
 

@@ -223,6 +223,43 @@ int pww_xattn_fused_multi_bf16(const void* q, const void* k, const void* v, void
                                float* stats, void* workspace, size_t workspace_bytes, void* stream);
 
 /*
+ * Attention recording: pww_xattn_fused_multi_f16 / _bf16 that also ACCUMULATES, for every recorded image, head and
+ * query row, the softmax mass each painted region's tokens receive.  `out` (and `stats`) are bit-identical to the
+ * _multi call's on the same inputs.  Extra arguments, after `stream`:
+ *   ridx      [Br, 80 k] int8 : region slot (0 .. 15) of each token, in the cidx column layout (token 77 c + j of chunk
+ *               c at column 80 c + j, k key chunks as for cidx); -1 = the token belongs to no region
+ *   rec_index [B] int32        : image b's record (row of ridx and of rec_acc), -1 = image b is not recorded.  The
+ *               recorded images of one call must have distinct records.
+ *   rec_acc   [Br, H, N, 16] fp32, 16-byte aligned, record i at rec_acc + i * rec_batch_stride:
+ *               rec_acc[i, h, n, r] += sum_{t : ridx[t] = r} P[n, t] / sum_t P[n, t]
+ *               with P the softmax probabilities of head h (after the bias, for biased images).  Slots no token maps to
+ *               get 0; when every real token has a slot, the slots sum to 1 up to fp32 rounding.  A plain read-add-write
+ *               in stream order (no atomics): zero the buffer before the first call, and calls on one stream add up.
+ *   rec_batch_stride : elements between records, >= H * N * 16
+ * Recording covers biased and unbiased images alike; mpack == NULL (no image biased) records plain attention.  A NULL
+ * ridx / rec_index / rec_acc, a misaligned rec_acc or a too small rec_batch_stride returns PWW_ERR_BAD_ARG before any
+ * CUDA call.  Batch splits offset rec_index with the images, as they do wmap_index.
+ */
+int pww_xattn_fused_rec_f16(const void* q, const void* k, const void* v, void* out,
+                            int B, int H, int N, int T, int D,
+                            int64_t q_batch_stride, int64_t q_row_stride,
+                            int64_t k_batch_stride, int64_t k_row_stride,
+                            int64_t o_batch_stride, int64_t o_row_stride,
+                            const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+                            const int32_t* wmap_index, const int32_t* stat, const float* g_sigma, float scale,
+                            float* stats, void* workspace, size_t workspace_bytes, void* stream,
+                            const int8_t* ridx, const int32_t* rec_index, float* rec_acc, int64_t rec_batch_stride);
+int pww_xattn_fused_rec_bf16(const void* q, const void* k, const void* v, void* out,
+                             int B, int H, int N, int T, int D,
+                             int64_t q_batch_stride, int64_t q_row_stride,
+                             int64_t k_batch_stride, int64_t k_row_stride,
+                             int64_t o_batch_stride, int64_t o_row_stride,
+                             const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+                             const int32_t* wmap_index, const int32_t* stat, const float* g_sigma, float scale,
+                             float* stats, void* workspace, size_t workspace_bytes, void* stream,
+                             const int8_t* ridx, const int32_t* rec_index, float* rec_acc, int64_t rec_batch_stride);
+
+/*
  * Self-attention through the same patched function (context=None, paint_with_words.py:71-72):
  *   out = softmax(scale * Q_h K_h^T) V_h  with keys/values [B, N, H*D]; no bias; online softmax.
  */

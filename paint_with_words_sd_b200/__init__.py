@@ -7,12 +7,13 @@ directory) because the canonical project name is not an importable identifier.
 from .attention import PwWAttnProcessor, inj_forward, patch_unet, unpatch_all  # noqa: F401
 from .conditioning import (  # noqa: F401
     _blur_image_mask, _encode_text_color_inputs, _extract_seed_and_sigma_from_context, _get_binary_mask,
-    _image_context_seperator, _img_importance_flatten, _tokens_img_attention_weight, always_round,
+    _image_context_seperator, _img_importance_flatten, _tokens_img_attention_weight, always_round, region_token_index,
 )
 from .controlnet import ControlNetModel, pww_load_controlnet  # noqa: F401
 from .pipeline import (  # noqa: F401
     PaintWithWord_StableDiffusionInpaintPipeline, PaintWithWord_StableDiffusionPipeline, PwWSampler, paint_with_words,
-    paint_with_words_batch, paint_with_words_inpaint, preprocess, prepare_mask_and_masked_image, pww_load_tools,
+    RegionAttention, paint_with_words_batch, paint_with_words_inpaint, preprocess, prepare_mask_and_masked_image,
+    pww_load_tools,
 )
 from .scheduler import (  # noqa: F401
     DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler, EulerDiscreteScheduler, LMSDiscreteScheduler,

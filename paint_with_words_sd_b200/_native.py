@@ -30,6 +30,7 @@ EXPORTS = (
     "pww_control_inject_f16", "pww_control_inject_bf16",
     "pww_control_combine_f16", "pww_control_combine_bf16",
     "pww_resnet_residual_f16", "pww_resnet_residual_bf16",
+    "pww_xattn_fused_rec_f16", "pww_xattn_fused_rec_bf16",
 )
 
 
@@ -79,6 +80,9 @@ def lib() -> ctypes.CDLL:
     L.pww_xattn_fused_multi_f16.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i, c_i, c_i, c_i, c_i, c_i64, c_i64, c_i64, c_i64,
                                             c_i64, c_i64, c_vp, c_i64, c_i, c_vp, c_vp, c_vp, c_vp, c_f, c_vp, c_vp, c_sz,
                                             c_vp]
+    # the _multi arguments, then ridx, rec_index, rec_acc (device pointers) and rec_batch_stride (elements)
+    L.pww_xattn_fused_rec_f16.restype = c_i
+    L.pww_xattn_fused_rec_f16.argtypes = list(L.pww_xattn_fused_multi_f16.argtypes) + [c_vp, c_vp, c_vp, c_i64]
     L.pww_attn_fwd_f16.restype = c_i
     L.pww_attn_fwd_f16.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i, c_i, c_i, c_i, c_i64, c_i64, c_i64, c_i64, c_f, c_vp]
     L.pww_groupnorm_workspace_bytes.restype = c_sz

@@ -9,7 +9,8 @@ Same calling convention, context-dict schema and patch mechanism as the referenc
         "CROSS_ATTENTION_WEIGHT_ORIG" ([H,W,T] fp32 or int 0), "SIGMA", "WEIGHT_FUNCTION"
     T = 77 (one CLIP window, any T <= 80 works) or a long prompt of 2 or 3 concatenated 77-token chunks (T = 154, 231;
     `conditioning.chunk_prompt`, the A1111 / compel layout).
-        (optional, ours) "WMAP_INDEX", "G_SIGMA", "STAT_KIND", "CROSS_ATTENTION_PACKED_{N}", "PWW_SCRATCH"
+        (optional, ours) "WMAP_INDEX", "G_SIGMA", "STAT_KIND", "CROSS_ATTENTION_PACKED_{N}", "PWW_SCRATCH",
+        "ATTN_RECORD" (per-region attention recording, see RECORD_KEY)
 
 Everything between the q/k/v projections and the output projection runs in libpww_b200.so through
 the C ABI (include/pww_b200.h): ONE launch of `pww_xattn_fused_f16` (per-image max/std of QK^T over all heads,
@@ -46,6 +47,9 @@ from .conditioning import PACK_TOKENS, expand_orig_weight_map, key_chunks, pack_
 from .weight_function import g_of_sigma, probe_weight_function
 
 _ORIG_KEY = "CROSS_ATTENTION_WEIGHT_ORIG"
+# Attention recording (kept by PwWSampler(record_attention=True)): {N: (ridx, rec_index, rec_acc)}, the `record` of every
+# cross-attention call with N query rows (see cross_attention).  A dict without it records nothing.
+RECORD_KEY = "ATTN_RECORD"
 
 
 class _DeviceState:
@@ -162,14 +166,17 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                     wmap: Optional[torch.Tensor] = None, wmap_index: Optional[torch.Tensor] = None,
                     stat: Union[int, torch.Tensor] = _native.PWW_STAT_MAX, g_sigma: Optional[torch.Tensor] = None,
                     return_stats: bool = False, packed=None, stats_out: Optional[torch.Tensor] = None,
-                    workspace: Optional[torch.Tensor] = None):
+                    workspace: Optional[torch.Tensor] = None, record=None):
     """Fused region for a key sequence of T <= 80 tokens or of 2 / 3 CLIP chunks (T = 154, 231; any other T raises).
     q [B,N,C]; k,v [B,T,C]; wmap [Bw,N,T] fp32 or None; `packed` = (mpack [Bw,N,32] fp16, cidx [Bw,80 k] int8, k key
     chunks) from `conditioning.pack_weight_map` (built from `wmap` and cached when not given).  `stat` is one kind for
     every image (an int) with `g_sigma` a 1-element fp32 device tensor holding G(sigma), or per-image settings: an int32
     [B] device tensor of kinds with `g_sigma` an fp32 [B] device tensor (entry b = image b; the `_multi` entry points).
     `stats_out` / `workspace` let a caller that captures CUDA graphs own the scratch (defaults: per-device scratch of
-    this module).  The call runs in bf16 when q is bf16 and in fp16 otherwise (see the module docstring)."""
+    this module).  The call runs in bf16 when q is bf16 and in fp16 otherwise (see the module docstring).
+    `record` = (ridx [Br, 80 k] int8, rec_index [B] int32, rec_acc [Br, heads, N, 16] fp32), all on q's device: the call
+    goes to `pww_xattn_fused_rec_*`, which also adds every recorded image's per-region softmax mass into rec_acc
+    (include/pww_b200.h).  It needs the one-launch kernel: a call that would take the dense pair raises."""
     L = _native.lib()
     dt = _elem_dtype(q)
     q, k, v = _rows(q, dt), _rows(k, dt), _rows(v, dt)
@@ -210,6 +217,25 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                                  f"{q.device}")
             kind_ptr = stat.data_ptr()
         stats = None
+        rec_args = ()
+        if record is not None:
+            if not use_fused:
+                why = ("XATTN_IMPL is 'dense'" if impl == "dense" else
+                       "the weight map has more than 10 distinct columns and takes the dense two-launch path")
+                raise _native.NativeError(f"attention recording needs the one-launch kernel, but {why}")
+            ridx, rec_index, rec_acc = record
+            if (ridx.dtype != torch.int8 or ridx.dim() != 2 or ridx.shape[1] != PACK_TOKENS * max(1, key_chunks(T))
+                    or not ridx.is_contiguous() or rec_index.dtype != torch.int32 or rec_index.numel() != B
+                    or not rec_index.is_contiguous() or rec_acc.dtype != torch.float32 or rec_acc.dim() != 4
+                    or tuple(rec_acc.shape[1:]) != (heads, N, 16) or not rec_acc[0].is_contiguous()
+                    or any(t.device != q.device for t in (ridx, rec_index, rec_acc))):
+                raise ValueError(f"record needs int8 [Br, {PACK_TOKENS * max(1, key_chunks(T))}] ridx, int32 [{B}] "
+                                 f"rec_index and fp32 [Br, {heads}, {N}, 16] rec_acc on {q.device}")
+            if not per_image and biased:           # the recording entry takes per-image kinds and G(sigma)
+                stat = torch.full((B,), int(stat), dtype=torch.int32, device=q.device)
+                g_sigma = g_sigma.reshape(-1)[:1].expand(B).contiguous()
+                kind_ptr, per_image = stat.data_ptr(), True
+            rec_args = (ridx.data_ptr(), rec_index.data_ptr(), rec_acc.data_ptr(), rec_acc.stride(0))
         if use_fused:
             mp_ptr = ci_ptr = idx_ptr = g_ptr = st_ptr = ws_ptr = None
             mp_bs = bw = ws_bytes = 0
@@ -224,11 +250,12 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                 mp_ptr, ci_ptr, idx_ptr = mpack.data_ptr(), cidx.data_ptr(), wmap_index.data_ptr()
                 g_ptr, st_ptr, ws_ptr = g_sigma.data_ptr(), stats.data_ptr(), ws.data_ptr()
                 mp_bs, bw, ws_bytes = mpack.stride(0), mpack.shape[0], ws.numel()
-            fn = _native.entry("pww_xattn_fused_multi" if per_image else "pww_xattn_fused", dt)
+            name = "pww_xattn_fused_rec" if rec_args else ("pww_xattn_fused_multi" if per_image else "pww_xattn_fused")
+            fn = _native.entry(name, dt)
             rc = fn(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, heads, N, T, D,
                     q.stride(0), q.stride(1), k.stride(0), k.stride(1), out.stride(0), out.stride(1),
-                    mp_ptr, mp_bs, bw, ci_ptr, idx_ptr, kind_ptr if per_image else stat, g_ptr, float(scale), st_ptr,
-                    ws_ptr, ws_bytes, stream)
+                    mp_ptr, mp_bs, bw, ci_ptr, idx_ptr, kind_ptr if per_image or rec_args else stat, g_ptr,
+                    float(scale), st_ptr, ws_ptr, ws_bytes, stream, *rec_args)
             _native.check(rc, fn.__name__)
             _native.launch_count += 1
         else:
@@ -378,11 +405,18 @@ def inj_forward(self, hidden_states, context=None, mask=None):
                 wmap_index = context.get("WMAP_INDEX")
                 packed = context.get(packed_key(q.shape[1]))          # (mpack, cidx) prepared by PwWSampler
                 scratch = context.get("PWW_SCRATCH", scratch)         # (stats, workspace) owned by the sampler
+        record = None
+        recs = context.get(RECORD_KEY) if is_dict else None
+        if recs is not None:
+            record = recs.get(q.shape[1])
+            if record is None:
+                raise _native.NativeError(f"attention recording has no accumulator for N = {q.shape[1]} query rows "
+                                          f"(levels: {sorted(recs)})")
         if k.shape[0] != q.shape[0]:
             k = k.expand(q.shape[0], -1, -1)
             v = v.expand(q.shape[0], -1, -1)
         o = cross_attention(q, k, v, self.heads, self.scale, wmap, wmap_index, stat, g_dev, packed=packed,
-                            stats_out=scratch[0], workspace=scratch[1])
+                            stats_out=scratch[0], workspace=scratch[1], record=record)
 
     with torch.autocast("cuda", dtype=act):
         o = self.to_out[0](o)

@@ -88,6 +88,54 @@ def _tokens_img_attention_weight(img_context_seperated, tokenized_texts, ratio: 
     return out.reshape(r0, r1, len(token_lis)) if original_shape else out
 
 
+def _token_region_counts(img_context_seperated, token_lis: List[int]) -> List[Optional[torch.Tensor]]:
+    """Per region (in order): fp32 [T] counts of the matched spans of its label covering each token -- the columns
+    `_tokens_img_attention_weight` adds the region's mask into -- or None when the label is not in the prompt."""
+    out: List[Optional[torch.Tensor]] = []
+    for label, _ in img_context_seperated:
+        starts = _match_positions(token_lis, label)
+        if not starts:
+            out.append(None)
+            continue
+        cnt = torch.zeros(len(token_lis), dtype=torch.float32)
+        for s in starts:
+            cnt[s:s + len(label)] += 1.0
+        out.append(cnt)
+    return out
+
+
+MAX_RECORDED_REGIONS = 16    # region slots of the attention recording (csrc/xattn_core.cuh: kRegions)
+REGION_INDEX_KEY = "REGION_TOKEN_INDEX"   # cond-dict key of `region_token_index`'s row
+REGION_COUNT_KEY = "REGION_COUNT"         # cond-dict key of the number of regions (the row's slots 0 .. count - 1)
+
+
+def region_token_index(img_context_seperated, tokenized_texts) -> torch.Tensor:
+    """Token -> region row of one image for attention recording (`pww_xattn_fused_rec_f16`): int8 [80 k] in the packed
+    map's column layout (k key chunks; token 77 c + j at column 80 c + j, `_cidx_columns`), entry = the index in
+    `color_context` order of the region whose label covers the token, -1 for tokens of no region.
+
+    A token belongs to region r when a matched span of r's label covers it: exactly the token columns the reference's
+    `_tokens_img_attention_weight` adds r's mask into (the incidence of `_tokens_img_attention_factors`).  A token
+    covered by the labels of several regions goes to the FIRST of them in `color_context` order.  A region whose label
+    is not in the prompt gets no tokens.  A long prompt (k = 2, 3) maps its concatenated ids.  More than 16 regions
+    raises ValueError."""
+    if len(img_context_seperated) > MAX_RECORDED_REGIONS:
+        raise ValueError(f"attention recording takes at most {MAX_RECORDED_REGIONS} regions, got "
+                         f"{len(img_context_seperated)}")
+    token_lis = tokenized_texts["input_ids"][0].tolist()
+    t = len(token_lis)
+    k = key_chunks(t)
+    if k == 0:
+        raise ValueError(f"no attention kernel for a context of {t} tokens")
+    owner = torch.full((t,), -1, dtype=torch.int8)
+    for r, cnt in enumerate(_token_region_counts(img_context_seperated, token_lis)):
+        if cnt is not None:
+            owner[(cnt > 0) & (owner < 0)] = r
+    row = torch.full((PACK_TOKENS * k,), -1, dtype=torch.int8)
+    row[_cidx_columns(t)] = owner
+    return row
+
+
 def _tokens_img_attention_factors(img_context_seperated, tokenized_texts, ratio: int = 8):
     """The same weight map as `_tokens_img_attention_weight`, kept in the factored form it is built from:
     W[n, t] = sum_r M[n, r] * C[t, r] with M [N, R] fp32 (column r = region r's resized strength mask,
@@ -101,13 +149,9 @@ def _tokens_img_attention_factors(img_context_seperated, tokenized_texts, ratio:
     dim0, dim1 = img_context_seperated[0][1].shape
     r0, r1 = always_round(dim0 / ratio), always_round(dim1 / ratio)
     cols, counts = [], []
-    for label, mask in img_context_seperated:
-        starts = _match_positions(token_lis, label)
-        if not starts:
+    for (label, mask), cnt in zip(img_context_seperated, _token_region_counts(img_context_seperated, token_lis)):
+        if cnt is None:
             continue
-        cnt = torch.zeros(len(token_lis), dtype=torch.float32)
-        for s in starts:
-            cnt[s:s + len(label)] += 1.0
         cols.append(_img_importance_flatten(mask, r0, r1).reshape(-1))
         counts.append(cnt)
     if not cols:
@@ -353,6 +397,10 @@ def _encode_text_color_inputs(text_encoder, tokenizer, device, color_map_image, 
         key = weight_key(always_round(height / r) * always_round(width / r))
         cond[key] = _tokens_img_attention_weight(seperated_word_contexts, text_input, ratio=r).to(device)
         uncond[key] = 0
+    # the token -> region row of attention recording (PwWSampler(record_attention=True)); None: too many regions to record
+    cond[REGION_INDEX_KEY] = (region_token_index(seperated_word_contexts, text_input)
+                              if len(seperated_word_contexts) <= MAX_RECORDED_REGIONS else None)
+    cond[REGION_COUNT_KEY] = len(seperated_word_contexts)
 
     if chunks > 1:
         cond["CONTEXT_TENSOR"] = _encode_chunked(text_encoder, text_input["input_ids"], device)

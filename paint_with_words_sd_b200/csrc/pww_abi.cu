@@ -210,11 +210,14 @@ int xattn_fused(const void* q, const void* k, const void* v, void* out, int B, i
                 int64_t o_batch_stride, int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw,
                 const int8_t* cidx, const int32_t* wmap_index, int stat, const int32_t* kinds, bool per_image,
                 const float* g_sigma, float scale, float* stats, void* workspace, size_t workspace_bytes,
-                void* stream) {
+                void* stream, const pww::fx::FxRecord* rec = nullptr) {
   int rc = check_common(q, k, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride);
   if (rc) return rc;
   if (!v || !out || !aligned16(v) || !aligned16(out)) return PWW_ERR_BAD_ARG;
   if ((o_batch_stride | o_row_stride) & 7 || o_row_stride < (int64_t)H * D || o_batch_stride <= 0) return PWW_ERR_BAD_ARG;
+  if (rec && (!rec->ridx || !rec->rec_index || !rec->rec_acc || !aligned16(rec->rec_acc) ||
+              rec->rec_bs < (int64_t)H * N * pww::core::kRegions))
+    return PWW_ERR_BAD_ARG;
   if (mpack) {
     if (!cidx || !g_sigma || !workspace || Bw <= 0 || !aligned16(mpack)) return PWW_ERR_BAD_ARG;
     if ((mpack_batch_stride & 7) || mpack_batch_stride < (int64_t)N * pww::fx::kMW) return PWW_ERR_BAD_ARG;
@@ -247,8 +250,13 @@ int xattn_fused(const void* q, const void* k, const void* v, void* out, int B, i
       ci = cidx + (int64_t)b0 * pww::core::kTP * pww::core::chunks_of(T);   // [Bw, 80 k]
     }
     c.wmap = (const float*)mp;                                     // non-null marks "maps present" for the kernel
+    pww::fx::FxRecord r;
+    if (rec) {                                                     // records are reached through rec_index
+      r = *rec;
+      r.rec_index += b0;
+    }
     const cudaError_t e = with_shape(D, T, [&](auto k) {
-      return pww::fx::launch_fused2<k.D, k.KC>(c, mp, mpack_batch_stride, ci, (cudaStream_t)stream);
+      return pww::fx::launch_fused2<k.D, k.KC>(c, mp, mpack_batch_stride, ci, (cudaStream_t)stream, rec ? &r : nullptr);
     });
     if (e == cudaErrorInvalidConfiguration) return PWW_ERR_UNSUPPORTED;
     if (e != cudaSuccess) return cuda_fail(e);
@@ -526,6 +534,30 @@ int pww_xattn_fused_multi_bf16(const void* q, const void* k, const void* v, void
       q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
       o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, PWW_STAT_MAX, stat, true,
       g_sigma, scale, stats, workspace, workspace_bytes, stream);
+}
+
+int pww_xattn_fused_rec_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+    int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int64_t o_batch_stride,
+    int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+    const int32_t* wmap_index, const int32_t* stat, const float* g_sigma, float scale, float* stats, void* workspace,
+    size_t workspace_bytes, void* stream, const int8_t* ridx, const int32_t* rec_index, float* rec_acc,
+    int64_t rec_batch_stride) {
+  const pww::fx::FxRecord rec = {ridx, rec_index, rec_acc, rec_batch_stride};
+  return xattn_fused<__half>(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+      o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, PWW_STAT_MAX, stat, true,
+      g_sigma, scale, stats, workspace, workspace_bytes, stream, &rec);
+}
+int pww_xattn_fused_rec_bf16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T, int D,
+    int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int64_t o_batch_stride,
+    int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+    const int32_t* wmap_index, const int32_t* stat, const float* g_sigma, float scale, float* stats, void* workspace,
+    size_t workspace_bytes, void* stream, const int8_t* ridx, const int32_t* rec_index, float* rec_acc,
+    int64_t rec_batch_stride) {
+  const pww::fx::FxRecord rec = {ridx, rec_index, rec_acc, rec_batch_stride};
+  return xattn_fused<__nv_bfloat16>(
+      q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+      o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, PWW_STAT_MAX, stat, true,
+      g_sigma, scale, stats, workspace, workspace_bytes, stream, &rec);
 }
 
 int pww_attn_fwd_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int D,

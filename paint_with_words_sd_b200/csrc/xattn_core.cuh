@@ -136,11 +136,19 @@ __device__ __forceinline__ void warp_online_begin(float (&o)[Tile<D>::NT][4], fl
   l0 = l1 = 0.f;
 }
 
+// What warp_online_chunk hands its hook after P V: the packed P fragments (the A operands) and the rescale factors of
+// the rows' running max.  The default hook does nothing and compiles to nothing.
+struct NoPHook {
+  template <int NK>
+  __device__ __forceinline__ void operator()(const uint32_t (&)[NK][4], float, float) const {}
+};
+
 // One key tile of NJ n-tiles (10: a cross-attention chunk of 80 padded keys; 8: a self-attention tile of 64): s holds
 // S (+ bias) of the tile, of which the first kv keys are real; vs is its V tile.  l0 / l1 are per-thread partial row sums.
-template <int D, typename E, int NJ>
+template <int D, typename E, int NJ, typename Hook = NoPHook>
 __device__ __forceinline__ void warp_online_chunk(float (&s)[NJ][4], int kv, float sl2, uint32_t vs, int lane,
-                                                  float (&o)[Tile<D>::NT][4], float& m0, float& m1, float& l0, float& l1) {
+                                                  float (&o)[Tile<D>::NT][4], float& m0, float& m1, float& l0, float& l1,
+                                                  const Hook& hook = Hook{}) {
   static_assert(NJ % 2 == 0, "P V takes two n-tiles of P per k-step");
   using C = Tile<D>;
   float t0 = -INFINITY, t1 = -INFINITY;
@@ -193,6 +201,7 @@ __device__ __forceinline__ void warp_online_chunk(float (&s)[NJ][4], int kv, flo
       ptx::mma16816<E>(o[C::NT - 1], pa[kk], b0, b1);
     }
   }
+  hook(pa, a0, a1);
 }
 
 // Divides O by the row sums (reduced over the quad) once every chunk has been accumulated.
@@ -206,6 +215,59 @@ __device__ __forceinline__ void warp_online_end(float (&o)[Tile<D>::NT][4], floa
 #pragma unroll
   for (int j = 0; j < Tile<D>::NT; ++j) {
     o[j][0] *= i0; o[j][1] *= i0; o[j][2] *= i1; o[j][3] *= i1;
+  }
+}
+
+// ---- per-region softmax mass (the recording instance of the cross-attention kernel) ----
+// The 16 region slots are two more 8-column "V" tiles: R[t, r] = (ridx[t] == r), a 0/1 matrix built in registers, so
+// mass[n, r] = sum_t P[n, t] R[t, r] is two MMAs per k-step of P V with the same packed P, rescaled like O when the row
+// max moves and divided by the same row sum at the end.  rm[2][4] holds the [16 rows x 16 slots] C fragments.
+constexpr int kRegions = 16;
+
+// After chunk c's P V: rescale rm by the chunk's factors a0 / a1 and add P R; rt = the chunk's 80 ridx entries.
+template <typename E, int NK>
+__device__ __forceinline__ void warp_region_chunk(const uint32_t (&pa)[NK][4], float a0, float a1, const int8_t* rt,
+                                                  int lane, float (&rm)[2][4]) {
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    rm[j][0] *= a0; rm[j][1] *= a0; rm[j][2] *= a1; rm[j][3] *= a1;
+  }
+  const int r = lane >> 2;
+#pragma unroll
+  for (int kk = 0; kk < NK; ++kk) {
+    // B fragment of m16n8k16: tokens 16 kk + 2 (lane & 3) + {0, 1} (b0) and + 8 (b1), column lane / 4 of the tile
+    const int t = 16 * kk + 2 * (lane & 3);
+    const int i0 = __ldg(rt + t), i1 = __ldg(rt + t + 1), i2 = __ldg(rt + t + 8), i3 = __ldg(rt + t + 9);
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int slot = r + 8 * j;
+      const uint32_t b0 = ptx::pack2<E>(i0 == slot ? 1.f : 0.f, i1 == slot ? 1.f : 0.f);
+      const uint32_t b1 = ptx::pack2<E>(i2 == slot ? 1.f : 0.f, i3 == slot ? 1.f : 0.f);
+      ptx::mma16816<E>(rm[j], pa[kk], b0, b1);
+    }
+  }
+}
+
+// Normalises rm by the row sums (the quad reduction of warp_online_end) and adds it to acc, the fp32 [N, 16] mass of
+// this (record, head): plain read-add-write, rows >= N dropped.  One job owns each (image, head, row) of a launch.
+__device__ __forceinline__ void warp_region_add(const float (&rm)[2][4], float l0, float l1, float* acc, int row0, int N,
+                                                int lane) {
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float inv[2] = {1.f / l0, 1.f / l1};
+  const int g = lane >> 2, q = lane & 3;
+#pragma unroll
+  for (int hf = 0; hf < 2; ++hf) {
+    const int row = row0 + g + 8 * hf;
+    if (row >= N) continue;
+    float* a = acc + (int64_t)row * kRegions + 2 * q;
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      a[8 * j] += rm[j][2 * hf] * inv[hf];
+      a[8 * j + 1] += rm[j][2 * hf + 1] * inv[hf];
+    }
   }
 }
 

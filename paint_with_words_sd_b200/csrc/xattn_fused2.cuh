@@ -29,8 +29,14 @@
 // and Mu is split into fp16 hi/lo halves:  mpack[n] = [ hi(Mu[n,0..9]) | lo(Mu[n,0..9]) | hi(Mu[n,0..9]) | 0 0 ]  (32 fp16,
 // 64 bytes per row instead of 308).  The kernel rebuilds W[n, t] = hi + lo in fp32 (exact to 2^-22 relative) from the row
 // tile's 8 KB of packed map in shared memory and adds x * W to the fp32 scores.
+//
+// Attention recording (REC = true, FxRecord): the softmax jobs of the recorded images also add each query row's softmax
+// mass per region slot (16 slots, a token -> slot row per image) into a caller-owned fp32 accumulator, computed from the
+// same packed P as P.V (xattn_core.cuh: warp_region_chunk / warp_region_add).  The plain instances (REC = false) are
+// the kernel without it: every recording instruction is behind `if constexpr`.
 #pragma once
 #include <algorithm>
+#include <type_traits>
 #include <vector>
 
 #include "mma_sm90.cuh"
@@ -56,6 +62,22 @@ struct FxParams {
   int hg;                   // head groups per row tile
   unsigned* jobs_dump;      // debug only: [grid][2 + 2 * 512] = njobs, nstat, job table of every CTA
 };
+
+// Attention recording (the REC instances): image b with rec_index[b] >= 0 adds, for every head h and query row n, the
+// softmax mass of each region slot r < 16,  mass[n, r] = sum_{t : ridx[t] = r} P[n, t] / sum_t P[n, t],  into
+// rec_acc[rec_index[b], h, n, r].  Biased and unbiased images alike; the plain instances never see these fields.
+struct FxRecord {
+  const int8_t* ridx;       // [Br, 80 k] region slot per token (the cidx column layout), -1 = no region
+  const int32_t* rec_index; // [B] record of image b, -1 = not recorded
+  float* rec_acc;           // [Br, H, N, 16] fp32, accumulated into
+  int64_t rec_bs;           // elements between records (>= H * N * 16)
+};
+template <typename E>
+struct FxRecParams : FxParams<E> {
+  FxRecord rec;
+};
+template <typename E, bool REC>
+using FxArgs = std::conditional_t<REC, FxRecParams<E>, FxParams<E>>;
 
 template <int D, int KC = 1>
 struct Cfg2 {
@@ -232,8 +254,10 @@ __device__ __forceinline__ float key_f32(unsigned k) {
   return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
 }
 
-template <int D, int KC, typename E>
-__global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const FxParams<E> fp) {
+// REC = true: the recording instance (FxRecord above).  Its extra work is behind `if constexpr`, so the plain
+// instances are the kernel without it.
+template <int D, int KC, typename E, bool REC = false>
+__global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const FxArgs<E, REC> fp) {
   using C = core::Tile<D>;
   using CF = Cfg2<D, KC>;
   constexpr int CW = core::kTP * KC;                    // cidx columns: token 77 c + j of chunk c at column 80 c + j
@@ -519,6 +543,13 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
       const __half* mrow = reinterpret_cast<const __half*>(smem + stage(i) + CF::OFF_M) + (warp * 16 + (lane >> 2)) * kMW;
       float o[C::NT][4], m0, m1, l0, l1;
       core::warp_online_begin<D>(o, m0, m1, l0, l1);
+      [[maybe_unused]] float rm[2][4] = {};                          // REC: region mass of the warp's rows
+      [[maybe_unused]] int ri = -1;
+      [[maybe_unused]] const int8_t* rrow = nullptr;                // REC: the image's token -> region row, or none
+      if constexpr (REC) {
+        ri = __ldg(fp.rec.rec_index + b);
+        if (ri >= 0) rrow = fp.rec.ridx + (int64_t)ri * CW;
+      }
 #pragma unroll 1
       for (int c = 0; c < KC; ++c) {
         float s[10][4];
@@ -536,7 +567,19 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
               }
             }
         }
-        core::warp_online_chunk<D, E>(s, kv, sl2, st + C::QBYTES + (KC + c) * C::KBYTES, lane, o, m0, m1, l0, l1);
+        if constexpr (REC) {
+          core::warp_online_chunk<D, E>(s, kv, sl2, st + C::QBYTES + (KC + c) * C::KBYTES, lane, o, m0, m1, l0, l1,
+                                        [&](const auto& pa, float a0, float a1) {
+                                          if (rrow != nullptr) core::warp_region_chunk<E>(pa, a0, a1, rrow + c * core::kTP, lane, rm);
+                                        });
+        } else {
+          core::warp_online_chunk<D, E>(s, kv, sl2, st + C::QBYTES + (KC + c) * C::KBYTES, lane, o, m0, m1, l0, l1);
+        }
+      }
+      if constexpr (REC) {
+        if (rrow != nullptr)
+          core::warp_region_add(rm, l0, l1, fp.rec.rec_acc + (int64_t)ri * fp.rec.rec_bs + (int64_t)h * p.N * core::kRegions,
+                                row0, p.N, lane);
       }
       core::warp_online_end<D>(o, l0, l1);
       core::warp_store<D>(o, smem + stage(i) + warp * 16 * C::LD * 2, lane, p.out + (int64_t)b * p.o_bs + h * D, p.o_rs,
@@ -601,8 +644,29 @@ inline bool fused2_fits(int B, int hg, int tiles, int grid) {
   return fused_range_ok(B, hg, tiles, grid) && fused_units_ok(units, grid) && (units + grid - 1) / grid + 1 <= kMaxUnits;
 }
 
+template <int D, int KC, typename E, bool REC>
+cudaError_t launch_fused2_instance(const FxArgs<E, REC>& fp, cudaStream_t s) {
+  using CF = Cfg2<D, KC>;
+  const cudaError_t e = allow_dynamic_smem<xattn_fused2_kernel<D, KC, E, REC>>(CF::SMEM);
+  if (e != cudaSuccess) return e;
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3(fp.grid);
+  cfg.blockDim = dim3(core::kThreads);
+  cfg.dynamicSmemBytes = CF::SMEM;
+  cfg.stream = s;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeCooperative;     // all CTAs co-resident: the in-kernel grid barrier cannot deadlock
+  attr[0].val.cooperative = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  return cudaLaunchKernelEx(&cfg, xattn_fused2_kernel<D, KC, E, REC>, fp);
+}
+
+// rec == NULL: the plain instance; else the recording instance with *rec (rec_index starting at this launch's image 0).
 template <int D, int KC, typename E>
-cudaError_t launch_fused2(const XattnParams<E>& x, const void* mpack, int64_t mpack_bs, const int8_t* cidx, cudaStream_t s) {
+cudaError_t launch_fused2(const XattnParams<E>& x, const void* mpack, int64_t mpack_bs, const int8_t* cidx, cudaStream_t s,
+                          const FxRecord* rec = nullptr) {
   using CF = Cfg2<D, KC>;
   FxParams<E> fp;
   memset(&fp, 0, sizeof(fp));
@@ -616,20 +680,12 @@ cudaError_t launch_fused2(const XattnParams<E>& x, const void* mpack, int64_t mp
   fp.grid = fused_grid(fp.units);
   fp.jobs_dump = debug_jobs_dump();
   if (!fused2_fits(x.B, fp.hg, fp.tiles, fp.grid)) return cudaErrorInvalidConfiguration;
-  const cudaError_t e = allow_dynamic_smem<xattn_fused2_kernel<D, KC, E>>(CF::SMEM);
-  if (e != cudaSuccess) return e;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(fp.grid);
-  cfg.blockDim = dim3(core::kThreads);
-  cfg.dynamicSmemBytes = CF::SMEM;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeCooperative;     // all CTAs co-resident: the in-kernel grid barrier cannot deadlock
-  attr[0].val.cooperative = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, xattn_fused2_kernel<D, KC, E>, fp);
+  if (rec == nullptr) return launch_fused2_instance<D, KC, E, false>(fp, s);
+  FxRecParams<E> rp;
+  memset(&rp, 0, sizeof(rp));
+  static_cast<FxParams<E>&>(rp) = fp;
+  rp.rec = *rec;
+  return launch_fused2_instance<D, KC, E, true>(rp, s);
 }
 
 // Host replay of the job lists (test infrastructure): out[job] = {cta, i, kind, b, h, tile, biased, li} for every job of

@@ -14,6 +14,7 @@ What is different underneath (results equal within the stated fp16 tolerance):
 """
 from __future__ import annotations
 
+import dataclasses
 import inspect
 import math
 from typing import Callable, Dict, List, Optional, Sequence, Tuple, Union
@@ -24,7 +25,9 @@ import torch.nn.functional as F
 from PIL import Image
 
 from . import attention as _attention
-from .conditioning import _encode_text_color_inputs, _get_binary_mask, pack_weight_map, packed_key
+from .conditioning import (MAX_RECORDED_REGIONS, RATIOS, REGION_COUNT_KEY, REGION_INDEX_KEY,
+                           _encode_text_color_inputs, _extract_seed_and_sigma_from_context, _get_binary_mask,
+                           _rgb_of, always_round, pack_weight_map, packed_key)
 from . import _native, fused_ops
 from .scheduler import (SIGMA_SCHEDULERS, EulerAncestralDiscreteScheduler, LMSDiscreteScheduler, history_length,
                         step_form)
@@ -256,6 +259,11 @@ class PwWSampler:
     guess mode) and summed level by level in ONE native combine, and the UNet adds the sum.  If any unit is in guess
     mode, every unit runs on the m cond rows and only the cond half gets residuals (hook_pww.py:39-53, 199).  Each set
     of active units over the run has its own captured graph.
+
+    `record_attention=True` records, inside the UNet's cross-attention launches (`pww_xattn_fused_rec_*`), the softmax
+    mass every painted region's tokens receive from each pixel of each cond image, biased or not; `attention_maps()`
+    returns it per image as [R, h, w] maps.  The accumulators are zeroed at set-up and by `restart()`.  The latents are
+    the same bits as without recording.  The ControlNets' cross-attention is not recorded.
     """
 
     def __init__(self, unet, scheduler: LMSDiscreteScheduler, cond_ctxs: Sequence[dict], uncond_ctxs: Sequence[dict],
@@ -265,7 +273,8 @@ class PwWSampler:
                  noise_seed: Union[None, int, Sequence[int]] = None, controlnet=None,
                  control_image: Union[None, torch.Tensor, Sequence[torch.Tensor]] = None,
                  controlnet_conditioning_scale: Union[float, Sequence[float]] = 1.0, guess_mode: bool = False,
-                 control_guidance_start: float = 0.0, control_guidance_end: float = 1.0):
+                 control_guidance_start: float = 0.0, control_guidance_end: float = 1.0,
+                 record_attention: bool = False):
         if not isinstance(scheduler, SIGMA_SCHEDULERS):
             raise TypeError(f"PwWSampler does not support {type(scheduler).__name__}; use one of "
                             + ", ".join(c.__name__ for c in SIGMA_SCHEDULERS))
@@ -335,6 +344,53 @@ class PwWSampler:
             if len(units[0]) == 1:
                 self.controlnet = units[0][0]
             self._set_up_control(*units)
+        self.record_attention = bool(record_attention)
+        self._rec_levels: List[tuple] = []     # (N, h_r, w_r, accumulator [m, H, N, 16]) per cross-attention level
+        if self.record_attention:
+            self._set_up_recording(cond_ctxs)
+
+    def _set_up_recording(self, conds):
+        """record_attention: the cond images' token -> region rows, and one zeroed fp32 [m, H_l, N_l, 16] accumulator per
+        UNet level, at fixed addresses (captured graphs add into them).  Level l has N_l = h_r * w_r query rows, the grid
+        the weight-map builder uses at ratio 8 * 2^l, and the UNet config's head count of that level."""
+        m, dev = self.m, self.device
+        rows = [c.get(REGION_INDEX_KEY) for c in conds]
+        if any(r is None for r in rows):
+            raise ValueError(f"record_attention needs every cond dict's {REGION_INDEX_KEY} (set by the conditioning "
+                             f"builder for at most {MAX_RECORDED_REGIONS} regions)")
+        self._region_counts = [int(c[REGION_COUNT_KEY]) for c in conds]
+        ridx = torch.stack([r.to(torch.int8) for r in rows], 0).contiguous().to(dev)
+        rec_index = torch.tensor(list(range(m)) + [-1] * m, dtype=torch.int32, device=dev)   # only the cond rows
+        cfg = getattr(self.unet, "config", None)
+        heads = getattr(cfg, "attention_heads", getattr(cfg, "attention_head_dim", None))
+        channels = getattr(cfg, "block_out_channels", None)
+        if heads is None or channels is None:
+            raise TypeError(f"record_attention needs the UNet config's block_out_channels and attention heads "
+                            f"({type(self.unet).__name__} has none)")
+        heads = list(heads) if isinstance(heads, (list, tuple)) else [int(heads)] * len(channels)
+        h, w = self.latents.shape[-2:]
+        for lvl, r in enumerate(RATIOS[:len(channels)]):
+            hr, wr = always_round(8 * h / r), always_round(8 * w / r)
+            self._rec_levels.append((hr * wr, hr, wr, torch.zeros((m, int(heads[lvl]), hr * wr, MAX_RECORDED_REGIONS),
+                                                                   dtype=torch.float32, device=dev)))
+        self._ctx[_attention.RECORD_KEY] = {n: (ridx, rec_index, acc) for n, _, _, acc in self._rec_levels}
+        # every cross-attention module (a transformer block's attn2) is called once per UNet forward
+        self._rec_calls = sum(1 for name, _ in self.unet.named_modules() if name.split(".")[-1] == "attn2")
+
+    def attention_maps(self) -> List[torch.Tensor]:
+        """record_attention: per cond image, fp32 [R, h, w] on the CPU at latent resolution, R = its regions.  Map r is
+        the mean, over every recorded (step, cross-attention call, head), of the softmax mass the tokens of region r's
+        label receive, upsampled bilinearly (align_corners=False) from the call's grid to the latent grid."""
+        if not self.record_attention:
+            raise RuntimeError("attention_maps() needs PwWSampler(..., record_attention=True)")
+        m, (h, w) = self.m, self.latents.shape[-2:]
+        total = torch.zeros((m, MAX_RECORDED_REGIONS, h, w), dtype=torch.float32, device=self.device)
+        for _, hr, wr, acc in self._rec_levels:
+            mean = acc.sum(1) / acc.shape[1]                                   # head mean: [m, N, 16]
+            grid = mean.view(m, hr, wr, MAX_RECORDED_REGIONS).permute(0, 3, 1, 2)
+            total += F.interpolate(grid, size=(h, w), mode="bilinear", align_corners=False)
+        total /= max(1, self._rec_calls * self._step_no)
+        return [total[i, :r].cpu() for i, r in enumerate(self._region_counts)]
 
     def _set_up_control(self, nets, images, weights, guesses, starts, ends):
         """Validate every unit's ControlNet arguments (per-unit lists); embed the hints, build the scale tables and the
@@ -560,6 +616,8 @@ class PwWSampler:
         """Rewind to step 0 (empty history, the first noise row), optionally with new latents."""
         self._step_no = 0
         self._derivs.zero_()
+        for *_, acc in self._rec_levels:
+            acc.zero_()
         if latents is not None:
             self.latents.copy_(latents)
 
@@ -576,9 +634,10 @@ class PwWSampler:
             # one graph per set of active ControlNets (at most 2U + 1 over a run), each captured at the first step
             # that needs it; its two warm-up steps are undone, so the replay below is this step
             if active not in self._graphs:
-                snap = (self.latents.clone(), self._derivs.clone())
+                snap = [self.latents.clone(), self._derivs.clone()] + [acc.clone() for *_, acc in self._rec_levels]
                 self._graphs[active] = self._capture(lambda: self._step_body(active), warmup=2)
-                self.latents.copy_(snap[0]); self._derivs.copy_(snap[1])
+                for buf, old in zip([self.latents, self._derivs] + [acc for *_, acc in self._rec_levels], snap):
+                    buf.copy_(old)
             self._graphs[active][0].replay()
         self._step_no += 1
 
@@ -649,6 +708,7 @@ def paint_with_words(
     guess_mode: Union[bool, Sequence[bool]] = False,
     control_guidance_start: Union[float, Sequence[float]] = 0.0,
     control_guidance_end: Union[float, Sequence[float]] = 1.0,
+    return_attention_maps: bool = False,
 ):
     """paint_with_words.py:391-510.  Returns one PIL.Image (or the final latents with return_latents).
     `max_prompt_chunks` (1 .. 3): a prompt longer than 75 tokens fills up to that many 77-token CLIP chunks instead of
@@ -660,7 +720,9 @@ def paint_with_words(
     which words go where; `controlnet_conditioning_scale`, `guess_mode` and the guidance window as in `PwWSampler`.
     Several ControlNets (e.g. pose for the figure, edges for the background): `controlnet` a list of up to 10,
     `control_image` a list with one such image per ControlNet, and the other four arguments one value or one per
-    ControlNet."""
+    ControlNet.
+    `return_attention_maps=True` returns (image, RegionAttention): the per-region cross-attention maps of the cond image
+    recorded inside the attention kernels over the whole run, with each region's adherence to its painted area."""
     control = _control_arguments(controlnet, control_image, color_map_image.size, "color_map_image",
                                  controlnet_conditioning_scale, guess_mode, control_guidance_start,
                                  control_guidance_end)
@@ -678,8 +740,11 @@ def paint_with_words(
         # the reference draws img2img's noise from the global RNG as it stands: unseeded here
         latents, timesteps = _img2img_latents(vae, scheduler, init_image, num_inference_steps, strength, device)
     sampler = PwWSampler(unet, scheduler, [cond], [uncond], latents, weight_function, guidance_scale,
-                         timesteps=timesteps, noise_seed=seed, **control)
-    return _result(vae, sampler.run(), return_latents)
+                         timesteps=timesteps, noise_seed=seed, record_attention=return_attention_maps, **control)
+    result = _result(vae, sampler.run(), return_latents)
+    if not return_attention_maps:
+        return result
+    return result, _region_attention(sampler.attention_maps()[0], cond, color_context, color_map_image)
 
 
 def _tools(preloaded_utils, device, scheduler_type, local_model_path, hf_model_path, model_token, torch_dtype):
@@ -720,6 +785,50 @@ def _img2img_latents(vae, scheduler, init_image, num_inference_steps: int, stren
 def _result(vae, latents: torch.Tensor, return_latents: bool):
     """What the public functions return for one image: its final latents, or the PIL image they decode to."""
     return latents if return_latents else _pil_from_latents(vae, latents)[0]
+
+
+@dataclasses.dataclass
+class RegionAttention:
+    """Where each painted word looked, from `return_attention_maps=True`.
+    labels    : the `color_context` labels, in order (region r = entry r)
+    maps      : fp32 [R, h, w] at latent resolution: mean softmax mass region r's tokens receive (PwWSampler.attention_maps)
+    coverage  : fp32 [R, h, w]: the fraction of each latent pixel that region r's colour covers in the colour map
+    adherence : fp32 [R]: sum(maps * coverage) / sum(maps) per region -- the share of the region's attention that falls
+                inside its painted area (NaN for a region whose label is not in the prompt)"""
+    labels: List[str]
+    maps: torch.Tensor
+    coverage: torch.Tensor
+    adherence: torch.Tensor
+
+
+def region_adherence(maps: torch.Tensor, coverage: torch.Tensor, has_tokens: Sequence[bool]) -> torch.Tensor:
+    """fp32 [R]: sum(maps[r] * coverage[r]) / sum(maps[r]) for every region with tokens, NaN for the others."""
+    num = (maps * coverage).flatten(1).sum(1)
+    den = maps.flatten(1).sum(1)
+    out = num / den
+    out[~torch.tensor([bool(t) for t in has_tokens], dtype=torch.bool)] = float("nan")
+    return out.to(torch.float32)
+
+
+def region_coverage(color_map_image: Image.Image, color_context: dict, size: Tuple[int, int]) -> torch.Tensor:
+    """fp32 [R, h, w]: region r's binary colour mask (exact colour match, as the conditioning builder matches it)
+    area-averaged to the latent size (h, w)."""
+    pixels = np.array(color_map_image.convert("RGB"))
+    masks = [torch.from_numpy((pixels == _rgb_of(c)).all(axis=-1)).to(torch.float32) for c in color_context]
+    if not masks:
+        return torch.zeros((0,) + tuple(size), dtype=torch.float32)
+    return F.interpolate(torch.stack(masks, 0)[:, None], size=tuple(size), mode="area")[:, 0]
+
+
+def _region_attention(maps: torch.Tensor, cond: dict, color_context: dict, color_map_image) -> RegionAttention:
+    """The RegionAttention of one image from its recorded maps, cond dict and colour inputs."""
+    labels = [spec.rpartition(",")[0]
+              for spec in _extract_seed_and_sigma_from_context(dict(color_context))[0].values()]
+    coverage = region_coverage(color_map_image, color_context, tuple(maps.shape[-2:]))
+    ridx = cond[REGION_INDEX_KEY]
+    has_tokens = [bool((ridx == r).any()) for r in range(len(labels))]
+    maps = maps[:len(labels)]
+    return RegionAttention(labels, maps, coverage, region_adherence(maps, coverage, has_tokens))
 
 
 def _control_arguments(controlnet, control_image, size: Tuple[int, int], size_of: str, conditioning_scale,
@@ -800,6 +909,7 @@ def paint_with_words_batch(
     guess_mode: Union[bool, Sequence[bool]] = False,
     control_guidance_start: Union[float, Sequence[float]] = 0.0,
     control_guidance_end: Union[float, Sequence[float]] = 1.0,
+    return_attention_maps: bool = False,
 ):
     """Many images, each with its own settings, in as few samplers as possible.  `settings[i]` is a dict of the
     per-image keyword arguments of `paint_with_words` (BATCH_SETTING_KEYS: color_context, color_map_image, input_prompt,
@@ -815,7 +925,8 @@ def paint_with_words_batch(
     2 * max_batch_size UNet batch with CFG), whatever their weight functions and guidance scales.  The default of 8 gave
     the most images/s of k = 1, 2, 4, 8 at 512x512 (BASELINE.md section 4) and bounds memory.  Sizes that are not multiples of 64 need the single-image weight-map fallback and
     run one image per sampler.  img2img (init_image / strength) is not batched.  `torch_dtype` as in
-    `paint_with_words`."""
+    `paint_with_words`.  `return_attention_maps=True` returns a list of (image, RegionAttention) pairs in input order
+    (see `paint_with_words`)."""
     entries = _batch_settings(settings)
     if max_batch_size < 1:
         raise ValueError("max_batch_size must be >= 1")
@@ -840,6 +951,7 @@ def paint_with_words_batch(
         solo = width % 64 != 0 or height % 64 != 0
         keys.append(None if solo else (height // 8, width // 8, int(cond["CONTEXT_TENSOR"].shape[1])))
     results: List[Optional[torch.Tensor]] = [None] * len(entries)
+    attention: List[Optional[RegionAttention]] = [None] * len(entries)
     for idx in batch_groups(keys, max_batch_size):
         control = controls[idx[0]]
         if control and isinstance(controlnet, (list, tuple)):
@@ -857,12 +969,18 @@ def paint_with_words_batch(
         sampler = PwWSampler(unet, scheduler, [encoded[i][0] for i in idx], [encoded[i][1] for i in idx],
                              torch.cat([encoded[i][2] for i in idx], 0),
                              [entries[i]["weight_function"] for i in idx], [entries[i]["guidance_scale"] for i in idx],
-                             timesteps=scheduler.timesteps, noise_seed=[entries[i]["seed"] for i in idx], **control)
+                             timesteps=scheduler.timesteps, noise_seed=[entries[i]["seed"] for i in idx],
+                             record_attention=return_attention_maps, **control)
         latents = sampler.run()
+        maps = sampler.attention_maps() if return_attention_maps else None
         for j, i in enumerate(idx):
             results[i] = latents[j:j + 1].clone()
+            if maps is not None:
+                attention[i] = _region_attention(maps[j], encoded[i][0], entries[i]["color_context"],
+                                                 entries[i]["color_map_image"])
         del sampler
-    return [_result(vae, lat, return_latents) for lat in results]
+    images = [_result(vae, lat, return_latents) for lat in results]
+    return list(zip(images, attention)) if return_attention_maps else images
 
 
 def prepare_mask_and_masked_image(image, mask):
@@ -921,11 +1039,13 @@ def paint_with_words_inpaint(
     guess_mode: Union[bool, Sequence[bool]] = False,
     control_guidance_start: Union[float, Sequence[float]] = 0.0,
     control_guidance_end: Union[float, Sequence[float]] = 1.0,
+    return_attention_maps: bool = False,
 ):
     """paint_with_words_inpaint.py:137-270: 9-channel UNet input cat[latents, mask, masked-image latents].
     `max_prompt_chunks`, `torch_dtype` and the ControlNet arguments as in `paint_with_words`; the colour map is resized
     to the init image, so `control_image` has the init image's size.  The ControlNet sees the 4 latent channels of
-    the UNet input (hook_pww.py:113-119)."""
+    the UNet input (hook_pww.py:113-119).  `return_attention_maps` as in `paint_with_words` (coverage from the resized
+    colour map)."""
     width, height = init_image.size
     control = _control_arguments(controlnet, control_image, (width, height), "init_image (and resized color_map_image)",
                                  controlnet_conditioning_scale, guess_mode, control_guidance_start,
@@ -956,8 +1076,11 @@ def paint_with_words_inpaint(
             f"num_channels_masked_image: {masked_image_latents.shape[1]} = {total}.")
     sampler = PwWSampler(unet, scheduler, [cond], [uncond], latents, weight_function, guidance_scale,
                          extra_input=torch.cat([mask, masked_image_latents], 1).float(), timesteps=timesteps,
-                         noise_seed=seed, **control)
-    return _result(vae, sampler.run(), return_latents)
+                         noise_seed=seed, record_attention=return_attention_maps, **control)
+    result = _result(vae, sampler.run(), return_latents)
+    if not return_attention_maps:
+        return result
+    return result, _region_attention(sampler.attention_maps()[0], cond, color_context, color_map_image)
 
 
 # ---------------------------------------------------------------------------------------------

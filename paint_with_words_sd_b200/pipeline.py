@@ -180,11 +180,12 @@ MAX_CONTROLNET_UNITS = 10      # the reference extension's "Multi ControlNet: Ma
 
 
 def _control_units(controlnet, control_image, conditioning_scale, guess_mode, start, end) -> tuple:
-    """PwWSampler's ControlNet arguments as per-unit lists (nets, images, weights, guesses, starts, ends).  One
-    ControlNetModel is one unit with the arguments as they are.  A list of U (1..10) units takes `control_image` as a
-    list of U entries (each one tensor or one per image), `controlnet_conditioning_scale` as one float or U entries
-    (each one float or one per image), and `guess_mode` and the window each as one value or U values; lists are indexed
-    by unit first."""
+    """The ControlNet arguments as per-unit lists (nets, images, weights, guesses, starts, ends), for one ControlNet or
+    a list of them.  One ControlNetModel is one unit with the arguments as they are.  A list of U (1..10) units takes
+    `control_image` as a list of U entries (each one tensor or one per image), `controlnet_conditioning_scale` as one
+    float or U entries (each one float or one per image), and `guess_mode` and the window each as one value or U values;
+    lists are indexed by unit first.  The per-unit lists, passed in again, come out unchanged (`_control_arguments`
+    hands them to PwWSampler)."""
     if not isinstance(controlnet, (list, tuple)):
         return [controlnet], [control_image], [conditioning_scale], [bool(guess_mode)], [start], [end]
     U = len(controlnet)
@@ -254,11 +255,12 @@ class PwWSampler:
 
     Multi-ControlNet (the extension's control units): `controlnet` a list of 1..10 ControlNetModels, `control_image` a
     list with one entry per unit (each one tensor or m), and `controlnet_conditioning_scale`, `guess_mode` and the window
-    each one value or one per unit (a unit's weight may again be m floats).  A list of one is the single path above.
-    With several, the units active at a step run in unit order, their residuals scaled (0.825 ** (12 - k) for a unit in
-    guess mode) and summed level by level in ONE native combine, and the UNet adds the sum.  If any unit is in guess
-    mode, every unit runs on the m cond rows and only the cond half gets residuals (hook_pww.py:39-53, 199).  Each set
-    of active units over the run has its own captured graph.
+    each one value or one per unit (a unit's weight may again be m floats); one ControlNet is a list of one.  The units
+    active at a step run in unit order.  With one active unit, the UNet's inject scales its residuals as above.  With
+    two or more, their residuals are scaled (0.825 ** (12 - k) for a unit in guess mode) and summed level by level in
+    ONE native combine, and the UNet adds the sum.  If any unit is in guess mode, every unit runs on the m cond rows and
+    only the cond half gets residuals (hook_pww.py:39-53, 199).  Each set of active units over the run has its own
+    captured graph.
 
     `record_attention=True` records, inside the UNet's cross-attention launches (`pww_xattn_fused_rec_*`), the softmax
     mass every painted region's tokens receive from each pixel of each cond image, biased or not; `attention_maps()`
@@ -339,11 +341,8 @@ class PwWSampler:
             if control_image is not None:
                 raise ValueError("control_image is given but controlnet is None")
         else:
-            units = _control_units(controlnet, control_image, controlnet_conditioning_scale, guess_mode,
-                                   control_guidance_start, control_guidance_end)
-            if len(units[0]) == 1:
-                self.controlnet = units[0][0]
-            self._set_up_control(*units)
+            self._set_up_control(*_control_units(controlnet, control_image, controlnet_conditioning_scale, guess_mode,
+                                                 control_guidance_start, control_guidance_end))
         self.record_attention = bool(record_attention)
         self._rec_levels: List[tuple] = []     # (N, h_r, w_r, accumulator [m, H, N, 16]) per cross-attention level
         if self.record_attention:
@@ -393,9 +392,8 @@ class PwWSampler:
         return [total[i, :r].cpu() for i, r in enumerate(self._region_counts)]
 
     def _set_up_control(self, nets, images, weights, guesses, starts, ends):
-        """Validate every unit's ControlNet arguments (per-unit lists); embed the hints, build the scale tables and the
-        ControlNets' context.  One unit: CONTROL_SCALES for the UNet's inject.  Several: one [|A|, levels, rows] table
-        per active set A that occurs, for the combine."""
+        """Validate every unit's ControlNet arguments (per-unit lists); embed the hints, stack the scale tables of
+        every active set and build the ControlNets' context."""
         from .controlnet import ControlNetModel
         unet, m, U = self.unet, self.m, len(nets)
         h, w = self.latents.shape[-2:]
@@ -406,7 +404,7 @@ class PwWSampler:
         ucfg = getattr(unet, "config", None)
         for u, (net, start, end) in enumerate(zip(nets, starts, ends)):
             def arg(name):           # the argument, with the unit's index when there are several
-                return name if U == 1 else f"{name}[{u}]"
+                return f"{name}[{u}]" if U > 1 else name
             if not isinstance(net, ControlNetModel):
                 raise TypeError(f"{arg('controlnet')} must be a paint_with_words_sd_b200.controlnet.ControlNetModel, "
                                 f"got {type(net).__name__}")
@@ -447,12 +445,11 @@ class PwWSampler:
         rows = m if self.guess_mode else 2 * m
         tables = [control_scales(wt, g, len(net.controlnet_down_blocks) + 1)[:, :rows]
                   for net, wt, g in zip(nets, weights, guesses)]
-        if U == 1:
-            self._ctx["CONTROL_SCALES"] = tables[0].to(dev)
-        else:            # the scales are applied in the combine; the UNet adds the sum at scale 1
-            full = torch.stack(tables, 0)
-            self._combine_scales = {a: full[[u for u in range(U) if a[u]]].contiguous().to(dev)
-                                    for a in set(self._active_sets) if any(a)}
+        # per active set A that occurs, the active units' tables stacked: [|A|, levels, rows].  One unit's table is the
+        # UNet inject's CONTROL_SCALES; two or more are applied in the combine, and the UNet adds the sum at scale 1
+        full = torch.stack(tables, 0)
+        self._combine_scales = {a: full[[u for u in range(U) if a[u]]].contiguous().to(dev)
+                                for a in set(self._active_sets) if any(a)}
         # the ControlNets' own dict: the plain text context (cond rows only in guess mode), no weight maps, so every
         # cross-attention call is unbiased; its K/V are staged once like the UNet's (the cache is keyed by module, so
         # the units share the dict, and a model that appears twice its K/V)
@@ -524,11 +521,6 @@ class PwWSampler:
         return ctx
 
     # -- one step, expressed only with device tensors / device scalars --------------------------
-    @property
-    def _hint(self) -> torch.Tensor:
-        """The single ControlNet's hint embedding (unit 0's with several)."""
-        return self._hints[0]
-
     def _step_body(self, active: tuple = ()):
         m, (h, w) = self.m, self.latents.shape[-2:]
         L = _native.lib()
@@ -548,13 +540,16 @@ class PwWSampler:
             x = self._unet_in[:m, :4] if self.guess_mode else self._unet_in[:, :4]
             outs = [net(x, t, encoder_hidden_states=self._control_ctx, controlnet_cond_embedding=hint,
                         return_dict=False) for net, hint, on in zip(self._nets, self._hints, active) if on]
-            if len(self._nets) == 1:
-                down, mid = outs[0]
+            per_unit = [list(d) + [md] for d, md in outs]
+            scales = self._combine_scales[active]
+            if len(scales) == 1:
+                # one active unit: the UNet's inject scales its residuals (a captured graph keeps the table's address)
+                *down, mid = per_unit[0]
+                self._ctx["CONTROL_SCALES"] = scales[0]
             else:
-                # several units: their scaled residuals summed level by level in unit order (hook_pww.py:136-139), in
-                # place into the first active unit's, then added by the UNet at scale 1
-                per_unit = [list(d) + [md] for d, md in outs]
-                scales = self._combine_scales[active]
+                # several: their scaled residuals summed level by level in unit order (hook_pww.py:136-139), in place
+                # into the first active unit's, then added by the UNet at scale 1
+                self._ctx.pop("CONTROL_SCALES", None)
                 if fused_ops.is_fast(per_unit[0][0]):
                     *down, mid = fused_ops.control_combine(per_unit, scales)
                 else:
@@ -599,7 +594,7 @@ class PwWSampler:
         if "CONTEXT_TENSOR" in pinned and self._ctx.get("KV_CACHE"):
             # the cached K/V follow the new context: 16 small GEMMs, replayed as one CUDA graph (the ControlNet's
             # context is a view of the same tensor, so its cached K/V are refreshed too)
-            ctxs = [self._ctx] + ([self._control_ctx] if self.controlnet is not None else [])
+            ctxs = [self._ctx] + ([self._control_ctx] if self._nets else [])
 
             def refresh():
                 for c in ctxs:
@@ -833,27 +828,26 @@ def _region_attention(maps: torch.Tensor, cond: dict, color_context: dict, color
 
 def _control_arguments(controlnet, control_image, size: Tuple[int, int], size_of: str, conditioning_scale,
                        guess_mode: bool, start: float, end: float) -> dict:
-    """PwWSampler's ControlNet keyword arguments from the public ones, {} without a controlnet; the hint image must be
-    `size` (W, H).  With a list of ControlNets, `control_image` is a list of one such image per unit, and the other
-    arguments are one value or one per unit (`_control_units`)."""
+    """PwWSampler's ControlNet keyword arguments from the public ones, as per-unit lists (`_control_units`), {} without
+    a controlnet.  Every hint image must be `size` (W, H); with a list of ControlNets, `control_image` is a list of one
+    such image per unit."""
     if controlnet is None:
         if control_image is not None:
             raise ValueError("control_image is given but controlnet is None")
         return {}
-    multi = isinstance(controlnet, (list, tuple))
-    _control_units(controlnet, control_image, conditioning_scale, guess_mode, start, end)     # counts and lengths
-    images = list(control_image) if multi else [control_image]
+    nets, images, weights, guesses, starts, ends = _control_units(controlnet, control_image, conditioning_scale,
+                                                                  guess_mode, start, end)
+    indexed = isinstance(controlnet, (list, tuple))       # a list's images are named by unit
     for u, image in enumerate(images):
-        name = f"control_image[{u}]" if multi else "control_image"
+        name = f"control_image[{u}]" if indexed else "control_image"
         if not isinstance(image, Image.Image):
             raise ValueError(f"controlnet needs a {name} (a PIL image of the {size_of} size {size}), got "
                              f"{type(image).__name__}")
         if image.size != tuple(size):
             raise ValueError(f"{name} is {image.size}; it must have the {size_of} size {tuple(size)}")
-    tensors = [control_image_tensor(image) for image in images]
-    return dict(controlnet=controlnet, control_image=tensors if multi else tensors[0],
-                controlnet_conditioning_scale=conditioning_scale, guess_mode=guess_mode, control_guidance_start=start,
-                control_guidance_end=end)
+    return dict(controlnet=nets, control_image=[control_image_tensor(image) for image in images],
+                controlnet_conditioning_scale=weights, guess_mode=guesses, control_guidance_start=starts,
+                control_guidance_end=ends)
 
 
 # the per-image keyword arguments of paint_with_words that paint_with_words_batch takes per entry
@@ -954,18 +948,11 @@ def paint_with_words_batch(
     attention: List[Optional[RegionAttention]] = [None] * len(entries)
     for idx in batch_groups(keys, max_batch_size):
         control = controls[idx[0]]
-        if control and isinstance(controlnet, (list, tuple)):
-            # per unit u: the images' hints for u and their weights for u (an entry's one float is every unit's)
-            def unit_weight(s, u):
-                return s if isinstance(s, (int, float)) else s[u]
-            units = range(len(controlnet))
+        if control:         # the batch's ControlNets and windows; per unit, each image's own hint and weight
+            units = range(len(control["controlnet"]))
             control = dict(control, control_image=[[controls[i]["control_image"][u] for i in idx] for u in units],
-                           controlnet_conditioning_scale=[
-                               [unit_weight(controls[i]["controlnet_conditioning_scale"], u) for i in idx]
-                               for u in units])
-        elif control:       # the batch's ControlNet and window, each image's own hint and weight
-            control = dict(control, control_image=[controls[i]["control_image"] for i in idx],
-                           controlnet_conditioning_scale=[controls[i]["controlnet_conditioning_scale"] for i in idx])
+                           controlnet_conditioning_scale=[[controls[i]["controlnet_conditioning_scale"][u] for i in idx]
+                                                          for u in units])
         sampler = PwWSampler(unet, scheduler, [encoded[i][0] for i in idx], [encoded[i][1] for i in idx],
                              torch.cat([encoded[i][2] for i in idx], 0),
                              [entries[i]["weight_function"] for i in idx], [entries[i]["guidance_scale"] for i in idx],

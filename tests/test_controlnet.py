@@ -207,7 +207,7 @@ def _sampler_inputs(m=1, size=64):
 WF = lambda w, sigma, qk: 0.4 * w * qk.max()     # noqa: E731
 
 
-def test_sampler_builds_the_control_state_on_the_cpu(models):
+def test_sampler_builds_one_controlnets_state_on_the_cpu(models):
     unet, net = models
     sch, conds, unconds, lat = _sampler_inputs(m=2)
     imgs = [torch.rand(1, 3, 64, 64, generator=torch.manual_seed(i)) for i in range(2)]
@@ -215,13 +215,16 @@ def test_sampler_builds_the_control_state_on_the_cpu(models):
                       controlnet_conditioning_scale=[0.5, 1.5], control_guidance_start=0.25,
                       control_guidance_end=0.5)
     assert s._control_active == [False, True, True, False]
-    assert torch.equal(s._ctx["CONTROL_SCALES"], PL.control_scales([0.5, 1.5], False))
-    assert tuple(s._hint.shape) == (4, 160, 8, 8)
-    assert torch.equal(s._hint[:2], s._hint[2:]) and torch.equal(s._hint[:2], net.embed_condition(torch.cat(imgs)))
+    # one active unit: its table is the inject's CONTROL_SCALES, which the step puts into the context
+    assert list(s._combine_scales) == [(True,)] and "CONTROL_SCALES" not in s._ctx
+    assert torch.equal(s._combine_scales[(True,)], PL.control_scales([0.5, 1.5], False)[None])
+    hint = s._hints[0]
+    assert len(s._hints) == 1 and tuple(hint.shape) == (4, 160, 8, 8)
+    assert torch.equal(hint[:2], hint[2:]) and torch.equal(hint[:2], net.embed_condition(torch.cat(imgs)))
     assert s._control_ctx["CONTEXT_TENSOR"].data_ptr() == s._ctx["CONTEXT_TENSOR"].data_ptr()
     g = PL.PwWSampler(unet, sch, conds, unconds, lat, WF, controlnet=net, control_image=imgs[0], guess_mode=True)
-    assert tuple(g._hint.shape) == (2, 160, 8, 8) and g._control_ctx["CONTEXT_TENSOR"].shape[0] == 2
-    assert torch.equal(g._ctx["CONTROL_SCALES"], PL.control_scales([1.0, 1.0], True))
+    assert tuple(g._hints[0].shape) == (2, 160, 8, 8) and g._control_ctx["CONTEXT_TENSOR"].shape[0] == 2
+    assert torch.equal(g._combine_scales[(True,)], PL.control_scales([1.0, 1.0], True)[None])
 
 
 class _NoResidualUNet(torch.nn.Module):

@@ -223,7 +223,7 @@ def test_closed_window_is_the_plain_sampler_bit_for_bit(use_graph):
         assert s.native_launches_per_step_without_control == p.native_launches_per_step
 
 
-def test_launch_accounting_of_the_two_graphs():
+def test_launch_accounting_in_and_out_of_the_window():
     """In the window: the plain step + the ControlNet's launches + ONE injection launch; outside it: the plain step."""
     cfg = UNetConfig.tiny()
     net = build_controlnet(cfg, seed=1, dtype=torch.float16, device="cuda")
@@ -234,7 +234,7 @@ def test_launch_accounting_of_the_two_graphs():
         x = torch.randn(2, 4, SIZE // 8, SIZE // 8, device="cuda", dtype=torch.float16)
         before = _native.launch_count
         net(x, torch.tensor([500.0], device="cuda"), encoder_hidden_states=s._control_ctx,
-            controlnet_cond_embedding=s._hint)
+            controlnet_cond_embedding=s._hints[0])
         net_launches = _native.launch_count - before
     finally:
         P.unpatch_all()

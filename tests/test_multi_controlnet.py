@@ -111,7 +111,7 @@ def test_active_sets_and_their_tables(models, windows, sets):
         assert torch.equal(t, torch.tensor(want)[:, None, None].expand(len(want), 13, 2))
 
 
-def test_a_list_of_one_is_the_single_path(models):
+def test_a_list_of_one_sets_up_as_one_controlnet(models):
     unet, a, _ = models
     sch, conds, unconds, lat = _sampler_inputs(m=2)
     img = _imgs(1)[0]
@@ -119,10 +119,12 @@ def test_a_list_of_one_is_the_single_path(models):
                         controlnet_conditioning_scale=[0.7], guess_mode=[True], control_guidance_start=[0.25])
     single = PL.PwWSampler(unet, sch, conds, unconds, lat, WF, controlnet=a, control_image=img,
                            controlnet_conditioning_scale=0.7, guess_mode=True, control_guidance_start=0.25)
-    assert one.controlnet is a and one._nets == [a]
-    assert torch.equal(one._ctx["CONTROL_SCALES"], single._ctx["CONTROL_SCALES"])
+    assert one.controlnet == [a] and single.controlnet is a and one._nets == single._nets == [a]
+    assert list(one._combine_scales) == list(single._combine_scales) == [(True,)]
+    assert torch.equal(one._combine_scales[(True,)], single._combine_scales[(True,)])
+    assert torch.equal(one._combine_scales[(True,)], PL.control_scales([0.7, 0.7], True)[None])
     assert one._active_sets == single._active_sets == [(False,), (True,), (True,), (True,)]
-    assert torch.equal(one._hint, single._hint)
+    assert len(one._hints) == len(single._hints) == 1 and torch.equal(one._hints[0], single._hints[0])
 
 
 def test_sampler_rejects_bad_multi_control_arguments(models):

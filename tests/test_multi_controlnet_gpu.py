@@ -3,9 +3,9 @@
 Kernel: `pww_control_combine_{f16,bf16}` is bitwise the torch left fold `(r0 * s0).to(E) + (r1 * s1).to(E) + ...` at
 the SD1.5, SD2.1 and tiny residual shapes, for U = 2, 3, 10 units, m = 1, 8, rows = B and B / 2, in place into unit 0's
 residuals and out of place.  Loop: `PwWSampler(controlnet=[a, b])` with tiny ControlNets against
-`reference_multi_controlnet_loop` (rel RMSE < 3e-2, the bar of the other loop tests), a weight-0 second unit against
-the single-ControlNet sampler bit for bit, launch accounting per active set, guess-mode routing, batching and the
-public API."""
+`reference_multi_controlnet_loop` (rel RMSE < 3e-2, the bar of the other loop tests), a weight-0 second unit and a
+second unit that is never in its window against the single-ControlNet sampler bit for bit, launch accounting per
+active set, guess-mode routing, batching and the public API."""
 import pytest
 import torch
 from PIL import Image
@@ -148,6 +148,22 @@ def test_a_weight_zero_second_unit_is_the_single_sampler_bit_for_bit(use_graph):
         assert set(s._graphs) == {(True, True)}
 
 
+@pytest.mark.parametrize("use_graph", [False, True])
+def test_a_second_unit_never_in_its_window_is_the_single_sampler_bit_for_bit(use_graph):
+    """A step with one active unit of several runs no combine: the single ControlNet's step, bits and launches."""
+    cfg = UNetConfig.tiny()
+    a = build_controlnet(cfg, seed=1, dtype=torch.float16, device="cuda")
+    b = build_controlnet(cfg, seed=2, dtype=torch.float16, device="cuda")
+    two, s = _gpu([a, b], use_graph, controlnet_conditioning_scale=0.7, control_guidance_start=[0.0, 1.0],
+                  control_guidance_end=[1.0, 1.0])
+    one, single = _gpu(a, use_graph, controlnet_conditioning_scale=0.7)
+    assert s._active_sets == [(True, False)] * STEPS
+    assert torch.equal(two, one)
+    if use_graph:
+        assert s.native_launches_per_active_set == {(True, False): single.native_launches_per_step}
+        assert s.native_launches_per_step is None
+
+
 def _net_launches(net, s, unit):
     P.patch_unet(net)
     try:
@@ -160,8 +176,9 @@ def _net_launches(net, s, unit):
         P.unpatch_all()
 
 
-def test_launch_accounting_per_active_set():
-    """A step with active set A: the plain step + each active ControlNet's launches + the combine + the inject."""
+def test_launch_accounting_per_active_set_and_its_size():
+    """A step with active set A: the plain step + each active ControlNet's launches + the inject, and the combine
+    before it when two or more units are active."""
     cfg = UNetConfig.tiny()
     nets = [build_controlnet(cfg, seed=s, dtype=torch.float16, device="cuda") for s in (1, 2)]
     _, s = _gpu(nets, control_guidance_start=[0.0, 0.25], control_guidance_end=[0.5, 0.75])
@@ -172,7 +189,7 @@ def test_launch_accounting_per_active_set():
     launches = s.native_launches_per_active_set
     assert set(launches) == {(True, False), (True, True), (False, True)} and len(s._graphs) == 3
     for a, got in launches.items():
-        want = plain.native_launches_per_step + sum(n for n, on in zip(per_net, a) if on) + 2
+        want = plain.native_launches_per_step + sum(n for n, on in zip(per_net, a) if on) + (2 if sum(a) > 1 else 1)
         assert got == want, (a, got, want)
     assert s.native_launches_per_step == launches[(True, True)]
     assert s.native_launches_per_step_without_control is None

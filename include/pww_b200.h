@@ -318,6 +318,21 @@ int pww_resnet_residual_f16(const void* a, const void* h, const float* bias, voi
 int pww_resnet_residual_bf16(const void* a, const void* h, const float* bias, void* out, int64_t rows, int C,
                              void* stream);
 
+/* T2I-Adapter feature add fused into a residual epilogue, over [rows, pixels, C] channels-last activations:
+ *   s = E( a + b [+ bias[c]] )                               every row
+ *   out = E( s + feat )  for rows r < feat_rows,  out = s  otherwise
+ * a and b are the two residual operands (a transformer's projection and its input, or a ResNet block's shortcut and its
+ * bias-free conv2 output), bias an fp32 [C] array or NULL (no bias term), feat a [feat_rows, pixels, C] adapter
+ * feature (NULL when feat_rows == 0).  fp32 arithmetic, rounded to E after each add: with feat_rows == 0 and a bias
+ * this is bitwise pww_resnet_residual, without a bias torch's `a + b`.  out may be a or b (in place); it must not
+ * otherwise overlap a, b or feat.  Returns PWW_ERR_BAD_ARG, before any CUDA call, for a null a, b or out, rows <= 0,
+ * pixels <= 0, C <= 0, C % 8 != 0, feat_rows outside 0..rows, a null feat with feat_rows > 0, or a pointer that is not
+ * 16-byte aligned. */
+int pww_adapter_residual_f16(const void* a, const void* b, const float* bias, const void* feat, void* out, int rows,
+                             int64_t pixels, int C, int feat_rows, void* stream);
+int pww_adapter_residual_bf16(const void* a, const void* b, const float* bias, const void* feat, void* out, int rows,
+                              int64_t pixels, int C, int feat_rows, void* stream);
+
 /*
  * The sampler step around the UNet (LMS, Euler, Euler ancestral, DPM++ 2M), two launches per denoising step.
  * Latents are [m, 4, h, w] fp32 contiguous; dtype codes name the UNet's input / output type.

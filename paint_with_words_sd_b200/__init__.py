@@ -9,6 +9,7 @@ from .conditioning import (  # noqa: F401
     _blur_image_mask, _encode_text_color_inputs, _extract_seed_and_sigma_from_context, _get_binary_mask,
     _image_context_seperator, _img_importance_flatten, _tokens_img_attention_weight, always_round, region_token_index,
 )
+from .adapter import T2IAdapter, build_adapter, pww_load_adapter  # noqa: F401
 from .controlnet import ControlNetModel, pww_load_controlnet  # noqa: F401
 from .pipeline import (  # noqa: F401
     PaintWithWord_StableDiffusionInpaintPipeline, PaintWithWord_StableDiffusionPipeline, PwWSampler, paint_with_words,

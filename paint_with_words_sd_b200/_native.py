@@ -31,6 +31,7 @@ EXPORTS = (
     "pww_control_combine_f16", "pww_control_combine_bf16",
     "pww_resnet_residual_f16", "pww_resnet_residual_bf16",
     "pww_xattn_fused_rec_f16", "pww_xattn_fused_rec_bf16",
+    "pww_adapter_residual_f16", "pww_adapter_residual_bf16",
 )
 
 
@@ -95,6 +96,9 @@ def lib() -> ctypes.CDLL:
     L.pww_add_layernorm_f16.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i, c_f, c_vp]
     L.pww_resnet_residual_f16.restype = c_i
     L.pww_resnet_residual_f16.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i64, c_i, c_vp]
+    # a, b, bias (or NULL), feat (or NULL), out, rows, pixels, C, feat_rows, stream
+    L.pww_adapter_residual_f16.restype = c_i
+    L.pww_adapter_residual_f16.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_i, c_i64, c_i, c_i, c_vp]
     # n, dst[n], res[n], elems_per_image[n] (host arrays), rows, scales (device [n, rows] fp32 or NULL), stream
     L.pww_control_inject_f16.restype = c_i
     L.pww_control_inject_f16.argtypes = [c_i, ctypes.POINTER(c_vp), ctypes.POINTER(c_vp), ctypes.POINTER(c_i64), c_i,

@@ -10,6 +10,7 @@
 #include "sampler_step.cuh"
 #include "control_inject.cuh"
 #include "control_combine.cuh"
+#include "adapter_residual.cuh"
 #include <stdlib.h>
 #include <algorithm>
 #include <type_traits>
@@ -356,6 +357,20 @@ int resnet_residual(const void* a, const void* h, const float* bias, void* out, 
 }
 
 template <typename E>
+int adapter_residual(const void* a, const void* b, const float* bias, const void* feat, void* out, int rows,
+                     int64_t pixels, int C, int feat_rows, void* stream) {
+  if (!a || !b || !out || rows <= 0 || pixels <= 0 || C <= 0 || (C & 7)) return PWW_ERR_BAD_ARG;
+  if (feat_rows < 0 || feat_rows > rows || (feat_rows > 0 && !feat)) return PWW_ERR_BAD_ARG;
+  if (!aligned16(a) || !aligned16(b) || !aligned16(out) || (bias && !aligned16(bias)) || (feat && !aligned16(feat)))
+    return PWW_ERR_BAD_ARG;
+  const long long per_row = (long long)pixels * (C >> 3);
+  const cudaError_t e = pww::adp::launch<E>(a, b, bias, feat, out, (long long)rows * per_row,
+                                            (long long)feat_rows * per_row, C >> 3, (long long)pww::num_sms() * 16,
+                                            (cudaStream_t)stream);
+  return e == cudaSuccess ? PWW_OK : cuda_fail(e);
+}
+
+template <typename E>
 int attn_fwd(const void* q,const void* k, const void* v, void* out, int B, int H, int N, int D, int64_t qkv_batch_stride,
              int64_t qkv_row_stride, int64_t o_batch_stride, int64_t o_row_stride, float scale, void* stream) {
   if (!q || !k || !v || !out || B <= 0 || H <= 0 || N <= 0 || D <= 0) return PWW_ERR_BAD_ARG;
@@ -618,6 +633,15 @@ int pww_resnet_residual_f16(const void* a, const void* h, const float* bias, voi
 int pww_resnet_residual_bf16(const void* a, const void* h, const float* bias, void* out, int64_t rows, int C,
                              void* stream) {
   return resnet_residual<__nv_bfloat16>(a, h, bias, out, rows, C, stream);
+}
+
+int pww_adapter_residual_f16(const void* a, const void* b, const float* bias, const void* feat, void* out, int rows,
+                             int64_t pixels, int C, int feat_rows, void* stream) {
+  return adapter_residual<__half>(a, b, bias, feat, out, rows, pixels, C, feat_rows, stream);
+}
+int pww_adapter_residual_bf16(const void* a, const void* b, const float* bias, const void* feat, void* out, int rows,
+                              int64_t pixels, int C, int feat_rows, void* stream) {
+  return adapter_residual<__nv_bfloat16>(a, b, bias, feat, out, rows, pixels, C, feat_rows, stream);
 }
 
 int pww_sampler_input(const float* latents, const float* scale, const float* extra, void* out, int out_dtype, int m,

@@ -1,5 +1,6 @@
 """Python wrappers for the fused channels-last UNet ops of libpww_b200 (GroupNorm[+add][+SiLU], GEGLU, add+LayerNorm,
-the ResNet residual epilogue) and the ControlNet residual injection and multi-ControlNet combine.
+the ResNet residual epilogue, with or without a T2I-Adapter feature) and the ControlNet residual injection and
+multi-ControlNet combine.
 
 Used by `unet.py` on CUDA fp16 or bf16 activations (the `_f16` / `_bf16` entry points, picked from x.dtype); the
 CPU/fp32 route of the same modules stays plain PyTorch (it is what the CPU reference arm runs).  No fallback on CUDA: a
@@ -120,6 +121,43 @@ def resnet_residual(a: torch.Tensor, h: torch.Tensor, bias: torch.Tensor, out: O
     with torch.cuda.device(h.device):
         rc = fn(a.data_ptr(), h.data_ptr(), bias.data_ptr(), out.data_ptr(), h.numel() // C, C,
                 torch.cuda.current_stream(h.device).cuda_stream)
+    _native.check(rc, fn.__name__)
+    _native.launch_count += 1
+    return out
+
+
+def adapter_residual(a: torch.Tensor, b: torch.Tensor, bias: Optional[torch.Tensor], feat: Optional[torch.Tensor],
+                     out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """s = (a.float() + b.float() [+ bias]).to(E), then out[:r] = (s[:r].float() + feat.float()).to(E) and out[r:] =
+    s[r:] (r = feat.shape[0], 0 for feat None), in one launch (`pww_adapter_residual_*`): a residual epilogue with a
+    T2I-Adapter feature added before the skip is taken.  a, b: [rows, C, h, w] of one type E (fp16 or bf16), both
+    channels-last; feat: [r <= rows, C, h, w] of that type and format; bias: fp32 [C] or None.  `out` (channels-last)
+    defaults to b (in place).  Returns out."""
+    cl = torch.channels_last
+    out = b if out is None else out
+    C = b.shape[1]
+    ops = [("a", a), ("b", b), ("out", out)]
+    for name, t in ops:
+        if (t.dim() != 4 or tuple(t.shape) != tuple(b.shape) or t.dtype != b.dtype or t.device != b.device
+                or not t.is_contiguous(memory_format=cl)):
+            raise ValueError(f"adapter_residual {name} {tuple(t.shape)} {t.dtype} does not match b {tuple(b.shape)} "
+                             f"{b.dtype} (a, b and out: one shape, type and device, channels-last)")
+    rows = 0
+    if feat is not None:
+        rows = int(feat.shape[0]) if feat.dim() == 4 else -1
+        if (feat.dim() != 4 or tuple(feat.shape[1:]) != tuple(b.shape[1:]) or rows > b.shape[0]
+                or feat.dtype != b.dtype or feat.device != b.device or not feat.is_contiguous(memory_format=cl)):
+            raise ValueError(f"adapter_residual feat {tuple(feat.shape)} {feat.dtype} does not match b "
+                             f"{tuple(b.shape)} {b.dtype} (same type, channels and size, at most as many images, "
+                             "channels-last)")
+    if bias is not None and (bias.dtype != torch.float32 or tuple(bias.shape) != (C,) or not bias.is_contiguous()
+                             or bias.device != b.device):
+        raise ValueError(f"adapter_residual bias must be a contiguous fp32 [{C}] tensor on {b.device}")
+    fn = _native.entry("pww_adapter_residual", b.dtype)
+    with torch.cuda.device(b.device):
+        rc = fn(a.data_ptr(), b.data_ptr(), None if bias is None else bias.data_ptr(),
+                None if feat is None else feat.data_ptr(), out.data_ptr(), b.shape[0], b.shape[2] * b.shape[3], C,
+                rows, torch.cuda.current_stream(b.device).cuda_stream)
     _native.check(rc, fn.__name__)
     _native.launch_count += 1
     return out

@@ -262,6 +262,15 @@ class PwWSampler:
     only the cond half gets residuals (hook_pww.py:39-53, 199).  Each set of active units over the run has its own
     captured graph.
 
+    T2I-Adapters (`adapter.T2IAdapter`, from `pww_load_adapter`) are control units too: an entry of `controlnet` may
+    be one, with its `control_image`, weight, guess mode and window taken exactly as a ControlNet unit's.  At set-up
+    every adapter runs once on its hints (its features do not depend on the step), a feature is resized (nearest) where
+    its level's size differs from the UNet's, and for every active set the active adapters' features, scaled (weight *
+    (0.25, 0.62, 0.825, 1.0) per level in guess mode) and summed in unit order, are stored at fixed addresses.  A step
+    hands that sum to the UNet (`down_intrablock_additional_residuals`), which adds it inside the residual epilogue of
+    each encoder level's last layer: an adapter costs no extra launch per step.  ControlNet residuals reach the skips
+    after the encoder has run, so a skip carries its adapter feature and then its ControlNet residual.
+
     `record_attention=True` records, inside the UNet's cross-attention launches (`pww_xattn_fused_rec_*`), the softmax
     mass every painted region's tokens receive from each pixel of each cond image, biased or not; `attention_maps()`
     returns it per image as [R, h, w] maps.  The accumulators are zeroed at set-up and by `restart()`.  The latents are
@@ -334,7 +343,10 @@ class PwWSampler:
         self._step_no = 0
         self.controlnet = controlnet
         self.guess_mode = bool(guess_mode)
-        self._nets: List = []              # the ControlNet units, in unit order
+        self._nets: List = []              # the control units (ControlNets and T2I-Adapters), in unit order
+        self._is_adapter: List[bool] = []
+        self._combine_scales: Dict[tuple, torch.Tensor] = {}         # active set -> its ControlNets' scale tables
+        self._adapter_sums: Dict[tuple, List[torch.Tensor]] = {}     # active set -> its adapters' summed features
         self._active_sets = [()] * len(self.timesteps)      # step i -> which units run (one bool per unit)
         self._control_active = [False] * len(self.timesteps)
         if controlnet is None:
@@ -392,30 +404,42 @@ class PwWSampler:
         return [total[i, :r].cpu() for i, r in enumerate(self._region_counts)]
 
     def _set_up_control(self, nets, images, weights, guesses, starts, ends):
-        """Validate every unit's ControlNet arguments (per-unit lists); embed the hints, stack the scale tables of
-        every active set and build the ControlNets' context."""
+        """Validate every unit's arguments (per-unit lists); embed the ControlNets' hints, run every adapter once on
+        its hints, stack the ControlNet scale tables and sum the adapter features of every active set, and build the
+        ControlNets' context."""
+        from .adapter import T2IAdapter, adapter_scales, align_features, unet_level_sizes
         from .controlnet import ControlNetModel
         unet, m, U = self.unet, self.m, len(nets)
         h, w = self.latents.shape[-2:]
         params = inspect.signature(unet.forward).parameters
-        if "down_block_additional_residuals" not in params or "mid_block_additional_residual" not in params:
-            raise TypeError(f"the UNet ({type(unet).__name__}) does not take down_block_additional_residuals / "
-                            "mid_block_additional_residual, so it cannot take a controlnet")
         ucfg = getattr(unet, "config", None)
+        is_adapter = [isinstance(net, T2IAdapter) for net in nets]
         for u, (net, start, end) in enumerate(zip(nets, starts, ends)):
             def arg(name):           # the argument, with the unit's index when there are several
                 return f"{name}[{u}]" if U > 1 else name
-            if not isinstance(net, ControlNetModel):
-                raise TypeError(f"{arg('controlnet')} must be a paint_with_words_sd_b200.controlnet.ControlNetModel, "
-                                f"got {type(net).__name__}")
-            ccfg = net.config
-            for name in ("block_out_channels", "layers_per_block", "cross_attention_dim"):
-                if getattr(ucfg, name, None) != getattr(ccfg, name):
-                    raise ValueError(f"{arg('controlnet')} config {name} = {getattr(ccfg, name)} does not match the "
-                                     f"UNet's {getattr(ucfg, name, None)}")
-            if ccfg.in_channels != 4:
-                raise ValueError(f"{arg('controlnet')} config in_channels = {ccfg.in_channels}: a ControlNet takes the "
-                                 "4 latent channels")
+            if is_adapter[u]:
+                if "down_intrablock_additional_residuals" not in params:
+                    raise TypeError(f"the UNet ({type(unet).__name__}) does not take "
+                                    "down_intrablock_additional_residuals, so it cannot take a T2I-Adapter")
+                uch = getattr(ucfg, "block_out_channels", None)
+                if uch is None or tuple(uch) != tuple(net.channels):
+                    raise ValueError(f"{arg('controlnet')}: a T2I-Adapter of channels {list(net.channels)} does not "
+                                     f"match the UNet's block_out_channels {None if uch is None else list(uch)}")
+            elif not isinstance(net, ControlNetModel):
+                raise TypeError(f"{arg('controlnet')} must be a paint_with_words_sd_b200.controlnet.ControlNetModel or "
+                                f"a paint_with_words_sd_b200.adapter.T2IAdapter, got {type(net).__name__}")
+            else:
+                if "down_block_additional_residuals" not in params or "mid_block_additional_residual" not in params:
+                    raise TypeError(f"the UNet ({type(unet).__name__}) does not take down_block_additional_residuals "
+                                    "/ mid_block_additional_residual, so it cannot take a controlnet")
+                ccfg = net.config
+                for name in ("block_out_channels", "layers_per_block", "cross_attention_dim"):
+                    if getattr(ucfg, name, None) != getattr(ccfg, name):
+                        raise ValueError(f"{arg('controlnet')} config {name} = {getattr(ccfg, name)} does not match "
+                                         f"the UNet's {getattr(ucfg, name, None)}")
+                if ccfg.in_channels != 4:
+                    raise ValueError(f"{arg('controlnet')} config in_channels = {ccfg.in_channels}: a ControlNet takes "
+                                     "the 4 latent channels")
             if not start <= end:
                 raise ValueError(f"{arg('control_guidance_start')} ({start}) must not exceed "
                                  f"{arg('control_guidance_end')} ({end})")
@@ -429,27 +453,51 @@ class PwWSampler:
             weights[u] = _per_image(weights[u], m, arg("controlnet_conditioning_scale"),
                                     lambda s: isinstance(s, (int, float)) and not isinstance(s, bool))
         # guess-mode routing is global (hook_pww.py:39-53, 199): if any unit is in guess mode, every unit's residuals
-        # go to the cond half only, and every ControlNet runs on the m cond rows
-        self._nets, self.guess_mode = list(nets), any(guesses)
+        # and features go to the cond half only, and every ControlNet runs on the m cond rows
+        self._nets, self._is_adapter, self.guess_mode = list(nets), is_adapter, any(guesses)
         n = len(self.timesteps)
         self._active_sets = [tuple(control_step_active(i, n, s, e) for s, e in zip(starts, ends)) for i in range(n)]
         self._control_active = [any(a) for a in self._active_sets]
-        dev = self.device
-        self._hints = []
-        for net, imgs in zip(nets, images):
-            with torch.no_grad():
-                emb = net.embed_condition(torch.cat([img.to(dev) for img in imgs], 0))     # once: step-invariant
-            if not self.guess_mode:
-                emb = torch.cat([emb, emb], 0)                                          # rows i and m + i share image i
-            self._hints.append(emb.contiguous(memory_format=torch.channels_last) if emb.is_cuda else emb)
+        dev, udtype = self.device, _module_dtype(unet)
         rows = m if self.guess_mode else 2 * m
-        tables = [control_scales(wt, g, len(net.controlnet_down_blocks) + 1)[:, :rows]
-                  for net, wt, g in zip(nets, weights, guesses)]
-        # per active set A that occurs, the active units' tables stacked: [|A|, levels, rows].  One unit's table is the
-        # UNet inject's CONTROL_SCALES; two or more are applied in the combine, and the UNet adds the sum at scale 1
-        full = torch.stack(tables, 0)
-        self._combine_scales = {a: full[[u for u in range(U) if a[u]]].contiguous().to(dev)
-                                for a in set(self._active_sets) if any(a)}
+        sizes = unet_level_sizes(h, w)
+        self._hints, feats = [], {}         # per unit: a ControlNet's embedded hints (None for an adapter); features
+        for u, (net, imgs) in enumerate(zip(nets, images)):
+            with torch.no_grad():                                                       # once: step-invariant
+                hint = torch.cat([img.to(dev) for img in imgs], 0)
+                if is_adapter[u]:
+                    # PlugableAdapter.forward runs once and caches; the features go to the UNet's type
+                    out = [f.to(udtype) for f in align_features(net(hint), sizes)]
+                else:
+                    out = [net.embed_condition(hint)]
+            if not self.guess_mode:
+                out = [torch.cat([t, t], 0) for t in out]                              # rows i and m + i share image i
+            out = [t.contiguous(memory_format=torch.channels_last) if t.is_cuda else t for t in out]
+            if is_adapter[u]:
+                feats[u] = out
+            self._hints.append(None if is_adapter[u] else out[0])
+        tables = [(adapter_scales(wt, g) if ad else control_scales(wt, g, len(net.controlnet_down_blocks) + 1))[:, :rows]
+                  for net, wt, g, ad in zip(nets, weights, guesses, is_adapter)]
+        # per active set A that occurs, the active ControlNets' tables stacked: [|A|, levels, rows].  One unit's table is
+        # the UNet inject's CONTROL_SCALES; two or more are applied in the combine, and the UNet adds the sum at scale 1
+        self._combine_scales = {}
+        # ... and the active adapters' scaled features summed level by level in unit order (hook_pww.py:136-139), once
+        # here: 4 tensors at fixed addresses that the set's steps (and captured graphs) hand to the UNet
+        self._adapter_sums = {}
+        for a in set(self._active_sets):
+            cn = [u for u in range(U) if a[u] and not is_adapter[u]]
+            if cn:
+                self._combine_scales[a] = torch.stack([tables[u] for u in cn], 0).contiguous().to(dev)
+            ad = [u for u in range(U) if a[u] and is_adapter[u]]
+            if ad:
+                per_unit = [feats[u] for u in ad]
+                scales = torch.stack([tables[u] for u in ad], 0).contiguous().to(dev)
+                with torch.no_grad():
+                    if fused_ops.is_fast(per_unit[0][0]):
+                        self._adapter_sums[a] = fused_ops.control_combine(
+                            per_unit, scales, [torch.empty_like(f) for f in per_unit[0]])
+                    else:
+                        self._adapter_sums[a] = combine_control_residuals(per_unit, scales)
         # the ControlNets' own dict: the plain text context (cond rows only in guess mode), no weight maps, so every
         # cross-attention call is unbiased; its K/V are staged once like the UNet's (the cache is keyed by module, so
         # the units share the dict, and a model that appears twice its K/V)
@@ -534,12 +582,13 @@ class PwWSampler:
                                           self._unet_in.shape[1], h, w, stream), "pww_sampler_input")
         t = p[_T:_T + 1]
         residuals = {}
-        if any(active):
+        if active in self._combine_scales:
             # each active ControlNet sees the 4 latent channels of the UNet input (hook_pww.py:113-119), only the cond
             # rows in guess mode (the uncond rows' residuals would be discarded)
             x = self._unet_in[:m, :4] if self.guess_mode else self._unet_in[:, :4]
             outs = [net(x, t, encoder_hidden_states=self._control_ctx, controlnet_cond_embedding=hint,
-                        return_dict=False) for net, hint, on in zip(self._nets, self._hints, active) if on]
+                        return_dict=False)
+                    for net, hint, on, ad in zip(self._nets, self._hints, active, self._is_adapter) if on and not ad]
             per_unit = [list(d) + [md] for d, md in outs]
             scales = self._combine_scales[active]
             if len(scales) == 1:
@@ -555,6 +604,9 @@ class PwWSampler:
                 else:
                     *down, mid = combine_control_residuals(per_unit, scales)
             residuals = {"down_block_additional_residuals": down, "mid_block_additional_residual": mid}
+        if active in self._adapter_sums:
+            # the active adapters' summed features, added inside the encoder levels' last residual epilogues
+            residuals["down_intrablock_additional_residuals"] = self._adapter_sums[active]
         eps = self.unet(self._unet_in, t, encoder_hidden_states=self._ctx, **residuals).sample
         if tuple(eps.shape) != (2 * m, 4, h, w) or eps.device != self.device:
             raise ValueError(f"the UNet returned {tuple(eps.shape)} on {eps.device}; expected {(2 * m, 4, h, w)}")
@@ -594,7 +646,7 @@ class PwWSampler:
         if "CONTEXT_TENSOR" in pinned and self._ctx.get("KV_CACHE"):
             # the cached K/V follow the new context: 16 small GEMMs, replayed as one CUDA graph (the ControlNet's
             # context is a view of the same tensor, so its cached K/V are refreshed too)
-            ctxs = [self._ctx] + ([self._control_ctx] if self._nets else [])
+            ctxs = [self._ctx] + ([self._control_ctx] if self._combine_scales else [])
 
             def refresh():
                 for c in ctxs:
@@ -715,7 +767,7 @@ def paint_with_words(
     which words go where; `controlnet_conditioning_scale`, `guess_mode` and the guidance window as in `PwWSampler`.
     Several ControlNets (e.g. pose for the figure, edges for the background): `controlnet` a list of up to 10,
     `control_image` a list with one such image per ControlNet, and the other four arguments one value or one per
-    ControlNet.
+    ControlNet.  A T2I-Adapter from `pww_load_adapter` is a unit too, alone or in the list, with the same arguments.
     `return_attention_maps=True` returns (image, RegionAttention): the per-region cross-attention maps of the cond image
     recorded inside the attention kernels over the whole run, with each region's adherence to its painted area."""
     control = _control_arguments(controlnet, control_image, color_map_image.size, "color_map_image",

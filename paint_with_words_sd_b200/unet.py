@@ -149,9 +149,10 @@ class Transformer2DModel(nn.Module):
         self.transformer_blocks = nn.ModuleList([BasicTransformerBlock(inner, heads, dim_head, cross_attention_dim)])
         self.proj_out = nn.Linear(inner, in_channels) if linear_proj else nn.Conv2d(inner, in_channels, 1)
 
-    def _forward_fast(self, x, encoder_hidden_states):
+    def _forward_fast(self, x, encoder_hidden_states, adapter_feature=None):
         """Channels-last route: the token view [B,HW,C] of an NHWC activation is free, so GroupNorm is one fused
-        launch and the 1x1 projections are plain GEMMs -- no layout conversion anywhere."""
+        launch and the 1x1 projections are plain GEMMs -- no layout conversion anywhere.  An adapter feature is added
+        in the residual add's launch."""
         b, c, h, w = x.shape
         if not x.is_contiguous(memory_format=torch.channels_last):
             x = x.contiguous(memory_format=torch.channels_last)
@@ -162,12 +163,16 @@ class Transformer2DModel(nn.Module):
         for blk in self.transformer_blocks:
             t = blk(t, context=encoder_hidden_states)
         wo = self.proj_out.weight
-        t = F.linear(t, wo.reshape(wo.shape[0], wo.shape[1]), self.proj_out.bias) + res   # contiguous, vectorised add
+        t = F.linear(t, wo.reshape(wo.shape[0], wo.shape[1]), self.proj_out.bias)
+        if adapter_feature is not None:
+            return fused_ops.adapter_residual(x, t.reshape(b, h, w, c).permute(0, 3, 1, 2), None, adapter_feature)
+        t = t + res                                                 # contiguous, vectorised add
         return t.reshape(b, h, w, c).permute(0, 3, 1, 2)
 
-    def forward(self, x, encoder_hidden_states=None):
+    def forward(self, x, encoder_hidden_states=None, adapter_feature=None):
+        """`adapter_feature`: a T2I-Adapter feature [rows <= B, C, h, w] added to the output (to its first rows)."""
         if fused_ops.is_fast(x):
-            return self._forward_fast(x, encoder_hidden_states)
+            return self._forward_fast(x, encoder_hidden_states, adapter_feature)
         b, c, h, w = x.shape
         res = x
         x = self.norm(x)
@@ -181,7 +186,7 @@ class Transformer2DModel(nn.Module):
             x = self.proj_out(x).reshape(b, h, w, c).permute(0, 3, 1, 2)
         else:
             x = self.proj_out(x.reshape(b, h, w, -1).permute(0, 3, 1, 2))
-        return x + res
+        return add_adapter_feature(x + res, adapter_feature)
 
 
 class ResnetBlock2D(nn.Module):
@@ -194,7 +199,8 @@ class ResnetBlock2D(nn.Module):
         self.conv2 = nn.Conv2d(out_ch, out_ch, 3, padding=1)
         self.conv_shortcut = nn.Conv2d(in_ch, out_ch, 1) if in_ch != out_ch else None
 
-    def forward(self, x, temb):
+    def forward(self, x, temb, adapter_feature=None):
+        """`adapter_feature`: a T2I-Adapter feature [rows <= B, C, h, w] added to the output (to its first rows)."""
         if fused_ops.is_fast(x):
             # GroupNorm+SiLU fused; the convolutions run without bias, so no per-channel bias pass touches their outputs:
             # conv1's bias rides with the time embedding into the second GroupNorm's add, conv2's and the shortcut's go
@@ -208,11 +214,13 @@ class ResnetBlock2D(nn.Module):
                                          None)
             sc = self.conv_shortcut
             a = x if sc is None else sc._conv_forward(x, sc.weight, None)
+            if adapter_feature is not None:
+                return fused_ops.adapter_residual(a, h, res_bias, adapter_feature)
             return fused_ops.resnet_residual(a, h, res_bias)
         h = self.conv1(F.silu(self.norm1(x)))
         h = h + self.time_emb_proj(F.silu(temb))[:, :, None, None]
         h = self.conv2(F.silu(self.norm2(h)))
-        return (x if self.conv_shortcut is None else self.conv_shortcut(x)) + h
+        return add_adapter_feature((x if self.conv_shortcut is None else self.conv_shortcut(x)) + h, adapter_feature)
 
 
 class Downsample2D(nn.Module):
@@ -246,12 +254,17 @@ class _DownBlock(nn.Module):
                                              for _ in range(n_layers)])
         self.downsamplers = nn.ModuleList([Downsample2D(out_ch)]) if downsample else None
 
-    def forward(self, x, temb, ctx):
+    def forward(self, x, temb, ctx, adapter_feature=None):
+        """`adapter_feature` goes to the level's last layer (its transformer, else its ResNet block): added before the
+        skip is taken and before the downsampler."""
         outs = []
+        last = len(self.resnets) - 1
         for i, res in enumerate(self.resnets):
-            x = res(x, temb)
+            f = adapter_feature if i == last else None
             if self.attentions is not None:
-                x = self.attentions[i](x, ctx)
+                x = self.attentions[i](res(x, temb), ctx, f)
+            else:
+                x = res(x, temb, f)
             outs.append(x)
         if self.downsamplers is not None:
             x = self.downsamplers[0](x)
@@ -344,14 +357,22 @@ class UNet2DConditionModel(nn.Module):
         self.conv_out = nn.Conv2d(ch[0], cfg.out_channels, 3, padding=1)
 
     def forward(self, sample, timestep, encoder_hidden_states=None, down_block_additional_residuals=None,
-                mid_block_additional_residual=None):
+                mid_block_additional_residual=None, down_intrablock_additional_residuals=None):
         """`down_block_additional_residuals` (one per skip) and `mid_block_additional_residual` are a ControlNet's
         outputs, as in diffusers: residual k is added to skip k before the decoder concatenates it, the mid residual to
         the mid-block output.  Residuals of fewer images than the batch go into its first images (guess mode: the cond
         half).  A context dict may carry "CONTROL_SCALES", an fp32 [len(skips) + 1, rows] device tensor: residual k of
-        image b is multiplied by CONTROL_SCALES[k, b] first (absent: 1, diffusers' plain add)."""
+        image b is multiplied by CONTROL_SCALES[k, b] first (absent: 1, diffusers' plain add).
+
+        `down_intrablock_additional_residuals` are a T2I-Adapter's features, as in diffusers: one [rows <= B, C_l, h_l,
+        w_l] tensor per encoder level, added to the output of the level's last layer before its skip is taken and
+        before its downsampler (so the skip carries the feature, and a ControlNet residual is added to it later).  As
+        with the ControlNet residuals, rows < B means the first images."""
         if (down_block_additional_residuals is None) != (mid_block_additional_residual is None):
             raise ValueError("down_block_additional_residuals and mid_block_additional_residual go together")
+        feats = down_intrablock_additional_residuals
+        if feats is not None and len(feats) != len(self.down_blocks):
+            raise ValueError(f"{len(feats)} down_intrablock_additional_residuals for {len(self.down_blocks)} levels")
         if not torch.is_tensor(timestep):
             timestep = torch.tensor([timestep], dtype=torch.float32, device=sample.device)
         elif timestep.dim() == 0:
@@ -367,8 +388,8 @@ class UNet2DConditionModel(nn.Module):
             self._project_time_embeddings(temb)
         x = self.conv_in(x)
         skips = [x]
-        for blk in self.down_blocks:
-            x, outs = blk(x, temb, encoder_hidden_states)
+        for lvl, blk in enumerate(self.down_blocks):
+            x, outs = blk(x, temb, encoder_hidden_states, None if feats is None else feats[lvl])
             skips.extend(outs)
         x = self.mid_block(x, temb, encoder_hidden_states)
         if mid_block_additional_residual is not None:
@@ -402,6 +423,18 @@ def add_control_residuals(targets: Sequence[torch.Tensor], residuals: Sequence[t
         p = p.to(d.dtype)
         out.append(d + p if rows == d.shape[0] else torch.cat([d[:rows] + p, d[rows:]], 0))
     return out
+
+
+def add_adapter_feature(x: torch.Tensor, feat: Optional[torch.Tensor]) -> torch.Tensor:
+    """The torch statement of `pww_adapter_residual`'s feature add: x[:rows] + feat in x's type (rows =
+    feat.shape[0]); x itself when feat is None."""
+    if feat is None:
+        return x
+    rows = feat.shape[0]
+    if tuple(feat.shape[1:]) != tuple(x.shape[1:]) or rows > x.shape[0]:
+        raise ValueError(f"adapter feature {tuple(feat.shape)} does not match its target {tuple(x.shape)}")
+    feat = feat.to(x.dtype)
+    return x + feat if rows == x.shape[0] else torch.cat([x[:rows] + feat, x[rows:]], 0)
 
 
 def combine_control_residuals(res_per_unit: Sequence[Sequence[torch.Tensor]], scales: torch.Tensor) -> List[torch.Tensor]:

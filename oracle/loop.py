@@ -15,10 +15,14 @@ import torch
 from . import pww_oracle
 
 
-def patch_with_oracle(unet, emulate_fp16: bool = False) -> int:
-    """Class-level `__call__` patch as at paint_with_words.py:193-195, installing the oracle's inj_forward."""
+def patch_with_oracle(unet, emulate_fp16: bool = False, emulate_dtype: Optional[torch.dtype] = None) -> int:
+    """Class-level `__call__` patch as at paint_with_words.py:193-195, installing the oracle's inj_forward
+    (`emulate_fp16` / `emulate_dtype`: the rounding points of an eager fp16 / bf16 autocast, see attention_core)."""
+    pww_oracle._emulated_dtype(emulate_fp16, emulate_dtype)
+
     def fwd(self, hidden_states, context=None, mask=None):
-        return pww_oracle.inj_forward(self, hidden_states, context, mask, emulate_fp16=emulate_fp16)
+        return pww_oracle.inj_forward(self, hidden_states, context, mask, emulate_fp16=emulate_fp16,
+                                      emulate_dtype=emulate_dtype)
     n = 0
     for m in unet.modules():
         if m.__class__.__name__ == "CrossAttention":

@@ -170,33 +170,45 @@ def _b2h(x: torch.Tensor, heads: int) -> torch.Tensor:
 
 def attention_core(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, scale: float,
                    bias_fn: Optional[Callable[[torch.Tensor], object]] = None,
-                   emulate_fp16: bool = False) -> torch.Tensor:
+                   emulate_fp16: bool = False, emulate_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
     """Everything between to_q/to_k/to_v and to_out for ONE image (B=1 as in the reference).
 
     q [1,N,C], k/v [1,T,C].  Restates paint_with_words.py:83-118:
         S = Q_h K_h^T (unscaled) ; S' = (S + bias_fn(S)) * scale ; P = softmax(S') ; O = P V_h.
     `bias_fn(S[h,N,T])` returns the additive term (a [N,T] tensor or 0.0).
-    emulate_fp16=True reproduces the rounding points of the reference's CUDA-autocast path on fp32
-    hardware: inputs/S/P/O rounded to fp16 where eager fp16 autocast rounds them (SURVEY 8a-1)."""
-    def r16(t):
-        return t.to(torch.float16).to(torch.float32) if emulate_fp16 else t
-    q, k, v = r16(q.float()), r16(k.float()), r16(v.float())
+    emulate_dtype=torch.float16 (or emulate_fp16=True) reproduces the rounding points of the reference's CUDA-autocast
+    path on fp32 hardware: inputs/S/P/O rounded to fp16 where eager fp16 autocast rounds them (SURVEY 8a-1);
+    emulate_dtype=torch.bfloat16 rounds at the same points to bf16, as an eager bf16 autocast does."""
+    em = _emulated_dtype(emulate_fp16, emulate_dtype)
+
+    def rnd(t):
+        return t.to(em).to(torch.float32) if em is not None else t
+    q, k, v = rnd(q.float()), rnd(k.float()), rnd(v.float())
     qh, kh, vh = _h2b(q, heads), _h2b(k, heads), _h2b(v, heads)
-    s = r16(torch.matmul(qh, kh.transpose(-1, -2)))
-    bias = bias_fn(s.to(torch.float16) if emulate_fp16 else s) if bias_fn is not None else 0.0
+    s = rnd(torch.matmul(qh, kh.transpose(-1, -2)))
+    bias = bias_fn(s.to(em) if em is not None else s) if bias_fn is not None else 0.0
     if isinstance(bias, torch.Tensor):
         bias = bias.float()
         s = (s + bias) * scale
     else:
-        s = r16((s + bias) * scale)   # fp16 + python float stays fp16 under autocast
-    p = r16(s.softmax(dim=-1))
-    o = r16(torch.matmul(p, vh))
+        s = rnd((s + bias) * scale)   # half + python float stays half under autocast
+    p = rnd(s.softmax(dim=-1))
+    o = rnd(torch.matmul(p, vh))
     return _b2h(o, heads)
 
 
-def inj_forward(attn, hidden_states, context=None, mask=None, emulate_fp16: bool = False):
+def _emulated_dtype(emulate_fp16: bool, emulate_dtype: Optional[torch.dtype]) -> Optional[torch.dtype]:
+    if emulate_dtype not in (None, torch.float16, torch.bfloat16):
+        raise ValueError(f"emulate_dtype must be None, torch.float16 or torch.bfloat16, got {emulate_dtype}")
+    if emulate_fp16 and emulate_dtype not in (None, torch.float16):
+        raise ValueError(f"emulate_fp16=True contradicts emulate_dtype={emulate_dtype}")
+    return torch.float16 if emulate_fp16 else emulate_dtype
+
+
+def inj_forward(attn, hidden_states, context=None, mask=None, emulate_fp16: bool = False,
+                emulate_dtype: Optional[torch.dtype] = None):
     """Restates paint_with_words.py:60-125 for a module with the diffusers-0.10 CrossAttention contract
-    (to_q/to_k/to_v/to_out, heads, scale).  fp32 on CPU unless emulate_fp16."""
+    (to_q/to_k/to_v/to_out, heads, scale).  fp32 unless emulate_fp16 / emulate_dtype (see attention_core)."""
     is_dict = True
     if context is not None:
         if isinstance(context, dict):
@@ -225,7 +237,7 @@ def inj_forward(attn, hidden_states, context=None, mask=None, emulate_fp16: bool
     outs = []
     for b in range(q.shape[0]):            # reference is B=1; per-image stat scope for B>1
         outs.append(attention_core(q[b:b + 1], k[b:b + 1], v[b:b + 1], attn.heads, attn.scale,
-                                   bias_fn, emulate_fp16))
+                                   bias_fn, emulate_fp16, emulate_dtype))
     o = torch.cat(outs, 0)
     o = attn.to_out[0](o.to(hidden_states.dtype))
     return attn.to_out[1](o)

@@ -127,7 +127,7 @@ template <typename E>
 __global__ void __launch_bounds__(1024) gn_apply_kernel(GnParams<E> p, int rows_per_block) {
   using X = Elem<E>;
   using E2 = typename X::E2;
-  __shared__ float2 s_stat[64];   // (mean, rstd) of the slice's groups
+  __shared__ float3 s_stat[64];   // (shift, E[d], rstd) of the slice's groups: mean = shift + E[d]
   const int cg = p.C / p.G, sv = p.sv, rpp = blockDim.x / sv, b = blockIdx.z;
   const int v0 = blockIdx.y * sv, nv = min(sv, (p.C >> 3) - v0);
   const int c0 = v0 * 8, ng = nv * 8 / cg;
@@ -171,7 +171,7 @@ __global__ void __launch_bounds__(1024) gn_apply_kernel(GnParams<E> p, int rows_
       const float dm = ts / n;
       float var = tq / n - dm * dm;
       var = var < 0.f ? 0.f : var;
-      s_stat[lg] = make_float2(shift + dm, rsqrtf(var + p.eps));
+      s_stat[lg] = make_float3(shift, dm, rsqrtf(var + p.eps));
     }
   }
   __syncthreads();
@@ -181,9 +181,11 @@ __global__ void __launch_bounds__(1024) gn_apply_kernel(GnParams<E> p, int rows_
     const E* ah = reinterpret_cast<const E*>(&av);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      const float2 st = s_stat[(v * 8 + i) / cg];
-      sc[i] = st.y * X::to_float(gh[i]);
-      sh[i] = X::to_float(bh[i]) + (X::to_float(ah[i]) - st.x) * sc[i];
+      // add - mean as (add - shift) - E[d]: no fp32 rounding of the mean itself, which would err by 2^-24 |mean| where
+      // |add| >> std and rstd multiplies that by up to 1 / sqrt(eps)
+      const float3 st = s_stat[(v * 8 + i) / cg];
+      sc[i] = st.z * X::to_float(gh[i]);
+      sh[i] = X::to_float(bh[i]) + ((X::to_float(ah[i]) - st.x) - st.y) * sc[i];
     }
   }
   const int r = r0 + rl;

@@ -1,10 +1,12 @@
-"""Fused channels-last UNet ops (GroupNorm[+add][+SiLU], GEGLU) against plain PyTorch fp32 on the same inputs."""
+"""Fused channels-last UNet ops (GroupNorm[+add][+SiLU], GEGLU, add+LayerNorm) in fp16 against fp64 references to the
+per-element bound of tests/unet_ops_bound.py (the full sweep is tests/test_unet_ops_bound_gpu.py), and the fused UNet
+route against the plain one."""
 import pytest
 import torch
-import torch.nn.functional as F
 
 from paint_with_words_sd_b200 import fused_ops
 from paint_with_words_sd_b200.unet import UNetConfig, build_unet
+from tests import unet_ops_bound as U
 
 pytestmark = pytest.mark.gpu
 
@@ -20,29 +22,23 @@ def test_group_norm_nhwc(C, HW, G, silu, with_add):
     gn.weight.data = torch.randn(C, generator=g) * 0.5 + 1.0
     gn.bias.data = torch.randn(C, generator=g) * 0.2
     add = (torch.randn(B, C, generator=g) * 0.5).half() if with_add else None
-    xin = x.float() + (add.float()[:, :, None, None] if with_add else 0.0)
-    ref = F.group_norm(xin, G, gn.weight.float(), gn.bias.float(), 1e-5)
-    if silu:
-        ref = F.silu(ref)
     gn_h = gn.half().cuda()
     got = fused_ops.group_norm_nhwc(x.cuda().contiguous(memory_format=torch.channels_last), gn_h,
                                     None if add is None else add.cuda(), silu=silu)
     assert got.is_contiguous(memory_format=torch.channels_last)
-    # reference with fp16-rounded affine parameters, like the kernel sees them
-    ref = F.group_norm(xin, G, gn_h.weight.float().cpu(), gn_h.bias.float().cpu(), 1e-5)
-    if silu:
-        ref = F.silu(ref)
-    err = (got.float().cpu() - ref).abs().max().item()
-    assert err <= 4e-3 * max(1.0, ref.abs().max().item()), err
+    # reference on the inputs as the kernel sees them (fp16 activations and affine parameters)
+    ref, terms = U.gn_reference(x.cuda().flatten(2).transpose(1, 2), gn_h.weight, gn_h.bias, G, 1e-5,
+                                None if add is None else add.cuda(), silu)
+    U.check_within(got.flatten(2).transpose(1, 2), ref, terms, torch.float16, U.K_GN, f"gn {C} {HW} {G}")
 
 
 @pytest.mark.parametrize("M,I", [(2 * 4096, 1280), (2 * 64, 5120), (3, 8), (77, 2560)])
 def test_geglu(M, I):
     g = torch.Generator().manual_seed(M + I)
     h = (torch.randn(M, 2 * I, generator=g) * 2.0).half()
-    ref = h[:, :I].float() * F.gelu(h[:, I:].float())
-    got = fused_ops.geglu(h.cuda()).float().cpu()
-    assert (got - ref).abs().max().item() <= 2e-3 * ref.abs().max().item()
+    ref, terms = U.geglu_reference(h)
+    got = fused_ops.geglu(h.cuda()).cpu()
+    U.check_within(got, ref, terms, torch.float16, U.K_GEGLU, f"geglu {M} {I}")
 
 
 @pytest.mark.parametrize("M,C", [(2 * 4096, 320), (2 * 1024, 640), (2 * 256, 1280), (5, 1280), (3, 8), (7, 2048)])
@@ -56,10 +52,10 @@ def test_add_layer_norm(M, C, with_res):
     ln.bias.data = torch.randn(C, generator=g) * 0.2
     ln_h = ln.half().cuda()
     s_ref = (x.float() + res.float()).half() if with_res else x
-    y_ref = F.layer_norm(s_ref.float(), (C,), ln_h.weight.float().cpu(), ln_h.bias.float().cpu(), ln.eps)
+    y_ref, terms = U.ln_reference(s_ref, ln_h.weight.cpu(), ln_h.bias.cpu(), ln.eps)
     s, y = fused_ops.add_layer_norm(x.cuda(), None if res is None else res.cuda(), ln_h)
     assert torch.equal(s.cpu(), s_ref)                      # the residual stream is bit-identical to an fp16 add
-    assert (y.float().cpu() - y_ref).abs().max().item() <= 4e-3 * max(1.0, y_ref.abs().max().item())
+    U.check_within(y.cpu(), y_ref, terms, torch.float16, U.K_LN, f"add-layernorm {M} {C}")
 
 
 def test_unet_fast_route_matches_plain_route():

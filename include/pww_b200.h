@@ -365,6 +365,27 @@ int pww_sampler_update(const void* eps, int eps_dtype, int64_t eps_batch_stride,
                        int m, int height, int width, void* stream);
 
 /*
+ * pww_sampler_update_rescale: pww_sampler_update with guidance rescale (diffusers' `guidance_rescale`, Lin et al. 2023,
+ * section 3.4), in one launch.  Per image i, with phi = rescale[i] in [0, 1]:
+ *   cfg    = eps_u + guidance[i] (eps_c - eps_u)                                      (as pww_sampler_update)
+ *   k      = phi std(eps_c) / std(cfg) + (1 - phi)       std: unbiased, over the 4 h w values of image i, in fp32
+ *   eps'   = k cfg, then pww_sampler_update's step form with eps' for eps
+ * The means and the sums of squared deviations are two passes over the image, each folded in a fixed order, so image
+ * i's latents and stats row are the same bits alone, in any batch and at any position.  phi == 0 leaves k unapplied:
+ * that image's latents are bitwise pww_sampler_update's.  A std(cfg) of 0 gives a non-finite k, as the torch formula
+ * does; no special case.  `rescale` is an [m] fp32 device array; `stats_out` an [m, 3] fp32 device array that receives
+ * (std(eps_c), std(cfg), k) per image (k = 1 where phi == 0), or NULL.  One thread-block cluster per image.
+ * Returns PWW_ERR_BAD_ARG and PWW_ERR_UNSUPPORTED, before any CUDA call, as pww_sampler_update does, and
+ * PWW_ERR_BAD_ARG for a null `rescale`.
+ */
+int pww_sampler_update_rescale(const void* eps, int eps_dtype, int64_t eps_batch_stride, int64_t eps_channel_stride,
+                               int64_t eps_row_stride, int64_t eps_col_stride,
+                               float* latents, float* history, int history_len, const float* noise,
+                               const float* guidance, const float* beta, const float* form,
+                               const float* rescale, float* stats_out,
+                               int m, int height, int width, void* stream);
+
+/*
  * ControlNet residual injection: n (1..16) residuals added in place into n activations, in one launch.
  *   dst_k[b] = E( dst_k[b] + E( s[k, b] * res_k[b] ) )        k < n, b < rows
  * dst[k] points at a [B, elems_per_image[k]] tensor and res[k] at a [rows, elems_per_image[k]] one, both dense (a

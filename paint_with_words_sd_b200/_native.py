@@ -32,6 +32,7 @@ EXPORTS = (
     "pww_resnet_residual_f16", "pww_resnet_residual_bf16",
     "pww_xattn_fused_rec_f16", "pww_xattn_fused_rec_bf16",
     "pww_adapter_residual_f16", "pww_adapter_residual_bf16",
+    "pww_sampler_update_rescale",
 )
 
 
@@ -118,6 +119,10 @@ def lib() -> ctypes.CDLL:
     L.pww_sampler_update.restype = c_i
     L.pww_sampler_update.argtypes = [c_vp, c_i, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_i, c_vp, c_vp, c_vp, c_vp,
                                      c_i, c_i, c_i, c_vp]
+    # pww_sampler_update's arguments with rescale [m] and stats_out [m, 3] (or NULL) after `form`
+    L.pww_sampler_update_rescale.restype = c_i
+    L.pww_sampler_update_rescale.argtypes = L.pww_sampler_update.argtypes[:13] + [c_vp, c_vp] + \
+        L.pww_sampler_update.argtypes[13:]
     _lib = L
     return L
 

@@ -8,6 +8,7 @@
 #include "attn_tc.cuh"
 #include "unet_ops.cuh"
 #include "sampler_step.cuh"
+#include "sampler_rescale.cuh"
 #include "control_inject.cuh"
 #include "control_combine.cuh"
 #include "adapter_residual.cuh"
@@ -682,6 +683,34 @@ int pww_sampler_update(const void* eps, int eps_dtype, int64_t eps_batch_stride,
   const cudaError_t e = eps_dtype == PWW_DTYPE_F16    ? pww::smp::launch_update<__half>(a, px4, cl, s)
                         : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_update<__nv_bfloat16>(a, px4, cl, s)
                                                       : pww::smp::launch_update<float>(a, px4, cl, s);
+  return e == cudaSuccess ? PWW_OK : cuda_fail(e);
+}
+
+int pww_sampler_update_rescale(const void* eps, int eps_dtype, int64_t eps_batch_stride, int64_t eps_channel_stride,
+                               int64_t eps_row_stride, int64_t eps_col_stride, float* latents, float* history,
+                               int history_len, const float* noise, const float* guidance, const float* beta,
+                               const float* form, const float* rescale, float* stats_out, int m, int height, int width,
+                               void* stream) {
+  if (!eps || !latents || !history || !guidance || !beta || !form || !rescale) return PWW_ERR_BAD_ARG;
+  if (m <= 0 || height <= 0 || width <= 0 || history_len < 1 || history_len > 4) return PWW_ERR_BAD_ARG;
+  if (eps_dtype != PWW_DTYPE_F32 && eps_dtype != PWW_DTYPE_F16 && eps_dtype != PWW_DTYPE_BF16) return PWW_ERR_UNSUPPORTED;
+  pww::smp::UpdateArgs a;
+  a.eps = eps; a.e_sn = eps_batch_stride; a.e_sc = eps_channel_stride; a.e_sh = eps_row_stride; a.e_sw = eps_col_stride;
+  a.lat = latents; a.hist = history; a.noise = noise; a.gscale = guidance; a.beta = beta; a.form = form;
+  a.m = m; a.h = height; a.w = width; a.nh = history_len;
+  pww::smp::RescaleArgs r;
+  r.phi = rescale; r.stats = stats_out;
+  // the same pixel grouping and channels-last test as pww_sampler_update
+  const int64_t hw = (int64_t)height * width;
+  const size_t es = eps_dtype == PWW_DTYPE_F32 ? 4 : 2;
+  const bool px4 = (hw % 4) == 0 && aligned16(latents) && aligned16(history) && (!noise || aligned16(noise));
+  const size_t need = px4 ? 16 : 4 * es;
+  const bool cl = eps_channel_stride == 1 && eps_col_stride == 4 && eps_row_stride == 4 * (int64_t)width &&
+                  (reinterpret_cast<uintptr_t>(eps) % need) == 0 && ((size_t)eps_batch_stride * es) % need == 0;
+  cudaStream_t s = (cudaStream_t)stream;
+  const cudaError_t e = eps_dtype == PWW_DTYPE_F16    ? pww::smp::launch_update_rescale<__half>(a, r, px4, cl, s)
+                        : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_update_rescale<__nv_bfloat16>(a, r, px4, cl, s)
+                                                      : pww::smp::launch_update_rescale<float>(a, r, px4, cl, s);
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 

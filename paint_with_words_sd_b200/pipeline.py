@@ -16,7 +16,9 @@ from __future__ import annotations
 
 import dataclasses
 import inspect
+import json
 import math
+import os
 from typing import Callable, Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
@@ -57,13 +59,16 @@ _SYNTHETIC_CONFIGS = {
 
 def pww_load_tools(device: str = "cuda:0", scheduler_type=LMSDiscreteScheduler,
                    local_model_path: Optional[str] = None, hf_model_path: Optional[str] = None,
-                   model_token: Optional[str] = None, seed: int = 0, torch_dtype: Optional[torch.dtype] = None):
+                   model_token: Optional[str] = None, seed: int = 0, torch_dtype: Optional[torch.dtype] = None,
+                   prediction_type: Optional[str] = None):
     """paint_with_words.py:128-204: returns (vae, unet, text_encoder, tokenizer, scheduler) with the
     attention of `unet` patched.  `"synthetic:<sd15|sd15-inpaint|sd21|tiny>"` model paths build seeded
     random-weight stand-ins (no weights or network exist in this environment); any other path is
     loaded with diffusers/transformers when those are installed.
     `torch_dtype`: the UNet's (and VAE's) dtype; None keeps the reference's rule (fp16, fp32 on mps), and
-    torch.bfloat16 runs every native kernel in bf16."""
+    torch.bfloat16 runs every native kernel in bf16.
+    `prediction_type` ("epsilon" or "v_prediction") goes to `scheduler_type`; None takes the model's own
+    (`model_prediction_type`): a v-prediction checkpoint such as stable-diffusion-2-1 gets its v scheduler."""
     assert local_model_path or hf_model_path, "either local_model_path or hf_model_path must be provided"
     model_path = local_model_path if local_model_path is not None else hf_model_path
     dtype = torch_dtype if torch_dtype is not None else (torch.float16 if device != "mps" else torch.float32)
@@ -87,9 +92,29 @@ def pww_load_tools(device: str = "cuda:0", scheduler_type=LMSDiscreteScheduler,
         unet = _HFUNet.from_pretrained(model_path, subfolder="unet", torch_dtype=dtype,
                                        local_files_only=local_only).to(device)
     _attention.patch_unet(unet)
+    if prediction_type is None:
+        prediction_type = model_prediction_type(model_path)
     scheduler = scheduler_type(beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear",
-                               num_train_timesteps=1000)
+                               num_train_timesteps=1000, prediction_type=prediction_type)
     return vae, unet, text_encoder, tokenizer, scheduler
+
+
+def model_prediction_type(model_path: str) -> str:
+    """The `prediction_type` of a model's `scheduler/scheduler_config.json`: read with json from a local diffusers
+    directory, through diffusers' config loader for a hub id; "epsilon" for the synthetic models, a directory without
+    that file, or a config without the key."""
+    if model_path in _SYNTHETIC_CONFIGS:
+        return "epsilon"
+    if os.path.isdir(model_path):
+        path = os.path.join(model_path, "scheduler", "scheduler_config.json")
+        if not os.path.isfile(path):
+            return "epsilon"
+        with open(path) as f:
+            config = json.load(f)
+    else:
+        from diffusers import LMSDiscreteScheduler as _HFLMS
+        config = _HFLMS.load_config(model_path, subfolder="scheduler")
+    return config.get("prediction_type", "epsilon")
 
 
 def _dtype_code(dtype) -> int:
@@ -271,6 +296,13 @@ class PwWSampler:
     each encoder level's last layer: an adapter costs no extra launch per step.  ControlNet residuals reach the skips
     after the encoder has run, so a skip carries its adapter feature and then its ControlNet residual.
 
+    `guidance_rescale` (diffusers' name; Lin et al. 2023, section 3.4) is one phi in [0, 1] for every image or m of
+    them: image i's guided output is scaled by k_i = phi_i std(cond output) / std(guided output) + (1 - phi_i) before
+    the step form, which corrects the over-exposure of high guidance scales (mostly used with v-prediction models).
+    If any phi is non-zero, the update is `pww_sampler_update_rescale`, in place of `pww_sampler_update`: the same two
+    native launches per step, and images with phi = 0 get exactly the plain update.  A v-prediction scheduler
+    (`prediction_type="v_prediction"` in its config) needs nothing here: its step forms take the v output.
+
     `record_attention=True` records, inside the UNet's cross-attention launches (`pww_xattn_fused_rec_*`), the softmax
     mass every painted region's tokens receive from each pixel of each cond image, biased or not; `attention_maps()`
     returns it per image as [R, h, w] maps.  The accumulators are zeroed at set-up and by `restart()`.  The latents are
@@ -285,7 +317,7 @@ class PwWSampler:
                  control_image: Union[None, torch.Tensor, Sequence[torch.Tensor]] = None,
                  controlnet_conditioning_scale: Union[float, Sequence[float]] = 1.0, guess_mode: bool = False,
                  control_guidance_start: float = 0.0, control_guidance_end: float = 1.0,
-                 record_attention: bool = False):
+                 record_attention: bool = False, guidance_rescale: Union[float, Sequence[float]] = 0.0):
         if not isinstance(scheduler, SIGMA_SCHEDULERS):
             raise TypeError(f"PwWSampler does not support {type(scheduler).__name__}; use one of "
                             + ", ".join(c.__name__ for c in SIGMA_SCHEDULERS))
@@ -297,6 +329,12 @@ class PwWSampler:
                                else [float(g) for g in guidance_scale])
         self._fns = _per_image(weight_function, self.m, "weight_function", callable)
         scales = _per_image(self.guidance_scale, self.m, "guidance_scale", lambda g: isinstance(g, float))
+        phis = list(guidance_rescale) if isinstance(guidance_rescale, (list, tuple)) else [guidance_rescale] * self.m
+        if len(phis) != self.m or not all(isinstance(v, (int, float)) and not isinstance(v, bool) and 0.0 <= v <= 1.0
+                                          for v in phis):        # NaN fails the range test too
+            raise ValueError(f"guidance_rescale must be one value in [0, 1] or {self.m} (one per image), got "
+                             f"{guidance_rescale!r}")
+        self.guidance_rescale = [float(v) for v in phis]
         self.timesteps = list((scheduler.timesteps if timesteps is None else timesteps).tolist())
         # the sampler kernels index latents [m,4,h,w] and extra_input [m,5,h,w] as contiguous fp32 buffers: a private
         # contiguous copy, whatever the caller's layout, and shapes checked against the m images
@@ -331,6 +369,8 @@ class PwWSampler:
         self._derivs = torch.zeros((self._hist_len,) + tuple(self.latents.shape), dtype=torch.float32, device=dev)
         self._ctx["G_SIGMA"] = self._params[_G:self._form]
         self._gscale = torch.tensor(scales, dtype=torch.float32, device=dev).view(m, 1, 1, 1)
+        # phi per image ([m]); None when every phi is 0 and a step launches the plain update
+        self._rescale = torch.tensor(self.guidance_rescale, dtype=torch.float32, device=dev) if any(phis) else None
         self._noise = None
         if isinstance(scheduler, EulerAncestralDiscreteScheduler):
             if noise_seed is None:
@@ -610,12 +650,16 @@ class PwWSampler:
         eps = self.unet(self._unet_in, t, encoder_hidden_states=self._ctx, **residuals).sample
         if tuple(eps.shape) != (2 * m, 4, h, w) or eps.device != self.device:
             raise ValueError(f"the UNet returned {tuple(eps.shape)} on {eps.device}; expected {(2 * m, 4, h, w)}")
-        # CFG with the per-image scale, then the step form; eps is read in place through its strides
-        _native.check(L.pww_sampler_update(eps.data_ptr(), _dtype_code(eps.dtype), *eps.stride(),
-                                           self.latents.data_ptr(), self._derivs.data_ptr(), self._hist_len,
-                                           None if self._noise is None else self._noise.data_ptr(),
-                                           self._gscale.data_ptr(), p[_BETA:].data_ptr(), p[self._form:].data_ptr(),
-                                           m, h, w, stream), "pww_sampler_update")
+        # CFG with the per-image scale (and guidance rescale), then the step form; eps is read in place through its
+        # strides
+        args = (eps.data_ptr(), _dtype_code(eps.dtype), *eps.stride(), self.latents.data_ptr(), self._derivs.data_ptr(),
+                self._hist_len, None if self._noise is None else self._noise.data_ptr(), self._gscale.data_ptr(),
+                p[_BETA:].data_ptr(), p[self._form:].data_ptr())
+        if self._rescale is None:
+            _native.check(L.pww_sampler_update(*args, m, h, w, stream), "pww_sampler_update")
+        else:
+            _native.check(L.pww_sampler_update_rescale(*args, self._rescale.data_ptr(), None, m, h, w, stream),
+                          "pww_sampler_update_rescale")
         _native.launch_count += 2
 
     def _set_step_scalars(self, i: int, step_index: int):
@@ -756,6 +800,8 @@ def paint_with_words(
     control_guidance_start: Union[float, Sequence[float]] = 0.0,
     control_guidance_end: Union[float, Sequence[float]] = 1.0,
     return_attention_maps: bool = False,
+    guidance_rescale: float = 0.0,
+    prediction_type: Optional[str] = None,
 ):
     """paint_with_words.py:391-510.  Returns one PIL.Image (or the final latents with return_latents).
     `max_prompt_chunks` (1 .. 3): a prompt longer than 75 tokens fills up to that many 77-token CLIP chunks instead of
@@ -769,11 +815,15 @@ def paint_with_words(
     `control_image` a list with one such image per ControlNet, and the other four arguments one value or one per
     ControlNet.  A T2I-Adapter from `pww_load_adapter` is a unit too, alone or in the list, with the same arguments.
     `return_attention_maps=True` returns (image, RegionAttention): the per-region cross-attention maps of the cond image
-    recorded inside the attention kernels over the whole run, with each region's adherence to its painted area."""
+    recorded inside the attention kernels over the whole run, with each region's adherence to its painted area.
+    `guidance_rescale` (0..1) as in `PwWSampler`.  `prediction_type` ("epsilon" or "v_prediction") is passed to
+    `pww_load_tools` when this call loads the models (None: the model's own); with `preloaded_utils` the scheduler's
+    config decides."""
     control = _control_arguments(controlnet, control_image, color_map_image.size, "color_map_image",
                                  controlnet_conditioning_scale, guess_mode, control_guidance_start,
                                  control_guidance_end)
-    tools = _tools(preloaded_utils, device, scheduler_type, local_model_path, hf_model_path, model_token, torch_dtype)
+    tools = _tools(preloaded_utils, device, scheduler_type, local_model_path, hf_model_path, model_token, torch_dtype,
+                   prediction_type)
     vae, unet, text_encoder, tokenizer, scheduler = tools
     scheduler.set_timesteps(num_inference_steps)
     if init_image is None:
@@ -787,19 +837,21 @@ def paint_with_words(
         # the reference draws img2img's noise from the global RNG as it stands: unseeded here
         latents, timesteps = _img2img_latents(vae, scheduler, init_image, num_inference_steps, strength, device)
     sampler = PwWSampler(unet, scheduler, [cond], [uncond], latents, weight_function, guidance_scale,
-                         timesteps=timesteps, noise_seed=seed, record_attention=return_attention_maps, **control)
+                         timesteps=timesteps, noise_seed=seed, record_attention=return_attention_maps,
+                         guidance_rescale=guidance_rescale, **control)
     result = _result(vae, sampler.run(), return_latents)
     if not return_attention_maps:
         return result
     return result, _region_attention(sampler.attention_maps()[0], cond, color_context, color_map_image)
 
 
-def _tools(preloaded_utils, device, scheduler_type, local_model_path, hf_model_path, model_token, torch_dtype):
+def _tools(preloaded_utils, device, scheduler_type, local_model_path, hf_model_path, model_token, torch_dtype,
+           prediction_type=None):
     """The caller's (vae, unet, text_encoder, tokenizer, scheduler), or `pww_load_tools`'s when it passes none."""
     if preloaded_utils is not None:
         return preloaded_utils
     return pww_load_tools(device, scheduler_type, local_model_path=local_model_path, hf_model_path=hf_model_path,
-                          model_token=model_token, torch_dtype=torch_dtype)
+                          model_token=model_token, torch_dtype=torch_dtype, prediction_type=prediction_type)
 
 
 def _txt2img_inputs(tools, device, color_map_image, color_context, input_prompt, unconditional_input_prompt, seed,
@@ -905,7 +957,7 @@ def _control_arguments(controlnet, control_image, size: Tuple[int, int], size_of
 # the per-image keyword arguments of paint_with_words that paint_with_words_batch takes per entry
 BATCH_SETTING_KEYS = ("color_context", "color_map_image", "input_prompt", "unconditional_input_prompt", "seed",
                       "weight_function", "guidance_scale", "max_prompt_chunks", "control_image",
-                      "controlnet_conditioning_scale")
+                      "controlnet_conditioning_scale", "guidance_rescale")
 
 
 def _batch_settings(settings) -> List[dict]:
@@ -956,23 +1008,25 @@ def paint_with_words_batch(
     control_guidance_start: Union[float, Sequence[float]] = 0.0,
     control_guidance_end: Union[float, Sequence[float]] = 1.0,
     return_attention_maps: bool = False,
+    prediction_type: Optional[str] = None,
 ):
     """Many images, each with its own settings, in as few samplers as possible.  `settings[i]` is a dict of the
     per-image keyword arguments of `paint_with_words` (BATCH_SETTING_KEYS: color_context, color_map_image, input_prompt,
     unconditional_input_prompt, seed, weight_function, guidance_scale, max_prompt_chunks, control_image,
-    controlnet_conditioning_scale); missing keys take paint_with_words's defaults.  Returns a list of PIL images (or
-    [1,4,h,w] latents) in input order; image i equals `paint_with_words(**settings[i])` up to fp16 noise.
+    controlnet_conditioning_scale, guidance_rescale); missing keys take paint_with_words's defaults.  Returns a list of
+    PIL images (or [1,4,h,w] latents) in input order; image i equals `paint_with_words(**settings[i])` up to fp16 noise.
     With `controlnet` (one for the batch, with `guess_mode` and the guidance window) every entry needs a
     `control_image` of its colour map's size; its `controlnet_conditioning_scale` is its own.  With a list of
     ControlNets (`guess_mode` and the window each one value or one per ControlNet), an entry's `control_image` is a list
     of one image per ControlNet and its `controlnet_conditioning_scale` one float or one per ControlNet.
 
     Entries of the same latent size and text length run in one `PwWSampler` of at most `max_batch_size` images (a
-    2 * max_batch_size UNet batch with CFG), whatever their weight functions and guidance scales.  The default of 8 gave
-    the most images/s of k = 1, 2, 4, 8 at 512x512 (BASELINE.md section 4) and bounds memory.  Sizes that are not multiples of 64 need the single-image weight-map fallback and
-    run one image per sampler.  img2img (init_image / strength) is not batched.  `torch_dtype` as in
-    `paint_with_words`.  `return_attention_maps=True` returns a list of (image, RegionAttention) pairs in input order
-    (see `paint_with_words`)."""
+    2 * max_batch_size UNet batch with CFG), whatever their weight functions, guidance scales and guidance rescales.
+    The default of 8 gave the most images/s of k = 1, 2, 4, 8 at 512x512 (BASELINE.md section 4) and bounds memory.
+    Sizes that are not multiples of 64 need the single-image weight-map fallback and run one image per sampler.
+    img2img (init_image / strength) is not batched.  `torch_dtype` as in `paint_with_words`.
+    `return_attention_maps=True` returns a list of (image, RegionAttention) pairs in input order (see
+    `paint_with_words`).  `prediction_type` as in `paint_with_words`."""
     entries = _batch_settings(settings)
     if max_batch_size < 1:
         raise ValueError("max_batch_size must be >= 1")
@@ -984,7 +1038,8 @@ def paint_with_words_batch(
                                                control_guidance_start, control_guidance_end))
         except ValueError as err:
             raise ValueError(f"settings[{i}]: {err}") from err
-    tools = _tools(preloaded_utils, device, scheduler_type, local_model_path, hf_model_path, model_token, torch_dtype)
+    tools = _tools(preloaded_utils, device, scheduler_type, local_model_path, hf_model_path, model_token, torch_dtype,
+                   prediction_type)
     vae, unet, _, _, scheduler = tools
     scheduler.set_timesteps(num_inference_steps)
     encoded, keys = [], []
@@ -1009,7 +1064,8 @@ def paint_with_words_batch(
                              torch.cat([encoded[i][2] for i in idx], 0),
                              [entries[i]["weight_function"] for i in idx], [entries[i]["guidance_scale"] for i in idx],
                              timesteps=scheduler.timesteps, noise_seed=[entries[i]["seed"] for i in idx],
-                             record_attention=return_attention_maps, **control)
+                             record_attention=return_attention_maps,
+                             guidance_rescale=[entries[i]["guidance_rescale"] for i in idx], **control)
         latents = sampler.run()
         maps = sampler.attention_maps() if return_attention_maps else None
         for j, i in enumerate(idx):
@@ -1079,18 +1135,20 @@ def paint_with_words_inpaint(
     control_guidance_start: Union[float, Sequence[float]] = 0.0,
     control_guidance_end: Union[float, Sequence[float]] = 1.0,
     return_attention_maps: bool = False,
+    guidance_rescale: float = 0.0,
+    prediction_type: Optional[str] = None,
 ):
     """paint_with_words_inpaint.py:137-270: 9-channel UNet input cat[latents, mask, masked-image latents].
     `max_prompt_chunks`, `torch_dtype` and the ControlNet arguments as in `paint_with_words`; the colour map is resized
     to the init image, so `control_image` has the init image's size.  The ControlNet sees the 4 latent channels of
     the UNet input (hook_pww.py:113-119).  `return_attention_maps` as in `paint_with_words` (coverage from the resized
-    colour map)."""
+    colour map).  `guidance_rescale` and `prediction_type` as in `paint_with_words`."""
     width, height = init_image.size
     control = _control_arguments(controlnet, control_image, (width, height), "init_image (and resized color_map_image)",
                                  controlnet_conditioning_scale, guess_mode, control_guidance_start,
                                  control_guidance_end)
     vae, unet, text_encoder, tokenizer, scheduler = _tools(preloaded_utils, device, scheduler_type, local_model_path,
-                                                           hf_model_path, model_token, torch_dtype)
+                                                           hf_model_path, model_token, torch_dtype, prediction_type)
     color_map_image = color_map_image.resize((width, height), Image.NEAREST)
     mask_image = mask_image.resize((width, height), Image.NEAREST)
     _, _, cond, uncond = _encode_text_color_inputs(
@@ -1115,7 +1173,8 @@ def paint_with_words_inpaint(
             f"num_channels_masked_image: {masked_image_latents.shape[1]} = {total}.")
     sampler = PwWSampler(unet, scheduler, [cond], [uncond], latents, weight_function, guidance_scale,
                          extra_input=torch.cat([mask, masked_image_latents], 1).float(), timesteps=timesteps,
-                         noise_seed=seed, record_attention=return_attention_maps, **control)
+                         noise_seed=seed, record_attention=return_attention_maps, guidance_rescale=guidance_rescale,
+                         **control)
     result = _result(vae, sampler.run(), return_latents)
     if not return_attention_maps:
         return result
@@ -1135,7 +1194,8 @@ class PipelineOutput:
 class PaintWithWord_StableDiffusionPipeline:
     """Same constructor / `from_pretrained` / `plugin_cross_attention` / `__call__` surface as the reference class
     (paint_with_words.py:513-842); the work is `paint_with_words()` above (one `PwWSampler`).  Like the reference class
-    it always uses its own LMS scheduler (paint_with_words.py:534-539) and has no regional blur (:574)."""
+    it always uses its own LMS scheduler (paint_with_words.py:534-539), with the `prediction_type` of the scheduler it
+    is given (so `from_pretrained` keeps a v-prediction model's), and has no regional blur (:574)."""
 
     def __init__(self, vae, text_encoder, tokenizer, unet, scheduler=None, safety_checker=None, feature_extractor=None,
                  requires_safety_checker: bool = False, controlnet=None):
@@ -1144,8 +1204,9 @@ class PaintWithWord_StableDiffusionPipeline:
         self.vae, self.text_encoder, self.tokenizer, self.unet = vae, text_encoder, tokenizer, unet
         self.safety_checker, self.feature_extractor = safety_checker, feature_extractor
         self.controlnet = controlnet
+        prediction_type = dict(getattr(scheduler, "config", None) or {}).get("prediction_type", "epsilon")
         self.scheduler = LMSDiscreteScheduler(beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear",
-                                              num_train_timesteps=1000)
+                                              num_train_timesteps=1000, prediction_type=prediction_type)
         self.plugin_cross_attention()
 
     @classmethod
@@ -1193,9 +1254,11 @@ class PaintWithWord_StableDiffusionPipeline:
                  num_images_per_prompt: int = 1, eta: float = 0.5, seed: int = 0, generator=None, image=None, latents=None,
                  output_type: str = "pil", return_dict: bool = True, callback=None, callback_steps: int = 1,
                  max_prompt_chunks: int = 1, control_image=None, controlnet_conditioning_scale: float = 1.0,
-                 guess_mode: bool = False, control_guidance_start: float = 0.0, control_guidance_end: float = 1.0):
+                 guess_mode: bool = False, control_guidance_start: float = 0.0, control_guidance_end: float = 1.0,
+                 guidance_rescale: float = 0.0):
         extra = {} if image is None else {"init_image": image, "strength": eta}
         extra["max_prompt_chunks"] = max_prompt_chunks
+        extra["guidance_rescale"] = guidance_rescale
         extra.update(self._control(control_image, controlnet_conditioning_scale, guess_mode, control_guidance_start,
                                    control_guidance_end))
         return self._run(paint_with_words, prompt, color_map_image, dict(color_context), weight_function,
@@ -1220,10 +1283,11 @@ class PaintWithWord_StableDiffusionInpaintPipeline(PaintWithWord_StableDiffusion
                  num_images_per_prompt: int = 1, eta: float = 1.0, seed: int = 0, generator=None, latents=None,
                  output_type: str = "pil", return_dict: bool = True, callback=None, callback_steps: int = 1,
                  max_prompt_chunks: int = 1, control_image=None, controlnet_conditioning_scale: float = 1.0,
-                 guess_mode: bool = False, control_guidance_start: float = 0.0, control_guidance_end: float = 1.0):
+                 guess_mode: bool = False, control_guidance_start: float = 0.0, control_guidance_end: float = 1.0,
+                 guidance_rescale: float = 0.0):
         return self._run(paint_with_words_inpaint, prompt, color_map_image, dict(color_context), weight_function,
                          num_inference_steps, guidance_scale, negative_prompt, seed, output_type, return_dict, callback,
                          callback_steps, mask_image=mask_image, init_image=image, strength=eta,
-                         max_prompt_chunks=max_prompt_chunks,
+                         max_prompt_chunks=max_prompt_chunks, guidance_rescale=guidance_rescale,
                          **self._control(control_image, controlnet_conditioning_scale, guess_mode,
                                          control_guidance_start, control_guidance_end))

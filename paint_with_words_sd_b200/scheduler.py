@@ -14,6 +14,10 @@ GPU-first change: the multistep coefficients of every step are integrated once i
 Euler, Euler ancestral and DPM++ 2M (below) are restated the same way from their published definitions (Karras et al.
 2022; k-diffusion's `sample_euler_ancestral` / `sample_dpmpp_2m`; Lu et al. 2022), on the LMS schedule or the Karras
 schedule.  `step_form` writes any of the four as the one linear update the sampler kernel runs.
+
+Every scheduler takes `prediction_type`: "epsilon" (the model predicts the noise) or "v_prediction" (the SD2.x 768
+models: v = sqrt(abar) eps - sqrt(1 - abar) x0, Salimans & Ho 2022), converted in sigma space as diffusers' schedulers
+do: x0 = -sigma/sqrt(sigma^2+1) v + x/(sigma^2+1), eps = (x - x0)/sigma.
 """
 from __future__ import annotations
 
@@ -23,6 +27,28 @@ from typing import List, Optional
 import numpy as np
 import torch
 from scipy import integrate
+
+
+PREDICTION_TYPES = ("epsilon", "v_prediction")
+
+
+def check_prediction_type(prediction_type: str) -> None:
+    if prediction_type not in PREDICTION_TYPES:
+        raise ValueError(f"prediction_type must be one of {PREDICTION_TYPES}, got {prediction_type!r}")
+
+
+def predicted_original(prediction_type: str, model_output, sample, sigma: float):
+    """x0 from the model output at noise level sigma: x - sigma eps, or -sigma/sqrt(sigma^2+1) v + x/(sigma^2+1)."""
+    if prediction_type == "epsilon":
+        return sample - sigma * model_output
+    return model_output * (-sigma / (sigma ** 2 + 1) ** 0.5) + (sample / (sigma ** 2 + 1))
+
+
+def predicted_eps(prediction_type: str, model_output, sample, sigma: float):
+    """eps from the model output: the output itself, or (x - x0)/sigma for a v output."""
+    if prediction_type == "epsilon":
+        return model_output
+    return (sample - predicted_original(prediction_type, model_output, sample, sigma)) / sigma
 
 
 class _StepOutput:
@@ -35,7 +61,8 @@ class LMSDiscreteScheduler:
     order = 1
 
     def __init__(self, beta_start: float = 0.0001, beta_end: float = 0.02, beta_schedule: str = "linear",
-                 num_train_timesteps: int = 1000):
+                 num_train_timesteps: int = 1000, prediction_type: str = "epsilon"):
+        check_prediction_type(prediction_type)
         if beta_schedule == "linear":
             betas = np.linspace(beta_start, beta_end, num_train_timesteps, dtype=np.float32)
         elif beta_schedule == "scaled_linear":
@@ -43,7 +70,7 @@ class LMSDiscreteScheduler:
         else:
             raise NotImplementedError(beta_schedule)
         self.config = {"num_train_timesteps": num_train_timesteps, "beta_start": beta_start,
-                       "beta_end": beta_end, "beta_schedule": beta_schedule}
+                       "beta_end": beta_end, "beta_schedule": beta_schedule, "prediction_type": prediction_type}
         self.betas = torch.from_numpy(betas)
         self.alphas_cumprod = torch.cumprod(1.0 - self.betas, dim=0)
         sig = self._train_sigmas()
@@ -106,7 +133,7 @@ class LMSDiscreteScheduler:
     def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, order: int = 4):
         i = self.step_index_of(timestep)
         sigma = float(self.sigmas[i])
-        pred_original_sample = sample - sigma * model_output       # epsilon prediction
+        pred_original_sample = predicted_original(self.config["prediction_type"], model_output, sample, sigma)
         derivative = (sample - pred_original_sample) / sigma
         self.derivatives.append(derivative)
         if len(self.derivatives) > order:
@@ -126,7 +153,7 @@ class LMSDiscreteScheduler:
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# Euler, Euler ancestral and DPM++ 2M (sigma space, epsilon prediction)
+# Euler, Euler ancestral and DPM++ 2M (sigma space)
 # ---------------------------------------------------------------------------------------------------------------------
 def karras_sigmas(sigma_min: float, sigma_max: float, n: int, rho: float = 7.0) -> np.ndarray:
     """Karras et al. 2022, eq. (5): sigma_i = (max^(1/rho) + i/(n-1) (min^(1/rho) - max^(1/rho)))^rho, i = 0 .. n-1."""
@@ -151,8 +178,8 @@ class _SigmaScheduler:
     order = 1
 
     def __init__(self, beta_start: float = 0.0001, beta_end: float = 0.02, beta_schedule: str = "linear",
-                 num_train_timesteps: int = 1000, use_karras_sigmas: bool = False):
-        self._lms = LMSDiscreteScheduler(beta_start, beta_end, beta_schedule, num_train_timesteps)
+                 num_train_timesteps: int = 1000, use_karras_sigmas: bool = False, prediction_type: str = "epsilon"):
+        self._lms = LMSDiscreteScheduler(beta_start, beta_end, beta_schedule, num_train_timesteps, prediction_type)
         self.config = dict(self._lms.config, use_karras_sigmas=use_karras_sigmas)
         self.use_karras_sigmas = use_karras_sigmas
         self.betas, self.alphas_cumprod = self._lms.betas, self._lms.alphas_cumprod
@@ -204,6 +231,10 @@ class _SigmaScheduler:
         i = self.step_index_of(timestep)
         return i, float(self.sigmas[i]), float(self.sigmas[i + 1])
 
+    def _eps_and_original(self, model_output, sample, sigma: float):
+        p = self.config["prediction_type"]
+        return predicted_eps(p, model_output, sample, sigma), predicted_original(p, model_output, sample, sigma)
+
 
 class EulerDiscreteScheduler(_SigmaScheduler):
     """Euler method on the probability-flow ODE dx/dsigma = eps (Karras et al. 2022, Algorithm 1 without churn):
@@ -211,7 +242,8 @@ class EulerDiscreteScheduler(_SigmaScheduler):
 
     def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, **kw):
         _, sigma, sigma_next = self._sigma_pair(timestep)
-        return _StepOutput(sample + (sigma_next - sigma) * model_output, sample - sigma * model_output)
+        eps, original = self._eps_and_original(model_output, sample, sigma)
+        return _StepOutput(sample + (sigma_next - sigma) * eps, original)
 
 
 def ancestral_sigmas(sigma: float, sigma_next: float):
@@ -232,13 +264,14 @@ class EulerAncestralDiscreteScheduler(_SigmaScheduler):
         sigma_down, sigma_up = ancestral_sigmas(sigma, sigma_next)
         if noise is None:
             noise = torch.randn(sample.shape, generator=generator, dtype=sample.dtype).to(sample.device)
-        prev = sample + (sigma_down - sigma) * model_output + sigma_up * noise
-        return _StepOutput(prev, sample - sigma * model_output)
+        eps, original = self._eps_and_original(model_output, sample, sigma)
+        prev = sample + (sigma_down - sigma) * eps + sigma_up * noise
+        return _StepOutput(prev, original)
 
 
 class DPMSolverMultistepScheduler(_SigmaScheduler):
-    """DPM-Solver++(2M) in sigma space with epsilon prediction (Lu et al. 2022; k-diffusion `sample_dpmpp_2m`):
-    D = x - sigma eps, h = log sigma - log sigma',
+    """DPM-Solver++(2M) in sigma space (Lu et al. 2022; k-diffusion `sample_dpmpp_2m`):
+    D = x0 (x - sigma eps for an epsilon model), h = log sigma - log sigma',
       first order:  x' = (sigma'/sigma) x - expm1(-h) D
       second order: x' = (sigma'/sigma) x - expm1(-h) ((1 + 1/2r) D - (1/2r) D_prev),  r = h_prev / h.
     The first step of a run (or a step that does not follow the previous one) is first order, and the step to
@@ -250,7 +283,7 @@ class DPMSolverMultistepScheduler(_SigmaScheduler):
 
     def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, **kw):
         i, sigma, sigma_next = self._sigma_pair(timestep)
-        denoised = sample - sigma * model_output
+        denoised = predicted_original(self.config["prediction_type"], model_output, sample, sigma)
         prev, self._prev = self._prev, (i, denoised)
         if sigma_next == 0:
             return _StepOutput(denoised, denoised)
@@ -279,10 +312,22 @@ def history_length(scheduler) -> int:
 
 def step_form(scheduler, step_index: int, first: bool):
     """The step of `scheduler` at schedule position `step_index` as one linear update per image, in float64:
-        q      = a x + b eps                                        (the new history entry)
+        q      = a x + b out                                        (the new history entry)
         x_next = alpha x + (beta0 q + beta1 h1 + beta2 h2 + beta3 h3) + gamma z
-    with h_k the entry k steps old.  `first`: no earlier step of this run (DPM++ 2M's first step is first order).
-    Returns (alpha, a, b, [beta0..beta3], gamma).  Any other scheduler class raises TypeError."""
+    with out the (guided) model output and h_k the entry k steps old.  `first`: no earlier step of this run (DPM++ 2M's
+    first step is first order).  Returns (alpha, a, b, [beta0..beta3], gamma).  Any other scheduler class raises
+    TypeError.
+    For a v-prediction scheduler, eps = sigma/(sigma^2+1) x + v/sqrt(sigma^2+1) is linear in x and v, so its form is the
+    epsilon form with a_v = a + b sigma/(sigma^2+1) and b_v = b/sqrt(sigma^2+1); alpha, beta and gamma are unchanged."""
+    alpha, a, b, beta, gamma = _eps_step_form(scheduler, step_index, first)
+    if scheduler.config["prediction_type"] == "epsilon":
+        return alpha, a, b, beta, gamma
+    sigma = float(scheduler.sigmas[step_index])
+    return alpha, a + b * sigma / (sigma * sigma + 1.0), b / math.sqrt(sigma * sigma + 1.0), beta, gamma
+
+
+def _eps_step_form(scheduler, step_index: int, first: bool):
+    """`step_form` for an epsilon model: out = eps."""
     sch, i = scheduler, step_index
     if isinstance(sch, LMSDiscreteScheduler):
         # paint_with_words.py:506 -> order = min(step_index+1, 4) on the ABSOLUTE schedule index; missing history

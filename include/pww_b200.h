@@ -386,6 +386,29 @@ int pww_sampler_update_rescale(const void* eps, int eps_dtype, int64_t eps_batch
                                int m, int height, int width, void* stream);
 
 /*
+ * pww_sampler_update_masked: the update for masked img2img (inpainting with a model that has no mask input), in one
+ * launch.  The step is pww_sampler_update's (rescale == NULL) or pww_sampler_update_rescale's (rescale != NULL, with
+ * its `stats_out`), then every latent value is blended with the init image's noise path at the next sigma:
+ *   x_next = M x_step + (1 - M) (init + z sigma')
+ * x_step is the step's result (ancestral noise included), init = init_latents[i], z = init_noise[i] (the noise that
+ * made the start latents init + sigma_0 z), M = mask[i] broadcast over the 4 channels (1 = repaint), and sigma' =
+ * sigma_next[0], a device scalar (0 after the last step, which leaves init itself where M == 0).  fp32, rounded after
+ * every operation in the order written; init + z sigma' is the bits of the host's init + noise * sigma.  The history
+ * entry keeps the un-blended q = a x + b eps, as a host loop that blends after each scheduler step would.
+ * init_latents and init_noise are [m, 4, h, w], mask [m, 1, h, w], all fp32 contiguous device arrays.
+ * Returns PWW_ERR_BAD_ARG and PWW_ERR_UNSUPPORTED, before any CUDA call, as pww_sampler_update does, and
+ * PWW_ERR_BAD_ARG for a null init_latents, init_noise, mask or sigma_next, or a stats_out without rescale.
+ */
+int pww_sampler_update_masked(const void* eps, int eps_dtype, int64_t eps_batch_stride, int64_t eps_channel_stride,
+                              int64_t eps_row_stride, int64_t eps_col_stride,
+                              float* latents, float* history, int history_len, const float* noise,
+                              const float* guidance, const float* beta, const float* form,
+                              const float* rescale, float* stats_out,
+                              const float* init_latents, const float* init_noise, const float* mask,
+                              const float* sigma_next,
+                              int m, int height, int width, void* stream);
+
+/*
  * ControlNet residual injection: n (1..16) residuals added in place into n activations, in one launch.
  *   dst_k[b] = E( dst_k[b] + E( s[k, b] * res_k[b] ) )        k < n, b < rows
  * dst[k] points at a [B, elems_per_image[k]] tensor and res[k] at a [rows, elems_per_image[k]] one, both dense (a

@@ -32,7 +32,7 @@ EXPORTS = (
     "pww_resnet_residual_f16", "pww_resnet_residual_bf16",
     "pww_xattn_fused_rec_f16", "pww_xattn_fused_rec_bf16",
     "pww_adapter_residual_f16", "pww_adapter_residual_bf16",
-    "pww_sampler_update_rescale",
+    "pww_sampler_update_rescale", "pww_sampler_update_masked",
 )
 
 
@@ -122,6 +122,10 @@ def lib() -> ctypes.CDLL:
     # pww_sampler_update's arguments with rescale [m] and stats_out [m, 3] (or NULL) after `form`
     L.pww_sampler_update_rescale.restype = c_i
     L.pww_sampler_update_rescale.argtypes = L.pww_sampler_update.argtypes[:13] + [c_vp, c_vp] + \
+        L.pww_sampler_update.argtypes[13:]
+    # pww_sampler_update_rescale's arguments up to stats_out, then init_latents, init_noise, mask and sigma_next
+    L.pww_sampler_update_masked.restype = c_i
+    L.pww_sampler_update_masked.argtypes = L.pww_sampler_update_rescale.argtypes[:15] + [c_vp] * 4 + \
         L.pww_sampler_update.argtypes[13:]
     _lib = L
     return L

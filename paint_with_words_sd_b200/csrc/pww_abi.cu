@@ -680,9 +680,10 @@ int pww_sampler_update(const void* eps, int eps_dtype, int64_t eps_batch_stride,
   const bool cl = eps_channel_stride == 1 && eps_col_stride == 4 && eps_row_stride == 4 * (int64_t)width &&
                   (reinterpret_cast<uintptr_t>(eps) % need) == 0 && ((size_t)eps_batch_stride * es) % need == 0;
   cudaStream_t s = (cudaStream_t)stream;
-  const cudaError_t e = eps_dtype == PWW_DTYPE_F16    ? pww::smp::launch_update<__half>(a, px4, cl, s)
-                        : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_update<__nv_bfloat16>(a, px4, cl, s)
-                                                      : pww::smp::launch_update<float>(a, px4, cl, s);
+  const pww::smp::BlendArgs none{};
+  const cudaError_t e = eps_dtype == PWW_DTYPE_F16    ? pww::smp::launch_update<__half, false>(a, none, px4, cl, s)
+                        : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_update<__nv_bfloat16, false>(a, none, px4, cl, s)
+                                                      : pww::smp::launch_update<float, false>(a, none, px4, cl, s);
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 
@@ -708,9 +709,51 @@ int pww_sampler_update_rescale(const void* eps, int eps_dtype, int64_t eps_batch
   const bool cl = eps_channel_stride == 1 && eps_col_stride == 4 && eps_row_stride == 4 * (int64_t)width &&
                   (reinterpret_cast<uintptr_t>(eps) % need) == 0 && ((size_t)eps_batch_stride * es) % need == 0;
   cudaStream_t s = (cudaStream_t)stream;
-  const cudaError_t e = eps_dtype == PWW_DTYPE_F16    ? pww::smp::launch_update_rescale<__half>(a, r, px4, cl, s)
-                        : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_update_rescale<__nv_bfloat16>(a, r, px4, cl, s)
-                                                      : pww::smp::launch_update_rescale<float>(a, r, px4, cl, s);
+  const pww::smp::BlendArgs none{};
+  const cudaError_t e =
+      eps_dtype == PWW_DTYPE_F16    ? pww::smp::launch_update_rescale<__half, false>(a, r, none, px4, cl, s)
+      : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_update_rescale<__nv_bfloat16, false>(a, r, none, px4, cl, s)
+                                    : pww::smp::launch_update_rescale<float, false>(a, r, none, px4, cl, s);
+  return e == cudaSuccess ? PWW_OK : cuda_fail(e);
+}
+
+int pww_sampler_update_masked(const void* eps, int eps_dtype, int64_t eps_batch_stride, int64_t eps_channel_stride,
+                              int64_t eps_row_stride, int64_t eps_col_stride, float* latents, float* history,
+                              int history_len, const float* noise, const float* guidance, const float* beta,
+                              const float* form, const float* rescale, float* stats_out, const float* init_latents,
+                              const float* init_noise, const float* mask, const float* sigma_next, int m, int height,
+                              int width, void* stream) {
+  if (!eps || !latents || !history || !guidance || !beta || !form) return PWW_ERR_BAD_ARG;
+  if (!init_latents || !init_noise || !mask || !sigma_next || (stats_out && !rescale)) return PWW_ERR_BAD_ARG;
+  if (m <= 0 || height <= 0 || width <= 0 || history_len < 1 || history_len > 4) return PWW_ERR_BAD_ARG;
+  if (eps_dtype != PWW_DTYPE_F32 && eps_dtype != PWW_DTYPE_F16 && eps_dtype != PWW_DTYPE_BF16) return PWW_ERR_UNSUPPORTED;
+  pww::smp::UpdateArgs a;
+  a.eps = eps; a.e_sn = eps_batch_stride; a.e_sc = eps_channel_stride; a.e_sh = eps_row_stride; a.e_sw = eps_col_stride;
+  a.lat = latents; a.hist = history; a.noise = noise; a.gscale = guidance; a.beta = beta; a.form = form;
+  a.m = m; a.h = height; a.w = width; a.nh = history_len;
+  pww::smp::BlendArgs bl;
+  bl.init = init_latents; bl.noise0 = init_noise; bl.mask = mask; bl.sigma_next = sigma_next;
+  // pww_sampler_update's pixel grouping and channels-last test, with the blend inputs read 4 pixels at a time too
+  const int64_t hw = (int64_t)height * width;
+  const size_t es = eps_dtype == PWW_DTYPE_F32 ? 4 : 2;
+  const bool px4 = (hw % 4) == 0 && aligned16(latents) && aligned16(history) && (!noise || aligned16(noise)) &&
+                   aligned16(init_latents) && aligned16(init_noise) && aligned16(mask);
+  const size_t need = px4 ? 16 : 4 * es;
+  const bool cl = eps_channel_stride == 1 && eps_col_stride == 4 && eps_row_stride == 4 * (int64_t)width &&
+                  (reinterpret_cast<uintptr_t>(eps) % need) == 0 && ((size_t)eps_batch_stride * es) % need == 0;
+  cudaStream_t s = (cudaStream_t)stream;
+  cudaError_t e;
+  if (rescale) {
+    pww::smp::RescaleArgs r;
+    r.phi = rescale; r.stats = stats_out;
+    e = eps_dtype == PWW_DTYPE_F16    ? pww::smp::launch_update_rescale<__half, true>(a, r, bl, px4, cl, s)
+        : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_update_rescale<__nv_bfloat16, true>(a, r, bl, px4, cl, s)
+                                      : pww::smp::launch_update_rescale<float, true>(a, r, bl, px4, cl, s);
+  } else {
+    e = eps_dtype == PWW_DTYPE_F16    ? pww::smp::launch_update<__half, true>(a, bl, px4, cl, s)
+        : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_update<__nv_bfloat16, true>(a, bl, px4, cl, s)
+                                      : pww::smp::launch_update<float, true>(a, bl, px4, cl, s);
+  }
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 

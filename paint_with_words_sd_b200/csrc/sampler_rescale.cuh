@@ -93,11 +93,11 @@ __device__ __forceinline__ float2 cluster_sum(float2 v, float2* warp_part, float
   return t;
 }
 
-// out' = k cfg (phi == 0: cfg itself, k never applied), then sampler_update_kernel's step form, operation for
-// operation, on the 4 channels of pixels p0 .. p0 + PX - 1 of image i.
-template <int PX>
-__device__ __forceinline__ void rescaled_update(const UpdateArgs& a, int i, int p0, float (&eg)[4][PX], float phi,
-                                                float k) {
+// out' = k cfg (phi == 0: cfg itself, k never applied), then sampler_update_kernel's step form (and, BLEND, its
+// mask blend), operation for operation, on the 4 channels of pixels p0 .. p0 + PX - 1 of image i.
+template <int PX, bool BLEND>
+__device__ __forceinline__ void rescaled_update(const UpdateArgs& a, const BlendArgs& bl, int i, int p0,
+                                                float (&eg)[4][PX], float phi, float k) {
   if (phi != 0.f) {
 #pragma unroll
     for (int c = 0; c < 4; ++c)
@@ -110,6 +110,11 @@ __device__ __forceinline__ void rescaled_update(const UpdateArgs& a, int i, int 
   const float b0 = __ldg(a.beta + 0);
   const bool with_noise = a.noise != nullptr && gamma != 0.f;
   const int64_t entry = (int64_t)a.m * 4 * hw;
+  float mk[PX], sn = 0.f;
+  if constexpr (BLEND) {
+    load_px<PX>(bl.mask + (int64_t)i * hw + p0, mk);
+    sn = __ldg(bl.sigma_next);
+  }
 #pragma unroll
   for (int c = 0; c < 4; ++c) {
     const int64_t off = ((int64_t)i * 4 + c) * hw + p0;
@@ -137,14 +142,17 @@ __device__ __forceinline__ void rescaled_update(const UpdateArgs& a, int i, int 
 #pragma unroll
       for (int j = 0; j < PX; ++j) x[j] = __fadd_rn(x[j], __fmul_rn(gamma, z[j]));
     }
+    if constexpr (BLEND) blend_px<PX>(bl, off, mk, sn, x);
     store_px<PX>(a.lat + off, x);
   }
 }
 
 // One cluster per image; thread t of CTA rank r owns the PX-pixel groups r * 512 + t + k * (cluster size * 512).
-template <typename T, int PX, bool CL>
+// `bl` is read only by the BLEND instances.
+template <typename T, int PX, bool CL, bool BLEND>
 __global__ void __launch_bounds__(kRescaleThreads, 1) sampler_update_rescale_kernel(const UpdateArgs a,
-                                                                                    const RescaleArgs r) {
+                                                                                    const RescaleArgs r,
+                                                                                    const BlendArgs bl) {
   namespace cg = cooperative_groups;
   const cg::cluster_group cl = cg::this_cluster();
   __shared__ float2 warp_part[kRescaleThreads / 32];
@@ -191,11 +199,11 @@ __global__ void __launch_bounds__(kRescaleThreads, 1) sampler_update_rescale_ker
   }
 
   // pass 3: the update
-  if (own) rescaled_update<PX>(a, i, g0 * PX, f0, phi, k);
+  if (own) rescaled_update<PX, BLEND>(a, bl, i, g0 * PX, f0, phi, k);
   for (int g = g0 + stride; g < groups; g += stride) {
     float c[4][PX], f[4][PX];
     cond_and_cfg<T, PX, CL>(a, i, g * PX, c, f);
-    rescaled_update<PX>(a, i, g * PX, f, phi, k);
+    rescaled_update<PX, BLEND>(a, bl, i, g * PX, f, phi, k);
   }
   cl.sync();      // the other CTAs have read slots[1]
 }
@@ -207,8 +215,8 @@ inline int rescale_cluster_size(int64_t groups) {
   return cs;
 }
 
-template <typename T, int PX, bool CL>
-cudaError_t launch_rescale_instance(const UpdateArgs& a, const RescaleArgs& r, cudaStream_t s) {
+template <typename T, int PX, bool CL, bool BLEND>
+cudaError_t launch_rescale_instance(const UpdateArgs& a, const RescaleArgs& r, const BlendArgs& bl, cudaStream_t s) {
   const int cs = rescale_cluster_size((int64_t)a.h * a.w / PX);
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -222,13 +230,17 @@ cudaError_t launch_rescale_instance(const UpdateArgs& a, const RescaleArgs& r, c
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, sampler_update_rescale_kernel<T, PX, CL>, a, r);
+  return cudaLaunchKernelEx(&cfg, sampler_update_rescale_kernel<T, PX, CL, BLEND>, a, r, bl);
 }
 
-template <typename T>
-cudaError_t launch_update_rescale(const UpdateArgs& a, const RescaleArgs& r, bool px4, bool cl, cudaStream_t s) {
-  if (px4) return cl ? launch_rescale_instance<T, 4, true>(a, r, s) : launch_rescale_instance<T, 4, false>(a, r, s);
-  return cl ? launch_rescale_instance<T, 1, true>(a, r, s) : launch_rescale_instance<T, 1, false>(a, r, s);
+template <typename T, bool BLEND>
+cudaError_t launch_update_rescale(const UpdateArgs& a, const RescaleArgs& r, const BlendArgs& bl, bool px4, bool cl,
+                                  cudaStream_t s) {
+  if (px4)
+    return cl ? launch_rescale_instance<T, 4, true, BLEND>(a, r, bl, s)
+              : launch_rescale_instance<T, 4, false, BLEND>(a, r, bl, s);
+  return cl ? launch_rescale_instance<T, 1, true, BLEND>(a, r, bl, s)
+            : launch_rescale_instance<T, 1, false, BLEND>(a, r, bl, s);
 }
 
 }  // namespace smp

@@ -7,6 +7,9 @@
 //   eps    = eps_u + g_i (eps_c - eps_u)
 //   q      = a x + b eps                          (a == 0: q = b eps)
 //   x_next = alpha x + (beta0 q + beta1 h1 + ...)  (alpha == 1: x + (...))   [+ gamma z when gamma != 0 and z exists]
+// The BLEND instances (pww_sampler_update_masked) then put the area outside the mask M back on the init latents'
+// noise path at the next sigma (masked img2img):
+//   x_next = M x_next + (1 - M) (init + z0 sigma')
 #pragma once
 #include "pww_common.cuh"
 
@@ -26,6 +29,15 @@ struct UpdateArgs {
   const float* beta;                    // [4]
   const float* form;                    // [6]
   int m, h, w, nh;
+};
+
+// The masked instances' extra inputs.  A separate kernel parameter after the existing ones, not UpdateArgs fields, so
+// the parameter offsets, and with them the code, of the unmasked instances stay as they are.
+struct BlendArgs {
+  const float* init;                    // [m, 4, h, w] the init image's latents
+  const float* noise0;                  // [m, 4, h, w] the noise that made the start latents init + sigma0 noise0
+  const float* mask;                    // [m, 1, h, w] in [0, 1], 1 = repaint
+  const float* sigma_next;              // [1] the next step's sigma (0 after the last step)
 };
 
 struct InputArgs {
@@ -119,9 +131,23 @@ __device__ __forceinline__ void guided_eps(const UpdateArgs& a, int i, int p0, f
     for (int j = 0; j < PX; ++j) e[c][j] = __fadd_rn(eu[c][j], __fmul_rn(g, __fsub_rn(e[c][j], eu[c][j])));
 }
 
-// One thread per (image, PX consecutive pixels), all 4 channels.
-template <typename T, int PX, bool CL>
-__global__ void __launch_bounds__(kThreads) sampler_update_kernel(const UpdateArgs a) {
+// The masked instances' epilogue on one channel's PX values x of the step's result, at element offset `off`:
+//   x = M x + (1 - M) (init + z0 sigma')         mk: the pixels' mask values, sn: sigma'
+// For M == 1 this is x + 0 = x, for M == 0 it is 0 + (init + z0 sigma') (finite x and init + z0 sigma').
+template <int PX>
+__device__ __forceinline__ void blend_px(const BlendArgs& bl, int64_t off, const float (&mk)[PX], float sn,
+                                         float (&x)[PX]) {
+  float x0[PX], z0[PX];
+  load_px<PX>(bl.init + off, x0);
+  load_px<PX>(bl.noise0 + off, z0);
+#pragma unroll
+  for (int j = 0; j < PX; ++j)
+    x[j] = __fadd_rn(__fmul_rn(mk[j], x[j]), __fmul_rn(__fsub_rn(1.f, mk[j]), __fadd_rn(x0[j], __fmul_rn(z0[j], sn))));
+}
+
+// One thread per (image, PX consecutive pixels), all 4 channels.  `bl` is read only by the BLEND instances.
+template <typename T, int PX, bool CL, bool BLEND>
+__global__ void __launch_bounds__(kThreads) sampler_update_kernel(const UpdateArgs a, const BlendArgs bl) {
   const int hw = a.h * a.w, groups = hw / PX;
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (int64_t)a.m * groups) return;
@@ -129,6 +155,11 @@ __global__ void __launch_bounds__(kThreads) sampler_update_kernel(const UpdateAr
   const int p0 = (int)(idx - (int64_t)i * groups) * PX;
   float eg[4][PX];
   guided_eps<T, PX, CL>(a, i, p0, eg);
+  float mk[PX], sn = 0.f;
+  if constexpr (BLEND) {
+    load_px<PX>(bl.mask + (int64_t)i * hw + p0, mk);
+    sn = __ldg(bl.sigma_next);
+  }
   const float alpha = __ldg(a.form + 0), ca = __ldg(a.form + 1), cb = __ldg(a.form + 2), gamma = __ldg(a.form + 3);
   const int slot = (int)__ldg(a.form + 4), row = (int)__ldg(a.form + 5);
   const float b0 = __ldg(a.beta + 0);
@@ -161,6 +192,7 @@ __global__ void __launch_bounds__(kThreads) sampler_update_kernel(const UpdateAr
 #pragma unroll
       for (int j = 0; j < PX; ++j) x[j] = __fadd_rn(x[j], __fmul_rn(gamma, z[j]));
     }
+    if constexpr (BLEND) blend_px<PX>(bl, off, mk, sn, x);
     store_px<PX>(a.lat + off, x);
   }
 }
@@ -205,17 +237,17 @@ __global__ void __launch_bounds__(kThreads) sampler_input_kernel(const InputArgs
 
 inline unsigned blocks_for(int64_t threads) { return (unsigned)((threads + kThreads - 1) / kThreads); }
 
-template <typename T>
-cudaError_t launch_update(const UpdateArgs& a, bool px4, bool cl, cudaStream_t s) {
+template <typename T, bool BLEND>
+cudaError_t launch_update(const UpdateArgs& a, const BlendArgs& bl, bool px4, bool cl, cudaStream_t s) {
   const int64_t hw = (int64_t)a.h * a.w;
   if (px4) {
     const unsigned g = blocks_for(a.m * hw / 4);
-    if (cl) sampler_update_kernel<T, 4, true><<<g, kThreads, 0, s>>>(a);
-    else sampler_update_kernel<T, 4, false><<<g, kThreads, 0, s>>>(a);
+    if (cl) sampler_update_kernel<T, 4, true, BLEND><<<g, kThreads, 0, s>>>(a, bl);
+    else sampler_update_kernel<T, 4, false, BLEND><<<g, kThreads, 0, s>>>(a, bl);
   } else {
     const unsigned g = blocks_for(a.m * hw);
-    if (cl) sampler_update_kernel<T, 1, true><<<g, kThreads, 0, s>>>(a);
-    else sampler_update_kernel<T, 1, false><<<g, kThreads, 0, s>>>(a);
+    if (cl) sampler_update_kernel<T, 1, true, BLEND><<<g, kThreads, 0, s>>>(a, bl);
+    else sampler_update_kernel<T, 1, false, BLEND><<<g, kThreads, 0, s>>>(a, bl);
   }
   return cudaGetLastError();
 }

@@ -31,8 +31,8 @@ from .conditioning import (MAX_RECORDED_REGIONS, RATIOS, REGION_COUNT_KEY, REGIO
                            _encode_text_color_inputs, _extract_seed_and_sigma_from_context, _get_binary_mask,
                            _rgb_of, always_round, pack_weight_map, packed_key)
 from . import _native, fused_ops
-from .scheduler import (SIGMA_SCHEDULERS, EulerAncestralDiscreteScheduler, LMSDiscreteScheduler, history_length,
-                        step_form)
+from .scheduler import (FORM_COLUMNS, SIGMA_SCHEDULERS, EulerAncestralDiscreteScheduler, LMSDiscreteScheduler,
+                        history_length, step_form)
 from .synthetic import IdentityVAE, RandomTextEncoder, SimpleWordTokenizer
 from .unet import UNet2DConditionModel, UNetConfig, build_unet, combine_control_residuals
 from .weight_function import STAT_MAX, UnsupportedWeightFunction, g_of_sigma, probe_weight_function
@@ -249,6 +249,8 @@ _T = 2        # the timestep: the UNet's and the ControlNet's `timestep`
 _BETA = 3     # beta0..beta3: pww_sampler_update's `beta`
 _G = 7        # G_0(sigma) .. G_{m-1}(sigma), then m zeros for the uncond images: the attention's G_SIGMA
 # after them, at _G + 2m, scheduler.FORM_COLUMNS (alpha, a, b, gamma, slot, row): pww_sampler_update's `form`
+# with an inpaint mask, one more column after the form: sigma' = sigmas[step index + 1], pww_sampler_update_masked's
+# `sigma_next`
 
 
 class PwWSampler:
@@ -303,6 +305,14 @@ class PwWSampler:
     native launches per step, and images with phi = 0 get exactly the plain update.  A v-prediction scheduler
     (`prediction_type="v_prediction"` in its config) needs nothing here: its step forms take the v output.
 
+    Masked img2img (`init_latents`, `init_noise` and `inpaint_mask`, all three or none; inpainting with a model that
+    has no mask input): `init_latents` [m, 4, h, w] are the init images' VAE latents, `init_noise` [m, 4, h, w] the
+    noise that made the start latents `init_latents + sigma_0 init_noise`, and `inpaint_mask` [m, 1, h, w] in [0, 1]
+    (1 = repaint).  After the step from sigma to sigma' the latents are `M x + (1 - M) (init + z sigma')`: outside the
+    mask they stay on the init image's noise path and end, at sigma' = 0, as the init latents.  The blend is inside
+    the update launch (`pww_sampler_update_masked`), so a step keeps its two native launches, with every sampler,
+    guidance rescale, control unit and recording.  It composes with `extra_input` (a 9-channel model gets both).
+
     `record_attention=True` records, inside the UNet's cross-attention launches (`pww_xattn_fused_rec_*`), the softmax
     mass every painted region's tokens receive from each pixel of each cond image, biased or not; `attention_maps()`
     returns it per image as [R, h, w] maps.  The accumulators are zeroed at set-up and by `restart()`.  The latents are
@@ -317,7 +327,9 @@ class PwWSampler:
                  control_image: Union[None, torch.Tensor, Sequence[torch.Tensor]] = None,
                  controlnet_conditioning_scale: Union[float, Sequence[float]] = 1.0, guess_mode: bool = False,
                  control_guidance_start: float = 0.0, control_guidance_end: float = 1.0,
-                 record_attention: bool = False, guidance_rescale: Union[float, Sequence[float]] = 0.0):
+                 record_attention: bool = False, guidance_rescale: Union[float, Sequence[float]] = 0.0,
+                 init_latents: Optional[torch.Tensor] = None, init_noise: Optional[torch.Tensor] = None,
+                 inpaint_mask: Optional[torch.Tensor] = None):
         if not isinstance(scheduler, SIGMA_SCHEDULERS):
             raise TypeError(f"PwWSampler does not support {type(scheduler).__name__}; use one of "
                             + ", ".join(c.__name__ for c in SIGMA_SCHEDULERS))
@@ -346,6 +358,7 @@ class PwWSampler:
                              f"image latents per image), got {tuple(extra_input.shape)}")
         self.extra_input = (None if extra_input is None else     # inpaint: [m,5,h,w] (mask + masked-image latents)
                             extra_input.to(self.device, torch.float32, memory_format=torch.contiguous_format))
+        self._blend = self._blend_inputs(init_latents, init_noise, inpaint_mask)
         self.use_graph = use_graph and latents.is_cuda
         self._graphs = {}                  # "the step runs the ControlNet" -> (captured step, its native launches)
         self._kv_graph = None
@@ -399,6 +412,26 @@ class PwWSampler:
         self._rec_levels: List[tuple] = []     # (N, h_r, w_r, accumulator [m, H, N, 16]) per cross-attention level
         if self.record_attention:
             self._set_up_recording(cond_ctxs)
+
+    def _blend_inputs(self, init_latents, init_noise, inpaint_mask) -> Optional[Tuple[torch.Tensor, ...]]:
+        """Masked img2img's (init latents, init noise, mask) as private contiguous fp32 copies on the latents' device,
+        or None without a mask.  All three or none; shapes are checked against the latents, the mask against [0, 1]."""
+        given = [t is not None for t in (init_latents, init_noise, inpaint_mask)]
+        if not any(given):
+            return None
+        if not all(given):
+            raise ValueError("init_latents, init_noise and inpaint_mask go together: pass all three or none")
+        m, (h, w) = self.m, self.latents.shape[-2:]
+        out = []
+        for name, t, c in (("init_latents", init_latents, 4), ("init_noise", init_noise, 4),
+                           ("inpaint_mask", inpaint_mask, 1)):
+            if not torch.is_tensor(t) or tuple(t.shape) != (m, c, h, w):
+                got = tuple(t.shape) if torch.is_tensor(t) else type(t).__name__
+                raise ValueError(f"{name} must be [{m}, {c}, {h}, {w}] (one per image), got {got}")
+            out.append(t.to(self.device, torch.float32, memory_format=torch.contiguous_format, copy=True))
+        if not bool(((out[2] >= 0) & (out[2] <= 1)).all()):         # NaN fails too
+            raise ValueError("inpaint_mask values must be in [0, 1] (1 = repaint)")
+        return tuple(out)
 
     def _set_up_recording(self, conds):
         """record_attention: the cond images' token -> region rows, and one zeroed fp32 [m, H_l, N_l, 16] accumulator per
@@ -553,16 +586,17 @@ class PwWSampler:
         return [step_form(sch, sch.step_index_of(t), first=(i == 0)) for i, t in enumerate(self.timesteps)]
 
     def _build_rows(self) -> torch.Tensor:
-        """[steps, _G + 2m + 6] fp32: every step's row.  The step form ends with the history slot this step writes and
-        the noise row it reads."""
+        """[steps, _G + 2m + 6] fp32: every step's row, with one more column, sigma', for masked img2img.  The step
+        form ends with the history slot this step writes and the noise row it reads."""
         sch, zeros = self.scheduler, [0.0] * self.m
         rows = []
         for i, (t, (alpha, a, b, beta, gamma)) in enumerate(zip(self.timesteps, self.step_forms())):
             si = sch.step_index_of(t)
             sigma = float(sch.sigmas[si])
             gs = [g_of_sigma(f, pr, sch.sigmas[si]) for f, pr in zip(self._fns, self._probed)]
+            sigma_next = [] if self._blend is None else [float(sch.sigmas[si + 1])]
             rows.append([sigma, 1.0 / math.sqrt(sigma * sigma + 1.0), float(t), *beta, *gs, *zeros,
-                         alpha, a, b, gamma, float(i % self._hist_len), float(i)])
+                         alpha, a, b, gamma, float(i % self._hist_len), float(i), *sigma_next])
         return torch.tensor(rows, dtype=torch.float32)
 
     def _merge_contexts(self, conds, unconds) -> dict:
@@ -655,7 +689,14 @@ class PwWSampler:
         args = (eps.data_ptr(), _dtype_code(eps.dtype), *eps.stride(), self.latents.data_ptr(), self._derivs.data_ptr(),
                 self._hist_len, None if self._noise is None else self._noise.data_ptr(), self._gscale.data_ptr(),
                 p[_BETA:].data_ptr(), p[self._form:].data_ptr())
-        if self._rescale is None:
+        if self._blend is not None:
+            # masked img2img: the same update with the mask blend as its epilogue (sigma' after the form)
+            init, noise0, mask = self._blend
+            _native.check(L.pww_sampler_update_masked(*args, None if self._rescale is None else self._rescale.data_ptr(),
+                                                      None, init.data_ptr(), noise0.data_ptr(), mask.data_ptr(),
+                                                      p[self._form + len(FORM_COLUMNS):].data_ptr(), m, h, w, stream),
+                          "pww_sampler_update_masked")
+        elif self._rescale is None:
             _native.check(L.pww_sampler_update(*args, m, h, w, stream), "pww_sampler_update")
         else:
             _native.check(L.pww_sampler_update_rescale(*args, self._rescale.data_ptr(), None, m, h, w, stream),
@@ -802,6 +843,7 @@ def paint_with_words(
     return_attention_maps: bool = False,
     guidance_rescale: float = 0.0,
     prediction_type: Optional[str] = None,
+    mask_image: Optional[Image.Image] = None,
 ):
     """paint_with_words.py:391-510.  Returns one PIL.Image (or the final latents with return_latents).
     `max_prompt_chunks` (1 .. 3): a prompt longer than 75 tokens fills up to that many 77-token CLIP chunks instead of
@@ -818,7 +860,13 @@ def paint_with_words(
     recorded inside the attention kernels over the whole run, with each region's adherence to its painted area.
     `guidance_rescale` (0..1) as in `PwWSampler`.  `prediction_type` ("epsilon" or "v_prediction") is passed to
     `pww_load_tools` when this call loads the models (None: the model's own); with `preloaded_utils` the scheduler's
-    config decides."""
+    config decides.
+    `mask_image` (with `init_image`): masked img2img, inpainting with any model.  Only the white area of the mask is
+    repainted (values >= 0.5 after / 255, as `paint_with_words_inpaint` binarises them); elsewhere the latents follow
+    the init image's noise path and end as its latents (`PwWSampler`'s `inpaint_mask`).  The mask is resized (nearest)
+    to the init image's size, then to the latent grid."""
+    if mask_image is not None and init_image is None:
+        raise ValueError("mask_image needs an init_image: masked img2img repaints the masked area of the init image")
     control = _control_arguments(controlnet, control_image, color_map_image.size, "color_map_image",
                                  controlnet_conditioning_scale, guess_mode, control_guidance_start,
                                  control_guidance_end)
@@ -826,6 +874,7 @@ def paint_with_words(
                    prediction_type)
     vae, unet, text_encoder, tokenizer, scheduler = tools
     scheduler.set_timesteps(num_inference_steps)
+    blend = {}
     if init_image is None:
         cond, uncond, latents = _txt2img_inputs(tools, device, color_map_image, color_context, input_prompt,
                                                 unconditional_input_prompt, seed, max_prompt_chunks)
@@ -835,10 +884,14 @@ def paint_with_words(
             text_encoder, tokenizer, device, color_map_image, color_context, input_prompt, unconditional_input_prompt,
             max_prompt_chunks=max_prompt_chunks)
         # the reference draws img2img's noise from the global RNG as it stands: unseeded here
-        latents, timesteps = _img2img_latents(vae, scheduler, init_image, num_inference_steps, strength, device)
+        latents, timesteps, init, noise = _img2img_latents(vae, scheduler, init_image, num_inference_steps, strength,
+                                                           device)
+        if mask_image is not None:
+            blend = dict(init_latents=init, init_noise=noise,
+                         inpaint_mask=_latent_mask(init_image, mask_image, tuple(latents.shape[-2:]), device))
     sampler = PwWSampler(unet, scheduler, [cond], [uncond], latents, weight_function, guidance_scale,
                          timesteps=timesteps, noise_seed=seed, record_attention=return_attention_maps,
-                         guidance_rescale=guidance_rescale, **control)
+                         guidance_rescale=guidance_rescale, **control, **blend)
     result = _result(vae, sampler.run(), return_latents)
     if not return_attention_maps:
         return result
@@ -869,16 +922,27 @@ def _txt2img_inputs(tools, device, color_map_image, color_context, input_prompt,
 
 
 def _img2img_latents(vae, scheduler, init_image, num_inference_steps: int, strength: float, device,
-                     generator: Optional[torch.Generator] = None) -> Tuple[torch.Tensor, torch.Tensor]:
-    """(latents, timesteps) of an img2img run: the last `strength` of the schedule, and the init image's VAE latents
-    noised to its first timestep with noise from `generator` (None: the global RNG)."""
+                     generator: Optional[torch.Generator] = None) -> Tuple[torch.Tensor, ...]:
+    """(latents, timesteps, init latents, noise) of an img2img run: the last `strength` of the schedule, the init
+    image's VAE latents, and those latents noised to the schedule's first timestep with noise from `generator` (None:
+    the global RNG), latents = scheduler.add_noise(init, noise, timesteps[:1])."""
     init_timestep = min(int(num_inference_steps * strength), num_inference_steps)
     t_start = max(num_inference_steps - init_timestep, 0)
     timesteps = scheduler.timesteps[t_start:]
     image = preprocess(init_image).to(device=device)
     init_latents = 0.18215 * vae.encode(image.to(_module_dtype(vae, image.dtype))).latent_dist.sample().float()
     noise = torch.randn(init_latents.shape, generator=generator).to(device)
-    return scheduler.add_noise(init_latents, noise, timesteps[:1]), timesteps
+    return scheduler.add_noise(init_latents, noise, timesteps[:1]), timesteps, init_latents, noise
+
+
+def _latent_mask(init_image: Image.Image, mask_image: Image.Image, size: Tuple[int, int], device) -> torch.Tensor:
+    """Masked img2img's [1, 1, h, w] fp32 mask of latent size `size`: `mask_image` resized (nearest) to the init
+    image's size and binarised as `prepare_mask_and_masked_image` does (>= 0.5 after / 255, white = 1 = repaint), then
+    brought to the latent grid with nearest interpolation, as `paint_with_words_inpaint` does."""
+    width, height = init_image.size
+    mask, _ = prepare_mask_and_masked_image(init_image, mask_image.resize((width, height), Image.NEAREST))
+    mask = F.interpolate(mask, size=(height // 8, width // 8))
+    return F.interpolate(mask, size=tuple(size), mode="nearest").to(device)
 
 
 def _result(vae, latents: torch.Tensor, return_latents: bool):
@@ -1158,7 +1222,7 @@ def paint_with_words_inpaint(
 
     scheduler.set_timesteps(num_inference_steps)
     # seeded before the VAE encode, which draws from the same (global) generator
-    latents, timesteps = _img2img_latents(vae, scheduler, init_image, num_inference_steps, strength, device,
+    latents, timesteps, _, _ = _img2img_latents(vae, scheduler, init_image, num_inference_steps, strength, device,
                                           generator=torch.manual_seed(seed))
 
     mask = F.interpolate(mask, size=(height // 8, width // 8)).to(device=device, dtype=latents.dtype)
@@ -1255,8 +1319,10 @@ class PaintWithWord_StableDiffusionPipeline:
                  output_type: str = "pil", return_dict: bool = True, callback=None, callback_steps: int = 1,
                  max_prompt_chunks: int = 1, control_image=None, controlnet_conditioning_scale: float = 1.0,
                  guess_mode: bool = False, control_guidance_start: float = 0.0, control_guidance_end: float = 1.0,
-                 guidance_rescale: float = 0.0):
+                 guidance_rescale: float = 0.0, mask_image=None):
+        """`mask_image` with `image`: masked img2img (see `paint_with_words`)."""
         extra = {} if image is None else {"init_image": image, "strength": eta}
+        extra["mask_image"] = mask_image
         extra["max_prompt_chunks"] = max_prompt_chunks
         extra["guidance_rescale"] = guidance_rescale
         extra.update(self._control(control_image, controlnet_conditioning_scale, guess_mode, control_guidance_start,

@@ -409,6 +409,43 @@ int pww_sampler_update_masked(const void* eps, int eps_dtype, int64_t eps_batch_
                               int m, int height, int width, void* stream);
 
 /*
+ * MultiDiffusion panoramas: overlapping window x window crops of one canvas latent [1, 4, height, width] fp32 go
+ * through the UNet as a batch, and their guided outputs are averaged at every canvas value before the step form runs
+ * on the canvas.  Window v = iy * n_cols + ix (0 <= v < n_rows * n_cols) has its origin at (row_starts[iy],
+ * col_starts[ix]); both are int32 device arrays.  Every row start must satisfy 0 <= r0 <= height - window and every
+ * column start 0 <= c0 < width; a column start with c0 + window > width wraps, window column x reading canvas column
+ * (c0 + x) mod width (a circular panorama).  The windows are split into chunks of views_per_chunk (the last chunk may
+ * hold fewer), one UNet batch each.
+ *
+ * pww_window_input: chunk input [2n, 4, window, window] (contiguous, `out_dtype`) of windows first_view ..
+ *   first_view + n - 1 (n = n_views): rows j and n + j both get round(canvas[window first_view + j] * scale[0]).
+ *
+ * pww_window_update: one step of the canvas from every chunk's UNet output.  eps is a HOST array of n_chunks (1..64)
+ *   pointers; chunk k's output [2 n_k, 4, window, window] (cond rows, then uncond rows) is read in place through the
+ *   element strides given, which all chunks share.  For each canvas value, with the covering windows v1 < ... < vc:
+ *     g_v = eps_u,v + guidance[0] (eps_c,v - eps_u,v)          at the window-local position
+ *     E   = g_v1 + g_v2 + ... + g_vc                           summed left to right, starting from g_v1
+ *     e   = E / c
+ *   then pww_sampler_update's step form with m = 1: latents [1, 4, h, w], history [L, 1, 4, h, w], noise [n, 1, 4,
+ *   h, w] or NULL, and the same `beta` and `form` rows.  fp32, rounded after every operation in the order written.
+ *   One thread owns each canvas value: no atomics, and the bits do not depend on the chunking.  The pointer table
+ *   travels in the kernel parameters, so a captured CUDA graph carries it.
+ *
+ * Both return PWW_ERR_BAD_ARG for null pointers, a window larger than the canvas, non-positive sizes or views outside
+ * the n_rows * n_cols windows, and pww_window_update for n_chunks outside 1..64 or not ceil(views / views_per_chunk),
+ * and PWW_ERR_UNSUPPORTED for other dtypes, before any CUDA call.
+ */
+int pww_window_input(const float* latents, const float* scale, const int* row_starts, int n_rows,
+                     const int* col_starts, int n_cols, int first_view, int n_views, int window, void* out,
+                     int out_dtype, int height, int width, void* stream);
+int pww_window_update(const void* const* eps, int n_chunks, int views_per_chunk, int eps_dtype,
+                      int64_t eps_batch_stride, int64_t eps_channel_stride, int64_t eps_row_stride,
+                      int64_t eps_col_stride, const int* row_starts, int n_rows, const int* col_starts, int n_cols,
+                      int window, float* latents, float* history, int history_len, const float* noise,
+                      const float* guidance, const float* beta, const float* form, int height, int width,
+                      void* stream);
+
+/*
  * ControlNet residual injection: n (1..16) residuals added in place into n activations, in one launch.
  *   dst_k[b] = E( dst_k[b] + E( s[k, b] * res_k[b] ) )        k < n, b < rows
  * dst[k] points at a [B, elems_per_image[k]] tensor and res[k] at a [rows, elems_per_image[k]] one, both dense (a

@@ -16,6 +16,7 @@ from .pipeline import (  # noqa: F401
     RegionAttention, paint_with_words_batch, paint_with_words_inpaint, preprocess, prepare_mask_and_masked_image,
     pww_load_tools,
 )
+from .panorama import PanoramaSampler, paint_with_words_panorama, panorama_views  # noqa: F401
 from .scheduler import (  # noqa: F401
     DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler, EulerDiscreteScheduler, LMSDiscreteScheduler,
 )

@@ -33,6 +33,7 @@ EXPORTS = (
     "pww_xattn_fused_rec_f16", "pww_xattn_fused_rec_bf16",
     "pww_adapter_residual_f16", "pww_adapter_residual_bf16",
     "pww_sampler_update_rescale", "pww_sampler_update_masked",
+    "pww_window_input", "pww_window_update",
 )
 
 
@@ -127,6 +128,14 @@ def lib() -> ctypes.CDLL:
     L.pww_sampler_update_masked.restype = c_i
     L.pww_sampler_update_masked.argtypes = L.pww_sampler_update_rescale.argtypes[:15] + [c_vp] * 4 + \
         L.pww_sampler_update.argtypes[13:]
+    # latents, scale, row_starts, n_rows, col_starts, n_cols, first_view, n_views, window, out, out_dtype, h, w, stream
+    L.pww_window_input.restype = c_i
+    L.pww_window_input.argtypes = [c_vp, c_vp, c_vp, c_i, c_vp, c_i, c_i, c_i, c_i, c_vp, c_i, c_i, c_i, c_vp]
+    # eps[n_chunks] (host array), n_chunks, views_per_chunk, eps_dtype, 4 strides, row_starts, n_rows, col_starts,
+    # n_cols, window, then pww_sampler_update's latents .. form, height, width, stream
+    L.pww_window_update.restype = c_i
+    L.pww_window_update.argtypes = [ctypes.POINTER(c_vp), c_i, c_i, c_i, c_i64, c_i64, c_i64, c_i64, c_vp, c_i, c_vp,
+                                    c_i, c_i] + L.pww_sampler_update.argtypes[6:13] + [c_i, c_i, c_vp]
     _lib = L
     return L
 

@@ -9,6 +9,7 @@
 #include "unet_ops.cuh"
 #include "sampler_step.cuh"
 #include "sampler_rescale.cuh"
+#include "sampler_window.cuh"
 #include "control_inject.cuh"
 #include "control_combine.cuh"
 #include "adapter_residual.cuh"
@@ -754,6 +755,67 @@ int pww_sampler_update_masked(const void* eps, int eps_dtype, int64_t eps_batch_
         : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_update<__nv_bfloat16, true>(a, bl, px4, cl, s)
                                       : pww::smp::launch_update<float, true>(a, bl, px4, cl, s);
   }
+  return e == cudaSuccess ? PWW_OK : cuda_fail(e);
+}
+
+int pww_window_input(const float* latents, const float* scale, const int* row_starts, int n_rows,
+                     const int* col_starts, int n_cols, int first_view, int n_views, int window, void* out,
+                     int out_dtype, int height, int width, void* stream) {
+  if (!latents || !scale || !row_starts || !col_starts || !out) return PWW_ERR_BAD_ARG;
+  if (height <= 0 || width <= 0 || window <= 0 || window > height || window > width) return PWW_ERR_BAD_ARG;
+  if (n_rows <= 0 || n_cols <= 0 || n_views <= 0 || first_view < 0 ||
+      (int64_t)first_view + n_views > (int64_t)n_rows * n_cols)
+    return PWW_ERR_BAD_ARG;
+  if (out_dtype != PWW_DTYPE_F32 && out_dtype != PWW_DTYPE_F16 && out_dtype != PWW_DTYPE_BF16) return PWW_ERR_UNSUPPORTED;
+  pww::smp::WindowInputArgs a;
+  a.lat = latents; a.scale = scale; a.rows = row_starts; a.cols = col_starts; a.out = out;
+  a.n_cols = n_cols; a.first = first_view; a.n = n_views; a.window = window; a.H = height; a.W = width;
+  const bool px4 = (window % 4) == 0 && aligned16(out);
+  cudaStream_t s = (cudaStream_t)stream;
+  const cudaError_t e = out_dtype == PWW_DTYPE_F16    ? pww::smp::launch_window_input<__half>(a, px4, s)
+                        : out_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_window_input<__nv_bfloat16>(a, px4, s)
+                                                      : pww::smp::launch_window_input<float>(a, px4, s);
+  return e == cudaSuccess ? PWW_OK : cuda_fail(e);
+}
+
+int pww_window_update(const void* const* eps, int n_chunks, int views_per_chunk, int eps_dtype,
+                      int64_t eps_batch_stride, int64_t eps_channel_stride, int64_t eps_row_stride,
+                      int64_t eps_col_stride, const int* row_starts, int n_rows, const int* col_starts, int n_cols,
+                      int window, float* latents, float* history, int history_len, const float* noise,
+                      const float* guidance, const float* beta, const float* form, int height, int width,
+                      void* stream) {
+  if (!eps || !row_starts || !col_starts || !latents || !history || !guidance || !beta || !form) return PWW_ERR_BAD_ARG;
+  if (height <= 0 || width <= 0 || window <= 0 || window > height || window > width) return PWW_ERR_BAD_ARG;
+  if (history_len < 1 || history_len > 4 || n_rows <= 0 || n_cols <= 0 || views_per_chunk <= 0) return PWW_ERR_BAD_ARG;
+  if (n_chunks < 1 || n_chunks > pww::smp::kMaxWindowChunks) return PWW_ERR_BAD_ARG;
+  const int64_t views = (int64_t)n_rows * n_cols;
+  if ((views + views_per_chunk - 1) / views_per_chunk != n_chunks) return PWW_ERR_BAD_ARG;
+  if (eps_dtype != PWW_DTYPE_F32 && eps_dtype != PWW_DTYPE_F16 && eps_dtype != PWW_DTYPE_BF16) return PWW_ERR_UNSUPPORTED;
+  const size_t es = eps_dtype == PWW_DTYPE_F32 ? 4 : 2;
+  // window outputs are read one pixel (4 channels) at a time: channels-last packed rows take one 8- or 16-byte access
+  const size_t need = 4 * es;
+  bool cl = eps_channel_stride == 1 && eps_col_stride == 4 && eps_row_stride == 4 * (int64_t)window &&
+            ((size_t)eps_batch_stride * es) % need == 0;
+  pww::smp::WindowOutputs t;
+  for (int k = 0; k < n_chunks; ++k) {
+    if (!eps[k]) return PWW_ERR_BAD_ARG;
+    t.eps[k] = eps[k];
+    cl = cl && (reinterpret_cast<uintptr_t>(eps[k]) % need) == 0;
+  }
+  pww::smp::UpdateArgs a{}, o{};
+  a.lat = latents; a.hist = history; a.noise = noise; a.gscale = guidance; a.beta = beta; a.form = form;
+  a.m = 1; a.h = height; a.w = width; a.nh = history_len;
+  o.e_sn = eps_batch_stride; o.e_sc = eps_channel_stride; o.e_sh = eps_row_stride; o.e_sw = eps_col_stride;
+  o.w = window;
+  pww::smp::WindowArgs v;
+  v.rows = row_starts; v.cols = col_starts; v.n_rows = n_rows; v.n_cols = n_cols; v.window = window;
+  v.per_chunk = views_per_chunk; v.views = (int)views;
+  const bool px4 = (width % 4) == 0 && aligned16(latents) && aligned16(history) && (!noise || aligned16(noise));
+  cudaStream_t s = (cudaStream_t)stream;
+  const cudaError_t e =
+      eps_dtype == PWW_DTYPE_F16    ? pww::smp::launch_window_update<__half>(a, o, v, t, px4, cl, s)
+      : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_window_update<__nv_bfloat16>(a, o, v, t, px4, cl, s)
+                                    : pww::smp::launch_window_update<float>(a, o, v, t, px4, cl, s);
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 

@@ -602,8 +602,10 @@ class PwWSampler:
     def _merge_contexts(self, conds, unconds) -> dict:
         """Batch the per-image dicts: CONTEXT_TENSOR -> [2m,T,Dc]; weight maps -> [m,N,T] stacks;
         WMAP_INDEX = [0..m-1, -1 x m] with -1 also for images whose weight function is zero; STAT_KIND = the probed
-        statistic of every image (uncond images: max, ignored)."""
-        m = self.m
+        statistic of every image (uncond images: max, ignored).  The m images are the first len(conds) of the
+        sampler's (all of them here; a panorama chunk's windows in PanoramaSampler)."""
+        m = len(conds)
+        probed = self._probed[:m]
         lengths = {int(c["CONTEXT_TENSOR"].shape[1]) for c in list(conds) + list(unconds)}
         if len(lengths) != 1:
             raise ValueError(f"all images of a sampler need the same text length (got T = {sorted(lengths)}); encode them "
@@ -628,9 +630,9 @@ class PwWSampler:
                     ctx[packed_key(n)] = (packed[0].to(self.device), packed[1].to(self.device))
             else:
                 ctx[key] = 0
-        ctx["WMAP_INDEX"] = torch.tensor([-1 if pr.is_zero else i for i, pr in enumerate(self._probed)] + [-1] * m,
+        ctx["WMAP_INDEX"] = torch.tensor([-1 if pr.is_zero else i for i, pr in enumerate(probed)] + [-1] * m,
                                          dtype=torch.int32, device=self.device)
-        ctx["STAT_KIND"] = torch.tensor([STAT_MAX if pr.is_zero else pr.stat for pr in self._probed] + [STAT_MAX] * m,
+        ctx["STAT_KIND"] = torch.tensor([STAT_MAX if pr.is_zero else pr.stat for pr in probed] + [STAT_MAX] * m,
                                         dtype=torch.int32, device=self.device)
         ctx["WEIGHT_FUNCTION"] = self.weight_function
         ctx["SIGMA"] = None

@@ -260,6 +260,58 @@ int pww_xattn_fused_rec_bf16(const void* q, const void* k, const void* v, void* 
                              const int8_t* ridx, const int32_t* rec_index, float* rec_acc, int64_t rec_batch_stride);
 
 /*
+ * Region prompts: pww_xattn_fused_f16 / _multi_f16 (and the _bf16 twins) with one softmax per 77-key chunk, mixed per
+ * query row.  T must be 154 or 231 (k = 2, 3 chunks; any other T returns PWW_ERR_UNSUPPORTED).  For image b, head h and
+ * query row n:
+ *     out[n] = sum_c w_c(n) softmax_c(scale (S_c[n] + bias_c[n])) V_c
+ * where softmax_c runs over the 77 keys of chunk c alone and bias is the PwW bias of the sibling call (statistic over
+ * all H * N * T scores).  Extra arguments, after `stream`:
+ *   region_weights [Bw', N, k] fp32, 4-byte aligned: w_c(n) of weight row i at region_weights + i * region_batch_stride
+ *               + n * k + c.  Image b takes row wmap_index[b] (row b when wmap_index is NULL, whether or not mpack is
+ *               given); an image with index -1 takes w = (1, 0, ..) on every row.  Rows are meant to sum to 1 with
+ *               every w in [0, 1]; the kernel does not renormalise them.
+ *   region_batch_stride : elements between weight rows, >= N * k
+ * A chunk that no row of a 128-row tile weighs is neither read nor computed for that tile; a row with w_c = 0 gets
+ * exactly nothing from chunk c.
+ */
+int pww_xattn_fused_region_f16(const void* q, const void* k, const void* v, void* out,
+                               int B, int H, int N, int T, int D,
+                               int64_t q_batch_stride, int64_t q_row_stride,
+                               int64_t k_batch_stride, int64_t k_row_stride,
+                               int64_t o_batch_stride, int64_t o_row_stride,
+                               const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+                               const int32_t* wmap_index, int stat, const float* g_sigma, float scale,
+                               float* stats, void* workspace, size_t workspace_bytes, void* stream,
+                               const float* region_weights, int64_t region_batch_stride);
+int pww_xattn_fused_region_bf16(const void* q, const void* k, const void* v, void* out,
+                                int B, int H, int N, int T, int D,
+                                int64_t q_batch_stride, int64_t q_row_stride,
+                                int64_t k_batch_stride, int64_t k_row_stride,
+                                int64_t o_batch_stride, int64_t o_row_stride,
+                                const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+                                const int32_t* wmap_index, int stat, const float* g_sigma, float scale,
+                                float* stats, void* workspace, size_t workspace_bytes, void* stream,
+                                const float* region_weights, int64_t region_batch_stride);
+int pww_xattn_fused_region_multi_f16(const void* q, const void* k, const void* v, void* out,
+                                     int B, int H, int N, int T, int D,
+                                     int64_t q_batch_stride, int64_t q_row_stride,
+                                     int64_t k_batch_stride, int64_t k_row_stride,
+                                     int64_t o_batch_stride, int64_t o_row_stride,
+                                     const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+                                     const int32_t* wmap_index, const int32_t* stat, const float* g_sigma, float scale,
+                                     float* stats, void* workspace, size_t workspace_bytes, void* stream,
+                                     const float* region_weights, int64_t region_batch_stride);
+int pww_xattn_fused_region_multi_bf16(const void* q, const void* k, const void* v, void* out,
+                                      int B, int H, int N, int T, int D,
+                                      int64_t q_batch_stride, int64_t q_row_stride,
+                                      int64_t k_batch_stride, int64_t k_row_stride,
+                                      int64_t o_batch_stride, int64_t o_row_stride,
+                                      const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+                                      const int32_t* wmap_index, const int32_t* stat, const float* g_sigma, float scale,
+                                      float* stats, void* workspace, size_t workspace_bytes, void* stream,
+                                      const float* region_weights, int64_t region_batch_stride);
+
+/*
  * Self-attention through the same patched function (context=None, paint_with_words.py:71-72):
  *   out = softmax(scale * Q_h K_h^T) V_h  with keys/values [B, N, H*D]; no bias; online softmax.
  */

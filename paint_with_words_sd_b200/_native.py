@@ -34,6 +34,8 @@ EXPORTS = (
     "pww_adapter_residual_f16", "pww_adapter_residual_bf16",
     "pww_sampler_update_rescale", "pww_sampler_update_masked",
     "pww_window_input", "pww_window_update",
+    "pww_xattn_fused_region_f16", "pww_xattn_fused_region_bf16",
+    "pww_xattn_fused_region_multi_f16", "pww_xattn_fused_region_multi_bf16",
 )
 
 
@@ -86,6 +88,11 @@ def lib() -> ctypes.CDLL:
     # the _multi arguments, then ridx, rec_index, rec_acc (device pointers) and rec_batch_stride (elements)
     L.pww_xattn_fused_rec_f16.restype = c_i
     L.pww_xattn_fused_rec_f16.argtypes = list(L.pww_xattn_fused_multi_f16.argtypes) + [c_vp, c_vp, c_vp, c_i64]
+    # region prompts: the fused (or _multi) arguments, then region_weights (device pointer) and its batch stride
+    L.pww_xattn_fused_region_f16.restype = c_i
+    L.pww_xattn_fused_region_f16.argtypes = list(L.pww_xattn_fused_f16.argtypes) + [c_vp, c_i64]
+    L.pww_xattn_fused_region_multi_f16.restype = c_i
+    L.pww_xattn_fused_region_multi_f16.argtypes = list(L.pww_xattn_fused_multi_f16.argtypes) + [c_vp, c_i64]
     L.pww_attn_fwd_f16.restype = c_i
     L.pww_attn_fwd_f16.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i, c_i, c_i, c_i, c_i64, c_i64, c_i64, c_i64, c_f, c_vp]
     L.pww_groupnorm_workspace_bytes.restype = c_sz

@@ -10,7 +10,8 @@ Same calling convention, context-dict schema and patch mechanism as the referenc
     T = 77 (one CLIP window, any T <= 80 works) or a long prompt of 2 or 3 concatenated 77-token chunks (T = 154, 231;
     `conditioning.chunk_prompt`, the A1111 / compel layout).
         (optional, ours) "WMAP_INDEX", "G_SIGMA", "STAT_KIND", "CROSS_ATTENTION_PACKED_{N}", "PWW_SCRATCH",
-        "ATTN_RECORD" (per-region attention recording, see RECORD_KEY)
+        "ATTN_RECORD" (per-region attention recording, see RECORD_KEY), "REGION_WEIGHTS_{N}" (region prompts: fp32
+        [N, k] or [Bw, N, k] chunk weights of a k-chunk context, see cross_attention's `region`)
 
 Everything between the q/k/v projections and the output projection runs in libpww_b200.so through
 the C ABI (include/pww_b200.h): ONE launch of `pww_xattn_fused_f16` (per-image max/std of QK^T over all heads,
@@ -43,7 +44,8 @@ import torch
 import torch.nn.functional as F
 
 from . import _native
-from .conditioning import PACK_TOKENS, expand_orig_weight_map, key_chunks, pack_weight_map, packed_key, weight_key
+from .conditioning import (PACK_TOKENS, expand_orig_weight_map, key_chunks, pack_weight_map, packed_key, region_key,
+                           weight_key)
 from .weight_function import g_of_sigma, probe_weight_function
 
 _ORIG_KEY = "CROSS_ATTENTION_WEIGHT_ORIG"
@@ -166,7 +168,7 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                     wmap: Optional[torch.Tensor] = None, wmap_index: Optional[torch.Tensor] = None,
                     stat: Union[int, torch.Tensor] = _native.PWW_STAT_MAX, g_sigma: Optional[torch.Tensor] = None,
                     return_stats: bool = False, packed=None, stats_out: Optional[torch.Tensor] = None,
-                    workspace: Optional[torch.Tensor] = None, record=None):
+                    workspace: Optional[torch.Tensor] = None, record=None, region: Optional[torch.Tensor] = None):
     """Fused region for a key sequence of T <= 80 tokens or of 2 / 3 CLIP chunks (T = 154, 231; any other T raises).
     q [B,N,C]; k,v [B,T,C]; wmap [Bw,N,T] fp32 or None; `packed` = (mpack [Bw,N,32] fp16, cidx [Bw,80 k] int8, k key
     chunks) from `conditioning.pack_weight_map` (built from `wmap` and cached when not given).  `stat` is one kind for
@@ -176,7 +178,11 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
     this module).  The call runs in bf16 when q is bf16 and in fp16 otherwise (see the module docstring).
     `record` = (ridx [Br, 80 k] int8, rec_index [B] int32, rec_acc [Br, heads, N, 16] fp32), all on q's device: the call
     goes to `pww_xattn_fused_rec_*`, which also adds every recorded image's per-region softmax mass into rec_acc
-    (include/pww_b200.h).  It needs the one-launch kernel: a call that would take the dense pair raises."""
+    (include/pww_b200.h).  It needs the one-launch kernel: a call that would take the dense pair raises.
+    `region` = fp32 [Bw, N, k] chunk weights of a k = 2 or 3 chunk context (region prompts): the call goes to
+    `pww_xattn_fused_region_*`, which gives every chunk its own softmax and mixes them per query row by these weights.
+    Image b takes weight row `wmap_index[b]` (-1: (1, 0, ..), the first chunk alone), or row b without an index.  It
+    needs the one-launch kernel and cannot record."""
     L = _native.lib()
     dt = _elem_dtype(q)
     q, k, v = _rows(q, dt), _rows(k, dt), _rows(v, dt)
@@ -218,6 +224,22 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
             kind_ptr = stat.data_ptr()
         stats = None
         rec_args = ()
+        region_args = ()
+        if region is not None:
+            kc = key_chunks(T)
+            if region.dim() == 2:
+                region = region.unsqueeze(0)
+            if (kc < 2 or region.dtype != torch.float32 or region.dim() != 3 or tuple(region.shape[1:]) != (N, kc)
+                    or not region[0].is_contiguous() or region.device != q.device):
+                raise ValueError(f"region weights need fp32 [Bw, {N}, k] on {q.device} for a context of k = 2 or 3 "
+                                 f"chunks (T = {T})")
+            if not use_fused or record is not None:
+                raise _native.NativeError("region prompts need the one-launch kernel without attention recording")
+            if wmap_index is None and region.shape[0] != B:
+                wmap_index = (st.shared_index(B) if region.shape[0] == 1 else None)
+                if wmap_index is None:
+                    raise ValueError(f"{region.shape[0]} region weight rows for {B} images need a wmap_index")
+            region_args = (region.data_ptr(), region.stride(0))
         if record is not None:
             if not use_fused:
                 why = ("XATTN_IMPL is 'dense'" if impl == "dense" else
@@ -250,12 +272,16 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                 mp_ptr, ci_ptr, idx_ptr = mpack.data_ptr(), cidx.data_ptr(), wmap_index.data_ptr()
                 g_ptr, st_ptr, ws_ptr = g_sigma.data_ptr(), stats.data_ptr(), ws.data_ptr()
                 mp_bs, bw, ws_bytes = mpack.stride(0), mpack.shape[0], ws.numel()
+            if region_args and wmap_index is not None:
+                idx_ptr = wmap_index.data_ptr()    # the weight rows are reached through it with or without a bias
             name = "pww_xattn_fused_rec" if rec_args else ("pww_xattn_fused_multi" if per_image else "pww_xattn_fused")
+            if region_args:
+                name = "pww_xattn_fused_region_multi" if per_image else "pww_xattn_fused_region"
             fn = _native.entry(name, dt)
             rc = fn(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, heads, N, T, D,
                     q.stride(0), q.stride(1), k.stride(0), k.stride(1), out.stride(0), out.stride(1),
                     mp_ptr, mp_bs, bw, ci_ptr, idx_ptr, kind_ptr if per_image or rec_args else stat, g_ptr,
-                    float(scale), st_ptr, ws_ptr, ws_bytes, stream, *rec_args)
+                    float(scale), st_ptr, ws_ptr, ws_bytes, stream, *rec_args, *region_args)
             _native.check(rc, fn.__name__)
             _native.launch_count += 1
         else:
@@ -412,11 +438,14 @@ def inj_forward(self, hidden_states, context=None, mask=None):
             if record is None:
                 raise _native.NativeError(f"attention recording has no accumulator for N = {q.shape[1]} query rows "
                                           f"(levels: {sorted(recs)})")
+        region = context.get(region_key(q.shape[1])) if is_dict else None
+        if region is not None and wmap_index is None:
+            wmap_index = context.get("WMAP_INDEX")      # the sampler's image -> weight row (-1: uncond images)
         if k.shape[0] != q.shape[0]:
             k = k.expand(q.shape[0], -1, -1)
             v = v.expand(q.shape[0], -1, -1)
         o = cross_attention(q, k, v, self.heads, self.scale, wmap, wmap_index, stat, g_dev, packed=packed,
-                            stats_out=scratch[0], workspace=scratch[1], record=record)
+                            stats_out=scratch[0], workspace=scratch[1], record=record, region=region)
 
     with torch.autocast("cuda", dtype=act):
         o = self.to_out[0](o)

@@ -360,23 +360,90 @@ def chunk_prompt(tokenizer, prompt: str, labels: Sequence[str] = (), max_prompt_
     return _chunked_ids(tokenizer, windows, max(1, len(windows)))
 
 
+MAX_REGION_PROMPTS = 2          # 1 + 2 chunks of 77: the longest context the attention kernels take (T = 231)
+REGION_SIDE = 64                # colour-map sides must be multiples of this: every UNet level then has its weights
+
+
+def region_key(n: int) -> str:
+    """Dict key of the region-prompt chunk weights of the level with n query rows: fp32 [n, 1 + R] on the device."""
+    return f"REGION_WEIGHTS_{n}"
+
+
+def check_region_prompts(region_prompts, region_base_ratio: float, max_prompt_chunks: int = 1) -> None:
+    """The ValueErrors of region prompts that do not need the tokenizer or the colour map."""
+    if not isinstance(region_prompts, dict) or not 1 <= len(region_prompts) <= MAX_REGION_PROMPTS:
+        n = len(region_prompts) if isinstance(region_prompts, dict) else region_prompts
+        raise ValueError(f"region_prompts takes 1 .. {MAX_REGION_PROMPTS} colour -> sentence entries, got {n}")
+    if max_prompt_chunks > 1:
+        raise ValueError("region prompts and max_prompt_chunks > 1 do not combine: the base prompt is one 77-token chunk")
+    if not 0.0 <= float(region_base_ratio) <= 1.0:
+        raise ValueError(f"region_base_ratio must be in [0, 1], got {region_base_ratio}")
+
+
+def region_chunk_ids(tokenizer, input_prompt: str, region_prompts: dict) -> torch.Tensor:
+    """[1, 77 (1 + R)] ids: the base prompt, then each region's sentence in dict order, each as [BOS] + tokens + [EOS]
+    + padding in a chunk of its own.  A prompt longer than 75 tokens raises ValueError."""
+    width = tokenizer.model_max_length - 2
+    windows = []
+    for what, text in [("input_prompt", input_prompt)] + [(f"region prompt {k!r}", v) for k, v in region_prompts.items()]:
+        ids = list(tokenizer(text)["input_ids"])[1:-1]
+        if len(ids) > width:
+            raise ValueError(f"{what} is {len(ids)} tokens long; with region prompts every prompt must fit one "
+                             f"{width}-token window")
+        windows.append(ids)
+    return _chunked_ids(tokenizer, windows, len(windows))
+
+
+def region_chunk_weights(color_map_image, region_prompts: dict, region_base_ratio: float, ratio: int) -> torch.Tensor:
+    """fp32 [N, 1 + R] chunk weights of the level with latent ratio `ratio` (CPU):
+        w_c = (1 - beta) * f_c   (c >= 1),   w_0 = 1 - sum_{c >= 1} w_c
+    with f_c the binary mask of region c's colour resized as the weight maps are (`_img_importance_flatten` to
+    always_round(side / ratio)).  A colour absent from the map gives f_c = 0."""
+    pixels = np.array(color_map_image)
+    dim0, dim1 = pixels.shape[:2]
+    r0, r1 = always_round(dim0 / ratio), always_round(dim1 / ratio)
+    beta = float(region_base_ratio)
+    cols = []
+    for color in region_prompts:
+        hit = torch.from_numpy((pixels == _rgb_of(color)).all(axis=-1)).to(torch.float32)
+        cols.append((1.0 - beta) * _img_importance_flatten(hit, r0, r1).reshape(-1))
+    w = torch.stack(cols, 1)
+    return torch.cat([1.0 - w.sum(1, keepdim=True), w], 1).contiguous()
+
+
 def _encode_text_color_inputs(text_encoder, tokenizer, device, color_map_image, color_context,
                               input_prompt, unconditional_input_prompt, use_blur: bool = True,
-                              max_prompt_chunks: int = 1):
+                              max_prompt_chunks: int = 1, region_prompts: Optional[dict] = None,
+                              region_base_ratio: float = 0.2):
     """paint_with_words.py:315-388 (and the pipeline-class copy 561-627, which ignores blur sigmas:
     pass use_blur=False for that behaviour).  Returns
     (extra_seeds, seperated_word_contexts, encoder_hidden_states, uncond_encoder_hidden_states).
 
     `max_prompt_chunks` > 1 lets a prompt longer than 75 tokens fill up to that many 77-token CLIP chunks (T = 77 k,
     see `chunk_prompt`); the uncond prompt is encoded to the same number of chunks, each chunk by the text encoder on its
-    own.  A prompt that fits one chunk gives the same dicts as max_prompt_chunks=1 (the reference's behaviour)."""
+    own.  A prompt that fits one chunk gives the same dicts as max_prompt_chunks=1 (the reference's behaviour).
+
+    `region_prompts` ({colour: sentence}, 1 or 2 entries, colours of `color_map_image` in `color_context`'s key forms)
+    gives every painted region a sentence of its own: the context is 1 + R chunks (the base prompt, then the sentences
+    in dict order), and both dicts get `region_key(N)` chunk weights per level (`region_chunk_weights`; the uncond
+    dict's are (1, 0, ..) on every row).  `region_base_ratio` is the base prompt's share beta inside a region."""
     if not 1 <= max_prompt_chunks <= MAX_PROMPT_CHUNKS:
         raise ValueError(f"max_prompt_chunks must be 1 .. {MAX_PROMPT_CHUNKS}, got {max_prompt_chunks}")
+    if region_prompts is not None:
+        check_region_prompts(region_prompts, region_base_ratio, max_prompt_chunks)
+        if color_map_image is None:
+            raise ValueError("region prompts need a color_map_image")
+        if color_map_image.size[0] % REGION_SIDE or color_map_image.size[1] % REGION_SIDE:
+            raise ValueError(f"region prompts need colour-map sides that are multiples of {REGION_SIDE}, got "
+                             f"{color_map_image.size}")
     text_input = tokenizer([input_prompt], padding="max_length", max_length=tokenizer.model_max_length,
                            truncation=True, return_tensors="pt")
     color_context, extra_seeds, extra_sigmas = _extract_seed_and_sigma_from_context(color_context)
     chunks = 1
-    if max_prompt_chunks > 1:
+    if region_prompts is not None:
+        text_input = {"input_ids": region_chunk_ids(tokenizer, input_prompt, region_prompts)}
+        chunks = 1 + len(region_prompts)
+    elif max_prompt_chunks > 1:
         labels = [spec.rpartition(",")[0] for spec in color_context.values()] if color_map_image is not None else []
         ids = chunk_prompt(tokenizer, input_prompt, labels, max_prompt_chunks)
         chunks = ids.shape[1] // CHUNK_TOKENS
@@ -401,6 +468,14 @@ def _encode_text_color_inputs(text_encoder, tokenizer, device, color_map_image, 
     cond[REGION_INDEX_KEY] = (region_token_index(seperated_word_contexts, text_input)
                               if len(seperated_word_contexts) <= MAX_RECORDED_REGIONS else None)
     cond[REGION_COUNT_KEY] = len(seperated_word_contexts)
+    if region_prompts is not None:
+        for r in RATIOS:
+            w = region_chunk_weights(color_map_image, region_prompts, region_base_ratio, r)
+            n = w.shape[0]
+            cond[region_key(n)] = w.to(device)
+            plain = torch.zeros_like(w)
+            plain[:, 0] = 1.0
+            uncond[region_key(n)] = plain.to(device)
 
     if chunks > 1:
         cond["CONTEXT_TENSOR"] = _encode_chunked(text_encoder, text_input["input_ids"], device)

@@ -213,9 +213,15 @@ int xattn_fused(const void* q, const void* k, const void* v, void* out, int B, i
                 int64_t o_batch_stride, int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw,
                 const int8_t* cidx, const int32_t* wmap_index, int stat, const int32_t* kinds, bool per_image,
                 const float* g_sigma, float scale, float* stats, void* workspace, size_t workspace_bytes,
-                void* stream, const pww::fx::FxRecord* rec = nullptr) {
+                void* stream, const pww::fx::FxRecord* rec = nullptr, const pww::fx::FxRegion* rg = nullptr) {
   int rc = check_common(q, k, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride);
   if (rc) return rc;
+  if (rg) {
+    if (pww::core::chunks_of(T) < 2) return PWW_ERR_UNSUPPORTED;       // region prompts: T = 154, 231
+    if (!rg->rw || (reinterpret_cast<uintptr_t>(rg->rw) & 3u) ||
+        rg->rw_bs < (int64_t)N * pww::core::chunks_of(T))
+      return PWW_ERR_BAD_ARG;
+  }
   if (!v || !out || !aligned16(v) || !aligned16(out)) return PWW_ERR_BAD_ARG;
   if ((o_batch_stride | o_row_stride) & 7 || o_row_stride < (int64_t)H * D || o_batch_stride <= 0) return PWW_ERR_BAD_ARG;
   if (rec && (!rec->ridx || !rec->rec_index || !rec->rec_acc || !aligned16(rec->rec_acc) ||
@@ -258,8 +264,15 @@ int xattn_fused(const void* q, const void* k, const void* v, void* out, int B, i
       r = *rec;
       r.rec_index += b0;
     }
+    pww::fx::FxRegion g;
+    if (rg) {                                                      // weights through wmap_index, else row b
+      g = *rg;
+      if (g.rw_index) g.rw_index += b0;
+      else g.rw += (int64_t)b0 * g.rw_bs;
+    }
     const cudaError_t e = with_shape(D, T, [&](auto k) {
-      return pww::fx::launch_fused2<k.D, k.KC>(c, mp, mpack_batch_stride, ci, (cudaStream_t)stream, rec ? &r : nullptr);
+      return pww::fx::launch_fused2<k.D, k.KC>(c, mp, mpack_batch_stride, ci, (cudaStream_t)stream, rec ? &r : nullptr,
+                                               rg ? &g : nullptr);
     });
     if (e == cudaErrorInvalidConfiguration) return PWW_ERR_UNSUPPORTED;
     if (e != cudaSuccess) return cuda_fail(e);
@@ -575,6 +588,47 @@ int pww_xattn_fused_rec_bf16(const void* q, const void* k, const void* v, void* 
       q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
       o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, PWW_STAT_MAX, stat, true,
       g_sigma, scale, stats, workspace, workspace_bytes, stream, &rec);
+}
+
+int pww_xattn_fused_region_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T,
+    int D, int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
+    int64_t o_batch_stride, int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw,
+    const int8_t* cidx, const int32_t* wmap_index, int stat, const float* g_sigma, float scale, float* stats,
+    void* workspace, size_t workspace_bytes, void* stream, const float* region_weights, int64_t region_batch_stride) {
+  const pww::fx::FxRegion rg = {region_weights, region_batch_stride, wmap_index};
+  return xattn_fused<__half>(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+      o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, stat, nullptr, false,
+      g_sigma, scale, stats, workspace, workspace_bytes, stream, nullptr, &rg);
+}
+int pww_xattn_fused_region_bf16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T,
+    int D, int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
+    int64_t o_batch_stride, int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw,
+    const int8_t* cidx, const int32_t* wmap_index, int stat, const float* g_sigma, float scale, float* stats,
+    void* workspace, size_t workspace_bytes, void* stream, const float* region_weights, int64_t region_batch_stride) {
+  const pww::fx::FxRegion rg = {region_weights, region_batch_stride, wmap_index};
+  return xattn_fused<__nv_bfloat16>(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride,
+      k_row_stride, o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, stat, nullptr, false,
+      g_sigma, scale, stats, workspace, workspace_bytes, stream, nullptr, &rg);
+}
+int pww_xattn_fused_region_multi_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N,
+    int T, int D, int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
+    int64_t o_batch_stride, int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw,
+    const int8_t* cidx, const int32_t* wmap_index, const int32_t* stat, const float* g_sigma, float scale, float* stats,
+    void* workspace, size_t workspace_bytes, void* stream, const float* region_weights, int64_t region_batch_stride) {
+  const pww::fx::FxRegion rg = {region_weights, region_batch_stride, wmap_index};
+  return xattn_fused<__half>(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+      o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, PWW_STAT_MAX, stat, true,
+      g_sigma, scale, stats, workspace, workspace_bytes, stream, nullptr, &rg);
+}
+int pww_xattn_fused_region_multi_bf16(const void* q, const void* k, const void* v, void* out, int B, int H, int N,
+    int T, int D, int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
+    int64_t o_batch_stride, int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw,
+    const int8_t* cidx, const int32_t* wmap_index, const int32_t* stat, const float* g_sigma, float scale, float* stats,
+    void* workspace, size_t workspace_bytes, void* stream, const float* region_weights, int64_t region_batch_stride) {
+  const pww::fx::FxRegion rg = {region_weights, region_batch_stride, wmap_index};
+  return xattn_fused<__nv_bfloat16>(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride,
+      k_row_stride, o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, PWW_STAT_MAX, stat,
+      true, g_sigma, scale, stats, workspace, workspace_bytes, stream, nullptr, &rg);
 }
 
 int pww_attn_fwd_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int D,

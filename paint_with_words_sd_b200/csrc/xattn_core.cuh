@@ -127,6 +127,22 @@ __device__ __forceinline__ void load_operands(uint32_t st, const XattnParams<E>&
     if (with_v) load_rows<D>(st + C::QBYTES + (KC + c) * C::KBYTES, p.v + off, p.k_rs, kTP, kv);
   }
 }
+// The same copies with K and V of the chunks in `chunks` (bit c = chunk c) only: a region-prompt job (with_v) skips
+// the chunks no row of its tile weighs.
+template <int D, int KC, typename E>
+__device__ __forceinline__ void load_operands_of(uint32_t st, const XattnParams<E>& p, int b, int h, int tile,
+                                                 unsigned chunks) {
+  using C = Tile<D>;
+  const int rows = p.N - tile * kBM;
+  load_rows<D>(st, p.q + (int64_t)b * p.q_bs + (int64_t)tile * kBM * p.q_rs + h * D, p.q_rs, kBM, rows < kBM ? rows : kBM);
+#pragma unroll 1
+  for (int c = 0; c < KC; ++c) {
+    if (!((chunks >> c) & 1u)) continue;
+    const int64_t off = (int64_t)b * p.k_bs + (int64_t)c * kChunk * p.k_rs + h * D;
+    load_rows<D>(st + C::QBYTES + c * C::KBYTES, p.k + off, p.k_rs, kTP, kChunk);
+    load_rows<D>(st + C::QBYTES + (KC + c) * C::KBYTES, p.v + off, p.k_rs, kTP, kChunk);
+  }
+}
 
 template <int D>
 __device__ __forceinline__ void warp_online_begin(float (&o)[Tile<D>::NT][4], float& m0, float& m1, float& l0, float& l1) {
@@ -142,6 +158,28 @@ struct NoPHook {
   template <int NK>
   __device__ __forceinline__ void operator()(const uint32_t (&)[NK][4], float, float) const {}
 };
+
+// O += P V for the packed P of one key tile (NK k-steps of 16 keys); vs is the tile's V in shared memory.
+template <int D, typename E, int NK>
+__device__ __forceinline__ void warp_pv(const uint32_t (&pa)[NK][4], uint32_t vs, int lane, float (&o)[Tile<D>::NT][4]) {
+  using C = Tile<D>;
+#pragma unroll
+  for (int kk = 0; kk < NK; ++kk) {
+    const int t = 16 * kk + (lane & 7) + ((lane >> 3) & 1) * 8;
+#pragma unroll
+    for (int jp = 0; jp < C::NT / 2; ++jp) {
+      uint32_t b0, b1, b2, b3;
+      ptx::ldsm_x4_t(vs + (uint32_t)(t * C::LD + 16 * jp + (lane >> 4) * 8) * 2u, b0, b1, b2, b3);
+      ptx::mma16816<E>(o[2 * jp], pa[kk], b0, b1);
+      ptx::mma16816<E>(o[2 * jp + 1], pa[kk], b2, b3);
+    }
+    if constexpr (C::NT & 1) {
+      uint32_t b0, b1;
+      ptx::ldsm_x2_t(vs + (uint32_t)(t * C::LD + 8 * (C::NT - 1)) * 2u, b0, b1);
+      ptx::mma16816<E>(o[C::NT - 1], pa[kk], b0, b1);
+    }
+  }
+}
 
 // One key tile of NJ n-tiles (10: a cross-attention chunk of 80 padded keys; 8: a self-attention tile of 64): s holds
 // S (+ bias) of the tile, of which the first kv keys are real; vs is its V tile.  l0 / l1 are per-thread partial row sums.
@@ -185,23 +223,51 @@ __device__ __forceinline__ void warp_online_chunk(float (&s)[NJ][4], int kv, flo
   for (int j = 0; j < C::NT; ++j) {
     o[j][0] *= a0; o[j][1] *= a0; o[j][2] *= a1; o[j][3] *= a1;
   }
-#pragma unroll
-  for (int kk = 0; kk < NJ / 2; ++kk) {
-    const int t = 16 * kk + (lane & 7) + ((lane >> 3) & 1) * 8;
-#pragma unroll
-    for (int jp = 0; jp < C::NT / 2; ++jp) {
-      uint32_t b0, b1, b2, b3;
-      ptx::ldsm_x4_t(vs + (uint32_t)(t * C::LD + 16 * jp + (lane >> 4) * 8) * 2u, b0, b1, b2, b3);
-      ptx::mma16816<E>(o[2 * jp], pa[kk], b0, b1);
-      ptx::mma16816<E>(o[2 * jp + 1], pa[kk], b2, b3);
-    }
-    if constexpr (C::NT & 1) {
-      uint32_t b0, b1;
-      ptx::ldsm_x2_t(vs + (uint32_t)(t * C::LD + 8 * (C::NT - 1)) * 2u, b0, b1);
-      ptx::mma16816<E>(o[C::NT - 1], pa[kk], b0, b1);
-    }
-  }
+  warp_pv<D, E>(pa, vs, lane, o);
   hook(pa, a0, a1);
+}
+
+// ---- region prompts (the RGN instances of the one-launch kernel) ----
+// Chunk c of a job gets a softmax of its own, mixed per query row by the row's chunk weight w_c:
+//     O += E(p * (w_c / l_c)) V_c,   p = 2^(log2e * scale * (S + bias - rowmax_c)) in fp32,  l_c = fp32 sum of those p
+// A chunk is one 80-key tile, so its row max and sum are complete before its P V: there is no rescale across chunks
+// and no division at the end.  A row with w_c = 0 multiplies exact zeros (l_c >= 1: the row max contributes 2^0).
+template <int D, typename E>
+__device__ __forceinline__ void warp_weighted_chunk(float (&s)[10][4], int kv, float sl2, uint32_t vs, int lane,
+                                                    float w0, float w1, float (&o)[Tile<D>::NT][4]) {
+  float t0 = -INFINITY, t1 = -INFINITY;
+#pragma unroll
+  for (int j = 0; j < 10; ++j)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      if (tok(j, e, lane) >= kv) s[j][e] = -INFINITY;
+      if (e < 2) t0 = fmaxf(t0, s[j][e]); else t1 = fmaxf(t1, s[j][e]);
+    }
+  t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, 1));
+  t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, 2));
+  t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, 1));
+  t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, 2));
+  const float n0 = -t0 * sl2, n1 = -t1 * sl2;
+  float r0 = 0.f, r1 = 0.f;
+#pragma unroll
+  for (int j = 0; j < 10; ++j) {
+    s[j][0] = ptx::ex2(fmaf(s[j][0], sl2, n0)); s[j][1] = ptx::ex2(fmaf(s[j][1], sl2, n0));
+    s[j][2] = ptx::ex2(fmaf(s[j][2], sl2, n1)); s[j][3] = ptx::ex2(fmaf(s[j][3], sl2, n1));
+    r0 += s[j][0] + s[j][1];
+    r1 += s[j][2] + s[j][3];
+  }
+  r0 += __shfl_xor_sync(0xffffffffu, r0, 1);
+  r0 += __shfl_xor_sync(0xffffffffu, r0, 2);
+  r1 += __shfl_xor_sync(0xffffffffu, r1, 1);
+  r1 += __shfl_xor_sync(0xffffffffu, r1, 2);
+  const float f0 = w0 / r0, f1 = w1 / r1;
+  uint32_t pa[5][4];
+#pragma unroll
+  for (int j = 0; j < 10; ++j) {
+    pa[j >> 1][(j & 1) * 2] = ptx::pack2<E>(s[j][0] * f0, s[j][1] * f0);
+    pa[j >> 1][(j & 1) * 2 + 1] = ptx::pack2<E>(s[j][2] * f1, s[j][3] * f1);
+  }
+  warp_pv<D, E>(pa, vs, lane, o);
 }
 
 // Divides O by the row sums (reduced over the quad) once every chunk has been accumulated.

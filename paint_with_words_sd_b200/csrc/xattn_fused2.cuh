@@ -34,6 +34,10 @@
 // mass per region slot (16 slots, a token -> slot row per image) into a caller-owned fp32 accumulator, computed from the
 // same packed P as P.V (xattn_core.cuh: warp_region_chunk / warp_region_add).  The plain instances (REC = false) are
 // the kernel without it: every recording instruction is behind `if constexpr`.
+//
+// Region prompts (RGN = true, FxRegion, KC = 2, 3): one softmax per key chunk, mixed per query row by fp32 chunk
+// weights (xattn_core.cuh: warp_weighted_chunk); the chunks no row of a tile weighs are not copied.  Every region
+// instruction is behind `if constexpr` as well.
 #pragma once
 #include <algorithm>
 #include <type_traits>
@@ -76,8 +80,22 @@ template <typename E>
 struct FxRecParams : FxParams<E> {
   FxRecord rec;
 };
-template <typename E, bool REC>
-using FxArgs = std::conditional_t<REC, FxRecParams<E>, FxParams<E>>;
+// Region prompts (the RGN instances, KC = 2, 3): chunk c of image b's context gets its own softmax over its 77 keys,
+// and query row n takes  out(n) = sum_c w_c(n) softmax_c(..) V_c  (xattn_core.cuh: warp_weighted_chunk).  The weights
+// of image b are row rw_index[b] (row b when rw_index is NULL) of rw; an image with index -1 takes (1, 0, ..) on every
+// row.  The K / V of a chunk that no row of a softmax job's tile weighs are neither copied nor multiplied; the
+// statistic jobs still see every chunk, so the statistic is the one over all H * N * 77 KC scores.
+struct FxRegion {
+  const float* rw;          // [Bw, N, KC] fp32 chunk weights
+  int64_t rw_bs;            // elements between weight rows (>= N * KC)
+  const int32_t* rw_index;  // [B] weight row of image b, -1 = none; NULL = row b
+};
+template <typename E>
+struct FxRgnParams : FxParams<E> {
+  FxRegion rg;
+};
+template <typename E, bool REC, bool RGN = false>
+using FxArgs = std::conditional_t<RGN, FxRgnParams<E>, std::conditional_t<REC, FxRecParams<E>, FxParams<E>>>;
 
 template <int D, int KC = 1>
 struct Cfg2 {
@@ -90,6 +108,9 @@ struct Cfg2 {
   static constexpr int NST = (2 * STAGE + 8192 <= 232448) ? 2 : 1;     // stages (see the header)
   static constexpr uint32_t SMEM = NST * STAGE;
   static_assert(SMEM + 8192 <= 232448, "shared memory budget (dynamic + ~7 KB of static tables incl. the 4 KB job table)");
+  // region instances: [2][kWarps] per-warp chunk bits and [2] chunk masks of the jobs in flight, after the stages
+  static constexpr uint32_t SMEM_RGN = SMEM + 128;
+  static_assert(SMEM_RGN + 8192 <= 232448, "shared memory budget of the region instances");
 };
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -254,10 +275,12 @@ __device__ __forceinline__ float key_f32(unsigned k) {
   return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
 }
 
-// REC = true: the recording instance (FxRecord above).  Its extra work is behind `if constexpr`, so the plain
-// instances are the kernel without it.
-template <int D, int KC, typename E, bool REC = false>
-__global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const FxArgs<E, REC> fp) {
+// REC = true: the recording instance (FxRecord above); RGN = true: the region-prompt instance (FxRegion above).  Their
+// extra work is behind `if constexpr`, so the plain instances are the kernel without it.
+template <int D, int KC, typename E, bool REC = false, bool RGN = false>
+__global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const FxArgs<E, REC, RGN> fp) {
+  static_assert(!(REC && RGN), "attention recording has no region-prompt instance");
+  static_assert(!RGN || KC > 1, "region prompts need 2 or 3 key chunks");
   using C = core::Tile<D>;
   using CF = Cfg2<D, KC>;
   constexpr int CW = core::kTP * KC;                    // cidx columns: token 77 c + j of chunk c at column 80 c + j
@@ -396,12 +419,50 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
 
   // the copies of job i into stage i % 2 (stage 0 when there is one)
   auto stage = [&](int i) { return (uint32_t)(CF::NST == 2 ? (i & 1) : 0) * CF::STAGE; };
+  // RGN: the chunks some row of softmax job i's tile weighs (bit c = chunk c), also left for the job in the mask word
+  // of slot i & 1.  Consecutive jobs of one (image, tile) -- the heads of a unit -- reuse the last scan.
+  struct RegionScan { unsigned key = ~0u, bits = 0u; };
+  struct NoScan {};
+  [[maybe_unused]] std::conditional_t<RGN, RegionScan, NoScan> rgs;
+  [[maybe_unused]] auto region_chunks = [&](int i, int b, int tile) -> unsigned {
+    if constexpr (!RGN) return 0u;
+    else {
+    unsigned* words = reinterpret_cast<unsigned*>(smem + CF::SMEM);
+    const unsigned key = (unsigned)b | ((unsigned)tile << 8);
+    if (key != rgs.key) {                           // CTA-uniform: every thread walks the same job list
+      const int ri = fp.rg.rw_index != nullptr ? __ldg(fp.rg.rw_index + b) : b;
+      unsigned bits = 1u;                           // no weights: chunk 0 alone
+      if (ri >= 0) {
+        const int rows = p.N - tile * core::kBM < core::kBM ? p.N - tile * core::kBM : core::kBM;
+        const float* wt = fp.rg.rw + (int64_t)ri * fp.rg.rw_bs + (int64_t)tile * core::kBM * KC;
+        bits = 0u;
+        for (int idx = threadIdx.x; idx < rows * KC; idx += blockDim.x)
+          if (__ldg(wt + idx) != 0.f) bits |= 1u << (idx % KC);
+        bits = __reduce_or_sync(0xffffffffu, bits);
+        if (lane == 0) words[(i & 1) * core::kWarps + warp] = bits;
+        __syncthreads();
+        bits = 0u;
+#pragma unroll
+        for (int w = 0; w < core::kWarps; ++w) bits |= words[(i & 1) * core::kWarps + w];
+      }
+      rgs.key = key;
+      rgs.bits = bits;
+    }
+    if (threadIdx.x == 0) words[2 * core::kWarps + (i & 1)] = rgs.bits;
+    return rgs.bits;
+    }
+  };
   auto issue = [&](int i) {
     const uint2 r = s_jobs[i];
     const int b = r.x & 0xff, h = (r.x >> 8) & 0xff, tile = r.x >> 16;
     const bool is_main = (r.y & JF_MAIN) != 0, biased = (r.y & JF_BIASED) != 0;
     const uint32_t st = smem0 + stage(i);
-    core::load_operands<D, KC>(st, p, b, h, tile, is_main);
+    if constexpr (RGN) {
+      if (is_main) core::load_operands_of<D, KC>(st, p, b, h, tile, region_chunks(i, b, tile));
+      else core::load_operands<D, KC>(st, p, b, h, tile, false);
+    } else {
+      core::load_operands<D, KC>(st, p, b, h, tile, is_main);
+    }
     if (is_main && biased) {
       const int rows = p.N - tile * core::kBM;
       const __half* mp = reinterpret_cast<const __half*>(fp.mpack) + (int64_t)s_widx[b] * fp.mpack_bs + (int64_t)tile * core::kBM * kMW;
@@ -538,6 +599,44 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
       dsum += (double)sum;
       dsq += (double)sumsq;
       if (i == ns - 1) flush();
+    } else if constexpr (RGN) {
+      const float x = biased ? s_coef[li] : 0.f;
+      const __half* mrow = reinterpret_cast<const __half*>(smem + stage(i) + CF::OFF_M) + (warp * 16 + (lane >> 2)) * kMW;
+      const unsigned cm = reinterpret_cast<const unsigned*>(smem + CF::SMEM)[2 * core::kWarps + (i & 1)];
+      const int ri = fp.rg.rw_index != nullptr ? __ldg(fp.rg.rw_index + b) : b;
+      const int ra = row0 + (lane >> 2), rb = ra + 8;          // this thread's two query rows
+      const float* wr = fp.rg.rw + (int64_t)(ri < 0 ? 0 : ri) * fp.rg.rw_bs;
+      float o[C::NT][4];
+#pragma unroll
+      for (int j = 0; j < C::NT; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
+#pragma unroll 1
+      for (int c = 0; c < KC; ++c) {
+        if (!((cm >> c) & 1u)) continue;                       // no row of the tile weighs chunk c: not even copied
+        float w0 = c == 0 ? 1.f : 0.f, w1 = w0;
+        if (ri >= 0) {
+          w0 = ra < p.N ? __ldg(wr + (int64_t)ra * KC + c) : 0.f;
+          w1 = rb < p.N ? __ldg(wr + (int64_t)rb * KC + c) : 0.f;
+        }
+        if (!__any_sync(0xffffffffu, w0 != 0.f || w1 != 0.f)) continue;   // nor of this warp's 16 rows
+        float s[10][4];
+        core::warp_qk<D, E>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
+        if (biased) {
+          const signed char* ci = s_cidx[li] + c * core::kTP;
+#pragma unroll
+          for (int j = 0; j < 10; ++j)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const int cc = ci[core::tok(j, e, lane)];
+              if (cc >= 0) {
+                const __half* mr = mrow + (e >> 1) * 8 * kMW;
+                s[j][e] = fmaf(x, __half2float(mr[cc]) + __half2float(mr[kRC + cc]), s[j][e]);
+              }
+            }
+        }
+        core::warp_weighted_chunk<D, E>(s, kv, sl2, st + C::QBYTES + (KC + c) * C::KBYTES, lane, w0, w1, o);
+      }
+      core::warp_store<D>(o, smem + stage(i) + warp * 16 * C::LD * 2, lane, p.out + (int64_t)b * p.o_bs + h * D, p.o_rs,
+                          row0, p.N);
     } else {
       const float x = biased ? s_coef[li] : 0.f;
       const __half* mrow = reinterpret_cast<const __half*>(smem + stage(i) + CF::OFF_M) + (warp * 16 + (lane >> 2)) * kMW;
@@ -644,29 +743,31 @@ inline bool fused2_fits(int B, int hg, int tiles, int grid) {
   return fused_range_ok(B, hg, tiles, grid) && fused_units_ok(units, grid) && (units + grid - 1) / grid + 1 <= kMaxUnits;
 }
 
-template <int D, int KC, typename E, bool REC>
-cudaError_t launch_fused2_instance(const FxArgs<E, REC>& fp, cudaStream_t s) {
+template <int D, int KC, typename E, bool REC, bool RGN = false>
+cudaError_t launch_fused2_instance(const FxArgs<E, REC, RGN>& fp, cudaStream_t s) {
   using CF = Cfg2<D, KC>;
-  const cudaError_t e = allow_dynamic_smem<xattn_fused2_kernel<D, KC, E, REC>>(CF::SMEM);
+  constexpr uint32_t smem_bytes = RGN ? CF::SMEM_RGN : CF::SMEM;
+  const cudaError_t e = allow_dynamic_smem<xattn_fused2_kernel<D, KC, E, REC, RGN>>(smem_bytes);
   if (e != cudaSuccess) return e;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(fp.grid);
   cfg.blockDim = dim3(core::kThreads);
-  cfg.dynamicSmemBytes = CF::SMEM;
+  cfg.dynamicSmemBytes = smem_bytes;
   cfg.stream = s;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeCooperative;     // all CTAs co-resident: the in-kernel grid barrier cannot deadlock
   attr[0].val.cooperative = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, xattn_fused2_kernel<D, KC, E, REC>, fp);
+  return cudaLaunchKernelEx(&cfg, xattn_fused2_kernel<D, KC, E, REC, RGN>, fp);
 }
 
 // rec == NULL: the plain instance; else the recording instance with *rec (rec_index starting at this launch's image 0).
+// rg != NULL: the region-prompt instance with *rg (KC = 2, 3 only; rec must be NULL).
 template <int D, int KC, typename E>
 cudaError_t launch_fused2(const XattnParams<E>& x, const void* mpack, int64_t mpack_bs, const int8_t* cidx, cudaStream_t s,
-                          const FxRecord* rec = nullptr) {
+                          const FxRecord* rec = nullptr, const FxRegion* rg = nullptr) {
   using CF = Cfg2<D, KC>;
   FxParams<E> fp;
   memset(&fp, 0, sizeof(fp));
@@ -680,6 +781,17 @@ cudaError_t launch_fused2(const XattnParams<E>& x, const void* mpack, int64_t mp
   fp.grid = fused_grid(fp.units);
   fp.jobs_dump = debug_jobs_dump();
   if (!fused2_fits(x.B, fp.hg, fp.tiles, fp.grid)) return cudaErrorInvalidConfiguration;
+  if (rg != nullptr) {
+    if constexpr (KC > 1) {
+      if (rec != nullptr) return cudaErrorInvalidValue;
+      FxRgnParams<E> gp;
+      memset(&gp, 0, sizeof(gp));
+      static_cast<FxParams<E>&>(gp) = fp;
+      gp.rg = *rg;
+      return launch_fused2_instance<D, KC, E, false, true>(gp, s);
+    }
+    return cudaErrorInvalidValue;
+  }
   if (rec == nullptr) return launch_fused2_instance<D, KC, E, false>(fp, s);
   FxRecParams<E> rp;
   memset(&rp, 0, sizeof(rp));

@@ -29,7 +29,7 @@ from PIL import Image
 from . import attention as _attention
 from .conditioning import (MAX_RECORDED_REGIONS, RATIOS, REGION_COUNT_KEY, REGION_INDEX_KEY,
                            _encode_text_color_inputs, _extract_seed_and_sigma_from_context, _get_binary_mask,
-                           _rgb_of, always_round, pack_weight_map, packed_key)
+                           _rgb_of, always_round, check_region_prompts, pack_weight_map, packed_key)
 from . import _native, fused_ops
 from .scheduler import (FORM_COLUMNS, SIGMA_SCHEDULERS, EulerAncestralDiscreteScheduler, LMSDiscreteScheduler,
                         history_length, step_form)
@@ -409,6 +409,8 @@ class PwWSampler:
             self._set_up_control(*_control_units(controlnet, control_image, controlnet_conditioning_scale, guess_mode,
                                                  control_guidance_start, control_guidance_end))
         self.record_attention = bool(record_attention)
+        if self.record_attention and any(k.startswith("REGION_WEIGHTS_") for k in self._ctx):
+            raise ValueError("attention recording does not combine with region prompts")
         self._rec_levels: List[tuple] = []     # (N, h_r, w_r, accumulator [m, H, N, 16]) per cross-attention level
         if self.record_attention:
             self._set_up_recording(cond_ctxs)
@@ -602,7 +604,10 @@ class PwWSampler:
     def _merge_contexts(self, conds, unconds) -> dict:
         """Batch the per-image dicts: CONTEXT_TENSOR -> [2m,T,Dc]; weight maps -> [m,N,T] stacks;
         WMAP_INDEX = [0..m-1, -1 x m] with -1 also for images whose weight function is zero; STAT_KIND = the probed
-        statistic of every image (uncond images: max, ignored).  The m images are the first len(conds) of the
+        statistic of every image (uncond images: max, ignored).  Region prompts: REGION_WEIGHTS_{N} -> [m, N, k] stacks
+        (every cond dict has them or none does), reached through WMAP_INDEX, which then keeps row i for an image whose
+        weight function is zero (its G(sigma) is 0, so its bias is exactly 0); the uncond images' -1 gives them the
+        first chunk alone.  The m images are the first len(conds) of the
         sampler's (all of them here; a panorama chunk's windows in PanoramaSampler)."""
         m = len(conds)
         probed = self._probed[:m]
@@ -630,8 +635,13 @@ class PwWSampler:
                     ctx[packed_key(n)] = (packed[0].to(self.device), packed[1].to(self.device))
             else:
                 ctx[key] = 0
-        ctx["WMAP_INDEX"] = torch.tensor([-1 if pr.is_zero else i for i, pr in enumerate(probed)] + [-1] * m,
-                                         dtype=torch.int32, device=self.device)
+        region_keys = [k for k in conds[0] if k.startswith("REGION_WEIGHTS_")]
+        if any(sorted(k for k in c if k.startswith("REGION_WEIGHTS_")) != sorted(region_keys) for c in conds):
+            raise ValueError("the images of one sampler either all have region prompts or none has")
+        for key in region_keys:
+            ctx[key] = torch.stack([c[key].to(self.device, torch.float32) for c in conds], 0).contiguous()
+        ctx["WMAP_INDEX"] = torch.tensor([-1 if pr.is_zero and not region_keys else i for i, pr in enumerate(probed)] +
+                                         [-1] * m, dtype=torch.int32, device=self.device)
         ctx["STAT_KIND"] = torch.tensor([STAT_MAX if pr.is_zero else pr.stat for pr in probed] + [STAT_MAX] * m,
                                         dtype=torch.int32, device=self.device)
         ctx["WEIGHT_FUNCTION"] = self.weight_function
@@ -846,6 +856,8 @@ def paint_with_words(
     guidance_rescale: float = 0.0,
     prediction_type: Optional[str] = None,
     mask_image: Optional[Image.Image] = None,
+    region_prompts: Optional[Dict] = None,
+    region_base_ratio: float = 0.2,
 ):
     """paint_with_words.py:391-510.  Returns one PIL.Image (or the final latents with return_latents).
     `max_prompt_chunks` (1 .. 3): a prompt longer than 75 tokens fills up to that many 77-token CLIP chunks instead of
@@ -866,7 +878,13 @@ def paint_with_words(
     `mask_image` (with `init_image`): masked img2img, inpainting with any model.  Only the white area of the mask is
     repainted (values >= 0.5 after / 255, as `paint_with_words_inpaint` binarises them); elsewhere the latents follow
     the init image's noise path and end as its latents (`PwWSampler`'s `inpaint_mask`).  The mask is resized (nearest)
-    to the init image's size, then to the latent grid."""
+    to the init image's size, then to the latent grid.
+    `region_prompts` ({colour: sentence}, 1 or 2 entries): every painted region of that colour also gets a sentence
+    of its own, attended with its own softmax and mixed per pixel with the base prompt, which keeps a share of
+    `region_base_ratio` (0..1) inside the region (README, Region prompts).  `input_prompt` and each sentence must fit
+    one 75-token window; not with max_prompt_chunks > 1, attention maps or colour-map sides that are not multiples of
+    64."""
+    _check_region_call(region_prompts, region_base_ratio, max_prompt_chunks, return_attention_maps)
     if mask_image is not None and init_image is None:
         raise ValueError("mask_image needs an init_image: masked img2img repaints the masked area of the init image")
     control = _control_arguments(controlnet, control_image, color_map_image.size, "color_map_image",
@@ -879,12 +897,13 @@ def paint_with_words(
     blend = {}
     if init_image is None:
         cond, uncond, latents = _txt2img_inputs(tools, device, color_map_image, color_context, input_prompt,
-                                                unconditional_input_prompt, seed, max_prompt_chunks)
+                                                unconditional_input_prompt, seed, max_prompt_chunks, region_prompts,
+                                                region_base_ratio)
         timesteps = scheduler.timesteps
     else:
         _, _, cond, uncond = _encode_text_color_inputs(
             text_encoder, tokenizer, device, color_map_image, color_context, input_prompt, unconditional_input_prompt,
-            max_prompt_chunks=max_prompt_chunks)
+            max_prompt_chunks=max_prompt_chunks, region_prompts=region_prompts, region_base_ratio=region_base_ratio)
         # the reference draws img2img's noise from the global RNG as it stands: unseeded here
         latents, timesteps, init, noise = _img2img_latents(vae, scheduler, init_image, num_inference_steps, strength,
                                                            device)
@@ -909,15 +928,24 @@ def _tools(preloaded_utils, device, scheduler_type, local_model_path, hf_model_p
                           model_token=model_token, torch_dtype=torch_dtype, prediction_type=prediction_type)
 
 
+def _check_region_call(region_prompts, region_base_ratio, max_prompt_chunks, return_attention_maps) -> None:
+    """The ValueErrors of a public call with region prompts that need no model."""
+    if region_prompts is None:
+        return
+    check_region_prompts(region_prompts, region_base_ratio, max_prompt_chunks)
+    if return_attention_maps:
+        raise ValueError("attention recording does not combine with region prompts")
+
+
 def _txt2img_inputs(tools, device, color_map_image, color_context, input_prompt, unconditional_input_prompt, seed,
-                    max_prompt_chunks) -> Tuple[dict, dict, torch.Tensor]:
+                    max_prompt_chunks, region_prompts=None, region_base_ratio=0.2) -> Tuple[dict, dict, torch.Tensor]:
     """One txt2img image's (cond, uncond, latents): its text and colour contexts, and its seeded initial noise scaled
     by the scheduler's initial sigma (so `scheduler.set_timesteps` comes first)."""
     _, unet, text_encoder, tokenizer, scheduler = tools
     width, height = color_map_image.size
     extra_seeds, seperated_word_contexts, cond, uncond = _encode_text_color_inputs(
         text_encoder, tokenizer, device, color_map_image, color_context, input_prompt, unconditional_input_prompt,
-        max_prompt_chunks=max_prompt_chunks)
+        max_prompt_chunks=max_prompt_chunks, region_prompts=region_prompts, region_base_ratio=region_base_ratio)
     latents = initial_latents((1, unet.in_channels, height // 8, width // 8), seed, extra_seeds,
                               seperated_word_contexts).to(device)
     return cond, uncond, latents * scheduler.init_noise_sigma
@@ -1023,7 +1051,7 @@ def _control_arguments(controlnet, control_image, size: Tuple[int, int], size_of
 # the per-image keyword arguments of paint_with_words that paint_with_words_batch takes per entry
 BATCH_SETTING_KEYS = ("color_context", "color_map_image", "input_prompt", "unconditional_input_prompt", "seed",
                       "weight_function", "guidance_scale", "max_prompt_chunks", "control_image",
-                      "controlnet_conditioning_scale", "guidance_rescale")
+                      "controlnet_conditioning_scale", "guidance_rescale", "region_prompts", "region_base_ratio")
 
 
 def _batch_settings(settings) -> List[dict]:
@@ -1042,6 +1070,10 @@ def _batch_settings(settings) -> List[dict]:
         full.update(entry)
         if full["color_map_image"] is None:
             raise ValueError(f"settings[{i}]: color_map_image is required")
+        try:
+            _check_region_call(full["region_prompts"], full["region_base_ratio"], full["max_prompt_chunks"], False)
+        except ValueError as err:
+            raise ValueError(f"settings[{i}]: {err}") from err
         out.append(full)
     return out
 
@@ -1079,7 +1111,8 @@ def paint_with_words_batch(
     """Many images, each with its own settings, in as few samplers as possible.  `settings[i]` is a dict of the
     per-image keyword arguments of `paint_with_words` (BATCH_SETTING_KEYS: color_context, color_map_image, input_prompt,
     unconditional_input_prompt, seed, weight_function, guidance_scale, max_prompt_chunks, control_image,
-    controlnet_conditioning_scale, guidance_rescale); missing keys take paint_with_words's defaults.  Returns a list of
+    controlnet_conditioning_scale, guidance_rescale, region_prompts, region_base_ratio); missing keys take
+    paint_with_words's defaults.  Entries with region prompts share a sampler only with each other.  Returns a list of
     PIL images (or [1,4,h,w] latents) in input order; image i equals `paint_with_words(**settings[i])` up to fp16 noise.
     With `controlnet` (one for the batch, with `guess_mode` and the guidance window) every entry needs a
     `control_image` of its colour map's size; its `controlnet_conditioning_scale` is its own.  With a list of
@@ -1096,6 +1129,8 @@ def paint_with_words_batch(
     entries = _batch_settings(settings)
     if max_batch_size < 1:
         raise ValueError("max_batch_size must be >= 1")
+    if return_attention_maps and any(e["region_prompts"] is not None for e in entries):
+        raise ValueError("attention recording does not combine with region prompts")
     controls = []
     for i, e in enumerate(entries):
         try:
@@ -1112,11 +1147,13 @@ def paint_with_words_batch(
     for e in entries:
         cond, uncond, latents = _txt2img_inputs(tools, device, e["color_map_image"], dict(e["color_context"]),
                                                 e["input_prompt"], e["unconditional_input_prompt"], e["seed"],
-                                                e["max_prompt_chunks"])
+                                                e["max_prompt_chunks"], e["region_prompts"], e["region_base_ratio"])
         encoded.append((cond, uncond, latents))
         width, height = e["color_map_image"].size
         solo = width % 64 != 0 or height % 64 != 0
-        keys.append(None if solo else (height // 8, width // 8, int(cond["CONTEXT_TENSOR"].shape[1])))
+        # region-prompt entries share a sampler with each other only: their chunks are softmaxed one by one
+        keys.append(None if solo else (height // 8, width // 8, int(cond["CONTEXT_TENSOR"].shape[1]),
+                                       e["region_prompts"] is not None))
     results: List[Optional[torch.Tensor]] = [None] * len(entries)
     attention: List[Optional[RegionAttention]] = [None] * len(entries)
     for idx in batch_groups(keys, max_batch_size):
@@ -1203,12 +1240,16 @@ def paint_with_words_inpaint(
     return_attention_maps: bool = False,
     guidance_rescale: float = 0.0,
     prediction_type: Optional[str] = None,
+    region_prompts: Optional[Dict] = None,
+    region_base_ratio: float = 0.2,
 ):
     """paint_with_words_inpaint.py:137-270: 9-channel UNet input cat[latents, mask, masked-image latents].
     `max_prompt_chunks`, `torch_dtype` and the ControlNet arguments as in `paint_with_words`; the colour map is resized
     to the init image, so `control_image` has the init image's size.  The ControlNet sees the 4 latent channels of
     the UNet input (hook_pww.py:113-119).  `return_attention_maps` as in `paint_with_words` (coverage from the resized
-    colour map).  `guidance_rescale` and `prediction_type` as in `paint_with_words`."""
+    colour map).  `guidance_rescale`, `prediction_type`, `region_prompts` and `region_base_ratio` as in
+    `paint_with_words` (the colour-map size checked is the init image's)."""
+    _check_region_call(region_prompts, region_base_ratio, max_prompt_chunks, return_attention_maps)
     width, height = init_image.size
     control = _control_arguments(controlnet, control_image, (width, height), "init_image (and resized color_map_image)",
                                  controlnet_conditioning_scale, guess_mode, control_guidance_start,
@@ -1219,7 +1260,7 @@ def paint_with_words_inpaint(
     mask_image = mask_image.resize((width, height), Image.NEAREST)
     _, _, cond, uncond = _encode_text_color_inputs(
         text_encoder, tokenizer, device, color_map_image, color_context, input_prompt, unconditional_input_prompt,
-        max_prompt_chunks=max_prompt_chunks)
+        max_prompt_chunks=max_prompt_chunks, region_prompts=region_prompts, region_base_ratio=region_base_ratio)
     mask, masked_image = prepare_mask_and_masked_image(init_image, mask_image)
 
     scheduler.set_timesteps(num_inference_steps)
@@ -1321,10 +1362,11 @@ class PaintWithWord_StableDiffusionPipeline:
                  output_type: str = "pil", return_dict: bool = True, callback=None, callback_steps: int = 1,
                  max_prompt_chunks: int = 1, control_image=None, controlnet_conditioning_scale: float = 1.0,
                  guess_mode: bool = False, control_guidance_start: float = 0.0, control_guidance_end: float = 1.0,
-                 guidance_rescale: float = 0.0, mask_image=None):
-        """`mask_image` with `image`: masked img2img (see `paint_with_words`)."""
+                 guidance_rescale: float = 0.0, mask_image=None, region_prompts=None, region_base_ratio: float = 0.2):
+        """`mask_image` with `image`: masked img2img; `region_prompts` / `region_base_ratio` (see `paint_with_words`)."""
         extra = {} if image is None else {"init_image": image, "strength": eta}
         extra["mask_image"] = mask_image
+        extra["region_prompts"], extra["region_base_ratio"] = region_prompts, region_base_ratio
         extra["max_prompt_chunks"] = max_prompt_chunks
         extra["guidance_rescale"] = guidance_rescale
         extra.update(self._control(control_image, controlnet_conditioning_scale, guess_mode, control_guidance_start,
@@ -1352,10 +1394,11 @@ class PaintWithWord_StableDiffusionInpaintPipeline(PaintWithWord_StableDiffusion
                  output_type: str = "pil", return_dict: bool = True, callback=None, callback_steps: int = 1,
                  max_prompt_chunks: int = 1, control_image=None, controlnet_conditioning_scale: float = 1.0,
                  guess_mode: bool = False, control_guidance_start: float = 0.0, control_guidance_end: float = 1.0,
-                 guidance_rescale: float = 0.0):
+                 guidance_rescale: float = 0.0, region_prompts=None, region_base_ratio: float = 0.2):
         return self._run(paint_with_words_inpaint, prompt, color_map_image, dict(color_context), weight_function,
                          num_inference_steps, guidance_scale, negative_prompt, seed, output_type, return_dict, callback,
                          callback_steps, mask_image=mask_image, init_image=image, strength=eta,
                          max_prompt_chunks=max_prompt_chunks, guidance_rescale=guidance_rescale,
+                         region_prompts=region_prompts, region_base_ratio=region_base_ratio,
                          **self._control(control_image, controlnet_conditioning_scale, guess_mode,
                                          control_guidance_start, control_guidance_end))

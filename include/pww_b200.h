@@ -312,6 +312,60 @@ int pww_xattn_fused_region_multi_bf16(const void* q, const void* k, const void* 
                                       const float* region_weights, int64_t region_batch_stride);
 
 /*
+ * Region prompts with a weight row per image independent of its bias (negative region prompts: the uncond images of
+ * a CFG batch get chunk weights of their own without a PwW bias): pww_xattn_fused_region_* with two more arguments.
+ *   region_index [B] int32 (device): image b takes weight row region_index[b] of region_weights, -1 = w = (1, 0, ..)
+ *               on every row; NULL = row b.  wmap_index keeps its one job, the packed map of a biased image, so an
+ *               unbiased image (index -1 there, or mpack NULL) with a weight row runs the mixed softmax with no bias,
+ *               and a biased image with region_index -1 takes its first chunk alone, with the bias.
+ *   stat_chunks  [B] int32 (device) or NULL: bit c set = chunk c is in image b's statistic; chunk 0 always is, and
+ *               bits >= k are ignored.  A biased image's max / std covers the H * N * 77 * popcount(mask) scores of
+ *               those chunks alone (their K is the only K its statistic reads); NULL = every chunk, H * N * T.
+ * With region_index == wmap_index and stat_chunks == NULL these give the bits of pww_xattn_fused_region_*; the unit
+ * order, job lists and grid barrier depend on wmap_index alone, as there.
+ */
+int pww_xattn_fused_region_rows_f16(const void* q, const void* k, const void* v, void* out,
+                                    int B, int H, int N, int T, int D,
+                                    int64_t q_batch_stride, int64_t q_row_stride,
+                                    int64_t k_batch_stride, int64_t k_row_stride,
+                                    int64_t o_batch_stride, int64_t o_row_stride,
+                                    const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+                                    const int32_t* wmap_index, int stat, const float* g_sigma, float scale,
+                                    float* stats, void* workspace, size_t workspace_bytes, void* stream,
+                                    const float* region_weights, int64_t region_batch_stride,
+                                    const int32_t* region_index, const int32_t* stat_chunks);
+int pww_xattn_fused_region_rows_bf16(const void* q, const void* k, const void* v, void* out,
+                                     int B, int H, int N, int T, int D,
+                                     int64_t q_batch_stride, int64_t q_row_stride,
+                                     int64_t k_batch_stride, int64_t k_row_stride,
+                                     int64_t o_batch_stride, int64_t o_row_stride,
+                                     const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+                                     const int32_t* wmap_index, int stat, const float* g_sigma, float scale,
+                                     float* stats, void* workspace, size_t workspace_bytes, void* stream,
+                                     const float* region_weights, int64_t region_batch_stride,
+                                     const int32_t* region_index, const int32_t* stat_chunks);
+int pww_xattn_fused_region_rows_multi_f16(const void* q, const void* k, const void* v, void* out,
+                                          int B, int H, int N, int T, int D,
+                                          int64_t q_batch_stride, int64_t q_row_stride,
+                                          int64_t k_batch_stride, int64_t k_row_stride,
+                                          int64_t o_batch_stride, int64_t o_row_stride,
+                                          const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+                                          const int32_t* wmap_index, const int32_t* stat, const float* g_sigma,
+                                          float scale, float* stats, void* workspace, size_t workspace_bytes,
+                                          void* stream, const float* region_weights, int64_t region_batch_stride,
+                                          const int32_t* region_index, const int32_t* stat_chunks);
+int pww_xattn_fused_region_rows_multi_bf16(const void* q, const void* k, const void* v, void* out,
+                                           int B, int H, int N, int T, int D,
+                                           int64_t q_batch_stride, int64_t q_row_stride,
+                                           int64_t k_batch_stride, int64_t k_row_stride,
+                                           int64_t o_batch_stride, int64_t o_row_stride,
+                                           const void* mpack, int64_t mpack_batch_stride, int Bw, const int8_t* cidx,
+                                           const int32_t* wmap_index, const int32_t* stat, const float* g_sigma,
+                                           float scale, float* stats, void* workspace, size_t workspace_bytes,
+                                           void* stream, const float* region_weights, int64_t region_batch_stride,
+                                           const int32_t* region_index, const int32_t* stat_chunks);
+
+/*
  * Self-attention through the same patched function (context=None, paint_with_words.py:71-72):
  *   out = softmax(scale * Q_h K_h^T) V_h  with keys/values [B, N, H*D]; no bias; online softmax.
  */

@@ -36,6 +36,8 @@ EXPORTS = (
     "pww_window_input", "pww_window_update",
     "pww_xattn_fused_region_f16", "pww_xattn_fused_region_bf16",
     "pww_xattn_fused_region_multi_f16", "pww_xattn_fused_region_multi_bf16",
+    "pww_xattn_fused_region_rows_f16", "pww_xattn_fused_region_rows_bf16",
+    "pww_xattn_fused_region_rows_multi_f16", "pww_xattn_fused_region_rows_multi_bf16",
 )
 
 
@@ -93,6 +95,11 @@ def lib() -> ctypes.CDLL:
     L.pww_xattn_fused_region_f16.argtypes = list(L.pww_xattn_fused_f16.argtypes) + [c_vp, c_i64]
     L.pww_xattn_fused_region_multi_f16.restype = c_i
     L.pww_xattn_fused_region_multi_f16.argtypes = list(L.pww_xattn_fused_multi_f16.argtypes) + [c_vp, c_i64]
+    # negative region prompts: the region arguments, then region_index and stat_chunks (device pointers or NULL)
+    L.pww_xattn_fused_region_rows_f16.restype = c_i
+    L.pww_xattn_fused_region_rows_f16.argtypes = list(L.pww_xattn_fused_region_f16.argtypes) + [c_vp, c_vp]
+    L.pww_xattn_fused_region_rows_multi_f16.restype = c_i
+    L.pww_xattn_fused_region_rows_multi_f16.argtypes = list(L.pww_xattn_fused_region_multi_f16.argtypes) + [c_vp, c_vp]
     L.pww_attn_fwd_f16.restype = c_i
     L.pww_attn_fwd_f16.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i, c_i, c_i, c_i, c_i64, c_i64, c_i64, c_i64, c_f, c_vp]
     L.pww_groupnorm_workspace_bytes.restype = c_sz

@@ -11,7 +11,9 @@ Same calling convention, context-dict schema and patch mechanism as the referenc
     `conditioning.chunk_prompt`, the A1111 / compel layout).
         (optional, ours) "WMAP_INDEX", "G_SIGMA", "STAT_KIND", "CROSS_ATTENTION_PACKED_{N}", "PWW_SCRATCH",
         "ATTN_RECORD" (per-region attention recording, see RECORD_KEY), "REGION_WEIGHTS_{N}" (region prompts: fp32
-        [N, k] or [Bw, N, k] chunk weights of a k-chunk context, see cross_attention's `region`)
+        [N, k] or [Bw, N, k] chunk weights of a k-chunk context, see cross_attention's `region`), "REGION_ROWS" and
+        "REGION_STAT_CHUNKS" (negative region prompts: int32 [B] weight row and statistic chunks of every image, see
+        cross_attention's `region_rows`)
 
 Everything between the q/k/v projections and the output projection runs in libpww_b200.so through
 the C ABI (include/pww_b200.h): ONE launch of `pww_xattn_fused_f16` (per-image max/std of QK^T over all heads,
@@ -44,8 +46,8 @@ import torch
 import torch.nn.functional as F
 
 from . import _native
-from .conditioning import (PACK_TOKENS, expand_orig_weight_map, key_chunks, pack_weight_map, packed_key, region_key,
-                           weight_key)
+from .conditioning import (PACK_TOKENS, REGION_ROWS_KEY, STAT_CHUNKS_KEY, expand_orig_weight_map, key_chunks,
+                           pack_weight_map, packed_key, region_key, weight_key)
 from .weight_function import g_of_sigma, probe_weight_function
 
 _ORIG_KEY = "CROSS_ATTENTION_WEIGHT_ORIG"
@@ -168,7 +170,8 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                     wmap: Optional[torch.Tensor] = None, wmap_index: Optional[torch.Tensor] = None,
                     stat: Union[int, torch.Tensor] = _native.PWW_STAT_MAX, g_sigma: Optional[torch.Tensor] = None,
                     return_stats: bool = False, packed=None, stats_out: Optional[torch.Tensor] = None,
-                    workspace: Optional[torch.Tensor] = None, record=None, region: Optional[torch.Tensor] = None):
+                    workspace: Optional[torch.Tensor] = None, record=None, region: Optional[torch.Tensor] = None,
+                    region_rows=None):
     """Fused region for a key sequence of T <= 80 tokens or of 2 / 3 CLIP chunks (T = 154, 231; any other T raises).
     q [B,N,C]; k,v [B,T,C]; wmap [Bw,N,T] fp32 or None; `packed` = (mpack [Bw,N,32] fp16, cidx [Bw,80 k] int8, k key
     chunks) from `conditioning.pack_weight_map` (built from `wmap` and cached when not given).  `stat` is one kind for
@@ -182,7 +185,11 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
     `region` = fp32 [Bw, N, k] chunk weights of a k = 2 or 3 chunk context (region prompts): the call goes to
     `pww_xattn_fused_region_*`, which gives every chunk its own softmax and mixes them per query row by these weights.
     Image b takes weight row `wmap_index[b]` (-1: (1, 0, ..), the first chunk alone), or row b without an index.  It
-    needs the one-launch kernel and cannot record."""
+    needs the one-launch kernel and cannot record.
+    `region_rows` = (region_index int32 [B], stat_chunks int32 [B] or None), on q's device, with `region`: image b
+    takes weight row region_index[b] whether or not it is biased (wmap_index then only picks its map), and a biased
+    image's statistic covers the chunks of its bit mask stat_chunks[b] (chunk 0 always; None: every chunk).  The call
+    goes to `pww_xattn_fused_region_rows_*` (negative region prompts)."""
     L = _native.lib()
     dt = _elem_dtype(q)
     q, k, v = _rows(q, dt), _rows(k, dt), _rows(v, dt)
@@ -235,11 +242,19 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                                  f"chunks (T = {T})")
             if not use_fused or record is not None:
                 raise _native.NativeError("region prompts need the one-launch kernel without attention recording")
-            if wmap_index is None and region.shape[0] != B:
-                wmap_index = (st.shared_index(B) if region.shape[0] == 1 else None)
-                if wmap_index is None:
-                    raise ValueError(f"{region.shape[0]} region weight rows for {B} images need a wmap_index")
-            region_args = (region.data_ptr(), region.stride(0))
+            if region_rows is not None:
+                rows, chunks = region_rows
+                for t in (rows,) if chunks is None else (rows, chunks):
+                    if t.dtype != torch.int32 or t.numel() != B or not t.is_contiguous() or t.device != q.device:
+                        raise ValueError(f"region_rows need int32 [{B}] region_index / stat_chunks on {q.device}")
+                region_args = (region.data_ptr(), region.stride(0), rows.data_ptr(),
+                               None if chunks is None else chunks.data_ptr())
+            else:
+                if wmap_index is None and region.shape[0] != B:
+                    wmap_index = (st.shared_index(B) if region.shape[0] == 1 else None)
+                    if wmap_index is None:
+                        raise ValueError(f"{region.shape[0]} region weight rows for {B} images need a wmap_index")
+                region_args = (region.data_ptr(), region.stride(0))
         if record is not None:
             if not use_fused:
                 why = ("XATTN_IMPL is 'dense'" if impl == "dense" else
@@ -272,11 +287,13 @@ def cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: in
                 mp_ptr, ci_ptr, idx_ptr = mpack.data_ptr(), cidx.data_ptr(), wmap_index.data_ptr()
                 g_ptr, st_ptr, ws_ptr = g_sigma.data_ptr(), stats.data_ptr(), ws.data_ptr()
                 mp_bs, bw, ws_bytes = mpack.stride(0), mpack.shape[0], ws.numel()
-            if region_args and wmap_index is not None:
+            if region_args and region_rows is None and wmap_index is not None:
                 idx_ptr = wmap_index.data_ptr()    # the weight rows are reached through it with or without a bias
             name = "pww_xattn_fused_rec" if rec_args else ("pww_xattn_fused_multi" if per_image else "pww_xattn_fused")
             if region_args:
                 name = "pww_xattn_fused_region_multi" if per_image else "pww_xattn_fused_region"
+                if region_rows is not None:
+                    name = name.replace("_region", "_region_rows")
             fn = _native.entry(name, dt)
             rc = fn(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, heads, N, T, D,
                     q.stride(0), q.stride(1), k.stride(0), k.stride(1), out.stride(0), out.stride(1),
@@ -439,13 +456,17 @@ def inj_forward(self, hidden_states, context=None, mask=None):
                 raise _native.NativeError(f"attention recording has no accumulator for N = {q.shape[1]} query rows "
                                           f"(levels: {sorted(recs)})")
         region = context.get(region_key(q.shape[1])) if is_dict else None
-        if region is not None and wmap_index is None:
+        rows = context.get(REGION_ROWS_KEY) if region is not None else None
+        if rows is not None:
+            rows = (rows, context.get(STAT_CHUNKS_KEY))   # negative region prompts: weight rows of their own
+        elif region is not None and wmap_index is None:
             wmap_index = context.get("WMAP_INDEX")      # the sampler's image -> weight row (-1: uncond images)
         if k.shape[0] != q.shape[0]:
             k = k.expand(q.shape[0], -1, -1)
             v = v.expand(q.shape[0], -1, -1)
         o = cross_attention(q, k, v, self.heads, self.scale, wmap, wmap_index, stat, g_dev, packed=packed,
-                            stats_out=scratch[0], workspace=scratch[1], record=record, region=region)
+                            stats_out=scratch[0], workspace=scratch[1], record=record, region=region,
+                            region_rows=rows)
 
     with torch.autocast("cuda", dtype=act):
         o = self.to_out[0](o)

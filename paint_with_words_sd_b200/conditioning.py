@@ -380,12 +380,14 @@ def check_region_prompts(region_prompts, region_base_ratio: float, max_prompt_ch
         raise ValueError(f"region_base_ratio must be in [0, 1], got {region_base_ratio}")
 
 
-def region_chunk_ids(tokenizer, input_prompt: str, region_prompts: dict) -> torch.Tensor:
+def region_chunk_ids(tokenizer, input_prompt: str, region_prompts: dict, base_name: str = "input_prompt",
+                     sentence_name: str = "region prompt") -> torch.Tensor:
     """[1, 77 (1 + R)] ids: the base prompt, then each region's sentence in dict order, each as [BOS] + tokens + [EOS]
-    + padding in a chunk of its own.  A prompt longer than 75 tokens raises ValueError."""
+    + padding in a chunk of its own.  A prompt longer than 75 tokens raises ValueError (naming it `base_name` or
+    `sentence_name` and its colour)."""
     width = tokenizer.model_max_length - 2
     windows = []
-    for what, text in [("input_prompt", input_prompt)] + [(f"region prompt {k!r}", v) for k, v in region_prompts.items()]:
+    for what, text in [(base_name, input_prompt)] + [(f"{sentence_name} {k!r}", v) for k, v in region_prompts.items()]:
         ids = list(tokenizer(text)["input_ids"])[1:-1]
         if len(ids) > width:
             raise ValueError(f"{what} is {len(ids)} tokens long; with region prompts every prompt must fit one "
@@ -394,27 +396,83 @@ def region_chunk_ids(tokenizer, input_prompt: str, region_prompts: dict) -> torc
     return _chunked_ids(tokenizer, windows, len(windows))
 
 
-def region_chunk_weights(color_map_image, region_prompts: dict, region_base_ratio: float, ratio: int) -> torch.Tensor:
+def region_chunk_weights(color_map_image, region_prompts: dict, region_base_ratio: float, ratio: int,
+                         layout: Optional[Sequence] = None) -> torch.Tensor:
     """fp32 [N, 1 + R] chunk weights of the level with latent ratio `ratio` (CPU):
         w_c = (1 - beta) * f_c   (c >= 1),   w_0 = 1 - sum_{c >= 1} w_c
     with f_c the binary mask of region c's colour resized as the weight maps are (`_img_importance_flatten` to
-    always_round(side / ratio)).  A colour absent from the map gives f_c = 0."""
+    always_round(side / ratio)).  A colour absent from the map gives f_c = 0.  `layout` (default: region_prompts'
+    colours) is the colour of every chunk c >= 1; a colour of it that region_prompts lacks gets f_c = 0 too."""
     pixels = np.array(color_map_image)
     dim0, dim1 = pixels.shape[:2]
     r0, r1 = always_round(dim0 / ratio), always_round(dim1 / ratio)
     beta = float(region_base_ratio)
+    mine = {tuple(_rgb_of(c)) for c in region_prompts}
     cols = []
-    for color in region_prompts:
+    for color in (region_prompts if layout is None else layout):
+        if tuple(_rgb_of(color)) not in mine:
+            cols.append(torch.zeros(r0 * r1, dtype=torch.float32))
+            continue
         hit = torch.from_numpy((pixels == _rgb_of(color)).all(axis=-1)).to(torch.float32)
         cols.append((1.0 - beta) * _img_importance_flatten(hit, r0, r1).reshape(-1))
     w = torch.stack(cols, 1)
     return torch.cat([1.0 - w.sum(1, keepdim=True), w], 1).contiguous()
 
 
+REGION_SENTENCES_KEY = "REGION_SENTENCE_CHUNKS"   # dict key: bit c = chunk c holds a sentence of this side (int)
+REGION_ROWS_KEY = "REGION_ROWS"                   # batched-dict key: int32 [B] weight row of every image, -1 = none
+STAT_CHUNKS_KEY = "REGION_STAT_CHUNKS"            # batched-dict key: int32 [B] chunks of every image's statistic
+
+
+def region_layout(region_prompts: Optional[dict], negative_region_prompts: Optional[dict]) -> list:
+    """The colour of every chunk c >= 1 of a context with region or negative region prompts: region_prompts' colours
+    in dict order, then negative_region_prompts' colours that region_prompts lacks, in dict order (one colour in two
+    key forms, "#ff0000" and (255, 0, 0), is one colour)."""
+    layout, seen = [], set()
+    for prompts in (region_prompts or {}, negative_region_prompts or {}):
+        for color in prompts:
+            if tuple(_rgb_of(color)) not in seen:
+                seen.add(tuple(_rgb_of(color)))
+                layout.append(color)
+    return layout
+
+
+def _side_sentences(layout: Sequence, prompts: Optional[dict], base: str) -> Tuple[dict, int]:
+    """One side's sentence for every chunk c >= 1 of `layout` (its own, else `base` again) and the bit mask of the
+    chunks that hold its own sentences."""
+    own = {tuple(_rgb_of(c)): text for c, text in (prompts or {}).items()}
+    texts, bits = {}, 0
+    for c, color in enumerate(layout, start=1):
+        text = own.get(tuple(_rgb_of(color)))
+        texts[color] = base if text is None else text
+        bits |= 0 if text is None else 1 << c
+    return texts, bits
+
+
+def check_negative_region_prompts(region_prompts, negative_region_prompts, region_base_ratio: float,
+                                  max_prompt_chunks: int = 1) -> None:
+    """The ValueErrors of negative region prompts that need neither a model nor the colour map (region_prompts may be
+    None)."""
+    if region_prompts is not None:
+        check_region_prompts(region_prompts, region_base_ratio, max_prompt_chunks)
+    if not isinstance(negative_region_prompts, dict) or not negative_region_prompts:
+        n = len(negative_region_prompts) if isinstance(negative_region_prompts, dict) else negative_region_prompts
+        raise ValueError(f"negative_region_prompts takes 1 .. {MAX_REGION_PROMPTS} colour -> sentence entries, got {n}")
+    n = len(region_layout(region_prompts, negative_region_prompts))
+    if n > MAX_REGION_PROMPTS:
+        raise ValueError(f"region_prompts and negative_region_prompts name {n} colours in all; at most "
+                         f"{MAX_REGION_PROMPTS} (1 .. {MAX_REGION_PROMPTS} extra 77-token chunks)")
+    if max_prompt_chunks > 1:
+        raise ValueError("negative region prompts and max_prompt_chunks > 1 do not combine: the base prompts are one "
+                         "77-token chunk")
+    if not 0.0 <= float(region_base_ratio) <= 1.0:
+        raise ValueError(f"region_base_ratio must be in [0, 1], got {region_base_ratio}")
+
+
 def _encode_text_color_inputs(text_encoder, tokenizer, device, color_map_image, color_context,
                               input_prompt, unconditional_input_prompt, use_blur: bool = True,
                               max_prompt_chunks: int = 1, region_prompts: Optional[dict] = None,
-                              region_base_ratio: float = 0.2):
+                              region_base_ratio: float = 0.2, negative_region_prompts: Optional[dict] = None):
     """paint_with_words.py:315-388 (and the pipeline-class copy 561-627, which ignores blur sigmas:
     pass use_blur=False for that behaviour).  Returns
     (extra_seeds, seperated_word_contexts, encoder_hidden_states, uncond_encoder_hidden_states).
@@ -426,11 +484,21 @@ def _encode_text_color_inputs(text_encoder, tokenizer, device, color_map_image, 
     `region_prompts` ({colour: sentence}, 1 or 2 entries, colours of `color_map_image` in `color_context`'s key forms)
     gives every painted region a sentence of its own: the context is 1 + R chunks (the base prompt, then the sentences
     in dict order), and both dicts get `region_key(N)` chunk weights per level (`region_chunk_weights`; the uncond
-    dict's are (1, 0, ..) on every row).  `region_base_ratio` is the base prompt's share beta inside a region."""
+    dict's are (1, 0, ..) on every row).  `region_base_ratio` is the base prompt's share beta inside a region.
+
+    `negative_region_prompts` ({colour: sentence}) does the same on the uncond side.  The chunks c >= 1 are the colours
+    of `region_layout` (at most 2 in all); a side without a sentence for colour c holds its own base prompt again in
+    chunk c, with weight 0.  The uncond prompt is then one 75-token chunk, and the uncond dict's weights are
+    `region_chunk_weights` over the negative colours.  Both dicts carry REGION_SENTENCES_KEY, the bit mask of the
+    chunks holding their own sentences (0 for a side without any), whenever they carry region weights."""
     if not 1 <= max_prompt_chunks <= MAX_PROMPT_CHUNKS:
         raise ValueError(f"max_prompt_chunks must be 1 .. {MAX_PROMPT_CHUNKS}, got {max_prompt_chunks}")
-    if region_prompts is not None:
+    if negative_region_prompts is not None:
+        check_negative_region_prompts(region_prompts, negative_region_prompts, region_base_ratio, max_prompt_chunks)
+    elif region_prompts is not None:
         check_region_prompts(region_prompts, region_base_ratio, max_prompt_chunks)
+    sided = region_prompts is not None or negative_region_prompts is not None
+    if sided:
         if color_map_image is None:
             raise ValueError("region prompts need a color_map_image")
         if color_map_image.size[0] % REGION_SIDE or color_map_image.size[1] % REGION_SIDE:
@@ -440,9 +508,16 @@ def _encode_text_color_inputs(text_encoder, tokenizer, device, color_map_image, 
                            truncation=True, return_tensors="pt")
     color_context, extra_seeds, extra_sigmas = _extract_seed_and_sigma_from_context(color_context)
     chunks = 1
-    if region_prompts is not None:
-        text_input = {"input_ids": region_chunk_ids(tokenizer, input_prompt, region_prompts)}
-        chunks = 1 + len(region_prompts)
+    layout = region_layout(region_prompts, negative_region_prompts)
+    un_ids = None
+    if sided:
+        texts, cond_bits = _side_sentences(layout, region_prompts, input_prompt)
+        text_input = {"input_ids": region_chunk_ids(tokenizer, input_prompt, texts)}
+        chunks = 1 + len(layout)
+        un_texts, un_bits = _side_sentences(layout, negative_region_prompts, unconditional_input_prompt)
+        if negative_region_prompts is not None:
+            un_ids = region_chunk_ids(tokenizer, unconditional_input_prompt, un_texts, "unconditional_input_prompt",
+                                      "negative region prompt")
     elif max_prompt_chunks > 1:
         labels = [spec.rpartition(",")[0] for spec in color_context.values()] if color_map_image is not None else []
         ids = chunk_prompt(tokenizer, input_prompt, labels, max_prompt_chunks)
@@ -468,21 +543,28 @@ def _encode_text_color_inputs(text_encoder, tokenizer, device, color_map_image, 
     cond[REGION_INDEX_KEY] = (region_token_index(seperated_word_contexts, text_input)
                               if len(seperated_word_contexts) <= MAX_RECORDED_REGIONS else None)
     cond[REGION_COUNT_KEY] = len(seperated_word_contexts)
-    if region_prompts is not None:
+    if sided:
         for r in RATIOS:
-            w = region_chunk_weights(color_map_image, region_prompts, region_base_ratio, r)
+            w = region_chunk_weights(color_map_image, region_prompts or {}, region_base_ratio, r, layout)
             n = w.shape[0]
             cond[region_key(n)] = w.to(device)
-            plain = torch.zeros_like(w)
-            plain[:, 0] = 1.0
-            uncond[region_key(n)] = plain.to(device)
+            if negative_region_prompts is None:
+                plain = torch.zeros_like(w)
+                plain[:, 0] = 1.0
+                uncond[region_key(n)] = plain.to(device)
+            else:
+                uncond[region_key(n)] = region_chunk_weights(color_map_image, negative_region_prompts,
+                                                             region_base_ratio, r, layout).to(device)
+        cond[REGION_SENTENCES_KEY] = cond_bits
+        uncond[REGION_SENTENCES_KEY] = un_bits
 
     if chunks > 1:
         cond["CONTEXT_TENSOR"] = _encode_chunked(text_encoder, text_input["input_ids"], device)
-        width = tokenizer.model_max_length - 2
-        un_ids = list(tokenizer(unconditional_input_prompt)["input_ids"])[1:-1]
-        un_windows = _prompt_windows(un_ids, [], chunks, width)
-        uncond["CONTEXT_TENSOR"] = _encode_chunked(text_encoder, _chunked_ids(tokenizer, un_windows, chunks), device)
+        if un_ids is None:
+            width = tokenizer.model_max_length - 2
+            un_tokens = list(tokenizer(unconditional_input_prompt)["input_ids"])[1:-1]
+            un_ids = _chunked_ids(tokenizer, _prompt_windows(un_tokens, [], chunks, width), chunks)
+        uncond["CONTEXT_TENSOR"] = _encode_chunked(text_encoder, un_ids, device)
         return extra_seeds, seperated_word_contexts, cond, uncond
     cond["CONTEXT_TENSOR"] = text_encoder(text_input.input_ids.to(device))[0]
     uncond_input = tokenizer([unconditional_input_prompt], padding="max_length",

@@ -265,10 +265,11 @@ int xattn_fused(const void* q, const void* k, const void* v, void* out, int B, i
       r.rec_index += b0;
     }
     pww::fx::FxRegion g;
-    if (rg) {                                                      // weights through wmap_index, else row b
+    if (rg) {                                                      // weights through rw_index, else row b
       g = *rg;
       if (g.rw_index) g.rw_index += b0;
       else g.rw += (int64_t)b0 * g.rw_bs;
+      if (g.stat_chunks) g.stat_chunks += b0;
     }
     const cudaError_t e = with_shape(D, T, [&](auto k) {
       return pww::fx::launch_fused2<k.D, k.KC>(c, mp, mpack_batch_stride, ci, (cudaStream_t)stream, rec ? &r : nullptr,
@@ -626,6 +627,51 @@ int pww_xattn_fused_region_multi_bf16(const void* q, const void* k, const void* 
     const int8_t* cidx, const int32_t* wmap_index, const int32_t* stat, const float* g_sigma, float scale, float* stats,
     void* workspace, size_t workspace_bytes, void* stream, const float* region_weights, int64_t region_batch_stride) {
   const pww::fx::FxRegion rg = {region_weights, region_batch_stride, wmap_index};
+  return xattn_fused<__nv_bfloat16>(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride,
+      k_row_stride, o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, PWW_STAT_MAX, stat,
+      true, g_sigma, scale, stats, workspace, workspace_bytes, stream, nullptr, &rg);
+}
+
+int pww_xattn_fused_region_rows_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N, int T,
+    int D, int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
+    int64_t o_batch_stride, int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw,
+    const int8_t* cidx, const int32_t* wmap_index, int stat, const float* g_sigma, float scale, float* stats,
+    void* workspace, size_t workspace_bytes, void* stream, const float* region_weights, int64_t region_batch_stride,
+    const int32_t* region_index, const int32_t* stat_chunks) {
+  const pww::fx::FxRegion rg = {region_weights, region_batch_stride, region_index, stat_chunks};
+  return xattn_fused<__half>(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+      o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, stat, nullptr, false,
+      g_sigma, scale, stats, workspace, workspace_bytes, stream, nullptr, &rg);
+}
+int pww_xattn_fused_region_rows_bf16(const void* q, const void* k, const void* v, void* out, int B, int H, int N,
+    int T, int D, int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
+    int64_t o_batch_stride, int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw,
+    const int8_t* cidx, const int32_t* wmap_index, int stat, const float* g_sigma, float scale, float* stats,
+    void* workspace, size_t workspace_bytes, void* stream, const float* region_weights, int64_t region_batch_stride,
+    const int32_t* region_index, const int32_t* stat_chunks) {
+  const pww::fx::FxRegion rg = {region_weights, region_batch_stride, region_index, stat_chunks};
+  return xattn_fused<__nv_bfloat16>(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride,
+      k_row_stride, o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, stat, nullptr, false,
+      g_sigma, scale, stats, workspace, workspace_bytes, stream, nullptr, &rg);
+}
+int pww_xattn_fused_region_rows_multi_f16(const void* q, const void* k, const void* v, void* out, int B, int H, int N,
+    int T, int D, int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
+    int64_t o_batch_stride, int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw,
+    const int8_t* cidx, const int32_t* wmap_index, const int32_t* stat, const float* g_sigma, float scale, float* stats,
+    void* workspace, size_t workspace_bytes, void* stream, const float* region_weights, int64_t region_batch_stride,
+    const int32_t* region_index, const int32_t* stat_chunks) {
+  const pww::fx::FxRegion rg = {region_weights, region_batch_stride, region_index, stat_chunks};
+  return xattn_fused<__half>(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride, k_row_stride,
+      o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, PWW_STAT_MAX, stat, true,
+      g_sigma, scale, stats, workspace, workspace_bytes, stream, nullptr, &rg);
+}
+int pww_xattn_fused_region_rows_multi_bf16(const void* q, const void* k, const void* v, void* out, int B, int H, int N,
+    int T, int D, int64_t q_batch_stride, int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride,
+    int64_t o_batch_stride, int64_t o_row_stride, const void* mpack, int64_t mpack_batch_stride, int Bw,
+    const int8_t* cidx, const int32_t* wmap_index, const int32_t* stat, const float* g_sigma, float scale, float* stats,
+    void* workspace, size_t workspace_bytes, void* stream, const float* region_weights, int64_t region_batch_stride,
+    const int32_t* region_index, const int32_t* stat_chunks) {
+  const pww::fx::FxRegion rg = {region_weights, region_batch_stride, region_index, stat_chunks};
   return xattn_fused<__nv_bfloat16>(q, k, v, out, B, H, N, T, D, q_batch_stride, q_row_stride, k_batch_stride,
       k_row_stride, o_batch_stride, o_row_stride, mpack, mpack_batch_stride, Bw, cidx, wmap_index, PWW_STAT_MAX, stat,
       true, g_sigma, scale, stats, workspace, workspace_bytes, stream, nullptr, &rg);

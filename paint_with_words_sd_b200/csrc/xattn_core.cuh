@@ -127,11 +127,11 @@ __device__ __forceinline__ void load_operands(uint32_t st, const XattnParams<E>&
     if (with_v) load_rows<D>(st + C::QBYTES + (KC + c) * C::KBYTES, p.v + off, p.k_rs, kTP, kv);
   }
 }
-// The same copies with K and V of the chunks in `chunks` (bit c = chunk c) only: a region-prompt job (with_v) skips
-// the chunks no row of its tile weighs.
+// The same copies with K (and V) of the chunks in `chunks` (bit c = chunk c) only: a region-prompt softmax job skips
+// the chunks no row of its tile weighs, and a statistic job the chunks outside its image's statistic.
 template <int D, int KC, typename E>
 __device__ __forceinline__ void load_operands_of(uint32_t st, const XattnParams<E>& p, int b, int h, int tile,
-                                                 unsigned chunks) {
+                                                 unsigned chunks, bool with_v) {
   using C = Tile<D>;
   const int rows = p.N - tile * kBM;
   load_rows<D>(st, p.q + (int64_t)b * p.q_bs + (int64_t)tile * kBM * p.q_rs + h * D, p.q_rs, kBM, rows < kBM ? rows : kBM);
@@ -140,7 +140,7 @@ __device__ __forceinline__ void load_operands_of(uint32_t st, const XattnParams<
     if (!((chunks >> c) & 1u)) continue;
     const int64_t off = (int64_t)b * p.k_bs + (int64_t)c * kChunk * p.k_rs + h * D;
     load_rows<D>(st + C::QBYTES + c * C::KBYTES, p.k + off, p.k_rs, kTP, kChunk);
-    load_rows<D>(st + C::QBYTES + (KC + c) * C::KBYTES, p.v + off, p.k_rs, kTP, kChunk);
+    if (with_v) load_rows<D>(st + C::QBYTES + (KC + c) * C::KBYTES, p.v + off, p.k_rs, kTP, kChunk);
   }
 }
 
@@ -368,11 +368,12 @@ __device__ __forceinline__ void warp_reduce_stat(double& m, double& a, double& q
   }
 }
 
-// The statistic of an image from its totals over all H * N * T scores: the maximum, or the unbiased standard deviation
-// (variance clamped at 0), rounded to E as qk.max() / qk.std() return it in the reference's op sequence under an E autocast.
+// The statistic of an image from its totals over its H * N * keys scores (keys = T, or 77 per chunk of a region-prompt
+// image's statistic): the maximum, or the unbiased standard deviation (variance clamped at 0), rounded to E as
+// qk.max() / qk.std() return it in the reference's op sequence under an E autocast.
 template <typename E>
-__device__ __forceinline__ float stat_value(const XattnParams<E>& p, bool is_max, double m, double a, double q) {
-  const double cnt = (double)p.H * (double)p.N * (double)p.T;
+__device__ __forceinline__ float stat_value(const XattnParams<E>& p, bool is_max, double m, double a, double q, int keys) {
+  const double cnt = (double)p.H * (double)p.N * (double)keys;
   double r;
   if (is_max) {
     r = m;

@@ -36,8 +36,9 @@
 // the kernel without it: every recording instruction is behind `if constexpr`.
 //
 // Region prompts (RGN = true, FxRegion, KC = 2, 3): one softmax per key chunk, mixed per query row by fp32 chunk
-// weights (xattn_core.cuh: warp_weighted_chunk); the chunks no row of a tile weighs are not copied.  Every region
-// instruction is behind `if constexpr` as well.
+// weights (xattn_core.cuh: warp_weighted_chunk); the chunks no row of a tile weighs are not copied, and a biased
+// image's statistic jobs skip the chunks outside its statistic mask.  Every region instruction is behind
+// `if constexpr` as well.
 #pragma once
 #include <algorithm>
 #include <type_traits>
@@ -83,12 +84,16 @@ struct FxRecParams : FxParams<E> {
 // Region prompts (the RGN instances, KC = 2, 3): chunk c of image b's context gets its own softmax over its 77 keys,
 // and query row n takes  out(n) = sum_c w_c(n) softmax_c(..) V_c  (xattn_core.cuh: warp_weighted_chunk).  The weights
 // of image b are row rw_index[b] (row b when rw_index is NULL) of rw; an image with index -1 takes (1, 0, ..) on every
-// row.  The K / V of a chunk that no row of a softmax job's tile weighs are neither copied nor multiplied; the
-// statistic jobs still see every chunk, so the statistic is the one over all H * N * 77 KC scores.
+// row.  The K / V of a chunk that no row of a softmax job's tile weighs are neither copied nor multiplied.  The weight
+// row is independent of the bias: an unbiased image with a row runs the same mixed softmax with no bias, and a biased
+// image with -1 takes its first chunk alone with the bias.  A biased image's statistic covers the chunks of its mask
+// stat_chunks[b] (chunk 0 always; the other chunks' K is not even copied for it): its max, or its std over the
+// H * N * 77 * popcount(mask) scores; with stat_chunks NULL every chunk, all H * N * 77 KC scores.
 struct FxRegion {
-  const float* rw;          // [Bw, N, KC] fp32 chunk weights
-  int64_t rw_bs;            // elements between weight rows (>= N * KC)
-  const int32_t* rw_index;  // [B] weight row of image b, -1 = none; NULL = row b
+  const float* rw;              // [Bw, N, KC] fp32 chunk weights
+  int64_t rw_bs;                // elements between weight rows (>= N * KC)
+  const int32_t* rw_index;      // [B] weight row of image b, -1 = none; NULL = row b
+  const int32_t* stat_chunks;   // [B] bit c = chunk c is in image b's statistic; NULL = every chunk
 };
 template <typename E>
 struct FxRgnParams : FxParams<E> {
@@ -452,14 +457,20 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
     return rgs.bits;
     }
   };
+  // RGN: the chunks of image b's statistic (bit c = chunk c; chunk 0 always)
+  [[maybe_unused]] auto stat_chunks = [&](int b) -> unsigned {
+    constexpr unsigned all = (1u << KC) - 1u;
+    if constexpr (!RGN) return all;
+    else return fp.rg.stat_chunks != nullptr ? ((unsigned)__ldg(fp.rg.stat_chunks + b) | 1u) & all : all;
+  };
   auto issue = [&](int i) {
     const uint2 r = s_jobs[i];
     const int b = r.x & 0xff, h = (r.x >> 8) & 0xff, tile = r.x >> 16;
     const bool is_main = (r.y & JF_MAIN) != 0, biased = (r.y & JF_BIASED) != 0;
     const uint32_t st = smem0 + stage(i);
     if constexpr (RGN) {
-      if (is_main) core::load_operands_of<D, KC>(st, p, b, h, tile, region_chunks(i, b, tile));
-      else core::load_operands<D, KC>(st, p, b, h, tile, false);
+      if (is_main) core::load_operands_of<D, KC>(st, p, b, h, tile, region_chunks(i, b, tile), true);
+      else core::load_operands_of<D, KC>(st, p, b, h, tile, stat_chunks(b), false);
     } else {
       core::load_operands<D, KC>(st, p, b, h, tile, is_main);
     }
@@ -569,7 +580,8 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
             core::warp_reduce_stat(m, a, q);
           }
           if (lane == 0) {
-            const float stv = core::stat_value(p, is_max, m, a, q);
+            const int keys = RGN ? core::kChunk * __popc(stat_chunks(bl)) : p.T;
+            const float stv = core::stat_value(p, is_max, m, a, q, keys);
             s_coef[l] = (p.g_sigma != nullptr ? image_g(p, bl) : 0.f) * stv;
             if (p.stats_out != nullptr) p.stats_out[bl] = stv;   // every CTA of the image writes the same value
           }
@@ -590,8 +602,12 @@ __global__ void __launch_bounds__(core::kThreads, 1) xattn_fused2_kernel(const F
     if (!is_main) {
       if (li != cur_li) { flush(); cur_li = li; }
       float sum = 0.f, sumsq = 0.f;
+      [[maybe_unused]] const unsigned sc = stat_chunks(b);
 #pragma unroll 1
-      for (int c = 0; c < KC; ++c) {                // the real tokens of every chunk
+      for (int c = 0; c < KC; ++c) {                // the real tokens of every chunk (RGN: of the image's statistic)
+        if constexpr (RGN) {
+          if (!((sc >> c) & 1u)) continue;
+        }
         float s[10][4];
         core::warp_qk<D, E>(qs, st + C::QBYTES + c * C::KBYTES, lane, s);
         core::warp_stat<E>(s, kv, p.N - row0, lane, s_ismax[li], vmax, sum, sumsq);

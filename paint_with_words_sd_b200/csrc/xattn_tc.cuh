@@ -356,7 +356,7 @@ __global__ void __launch_bounds__(kThreads, 1) xattn_stats_kernel(const TcParams
       }
     }
     core::warp_reduce_stat(m, a, q);
-    if (lane == 0) p.stats_out[b] = core::stat_value(p, s_ismax[b], m, a, q);
+    if (lane == 0) p.stats_out[b] = core::stat_value(p, s_ismax[b], m, a, q, p.T);
   }
   if (threadIdx.x == 0) p.counters[0] = 0u;
 }

@@ -27,9 +27,10 @@ import torch.nn.functional as F
 from PIL import Image
 
 from . import attention as _attention
-from .conditioning import (MAX_RECORDED_REGIONS, RATIOS, REGION_COUNT_KEY, REGION_INDEX_KEY,
-                           _encode_text_color_inputs, _extract_seed_and_sigma_from_context, _get_binary_mask,
-                           _rgb_of, always_round, check_region_prompts, pack_weight_map, packed_key)
+from .conditioning import (MAX_RECORDED_REGIONS, RATIOS, REGION_COUNT_KEY, REGION_INDEX_KEY, REGION_ROWS_KEY,
+                           REGION_SENTENCES_KEY, STAT_CHUNKS_KEY, _encode_text_color_inputs,
+                           _extract_seed_and_sigma_from_context, _get_binary_mask, _rgb_of, always_round,
+                           check_negative_region_prompts, check_region_prompts, pack_weight_map, packed_key)
 from . import _native, fused_ops
 from .scheduler import (FORM_COLUMNS, SIGMA_SCHEDULERS, EulerAncestralDiscreteScheduler, LMSDiscreteScheduler,
                         history_length, step_form)
@@ -607,7 +608,10 @@ class PwWSampler:
         statistic of every image (uncond images: max, ignored).  Region prompts: REGION_WEIGHTS_{N} -> [m, N, k] stacks
         (every cond dict has them or none does), reached through WMAP_INDEX, which then keeps row i for an image whose
         weight function is zero (its G(sigma) is 0, so its bias is exactly 0); the uncond images' -1 gives them the
-        first chunk alone.  The m images are the first len(conds) of the
+        first chunk alone.  Negative region prompts (some uncond dict has sentences of its own): REGION_WEIGHTS_{N} ->
+        [2m, N, k] stacks of the cond then the uncond weights, reached through REGION_ROWS (row i of a side with
+        sentences, -1 for a side without), so WMAP_INDEX keeps -1 for a zero weight function; REGION_STAT_CHUNKS =
+        chunk 0 and the cond image's own sentences.  The m images are the first len(conds) of the
         sampler's (all of them here; a panorama chunk's windows in PanoramaSampler)."""
         m = len(conds)
         probed = self._probed[:m]
@@ -638,10 +642,18 @@ class PwWSampler:
         region_keys = [k for k in conds[0] if k.startswith("REGION_WEIGHTS_")]
         if any(sorted(k for k in c if k.startswith("REGION_WEIGHTS_")) != sorted(region_keys) for c in conds):
             raise ValueError("the images of one sampler either all have region prompts or none has")
+        negative = bool(region_keys) and any(u.get(REGION_SENTENCES_KEY, 0) for u in unconds)
+        sides = list(conds) + list(unconds) if negative else conds
         for key in region_keys:
-            ctx[key] = torch.stack([c[key].to(self.device, torch.float32) for c in conds], 0).contiguous()
-        ctx["WMAP_INDEX"] = torch.tensor([-1 if pr.is_zero and not region_keys else i for i, pr in enumerate(probed)] +
-                                         [-1] * m, dtype=torch.int32, device=self.device)
+            ctx[key] = torch.stack([c[key].to(self.device, torch.float32) for c in sides], 0).contiguous()
+        if negative:
+            ctx[REGION_ROWS_KEY] = torch.tensor([i if c.get(REGION_SENTENCES_KEY, 0) else -1 for i, c in enumerate(sides)],
+                                                dtype=torch.int32, device=self.device)
+            ctx[STAT_CHUNKS_KEY] = torch.tensor([1 | c.get(REGION_SENTENCES_KEY, 0) for c in conds] + [1] * m,
+                                                dtype=torch.int32, device=self.device)
+        ctx["WMAP_INDEX"] = torch.tensor([-1 if pr.is_zero and (negative or not region_keys) else i
+                                          for i, pr in enumerate(probed)] + [-1] * m,
+                                         dtype=torch.int32, device=self.device)
         ctx["STAT_KIND"] = torch.tensor([STAT_MAX if pr.is_zero else pr.stat for pr in probed] + [STAT_MAX] * m,
                                         dtype=torch.int32, device=self.device)
         ctx["WEIGHT_FUNCTION"] = self.weight_function
@@ -858,6 +870,7 @@ def paint_with_words(
     mask_image: Optional[Image.Image] = None,
     region_prompts: Optional[Dict] = None,
     region_base_ratio: float = 0.2,
+    negative_region_prompts: Optional[Dict] = None,
 ):
     """paint_with_words.py:391-510.  Returns one PIL.Image (or the final latents with return_latents).
     `max_prompt_chunks` (1 .. 3): a prompt longer than 75 tokens fills up to that many 77-token CLIP chunks instead of
@@ -883,8 +896,13 @@ def paint_with_words(
     of its own, attended with its own softmax and mixed per pixel with the base prompt, which keeps a share of
     `region_base_ratio` (0..1) inside the region (README, Region prompts).  `input_prompt` and each sentence must fit
     one 75-token window; not with max_prompt_chunks > 1, attention maps or colour-map sides that are not multiples of
-    64."""
-    _check_region_call(region_prompts, region_base_ratio, max_prompt_chunks, return_attention_maps)
+    64.
+    `negative_region_prompts` ({colour: sentence}): the same on the negative (uncond) side, so a sentence guides only
+    its region away from itself ("trees" in the blue region's entry: no trees there).  With region_prompts at most 2
+    colours in all; `unconditional_input_prompt` must then fit one 75-token window (README, Negative region
+    prompts)."""
+    _check_region_call(region_prompts, region_base_ratio, max_prompt_chunks, return_attention_maps,
+                       negative_region_prompts)
     if mask_image is not None and init_image is None:
         raise ValueError("mask_image needs an init_image: masked img2img repaints the masked area of the init image")
     control = _control_arguments(controlnet, control_image, color_map_image.size, "color_map_image",
@@ -898,12 +916,13 @@ def paint_with_words(
     if init_image is None:
         cond, uncond, latents = _txt2img_inputs(tools, device, color_map_image, color_context, input_prompt,
                                                 unconditional_input_prompt, seed, max_prompt_chunks, region_prompts,
-                                                region_base_ratio)
+                                                region_base_ratio, negative_region_prompts)
         timesteps = scheduler.timesteps
     else:
         _, _, cond, uncond = _encode_text_color_inputs(
             text_encoder, tokenizer, device, color_map_image, color_context, input_prompt, unconditional_input_prompt,
-            max_prompt_chunks=max_prompt_chunks, region_prompts=region_prompts, region_base_ratio=region_base_ratio)
+            max_prompt_chunks=max_prompt_chunks, region_prompts=region_prompts, region_base_ratio=region_base_ratio,
+            negative_region_prompts=negative_region_prompts)
         # the reference draws img2img's noise from the global RNG as it stands: unseeded here
         latents, timesteps, init, noise = _img2img_latents(vae, scheduler, init_image, num_inference_steps, strength,
                                                            device)
@@ -928,24 +947,30 @@ def _tools(preloaded_utils, device, scheduler_type, local_model_path, hf_model_p
                           model_token=model_token, torch_dtype=torch_dtype, prediction_type=prediction_type)
 
 
-def _check_region_call(region_prompts, region_base_ratio, max_prompt_chunks, return_attention_maps) -> None:
-    """The ValueErrors of a public call with region prompts that need no model."""
-    if region_prompts is None:
+def _check_region_call(region_prompts, region_base_ratio, max_prompt_chunks, return_attention_maps,
+                       negative_region_prompts=None) -> None:
+    """The ValueErrors of a public call with region or negative region prompts that need no model."""
+    if negative_region_prompts is not None:
+        check_negative_region_prompts(region_prompts, negative_region_prompts, region_base_ratio, max_prompt_chunks)
+    elif region_prompts is not None:
+        check_region_prompts(region_prompts, region_base_ratio, max_prompt_chunks)
+    else:
         return
-    check_region_prompts(region_prompts, region_base_ratio, max_prompt_chunks)
     if return_attention_maps:
         raise ValueError("attention recording does not combine with region prompts")
 
 
 def _txt2img_inputs(tools, device, color_map_image, color_context, input_prompt, unconditional_input_prompt, seed,
-                    max_prompt_chunks, region_prompts=None, region_base_ratio=0.2) -> Tuple[dict, dict, torch.Tensor]:
+                    max_prompt_chunks, region_prompts=None, region_base_ratio=0.2,
+                    negative_region_prompts=None) -> Tuple[dict, dict, torch.Tensor]:
     """One txt2img image's (cond, uncond, latents): its text and colour contexts, and its seeded initial noise scaled
     by the scheduler's initial sigma (so `scheduler.set_timesteps` comes first)."""
     _, unet, text_encoder, tokenizer, scheduler = tools
     width, height = color_map_image.size
     extra_seeds, seperated_word_contexts, cond, uncond = _encode_text_color_inputs(
         text_encoder, tokenizer, device, color_map_image, color_context, input_prompt, unconditional_input_prompt,
-        max_prompt_chunks=max_prompt_chunks, region_prompts=region_prompts, region_base_ratio=region_base_ratio)
+        max_prompt_chunks=max_prompt_chunks, region_prompts=region_prompts, region_base_ratio=region_base_ratio,
+        negative_region_prompts=negative_region_prompts)
     latents = initial_latents((1, unet.in_channels, height // 8, width // 8), seed, extra_seeds,
                               seperated_word_contexts).to(device)
     return cond, uncond, latents * scheduler.init_noise_sigma
@@ -1051,7 +1076,8 @@ def _control_arguments(controlnet, control_image, size: Tuple[int, int], size_of
 # the per-image keyword arguments of paint_with_words that paint_with_words_batch takes per entry
 BATCH_SETTING_KEYS = ("color_context", "color_map_image", "input_prompt", "unconditional_input_prompt", "seed",
                       "weight_function", "guidance_scale", "max_prompt_chunks", "control_image",
-                      "controlnet_conditioning_scale", "guidance_rescale", "region_prompts", "region_base_ratio")
+                      "controlnet_conditioning_scale", "guidance_rescale", "region_prompts", "region_base_ratio",
+                      "negative_region_prompts")
 
 
 def _batch_settings(settings) -> List[dict]:
@@ -1071,11 +1097,17 @@ def _batch_settings(settings) -> List[dict]:
         if full["color_map_image"] is None:
             raise ValueError(f"settings[{i}]: color_map_image is required")
         try:
-            _check_region_call(full["region_prompts"], full["region_base_ratio"], full["max_prompt_chunks"], False)
+            _check_region_call(full["region_prompts"], full["region_base_ratio"], full["max_prompt_chunks"], False,
+                               full["negative_region_prompts"])
         except ValueError as err:
             raise ValueError(f"settings[{i}]: {err}") from err
         out.append(full)
     return out
+
+
+def _has_region_sentence(entry: dict) -> bool:
+    """Does a batch entry give a region a sentence, on the cond or on the uncond side?"""
+    return entry["region_prompts"] is not None or entry["negative_region_prompts"] is not None
 
 
 def batch_groups(keys: Sequence, max_batch_size: int) -> List[List[int]]:
@@ -1111,9 +1143,10 @@ def paint_with_words_batch(
     """Many images, each with its own settings, in as few samplers as possible.  `settings[i]` is a dict of the
     per-image keyword arguments of `paint_with_words` (BATCH_SETTING_KEYS: color_context, color_map_image, input_prompt,
     unconditional_input_prompt, seed, weight_function, guidance_scale, max_prompt_chunks, control_image,
-    controlnet_conditioning_scale, guidance_rescale, region_prompts, region_base_ratio); missing keys take
-    paint_with_words's defaults.  Entries with region prompts share a sampler only with each other.  Returns a list of
-    PIL images (or [1,4,h,w] latents) in input order; image i equals `paint_with_words(**settings[i])` up to fp16 noise.
+    controlnet_conditioning_scale, guidance_rescale, region_prompts, region_base_ratio, negative_region_prompts);
+    missing keys take paint_with_words's defaults.  Entries with a region sentence (on either side) share a sampler
+    only with each other.  Returns a list of PIL images (or [1,4,h,w] latents) in input order; image i equals
+    `paint_with_words(**settings[i])` up to fp16 noise.
     With `controlnet` (one for the batch, with `guess_mode` and the guidance window) every entry needs a
     `control_image` of its colour map's size; its `controlnet_conditioning_scale` is its own.  With a list of
     ControlNets (`guess_mode` and the window each one value or one per ControlNet), an entry's `control_image` is a list
@@ -1129,7 +1162,7 @@ def paint_with_words_batch(
     entries = _batch_settings(settings)
     if max_batch_size < 1:
         raise ValueError("max_batch_size must be >= 1")
-    if return_attention_maps and any(e["region_prompts"] is not None for e in entries):
+    if return_attention_maps and any(_has_region_sentence(e) for e in entries):
         raise ValueError("attention recording does not combine with region prompts")
     controls = []
     for i, e in enumerate(entries):
@@ -1147,13 +1180,15 @@ def paint_with_words_batch(
     for e in entries:
         cond, uncond, latents = _txt2img_inputs(tools, device, e["color_map_image"], dict(e["color_context"]),
                                                 e["input_prompt"], e["unconditional_input_prompt"], e["seed"],
-                                                e["max_prompt_chunks"], e["region_prompts"], e["region_base_ratio"])
+                                                e["max_prompt_chunks"], e["region_prompts"], e["region_base_ratio"],
+                                                e["negative_region_prompts"])
         encoded.append((cond, uncond, latents))
         width, height = e["color_map_image"].size
         solo = width % 64 != 0 or height % 64 != 0
-        # region-prompt entries share a sampler with each other only: their chunks are softmaxed one by one
+        # entries with a region sentence on either side share a sampler with each other only: their chunks are
+        # softmaxed one by one
         keys.append(None if solo else (height // 8, width // 8, int(cond["CONTEXT_TENSOR"].shape[1]),
-                                       e["region_prompts"] is not None))
+                                       _has_region_sentence(e)))
     results: List[Optional[torch.Tensor]] = [None] * len(entries)
     attention: List[Optional[RegionAttention]] = [None] * len(entries)
     for idx in batch_groups(keys, max_batch_size):
@@ -1242,14 +1277,16 @@ def paint_with_words_inpaint(
     prediction_type: Optional[str] = None,
     region_prompts: Optional[Dict] = None,
     region_base_ratio: float = 0.2,
+    negative_region_prompts: Optional[Dict] = None,
 ):
     """paint_with_words_inpaint.py:137-270: 9-channel UNet input cat[latents, mask, masked-image latents].
     `max_prompt_chunks`, `torch_dtype` and the ControlNet arguments as in `paint_with_words`; the colour map is resized
     to the init image, so `control_image` has the init image's size.  The ControlNet sees the 4 latent channels of
     the UNet input (hook_pww.py:113-119).  `return_attention_maps` as in `paint_with_words` (coverage from the resized
-    colour map).  `guidance_rescale`, `prediction_type`, `region_prompts` and `region_base_ratio` as in
-    `paint_with_words` (the colour-map size checked is the init image's)."""
-    _check_region_call(region_prompts, region_base_ratio, max_prompt_chunks, return_attention_maps)
+    colour map).  `guidance_rescale`, `prediction_type`, `region_prompts`, `region_base_ratio` and
+    `negative_region_prompts` as in `paint_with_words` (the colour-map size checked is the init image's)."""
+    _check_region_call(region_prompts, region_base_ratio, max_prompt_chunks, return_attention_maps,
+                       negative_region_prompts)
     width, height = init_image.size
     control = _control_arguments(controlnet, control_image, (width, height), "init_image (and resized color_map_image)",
                                  controlnet_conditioning_scale, guess_mode, control_guidance_start,
@@ -1260,7 +1297,8 @@ def paint_with_words_inpaint(
     mask_image = mask_image.resize((width, height), Image.NEAREST)
     _, _, cond, uncond = _encode_text_color_inputs(
         text_encoder, tokenizer, device, color_map_image, color_context, input_prompt, unconditional_input_prompt,
-        max_prompt_chunks=max_prompt_chunks, region_prompts=region_prompts, region_base_ratio=region_base_ratio)
+        max_prompt_chunks=max_prompt_chunks, region_prompts=region_prompts, region_base_ratio=region_base_ratio,
+        negative_region_prompts=negative_region_prompts)
     mask, masked_image = prepare_mask_and_masked_image(init_image, mask_image)
 
     scheduler.set_timesteps(num_inference_steps)
@@ -1362,11 +1400,14 @@ class PaintWithWord_StableDiffusionPipeline:
                  output_type: str = "pil", return_dict: bool = True, callback=None, callback_steps: int = 1,
                  max_prompt_chunks: int = 1, control_image=None, controlnet_conditioning_scale: float = 1.0,
                  guess_mode: bool = False, control_guidance_start: float = 0.0, control_guidance_end: float = 1.0,
-                 guidance_rescale: float = 0.0, mask_image=None, region_prompts=None, region_base_ratio: float = 0.2):
-        """`mask_image` with `image`: masked img2img; `region_prompts` / `region_base_ratio` (see `paint_with_words`)."""
+                 guidance_rescale: float = 0.0, mask_image=None, region_prompts=None, region_base_ratio: float = 0.2,
+                 negative_region_prompts=None):
+        """`mask_image` with `image`: masked img2img; `region_prompts` / `region_base_ratio` /
+        `negative_region_prompts` (see `paint_with_words`)."""
         extra = {} if image is None else {"init_image": image, "strength": eta}
         extra["mask_image"] = mask_image
         extra["region_prompts"], extra["region_base_ratio"] = region_prompts, region_base_ratio
+        extra["negative_region_prompts"] = negative_region_prompts
         extra["max_prompt_chunks"] = max_prompt_chunks
         extra["guidance_rescale"] = guidance_rescale
         extra.update(self._control(control_image, controlnet_conditioning_scale, guess_mode, control_guidance_start,
@@ -1394,11 +1435,13 @@ class PaintWithWord_StableDiffusionInpaintPipeline(PaintWithWord_StableDiffusion
                  output_type: str = "pil", return_dict: bool = True, callback=None, callback_steps: int = 1,
                  max_prompt_chunks: int = 1, control_image=None, controlnet_conditioning_scale: float = 1.0,
                  guess_mode: bool = False, control_guidance_start: float = 0.0, control_guidance_end: float = 1.0,
-                 guidance_rescale: float = 0.0, region_prompts=None, region_base_ratio: float = 0.2):
+                 guidance_rescale: float = 0.0, region_prompts=None, region_base_ratio: float = 0.2,
+                 negative_region_prompts=None):
         return self._run(paint_with_words_inpaint, prompt, color_map_image, dict(color_context), weight_function,
                          num_inference_steps, guidance_scale, negative_prompt, seed, output_type, return_dict, callback,
                          callback_steps, mask_image=mask_image, init_image=image, strength=eta,
                          max_prompt_chunks=max_prompt_chunks, guidance_rescale=guidance_rescale,
                          region_prompts=region_prompts, region_base_ratio=region_base_ratio,
+                         negative_region_prompts=negative_region_prompts,
                          **self._control(control_image, controlnet_conditioning_scale, guess_mode,
                                          control_guidance_start, control_guidance_end))

@@ -72,6 +72,37 @@ void with_int(int v, F&& f) {
 
 size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// f(T{}) for the element type T of a PWW_DTYPE_* code the caller has checked: fp16, bf16, else fp32.
+template <typename F>
+cudaError_t with_dtype(int dtype, F&& f) {
+  if (dtype == PWW_DTYPE_F16) return f(__half{});
+  if (dtype == PWW_DTYPE_BF16) return f(__nv_bfloat16{});
+  return f(float{});
+}
+
+// The pww_sampler_update* entry points' shared part: the argument checks (every PWW_ERR_BAD_ARG before the dtype's
+// PWW_ERR_UNSUPPORTED, and none of them a CUDA call), the UpdateArgs and the layout.  PX = 4 needs h w % 4 == 0 and
+// 16-byte aligned latents, history and noise, and `px4_extra` (the caller's own inputs read 4 pixels at a time).
+int update_setup(const void* eps, int eps_dtype, int64_t e_sn, int64_t e_sc, int64_t e_sh, int64_t e_sw,
+                 float* latents, float* history, int history_len, const float* noise, const float* guidance,
+                 const float* beta, const float* form, int m, int height, int width, bool px4_extra,
+                 pww::smp::UpdateArgs& a, bool& px4, bool& cl) {
+  if (!eps || !latents || !history || !guidance || !beta || !form) return PWW_ERR_BAD_ARG;
+  if (m <= 0 || height <= 0 || width <= 0 || history_len < 1 || history_len > 4) return PWW_ERR_BAD_ARG;
+  if (eps_dtype != PWW_DTYPE_F32 && eps_dtype != PWW_DTYPE_F16 && eps_dtype != PWW_DTYPE_BF16) return PWW_ERR_UNSUPPORTED;
+  a.eps = eps; a.e_sn = e_sn; a.e_sc = e_sc; a.e_sh = e_sh; a.e_sw = e_sw;
+  a.lat = latents; a.hist = history; a.noise = noise; a.gscale = guidance; a.beta = beta; a.form = form;
+  a.m = m; a.h = height; a.w = width; a.nh = history_len;
+  const int64_t hw = (int64_t)height * width;
+  const size_t es = eps_dtype == PWW_DTYPE_F32 ? 4 : 2;
+  px4 = (hw % 4) == 0 && aligned16(latents) && aligned16(history) && (!noise || aligned16(noise)) && px4_extra;
+  // channels-last packed rows: pixel p's 4 channels at 4p (8 bytes per pixel in fp16 / bf16, 16 in fp32)
+  const size_t need = px4 ? 16 : 4 * es;
+  cl = e_sc == 1 && e_sw == 4 && e_sh == 4 * (int64_t)width && (reinterpret_cast<uintptr_t>(eps) % need) == 0 &&
+       ((size_t)e_sn * es) % need == 0;
+  return PWW_OK;
+}
+
 // Partial slots the statistics workspace reserves per image: one per CTA of the persistent grid, a device-independent
 // upper bound so that the size can be computed without a GPU.
 constexpr int kStatSlotsPerImage = 2048;
@@ -755,10 +786,9 @@ int pww_sampler_input(const float* latents, const float* scale, const float* ext
   pww::smp::InputArgs a;
   a.lat = latents; a.scale = scale; a.extra = extra; a.out = out; a.m = m; a.C = channels; a.hw = height * width;
   const bool px4 = (a.hw % 4) == 0 && aligned16(latents) && (!extra || aligned16(extra)) && aligned16(out);
-  cudaStream_t s = (cudaStream_t)stream;
-  const cudaError_t e = out_dtype == PWW_DTYPE_F16    ? pww::smp::launch_input<__half>(a, px4, s)
-                        : out_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_input<__nv_bfloat16>(a, px4, s)
-                                                      : pww::smp::launch_input<float>(a, px4, s);
+  const cudaError_t e = with_dtype(out_dtype, [&](auto t) {
+    return pww::smp::launch_input<decltype(t)>(a, px4, (cudaStream_t)stream);
+  });
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 
@@ -766,25 +796,15 @@ int pww_sampler_update(const void* eps, int eps_dtype, int64_t eps_batch_stride,
                        int64_t eps_row_stride, int64_t eps_col_stride, float* latents, float* history, int history_len,
                        const float* noise, const float* guidance, const float* beta, const float* form, int m,
                        int height, int width, void* stream) {
-  if (!eps || !latents || !history || !guidance || !beta || !form) return PWW_ERR_BAD_ARG;
-  if (m <= 0 || height <= 0 || width <= 0 || history_len < 1 || history_len > 4) return PWW_ERR_BAD_ARG;
-  if (eps_dtype != PWW_DTYPE_F32 && eps_dtype != PWW_DTYPE_F16 && eps_dtype != PWW_DTYPE_BF16) return PWW_ERR_UNSUPPORTED;
   pww::smp::UpdateArgs a;
-  a.eps = eps; a.e_sn = eps_batch_stride; a.e_sc = eps_channel_stride; a.e_sh = eps_row_stride; a.e_sw = eps_col_stride;
-  a.lat = latents; a.hist = history; a.noise = noise; a.gscale = guidance; a.beta = beta; a.form = form;
-  a.m = m; a.h = height; a.w = width; a.nh = history_len;
-  const int64_t hw = (int64_t)height * width;
-  const size_t es = eps_dtype == PWW_DTYPE_F32 ? 4 : 2;
-  const bool px4 = (hw % 4) == 0 && aligned16(latents) && aligned16(history) && (!noise || aligned16(noise));
-  // channels-last packed rows: pixel p's 4 channels at 4p (8 bytes per pixel in fp16 / bf16, 16 in fp32)
-  const size_t need = px4 ? 16 : 4 * es;
-  const bool cl = eps_channel_stride == 1 && eps_col_stride == 4 && eps_row_stride == 4 * (int64_t)width &&
-                  (reinterpret_cast<uintptr_t>(eps) % need) == 0 && ((size_t)eps_batch_stride * es) % need == 0;
-  cudaStream_t s = (cudaStream_t)stream;
-  const pww::smp::BlendArgs none{};
-  const cudaError_t e = eps_dtype == PWW_DTYPE_F16    ? pww::smp::launch_update<__half, false>(a, none, px4, cl, s)
-                        : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_update<__nv_bfloat16, false>(a, none, px4, cl, s)
-                                                      : pww::smp::launch_update<float, false>(a, none, px4, cl, s);
+  bool px4, cl;
+  const int st = update_setup(eps, eps_dtype, eps_batch_stride, eps_channel_stride, eps_row_stride, eps_col_stride,
+                              latents, history, history_len, noise, guidance, beta, form, m, height, width, true, a,
+                              px4, cl);
+  if (st != PWW_OK) return st;
+  const cudaError_t e = with_dtype(eps_dtype, [&](auto t) {
+    return pww::smp::launch_update<decltype(t), false>(a, pww::smp::BlendArgs{}, px4, cl, (cudaStream_t)stream);
+  });
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 
@@ -793,28 +813,19 @@ int pww_sampler_update_rescale(const void* eps, int eps_dtype, int64_t eps_batch
                                int history_len, const float* noise, const float* guidance, const float* beta,
                                const float* form, const float* rescale, float* stats_out, int m, int height, int width,
                                void* stream) {
-  if (!eps || !latents || !history || !guidance || !beta || !form || !rescale) return PWW_ERR_BAD_ARG;
-  if (m <= 0 || height <= 0 || width <= 0 || history_len < 1 || history_len > 4) return PWW_ERR_BAD_ARG;
-  if (eps_dtype != PWW_DTYPE_F32 && eps_dtype != PWW_DTYPE_F16 && eps_dtype != PWW_DTYPE_BF16) return PWW_ERR_UNSUPPORTED;
+  if (!rescale) return PWW_ERR_BAD_ARG;
   pww::smp::UpdateArgs a;
-  a.eps = eps; a.e_sn = eps_batch_stride; a.e_sc = eps_channel_stride; a.e_sh = eps_row_stride; a.e_sw = eps_col_stride;
-  a.lat = latents; a.hist = history; a.noise = noise; a.gscale = guidance; a.beta = beta; a.form = form;
-  a.m = m; a.h = height; a.w = width; a.nh = history_len;
+  bool px4, cl;
+  const int st = update_setup(eps, eps_dtype, eps_batch_stride, eps_channel_stride, eps_row_stride, eps_col_stride,
+                              latents, history, history_len, noise, guidance, beta, form, m, height, width, true, a,
+                              px4, cl);
+  if (st != PWW_OK) return st;
   pww::smp::RescaleArgs r;
   r.phi = rescale; r.stats = stats_out;
-  // the same pixel grouping and channels-last test as pww_sampler_update
-  const int64_t hw = (int64_t)height * width;
-  const size_t es = eps_dtype == PWW_DTYPE_F32 ? 4 : 2;
-  const bool px4 = (hw % 4) == 0 && aligned16(latents) && aligned16(history) && (!noise || aligned16(noise));
-  const size_t need = px4 ? 16 : 4 * es;
-  const bool cl = eps_channel_stride == 1 && eps_col_stride == 4 && eps_row_stride == 4 * (int64_t)width &&
-                  (reinterpret_cast<uintptr_t>(eps) % need) == 0 && ((size_t)eps_batch_stride * es) % need == 0;
-  cudaStream_t s = (cudaStream_t)stream;
-  const pww::smp::BlendArgs none{};
-  const cudaError_t e =
-      eps_dtype == PWW_DTYPE_F16    ? pww::smp::launch_update_rescale<__half, false>(a, r, none, px4, cl, s)
-      : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_update_rescale<__nv_bfloat16, false>(a, r, none, px4, cl, s)
-                                    : pww::smp::launch_update_rescale<float, false>(a, r, none, px4, cl, s);
+  const cudaError_t e = with_dtype(eps_dtype, [&](auto t) {
+    return pww::smp::launch_update_rescale<decltype(t), false>(a, r, pww::smp::BlendArgs{}, px4, cl,
+                                                               (cudaStream_t)stream);
+  });
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 
@@ -824,37 +835,24 @@ int pww_sampler_update_masked(const void* eps, int eps_dtype, int64_t eps_batch_
                               const float* form, const float* rescale, float* stats_out, const float* init_latents,
                               const float* init_noise, const float* mask, const float* sigma_next, int m, int height,
                               int width, void* stream) {
-  if (!eps || !latents || !history || !guidance || !beta || !form) return PWW_ERR_BAD_ARG;
   if (!init_latents || !init_noise || !mask || !sigma_next || (stats_out && !rescale)) return PWW_ERR_BAD_ARG;
-  if (m <= 0 || height <= 0 || width <= 0 || history_len < 1 || history_len > 4) return PWW_ERR_BAD_ARG;
-  if (eps_dtype != PWW_DTYPE_F32 && eps_dtype != PWW_DTYPE_F16 && eps_dtype != PWW_DTYPE_BF16) return PWW_ERR_UNSUPPORTED;
   pww::smp::UpdateArgs a;
-  a.eps = eps; a.e_sn = eps_batch_stride; a.e_sc = eps_channel_stride; a.e_sh = eps_row_stride; a.e_sw = eps_col_stride;
-  a.lat = latents; a.hist = history; a.noise = noise; a.gscale = guidance; a.beta = beta; a.form = form;
-  a.m = m; a.h = height; a.w = width; a.nh = history_len;
+  bool px4, cl;
+  // the blend inputs are read 4 pixels at a time too
+  const bool blend16 = aligned16(init_latents) && aligned16(init_noise) && aligned16(mask);
+  const int st = update_setup(eps, eps_dtype, eps_batch_stride, eps_channel_stride, eps_row_stride, eps_col_stride,
+                              latents, history, history_len, noise, guidance, beta, form, m, height, width, blend16, a,
+                              px4, cl);
+  if (st != PWW_OK) return st;
   pww::smp::BlendArgs bl;
   bl.init = init_latents; bl.noise0 = init_noise; bl.mask = mask; bl.sigma_next = sigma_next;
-  // pww_sampler_update's pixel grouping and channels-last test, with the blend inputs read 4 pixels at a time too
-  const int64_t hw = (int64_t)height * width;
-  const size_t es = eps_dtype == PWW_DTYPE_F32 ? 4 : 2;
-  const bool px4 = (hw % 4) == 0 && aligned16(latents) && aligned16(history) && (!noise || aligned16(noise)) &&
-                   aligned16(init_latents) && aligned16(init_noise) && aligned16(mask);
-  const size_t need = px4 ? 16 : 4 * es;
-  const bool cl = eps_channel_stride == 1 && eps_col_stride == 4 && eps_row_stride == 4 * (int64_t)width &&
-                  (reinterpret_cast<uintptr_t>(eps) % need) == 0 && ((size_t)eps_batch_stride * es) % need == 0;
-  cudaStream_t s = (cudaStream_t)stream;
-  cudaError_t e;
-  if (rescale) {
-    pww::smp::RescaleArgs r;
-    r.phi = rescale; r.stats = stats_out;
-    e = eps_dtype == PWW_DTYPE_F16    ? pww::smp::launch_update_rescale<__half, true>(a, r, bl, px4, cl, s)
-        : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_update_rescale<__nv_bfloat16, true>(a, r, bl, px4, cl, s)
-                                      : pww::smp::launch_update_rescale<float, true>(a, r, bl, px4, cl, s);
-  } else {
-    e = eps_dtype == PWW_DTYPE_F16    ? pww::smp::launch_update<__half, true>(a, bl, px4, cl, s)
-        : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_update<__nv_bfloat16, true>(a, bl, px4, cl, s)
-                                      : pww::smp::launch_update<float, true>(a, bl, px4, cl, s);
-  }
+  pww::smp::RescaleArgs r;
+  r.phi = rescale; r.stats = stats_out;
+  const cudaError_t e = with_dtype(eps_dtype, [&](auto t) {
+    using T = decltype(t);
+    return rescale ? pww::smp::launch_update_rescale<T, true>(a, r, bl, px4, cl, (cudaStream_t)stream)
+                   : pww::smp::launch_update<T, true>(a, bl, px4, cl, (cudaStream_t)stream);
+  });
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 
@@ -871,10 +869,9 @@ int pww_window_input(const float* latents, const float* scale, const int* row_st
   a.lat = latents; a.scale = scale; a.rows = row_starts; a.cols = col_starts; a.out = out;
   a.n_cols = n_cols; a.first = first_view; a.n = n_views; a.window = window; a.H = height; a.W = width;
   const bool px4 = (window % 4) == 0 && aligned16(out);
-  cudaStream_t s = (cudaStream_t)stream;
-  const cudaError_t e = out_dtype == PWW_DTYPE_F16    ? pww::smp::launch_window_input<__half>(a, px4, s)
-                        : out_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_window_input<__nv_bfloat16>(a, px4, s)
-                                                      : pww::smp::launch_window_input<float>(a, px4, s);
+  const cudaError_t e = with_dtype(out_dtype, [&](auto t) {
+    return pww::smp::launch_window_input<decltype(t)>(a, px4, (cudaStream_t)stream);
+  });
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 
@@ -902,20 +899,17 @@ int pww_window_update(const void* const* eps, int n_chunks, int views_per_chunk,
     t.eps[k] = eps[k];
     cl = cl && (reinterpret_cast<uintptr_t>(eps[k]) % need) == 0;
   }
-  pww::smp::UpdateArgs a{}, o{};
+  pww::smp::UpdateArgs a{};
   a.lat = latents; a.hist = history; a.noise = noise; a.gscale = guidance; a.beta = beta; a.form = form;
   a.m = 1; a.h = height; a.w = width; a.nh = history_len;
-  o.e_sn = eps_batch_stride; o.e_sc = eps_channel_stride; o.e_sh = eps_row_stride; o.e_sw = eps_col_stride;
-  o.w = window;
   pww::smp::WindowArgs v;
   v.rows = row_starts; v.cols = col_starts; v.n_rows = n_rows; v.n_cols = n_cols; v.window = window;
   v.per_chunk = views_per_chunk; v.views = (int)views;
+  v.e_sn = eps_batch_stride; v.e_sc = eps_channel_stride; v.e_sh = eps_row_stride; v.e_sw = eps_col_stride;
   const bool px4 = (width % 4) == 0 && aligned16(latents) && aligned16(history) && (!noise || aligned16(noise));
-  cudaStream_t s = (cudaStream_t)stream;
-  const cudaError_t e =
-      eps_dtype == PWW_DTYPE_F16    ? pww::smp::launch_window_update<__half>(a, o, v, t, px4, cl, s)
-      : eps_dtype == PWW_DTYPE_BF16 ? pww::smp::launch_window_update<__nv_bfloat16>(a, o, v, t, px4, cl, s)
-                                    : pww::smp::launch_window_update<float>(a, o, v, t, px4, cl, s);
+  const cudaError_t e = with_dtype(eps_dtype, [&](auto et) {
+    return pww::smp::launch_window_update<decltype(et)>(a, v, t, px4, cl, (cudaStream_t)stream);
+  });
   return e == cudaSuccess ? PWW_OK : cuda_fail(e);
 }
 

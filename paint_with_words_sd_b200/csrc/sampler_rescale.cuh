@@ -26,20 +26,6 @@ struct RescaleArgs {
   float* stats;                         // [m, 3] (std_cond, std_cfg, k), or NULL
 };
 
-// c = out_c and f = cfg of image i at pixels p0 .. p0 + PX - 1; f is guided_eps's arithmetic.
-template <typename T, int PX, bool CL>
-__device__ __forceinline__ void cond_and_cfg(const UpdateArgs& a, int i, int p0, float (&c)[4][PX],
-                                             float (&f)[4][PX]) {
-  const T* eps = static_cast<const T*>(a.eps);
-  const float g = __ldg(a.gscale + i);
-  load_eps<T, PX, CL>(eps + (int64_t)i * a.e_sn, a, p0, c);
-  load_eps<T, PX, CL>(eps + (int64_t)(i + a.m) * a.e_sn, a, p0, f);
-#pragma unroll
-  for (int ch = 0; ch < 4; ++ch)
-#pragma unroll
-    for (int j = 0; j < PX; ++j) f[ch][j] = __fadd_rn(f[ch][j], __fmul_rn(g, __fsub_rn(c[ch][j], f[ch][j])));
-}
-
 template <int PX>
 __device__ __forceinline__ void add_values(const float (&c)[4][PX], const float (&f)[4][PX], float2& s) {
 #pragma unroll
@@ -93,8 +79,8 @@ __device__ __forceinline__ float2 cluster_sum(float2 v, float2* warp_part, float
   return t;
 }
 
-// out' = k cfg (phi == 0: cfg itself, k never applied), then sampler_update_kernel's step form (and, BLEND, its
-// mask blend), operation for operation, on the 4 channels of pixels p0 .. p0 + PX - 1 of image i.
+// out' = k cfg (phi == 0: cfg itself, k never applied), then step_form on the 4 channels of pixels
+// p0 .. p0 + PX - 1 of image i.
 template <int PX, bool BLEND>
 __device__ __forceinline__ void rescaled_update(const UpdateArgs& a, const BlendArgs& bl, int i, int p0,
                                                 float (&eg)[4][PX], float phi, float k) {
@@ -104,47 +90,7 @@ __device__ __forceinline__ void rescaled_update(const UpdateArgs& a, const Blend
 #pragma unroll
       for (int j = 0; j < PX; ++j) eg[c][j] = __fmul_rn(k, eg[c][j]);
   }
-  const int hw = a.h * a.w;
-  const float alpha = __ldg(a.form + 0), ca = __ldg(a.form + 1), cb = __ldg(a.form + 2), gamma = __ldg(a.form + 3);
-  const int slot = (int)__ldg(a.form + 4), row = (int)__ldg(a.form + 5);
-  const float b0 = __ldg(a.beta + 0);
-  const bool with_noise = a.noise != nullptr && gamma != 0.f;
-  const int64_t entry = (int64_t)a.m * 4 * hw;
-  float mk[PX], sn = 0.f;
-  if constexpr (BLEND) {
-    load_px<PX>(bl.mask + (int64_t)i * hw + p0, mk);
-    sn = __ldg(bl.sigma_next);
-  }
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
-    const int64_t off = ((int64_t)i * 4 + c) * hw + p0;
-    float x[PX], q[PX], s[PX];
-    load_px<PX>(a.lat + off, x);
-#pragma unroll
-    for (int j = 0; j < PX; ++j) {
-      const float e = eg[c][j];
-      q[j] = ca == 0.f ? __fmul_rn(cb, e) : __fadd_rn(__fmul_rn(ca, x[j]), __fmul_rn(cb, e));
-      s[j] = __fmul_rn(b0, q[j]);
-    }
-    store_px<PX>(a.hist + slot * entry + off, q);
-    for (int k2 = 1; k2 < a.nh; ++k2) {
-      const float bk = __ldg(a.beta + k2);
-      float hk[PX];
-      load_px<PX>(a.hist + ((slot - k2 + a.nh) % a.nh) * entry + off, hk);
-#pragma unroll
-      for (int j = 0; j < PX; ++j) s[j] = __fadd_rn(s[j], __fmul_rn(bk, hk[j]));
-    }
-#pragma unroll
-    for (int j = 0; j < PX; ++j) x[j] = alpha == 1.f ? __fadd_rn(x[j], s[j]) : __fadd_rn(__fmul_rn(alpha, x[j]), s[j]);
-    if (with_noise) {
-      float z[PX];
-      load_px<PX>(a.noise + row * entry + off, z);
-#pragma unroll
-      for (int j = 0; j < PX; ++j) x[j] = __fadd_rn(x[j], __fmul_rn(gamma, z[j]));
-    }
-    if constexpr (BLEND) blend_px<PX>(bl, off, mk, sn, x);
-    store_px<PX>(a.lat + off, x);
-  }
+  step_form<PX, BLEND>(a, bl, i, p0, a.m, a.h * a.w, eg);
 }
 
 // One cluster per image; thread t of CTA rank r owns the PX-pixel groups r * 512 + t + k * (cluster size * 512).
@@ -236,11 +182,7 @@ cudaError_t launch_rescale_instance(const UpdateArgs& a, const RescaleArgs& r, c
 template <typename T, bool BLEND>
 cudaError_t launch_update_rescale(const UpdateArgs& a, const RescaleArgs& r, const BlendArgs& bl, bool px4, bool cl,
                                   cudaStream_t s) {
-  if (px4)
-    return cl ? launch_rescale_instance<T, 4, true, BLEND>(a, r, bl, s)
-              : launch_rescale_instance<T, 4, false, BLEND>(a, r, bl, s);
-  return cl ? launch_rescale_instance<T, 1, true, BLEND>(a, r, bl, s)
-            : launch_rescale_instance<T, 1, false, BLEND>(a, r, bl, s);
+  return with_layout(px4, cl, [&](auto px, auto c) { return launch_rescale_instance<T, px, c, BLEND>(a, r, bl, s); });
 }
 
 }  // namespace smp

@@ -11,6 +11,8 @@
 // noise path at the next sigma (masked img2img):
 //   x_next = M x_next + (1 - M) (init + z0 sigma')
 #pragma once
+#include <type_traits>
+
 #include "pww_common.cuh"
 
 namespace pww {
@@ -82,10 +84,12 @@ __device__ __forceinline__ void store_px(float* p, const float (&v)[PX]) {
   }
 }
 
-// e[c][j] = channel c of pixel p0 + j of one image's eps.  CL: channels-last packed rows (pixel p's 4 channels at
-// 4p .. 4p+3), read with 8- or 16-byte accesses; otherwise one strided load per element.
+// e[c][j] = channel c of pixel p0 + j of one image's eps, whose rows are w pixels wide.  CL: channels-last packed rows
+// (pixel p's 4 channels at 4p .. 4p+3), read with 8- or 16-byte accesses; otherwise one strided load per element, with
+// the channel, row and column strides sc, sh and sw.
 template <typename T, int PX, bool CL>
-__device__ __forceinline__ void load_eps(const T* base, const UpdateArgs& a, int p0, float (&e)[4][PX]) {
+__device__ __forceinline__ void load_eps(const T* base, int64_t sc, int64_t sh, int64_t sw, int w, int p0,
+                                         float (&e)[4][PX]) {
   if constexpr (CL && sizeof(T) == 4) {
     const float4* s = reinterpret_cast<const float4*>(base + (int64_t)p0 * 4);
 #pragma unroll
@@ -109,26 +113,31 @@ __device__ __forceinline__ void load_eps(const T* base, const UpdateArgs& a, int
   } else {
 #pragma unroll
     for (int j = 0; j < PX; ++j) {
-      const int p = p0 + j, y = p / a.w, x = p - y * a.w;
-      const T* px = base + y * a.e_sh + x * a.e_sw;
+      const int p = p0 + j, y = p / w, x = p - y * w;
+      const T* px = base + y * sh + x * sw;
 #pragma unroll
-      for (int c = 0; c < 4; ++c) e[c][j] = to_f(px[c * a.e_sc]);
+      for (int c = 0; c < 4; ++c) e[c][j] = to_f(px[c * sc]);
     }
   }
 }
 
-// e[c][j] = eps_u + g (eps_c - eps_u) of image i.
+// The CFG combine of one value: eps_u + g (eps_c - eps_u).
+__device__ __forceinline__ float cfg(float g, float ec, float eu) {
+  return __fadd_rn(eu, __fmul_rn(g, __fsub_rn(ec, eu)));
+}
+
+// c = eps_c and f = the guided eps of image i at pixels p0 .. p0 + PX - 1.
 template <typename T, int PX, bool CL>
-__device__ __forceinline__ void guided_eps(const UpdateArgs& a, int i, int p0, float (&e)[4][PX]) {
+__device__ __forceinline__ void cond_and_cfg(const UpdateArgs& a, int i, int p0, float (&c)[4][PX],
+                                             float (&f)[4][PX]) {
   const T* eps = static_cast<const T*>(a.eps);
   const float g = __ldg(a.gscale + i);
-  float eu[4][PX];
-  load_eps<T, PX, CL>(eps + (int64_t)i * a.e_sn, a, p0, e);
-  load_eps<T, PX, CL>(eps + (int64_t)(i + a.m) * a.e_sn, a, p0, eu);
+  load_eps<T, PX, CL>(eps + (int64_t)i * a.e_sn, a.e_sc, a.e_sh, a.e_sw, a.w, p0, c);
+  load_eps<T, PX, CL>(eps + (int64_t)(i + a.m) * a.e_sn, a.e_sc, a.e_sh, a.e_sw, a.w, p0, f);
 #pragma unroll
-  for (int c = 0; c < 4; ++c)
+  for (int ch = 0; ch < 4; ++ch)
 #pragma unroll
-    for (int j = 0; j < PX; ++j) e[c][j] = __fadd_rn(eu[c][j], __fmul_rn(g, __fsub_rn(e[c][j], eu[c][j])));
+    for (int j = 0; j < PX; ++j) f[ch][j] = cfg(g, c[ch][j], f[ch][j]);
 }
 
 // The masked instances' epilogue on one channel's PX values x of the step's result, at element offset `off`:
@@ -145,16 +154,12 @@ __device__ __forceinline__ void blend_px(const BlendArgs& bl, int64_t off, const
     x[j] = __fadd_rn(__fmul_rn(mk[j], x[j]), __fmul_rn(__fsub_rn(1.f, mk[j]), __fadd_rn(x0[j], __fmul_rn(z0[j], sn))));
 }
 
-// One thread per (image, PX consecutive pixels), all 4 channels.  `bl` is read only by the BLEND instances.
-template <typename T, int PX, bool CL, bool BLEND>
-__global__ void __launch_bounds__(kThreads) sampler_update_kernel(const UpdateArgs a, const BlendArgs bl) {
-  const int hw = a.h * a.w, groups = hw / PX;
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (int64_t)a.m * groups) return;
-  const int i = (int)(idx / groups);
-  const int p0 = (int)(idx - (int64_t)i * groups) * PX;
-  float eg[4][PX];
-  guided_eps<T, PX, CL>(a, i, p0, eg);
+// The step form, shared by the plain, rescale and panorama updates, on the guided eps eg of image i at pixels
+// p0 .. p0 + PX - 1 (m images of hw pixels in a history entry / noise row): writes the history entry, then the latents,
+// with the BLEND instances' mask blend before the store.  `bl` is read only by the BLEND instances.
+template <int PX, bool BLEND>
+__device__ __forceinline__ void step_form(const UpdateArgs& a, const BlendArgs& bl, int i, int p0, int m, int hw,
+                                          const float (&eg)[4][PX]) {
   float mk[PX], sn = 0.f;
   if constexpr (BLEND) {
     load_px<PX>(bl.mask + (int64_t)i * hw + p0, mk);
@@ -164,7 +169,7 @@ __global__ void __launch_bounds__(kThreads) sampler_update_kernel(const UpdateAr
   const int slot = (int)__ldg(a.form + 4), row = (int)__ldg(a.form + 5);
   const float b0 = __ldg(a.beta + 0);
   const bool with_noise = a.noise != nullptr && gamma != 0.f;
-  const int64_t entry = (int64_t)a.m * 4 * hw;   // elements of one history entry / noise row
+  const int64_t entry = (int64_t)m * 4 * hw;   // elements of one history entry / noise row
 #pragma unroll
   for (int c = 0; c < 4; ++c) {
     const int64_t off = ((int64_t)i * 4 + c) * hw + p0;
@@ -195,6 +200,19 @@ __global__ void __launch_bounds__(kThreads) sampler_update_kernel(const UpdateAr
     if constexpr (BLEND) blend_px<PX>(bl, off, mk, sn, x);
     store_px<PX>(a.lat + off, x);
   }
+}
+
+// One thread per (image, PX consecutive pixels), all 4 channels.  `bl` is read only by the BLEND instances.
+template <typename T, int PX, bool CL, bool BLEND>
+__global__ void __launch_bounds__(kThreads) sampler_update_kernel(const UpdateArgs a, const BlendArgs bl) {
+  const int hw = a.h * a.w, groups = hw / PX;
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (int64_t)a.m * groups) return;
+  const int i = (int)(idx / groups);
+  const int p0 = (int)(idx - (int64_t)i * groups) * PX;
+  float ec[4][PX], eg[4][PX];
+  cond_and_cfg<T, PX, CL>(a, i, p0, ec, eg);
+  step_form<PX, BLEND>(a, bl, i, p0, a.m, hw, eg);
 }
 
 template <typename T, int PX>
@@ -237,19 +255,22 @@ __global__ void __launch_bounds__(kThreads) sampler_input_kernel(const InputArgs
 
 inline unsigned blocks_for(int64_t threads) { return (unsigned)((threads + kThreads - 1) / kThreads); }
 
+// f(integral_constant<int, PX>{}, bool_constant<CL>{}) for the update kernels' layout: PX = 4 or 1 pixels per thread,
+// CL = channels-last packed eps rows or strided.
+template <typename F>
+cudaError_t with_layout(bool px4, bool cl, F&& f) {
+  using P1 = std::integral_constant<int, 1>;
+  using P4 = std::integral_constant<int, 4>;
+  if (px4) return cl ? f(P4{}, std::true_type{}) : f(P4{}, std::false_type{});
+  return cl ? f(P1{}, std::true_type{}) : f(P1{}, std::false_type{});
+}
+
 template <typename T, bool BLEND>
 cudaError_t launch_update(const UpdateArgs& a, const BlendArgs& bl, bool px4, bool cl, cudaStream_t s) {
-  const int64_t hw = (int64_t)a.h * a.w;
-  if (px4) {
-    const unsigned g = blocks_for(a.m * hw / 4);
-    if (cl) sampler_update_kernel<T, 4, true, BLEND><<<g, kThreads, 0, s>>>(a, bl);
-    else sampler_update_kernel<T, 4, false, BLEND><<<g, kThreads, 0, s>>>(a, bl);
-  } else {
-    const unsigned g = blocks_for(a.m * hw);
-    if (cl) sampler_update_kernel<T, 1, true, BLEND><<<g, kThreads, 0, s>>>(a, bl);
-    else sampler_update_kernel<T, 1, false, BLEND><<<g, kThreads, 0, s>>>(a, bl);
-  }
-  return cudaGetLastError();
+  return with_layout(px4, cl, [&](auto px, auto c) {
+    sampler_update_kernel<T, px, c, BLEND><<<blocks_for(a.m * (int64_t)a.h * a.w / px), kThreads, 0, s>>>(a, bl);
+    return cudaGetLastError();
+  });
 }
 
 template <typename T>

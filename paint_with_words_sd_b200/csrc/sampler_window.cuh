@@ -7,11 +7,11 @@
 //
 // The update's arithmetic, fp32 with explicit round-to-nearest intrinsics, per canvas value with the covering
 // windows v1 < v2 < ... < vc:
-//   g_v = eps_u,v + gs (eps_c,v - eps_u,v)        guided_eps's ops, at the window-local position
+//   g_v = eps_u,v + gs (eps_c,v - eps_u,v)        cfg's ops, at the window-local position
 //   E   = g_v1;  E = E + g_v2;  ...;  E = E + g_vc
 //   e   = E / c
-// then sampler_update_kernel's step form on (x, e) with m = 1.  One thread owns each canvas value, so the result does
-// not depend on how the windows are split into chunks.
+// then step_form on (x, e) with m = 1.  One thread owns each canvas value, so the result does not depend on how the
+// windows are split into chunks.
 #pragma once
 #include "sampler_step.cuh"
 
@@ -34,6 +34,7 @@ struct WindowArgs {
   const int* cols;                      // [n_cols]
   int n_rows, n_cols, window;
   int per_chunk, views;                 // windows per chunk (the last chunk may hold fewer), windows in all
+  int64_t e_sn, e_sc, e_sh, e_sw;       // the window outputs' element strides
 };
 
 // The UNet outputs of the chunks: chunk k's [2 n_k, 4, window, window] holds its windows' cond rows, then their
@@ -70,11 +71,10 @@ __global__ void __launch_bounds__(kThreads) window_input_kernel(const WindowInpu
 }
 
 // One thread per PX consecutive canvas pixels of one row, all 4 channels.  `a` describes the canvas (m = 1, h = H,
-// w = W, the latents, history, noise, guidance scale and step rows); `o` only the window outputs' strides and width
-// (o.w = window), for load_eps.
+// w = W, the latents, history, noise, guidance scale and step rows).
 template <typename T, int PX, bool CL>
-__global__ void __launch_bounds__(kThreads) window_update_kernel(const UpdateArgs a, const UpdateArgs o,
-                                                                  const WindowArgs v, const WindowOutputs t) {
+__global__ void __launch_bounds__(kThreads) window_update_kernel(const UpdateArgs a, const WindowArgs v,
+                                                                  const WindowOutputs t) {
   const int hw = a.h * a.w, groups = hw / PX;
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= groups) return;
@@ -96,11 +96,11 @@ __global__ void __launch_bounds__(kThreads) window_update_kernel(const UpdateArg
         const int n = min(v.per_chunk, v.views - chunk * v.per_chunk);
         const T* base = static_cast<const T*>(t.eps[chunk]);
         float ec[4][1], eu[4][1];
-        load_eps<T, 1, CL>(base + (int64_t)k * o.e_sn, o, ly * v.window + lx, ec);
-        load_eps<T, 1, CL>(base + (int64_t)(k + n) * o.e_sn, o, ly * v.window + lx, eu);
+        load_eps<T, 1, CL>(base + (int64_t)k * v.e_sn, v.e_sc, v.e_sh, v.e_sw, v.window, ly * v.window + lx, ec);
+        load_eps<T, 1, CL>(base + (int64_t)(k + n) * v.e_sn, v.e_sc, v.e_sh, v.e_sw, v.window, ly * v.window + lx, eu);
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
-          const float gv = __fadd_rn(eu[c][0], __fmul_rn(g, __fsub_rn(ec[c][0], eu[c][0])));
+          const float gv = cfg(g, ec[c][0], eu[c][0]);
           e[c] = cnt == 0 ? gv : __fadd_rn(e[c], gv);
         }
         ++cnt;
@@ -109,41 +109,7 @@ __global__ void __launch_bounds__(kThreads) window_update_kernel(const UpdateArg
 #pragma unroll
     for (int c = 0; c < 4; ++c) eg[c][j] = __fdiv_rn(e[c], (float)cnt);
   }
-  // sampler_update_kernel's step form for image 0 (that kernel stays as it is; the same operations in the same order)
-  const float alpha = __ldg(a.form + 0), ca = __ldg(a.form + 1), cb = __ldg(a.form + 2), gamma = __ldg(a.form + 3);
-  const int slot = (int)__ldg(a.form + 4), row = (int)__ldg(a.form + 5);
-  const float b0 = __ldg(a.beta + 0);
-  const bool with_noise = a.noise != nullptr && gamma != 0.f;
-  const int64_t entry = (int64_t)4 * hw;
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
-    const int64_t off = (int64_t)c * hw + p0;
-    float x[PX], q[PX], s[PX];
-    load_px<PX>(a.lat + off, x);
-#pragma unroll
-    for (int j = 0; j < PX; ++j) {
-      const float e = eg[c][j];
-      q[j] = ca == 0.f ? __fmul_rn(cb, e) : __fadd_rn(__fmul_rn(ca, x[j]), __fmul_rn(cb, e));
-      s[j] = __fmul_rn(b0, q[j]);
-    }
-    store_px<PX>(a.hist + slot * entry + off, q);
-    for (int k = 1; k < a.nh; ++k) {
-      const float bk = __ldg(a.beta + k);
-      float hk[PX];
-      load_px<PX>(a.hist + ((slot - k + a.nh) % a.nh) * entry + off, hk);
-#pragma unroll
-      for (int j = 0; j < PX; ++j) s[j] = __fadd_rn(s[j], __fmul_rn(bk, hk[j]));
-    }
-#pragma unroll
-    for (int j = 0; j < PX; ++j) x[j] = alpha == 1.f ? __fadd_rn(x[j], s[j]) : __fadd_rn(__fmul_rn(alpha, x[j]), s[j]);
-    if (with_noise) {
-      float z[PX];
-      load_px<PX>(a.noise + row * entry + off, z);
-#pragma unroll
-      for (int j = 0; j < PX; ++j) x[j] = __fadd_rn(x[j], __fmul_rn(gamma, z[j]));
-    }
-    store_px<PX>(a.lat + off, x);
-  }
+  step_form<PX, false>(a, BlendArgs{}, 0, p0, 1, hw, eg);
 }
 
 template <typename T>
@@ -155,19 +121,12 @@ cudaError_t launch_window_input(const WindowInputArgs& a, bool px4, cudaStream_t
 }
 
 template <typename T>
-cudaError_t launch_window_update(const UpdateArgs& a, const UpdateArgs& o, const WindowArgs& v,
-                                 const WindowOutputs& t, bool px4, bool cl, cudaStream_t s) {
-  const int64_t hw = (int64_t)a.h * a.w;
-  if (px4) {
-    const unsigned g = blocks_for(hw / 4);
-    if (cl) window_update_kernel<T, 4, true><<<g, kThreads, 0, s>>>(a, o, v, t);
-    else window_update_kernel<T, 4, false><<<g, kThreads, 0, s>>>(a, o, v, t);
-  } else {
-    const unsigned g = blocks_for(hw);
-    if (cl) window_update_kernel<T, 1, true><<<g, kThreads, 0, s>>>(a, o, v, t);
-    else window_update_kernel<T, 1, false><<<g, kThreads, 0, s>>>(a, o, v, t);
-  }
-  return cudaGetLastError();
+cudaError_t launch_window_update(const UpdateArgs& a, const WindowArgs& v, const WindowOutputs& t, bool px4, bool cl,
+                                 cudaStream_t s) {
+  return with_layout(px4, cl, [&](auto px, auto c) {
+    window_update_kernel<T, px, c><<<blocks_for((int64_t)a.h * a.w / px), kThreads, 0, s>>>(a, v, t);
+    return cudaGetLastError();
+  });
 }
 
 }  // namespace smp
